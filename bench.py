@@ -1,12 +1,12 @@
 #!/usr/bin/env python3
-"""bench.py — ECDSA-P256 verifies/s at batch = 64K (BASELINE.json configs[1]) on N B200s.
+"""bench.py — ECDSA-P256 verifies/s at batch = 64K (BASELINE.json configs[1]) on N H100s.
 
 A "step" is one pass of the hot path over one 65,536-signature batch PER GPU (batches shard embarrassingly, so per-GPU
 work is fixed as N grows: weak scaling); with N > 1 every step ends with the all-gather of the packed verdict bitmask
 over NCCL, issued by the engine itself (sbv_gather_verdicts_device: k_pack_bits + ncclAllGather, ordered behind the step on its stream) —
 the only exchange the path has.  No PyTorch kernel runs inside a step.
 
-  value      device-timed, inputs already resident in HBM (16 rotating copies = 168 MB > L2), steps rotating over 4 streams
+  value      device-timed, inputs already resident in HBM (16 rotating copies = 168 MB > 50 MB L2), steps rotating over 4 streams
   e2e        the same metric through the C ABI with pinned HOST buffers (sbv_verify_batch; sbv_verify_batch_ranked when
              N > 1, i.e. INCLUDING the gather): H2D of the 160 B/item batch and D2H of the verdicts inside the timed region
   roofline   dominant kernel (k_verify_kt: the fixed-base kernel the repeated keys of the batch take): achieved wide-MAC/s
@@ -18,6 +18,9 @@ the only exchange the path has.  No PyTorch kernel runs inside a step.
              C4 (n=16 commit-vote quorum stream, 262,144 signatures, sharded by instance over the ranks), C5 (mixed curves)
 
 `--impl reference` times the CPU implementation alone (the reference arm).
+`--dump-outputs DIR` writes the verdicts of the last timed step as DIR/verdicts.npy (float32, 1.0 = accept): the inputs
+are seeded, so two builds run with the same arguments can be compared output for output.  The reference arm verifies
+against its key table by index, not against the per-item (partly corrupted) keys, so its verdicts are its own.
 """
 from __future__ import annotations
 
@@ -39,7 +42,7 @@ MAC32_PER_VERIFY = 272_256       # SURVEY.md §8d canonical count (P-256)
 MAC32_PER_VERIFY_P384 = 902_880
 EXECUTED_MAC32_PER_VERIFY = 68 * (8 * 64 + 3 * 36) + (2 * 64 + 36)   # fixed-base path, P-256 (DESIGN.md §6)
 BYTES_PER_VERIFY = 161           # 160 B in + 1 B out
-N_COPIES = 16                    # rotating input copies: 16 x 10.5 MB > 126 MB L2
+N_COPIES = 16                    # rotating input copies: 16 x 10.5 MB > 50 MB L2 (H100)
 N_LANES = int(os.environ.get("SBV_BENCH_LANES", "4"))   # CUDA streams the device-timed steps rotate over
 METRIC = "ECDSA-P256 verifies/sec at batch=64K"
 WORKLOAD = "C2: ECDSA-P256 batch verify, 65,536 synthetic sigs per GPU, 1,024 keys, 1/16 corrupted"
@@ -48,19 +51,19 @@ WORKLOAD = "C2: ECDSA-P256 batch verify, 65,536 synthetic sigs per GPU, 1,024 ke
 def base_config(world):
     """The workload — the same dict, key for key, in both arms (the driver compares them)."""
     return {"workload": WORKLOAD, "batch_per_gpu": BATCH, "keys": KEYS, "seed": "1 + 1000*rank", "sharding": f"batch-parallel x{world}",
-            "l2": f"GPU arm: {N_COPIES} rotating input copies per rank (168 MB > 126 MB L2), no flush needed; CPU arm: the rank-0 batch (10.5 MB) every step"}
+            "l2": f"GPU arm: {N_COPIES} rotating input copies per rank (168 MB > 50 MB L2), no flush needed; CPU arm: the rank-0 batch (10.5 MB) every step"}
 
 
 def load_peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         with open(p) as f:
-            return json.load(f).get("hbm_gbs", 6650.0), "measured"
-    return 6650.0, "fallback"
+            return json.load(f).get("hbm_gbs", 3350.0), "measured"
+    return 3350.0, "H100 SXM data sheet"
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
 
     # (no power.draw: the power sensor read is the one query that can hold the GPU for milliseconds)
     Q = ("index,clocks.sm,clocks.max.sm,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
@@ -136,9 +139,12 @@ def run_reference(args, rank, world):
     for _ in range(max(args.warmup, 1)):
         oracle.bench_verify(oracle.P256, b["r"][:8192], b["s"][:8192], keys, b["key_idx"][:8192], b["digest"][:8192], nthreads=cores)
     total = 0.0
+    ok = None
     for _ in range(args.steps):
         t, ok = oracle.bench_verify(oracle.P256, b["r"], b["s"], keys, b["key_idx"], b["digest"], nthreads=cores)
         total += t
+    if args.dump_outputs and ok is not None:
+        dump_outputs(args.dump_outputs, {"verdicts": ok})
     value = BATCH * args.steps / total
     line = {
         "impl": "reference", "metric": METRIC, "value": value, "unit": "verifies/s", "n_gpus": args.gpus, "steps": args.steps,
@@ -151,6 +157,14 @@ def run_reference(args, rank, world):
         "gpu_launches": 0,
     }
     print(json.dumps(line), flush=True)
+
+
+def dump_outputs(out_dir, arrays):
+    """Writes each array as out_dir/<name>.npy in float32 (what the timed path returned to its caller)."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, f"{name}.npy"), np.asarray(a, dtype=np.float32))
 
 
 def pack_bits(ok):
@@ -166,6 +180,8 @@ def main():
     ap.add_argument("--impl", default="sbv", choices=["sbv", "reference"])
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-extras", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the verdicts of the last timed step to DIR/verdicts.npy (float32)")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3)
 
@@ -193,9 +209,8 @@ def main():
     eng = sbv.Engine(devices=[local_rank])
     # one-process-per-GPU: the engines form their own NCCL communicators (one channel per concurrent stream / caller);
     # torch.distributed only carries the 128-byte ids and the final max-over-ranks
-    # caller threads of the e2e leg: four keep one GPU busy; on the 8-GPU box three measured better than four
-    # (profiles/r02_scaling.txt: the ranks' synchronous calls meet in a gather every call, and more callers per rank made
-    # the slowest rank slower), so N = 8 runs with three
+    # caller threads of the e2e leg: four keep one GPU busy; at N = 8 three (the ranks' synchronous calls meet in a gather
+    # every call, and more callers per rank make the slowest rank slower)
     e2e_threads = int(os.environ.get("SBV_BENCH_E2E_THREADS", "4" if world <= 4 else "3"))
     n_channels = N_LANES + e2e_threads
     if world > 1:
@@ -278,7 +293,7 @@ def main():
     sampler.mark()
     e0.record()
     fork_lanes()
-    diag = os.environ.get("SBV_BENCH_DIAG", "0") != "0"   # per-step completion events cost 4-5 % of the throughput (profiles/r02_variants.md): off by default
+    diag = os.environ.get("SBV_BENCH_DIAG", "0") != "0"   # per-step completion events cost throughput: off by default
     step_done = [torch.cuda.Event(enable_timing=True) for _ in range(args.steps if diag else 0)]
     for i in range(args.steps):
         device_step(args.warmup + i)
@@ -302,6 +317,8 @@ def main():
             raise SystemExit("bench: pipelined verdicts differ from the oracle")
         if world > 1 and not np.array_equal(d_masks[k].cpu().numpy(), want_mask_all):
             raise SystemExit("bench: gathered verdict mask differs from the packed oracle verdicts of all ranks")
+    if args.dump_outputs and rank == 0 and args.steps > 0:
+        dump_outputs(args.dump_outputs, {"verdicts": d_oks[(args.warmup + args.steps - 1) % N_LANES].cpu().numpy()})
     clocks = sampler.stop() if rank == 0 else None
     value = world * BATCH * args.steps / (dev_ms * 1e-3)
 
@@ -427,18 +444,10 @@ def main():
         "frac_executed": BATCH * EXECUTED_MAC32_PER_VERIFY / (k_ms * 1e-3) / mad_peak if mad_peak else None,
         "note": "W = 272,256 MAC32 is SURVEY §8d's canonical double-scalar multiplication; the key-grouped pipeline does less arithmetic per "
                 "verify than the canonical algorithm (no doublings for repeated keys), so the fraction can exceed 1",
-        "traffic": None, "algorithmic_bytes_per_launch": BATCH * BYTES_PER_VERIFY,
+        "algorithmic_bytes_per_launch": BATCH * BYTES_PER_VERIFY,
         "hbm": {"achieved": BATCH * BYTES_PER_VERIFY / (k_ms * 1e-3) / 1e9, "peak": hbm_gbs, "unit": "GB/s",
                 "frac": BATCH * BYTES_PER_VERIFY / (k_ms * 1e-3) / 1e9 / hbm_gbs, "peak_source": hbm_src},
     }
-    tpath = os.path.join(ROOT, "profiles", "r02_traffic.json")
-    if os.path.exists(tpath):
-        try:
-            tj = json.load(open(tpath))
-            roofline["traffic"] = tj.get("dram_bytes_per_launch")
-            roofline["traffic_source"] = tj.get("source")
-        except Exception:
-            pass
 
     cfg = base_config(world)
     execution = dict({         # how THIS arm runs the workload (kept out of `config` so that both arms' configs are identical)

@@ -1,6 +1,6 @@
-"""consensus_b200 — B200-native batched signature verification behind SmartBFT's api.Verifier.
+"""consensus_b200 — H100-native batched signature verification behind SmartBFT's api.Verifier.
 
-The product is ``libsbv.so`` (hand-written sm_100a CUDA + a C ABI, include/sbv.h).  This package is
+The product is ``libsbv.so`` (hand-written sm_90a CUDA + a C ABI, include/sbv.h).  This package is
 the thin ctypes binding used by the tests and bench.py; it never falls back to a CPU
 implementation — if the library is missing or no CUDA device is usable, it raises.
 """

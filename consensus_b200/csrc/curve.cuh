@@ -22,7 +22,7 @@ static __device__ __noinline__ Fe8 p256_nmul_call(Fe8 a, Fe8 b);
 struct P256 {
     static constexpr int N = 8;
     static constexpr int BYTES = 32;
-    static constexpr int GW = 16;              // fixed-base comb window of G: 16 windows x 65536 entries (64 MB, L2-resident)
+    static constexpr int GW = 16;              // fixed-base comb window of G: 16 windows x 65536 entries (64 MB; H100's 50 MB L2 holds most of it)
     static constexpr int GWINS = 256 / GW;
     static constexpr uint32_t NINV = SBV_P256_NINV;
     static constexpr uint32_t PINV = SBV_P256_PINV;
@@ -211,7 +211,7 @@ struct P384 {
 #ifndef SBV_P384_GW
 #define SBV_P384_GW 16
 #endif
-    // fixed-base comb of G: 24 windows x 65,536 entries = 151 MB in HBM (not L2-resident like P-256's 64 MB, but the
+    // fixed-base comb of G: 24 windows x 65,536 entries = 151 MB, mostly in HBM (three times the L2, but the
     // gather of the next entry is in flight during the current addition and a P-384 addition takes microseconds);
     // 24 additions per verify instead of the 48 of an 8-bit comb.  The CPU simulation of tests/ builds an 8-bit one.
     static constexpr int GW = SBV_P384_GW;

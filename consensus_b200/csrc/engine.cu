@@ -1,4 +1,4 @@
-// engine.cu — host side of libsbv.so: the C ABI of include/sbv.h on top of the sm_100a kernels.
+// engine.cu — host side of libsbv.so: the C ABI of include/sbv.h on top of the sm_90a kernels.
 //
 // One engine owns 1..8 devices of one box (single process), or is one RANK of a one-process-per-GPU deployment
 // (sbv_comm_init_rank).  Every batch is sharded into contiguous ranges, one per device.  Every host-buffer entry point
@@ -323,7 +323,7 @@ struct BatchSrc {
 // digests in ln.d_dig) in ln.stream order.  The KEYS go first, so that the grouping and the table construction run while
 // the rest of the batch is still being copied.  A LARGE shard (>= chunk_items) then arrives in chunks on the lane's
 // second stream while the lane's first stream hashes and verifies the chunks that are already there: the call costs
-// max(upload, arithmetic) instead of their sum (C3: 1,048,576 requests of 256 B are 411 MB of upload and ~10 ms of kernels).
+// max(upload, arithmetic) instead of their sum (C3: 1,048,576 requests of 256 B are 411 MB of upload).
 // extra_pinned / so_out: the caller stages more arrays behind ours (the quorum columns) in the lane's pinned area.
 int stage_and_verify(sbv_engine *e, Dev &d, int lane, uint8_t curve, size_t lo, size_t cnt, const BatchSrc &b, size_t extra_pinned = 0,
                      size_t *so_out = nullptr) {

@@ -7,8 +7,8 @@
 namespace sbv {
 
 template <class C> struct Cfg;
-// P-256: the fixed-base kernel runs with its multiplications inlined at 6 blocks of 64 threads per SM (163 registers, no
-// spills; profiles/r02_variants.md: equal or slightly ahead of the out-of-line build at 7 blocks, which spills 80 B);
+// P-256: the fixed-base kernel runs with its multiplications inlined at 6 blocks of 64 threads per SM (168 registers, no
+// spills; equal or slightly ahead of the out-of-line build at 7 blocks, which spills);
 // the generic kernel likewise at 6 blocks (no spills) now that it only sees the keys that do not repeat.
 template <> struct Cfg<P256> { static constexpr int COZ_MINB = 6, KT_MINB = 7, KT_VARIANT = 2; };
 template <> struct Cfg<P384> { static constexpr int COZ_MINB = 4, KT_MINB = 4, KT_VARIANT = 0; };

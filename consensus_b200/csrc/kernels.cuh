@@ -1,7 +1,7 @@
-// kernels.cuh — sm_100a kernels of the sbv hot path (ECDSA verify over NIST prime curves).
+// kernels.cuh — sm_90a kernels of the sbv hot path (ECDSA verify over NIST prime curves).
 //
 //   k_gtable_init        one-time: affine fixed-base comb table  T[i][b] = b * 2^(GW*i) * G  (Montgomery form;
-//                        GW = 16 for both curves: 64 MiB for P-256, L2-resident; 151 MB for P-384, in HBM)
+//                        GW = 16 for both curves: 64 MiB for P-256, mostly in L2; 151 MB for P-384, in HBM)
 //   k_prep               per batch: range checks, batched inversion of s mod n (Montgomery's trick over S items
 //                        per thread, one binary-extended-GCD inversion per thread), u1 = e/s, u2 = r/s written
 //                        word-major ([2N][n] words) so that every consumer reads them coalesced and cuts its own
@@ -252,7 +252,7 @@ SBV_DEV bool load_key(uint32_t (&qxm)[C::N], uint32_t (&qym)[C::N], const uint8_
 }
 
 // acc += u1*G from the fixed-base comb: GWINS complete points.  The next entry (a random gather from the
-// L2-resident table) is in flight while the current one is added.
+// table, an L2 hit for most entries) is in flight while the current one is added.
 template <class C>
 SBV_DEV void add_u1G(Jac<C> &acc, const uint32_t *__restrict__ uw, uint32_t n, uint32_t idx, const uint4 *__restrict__ gtab) {
     constexpr int N = C::N;

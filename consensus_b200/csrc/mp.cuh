@@ -1,4 +1,4 @@
-// mp.cuh — register-resident multiprecision primitives for sm_100a (32-bit limbs, little-endian).
+// mp.cuh — register-resident multiprecision primitives for sm_90a (32-bit limbs, little-endian).
 //
 // The multiply uses the even/odd column split: every a[i]*b[j] with i+j even is a 64-bit value at
 // an even limb offset, so a row of them is one carry chain of IMAD.WIDE.U32.X instructions

@@ -143,7 +143,7 @@ void sbv_scratch_free(Dev &d) {
 int sbv_init_gtables(sbv_engine *e, Dev &d) {
     for (int c = 0; c < 2; c++) {
         const CurveOps &ops = sbv_ops(c);
-        CU(e, cudaMalloc(&d.gtab[c], ops.gtab_entries * 2 * ops.N * 4));  // P-256: 64 MiB, stays resident in the 126 MB L2
+        CU(e, cudaMalloc(&d.gtab[c], ops.gtab_entries * 2 * ops.N * 4));  // P-256: 64 MiB, mostly held by the 50 MB L2
         CU(e, ops.gtable_init(d.gtab[c], d.stream));
     }
     e->launches += 2;

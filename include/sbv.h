@@ -1,5 +1,5 @@
 /*
- * sbv.h — C ABI of the B200-native batched signature-verification engine.
+ * sbv.h — C ABI of the H100-native batched signature-verification engine.
  *
  * This is the drop-in boundary behind SmartBFT's application-implemented verifier plug-in:
  *   api.Verifier            /root/reference/pkg/api/dependencies.go:54-71
