@@ -401,8 +401,10 @@ SBV_DEV void pt_double(Jac<C> &P) {
 // MODE 2: z2 with its square and cube supplied (table points sharing one Z: 11M+3S).
 // `skip` leaves P unchanged (digit 0).  `neg` adds the negated point.  Handles every exceptional
 // case: P = inf -> result is the addend; P == addend -> doubling; P == -addend -> infinity (Z3 = 0).
-template <class C, int MODE>
-SBV_DEV void pt_add_m(Jac<C> &P, const uint32_t (&x2)[C::N], const uint32_t (&y2_in)[C::N], const uint32_t (&z2)[C::N],
+// DEFER: P == addend leaves P unchanged and returns true — the caller doubles P at its own doubling site, so that a
+// loop with one addition and one doubling does not carry a second inlined copy of the doubling.
+template <class C, int MODE, bool DEFER = false>
+SBV_DEV bool pt_add_m(Jac<C> &P, const uint32_t (&x2)[C::N], const uint32_t (&y2_in)[C::N], const uint32_t (&z2)[C::N],
                       const uint32_t (&z2sq)[C::N], const uint32_t (&z2cu)[C::N], bool neg, bool skip) {
     constexpr int N = C::N;
     uint32_t y2[N], zero[N];
@@ -436,8 +438,8 @@ SBV_DEV void pt_add_m(Jac<C> &P, const uint32_t (&x2)[C::N], const uint32_t (&y2
     C::fsub(r, s2, s1);
     const bool h0 = mp_is_zero<N>(h), r0 = mp_is_zero<N>(r);
     if (h0 && r0 && !p_inf && !skip) {  // same point: rare, data dependent — take the doubling path
-        pt_double<C>(P);
-        return;
+        if constexpr (!DEFER) pt_double<C>(P);
+        return true;
     }
     uint32_t hh[N], hhh[N], v[N], x3[N], y3[N], z3[N];
     C::fsqr(hh, h);
@@ -464,6 +466,7 @@ SBV_DEV void pt_add_m(Jac<C> &P, const uint32_t (&x2)[C::N], const uint32_t (&y2
         P.Y[i] = skip ? P.Y[i] : ny;
         P.Z[i] = skip ? P.Z[i] : nz;
     }
+    return false;
 }
 template <class C, bool AFFINE>
 SBV_DEV void pt_add(Jac<C> &P, const uint32_t (&x2)[C::N], const uint32_t (&y2)[C::N], const uint32_t (&z2)[C::N], bool neg, bool skip) {

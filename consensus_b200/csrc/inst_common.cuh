@@ -7,10 +7,11 @@
 namespace sbv {
 
 template <class C> struct Cfg;
-// P-256: the fixed-base kernel runs with its multiplications inlined at 6 blocks of 64 threads per SM (168 registers, no
-// spills; equal or slightly ahead of the out-of-line build at 7 blocks, which spills);
+// P-256: the fixed-base kernels run with their multiplications inlined at 6 blocks of 64 threads per SM (window kernel 168
+// registers, comb kernel 153, no spills; the window kernel is equal or slightly ahead of the out-of-line build at 7
+// blocks, which spills);
 // the generic kernel likewise at 6 blocks (no spills) now that it only sees the keys that do not repeat.
-template <> struct Cfg<P256> { static constexpr int COZ_MINB = 6, KT_MINB = 7, KT_VARIANT = 2; };
+template <> struct Cfg<P256> { static constexpr int COZ_MINB = 6, KT_MINB = 7, KT_VARIANT = 2, COMB_MINB = 6; static constexpr bool COMB_INL = true; };
 template <> struct Cfg<P384> { static constexpr int COZ_MINB = 4, KT_MINB = 4, KT_VARIANT = 0; };
 
 template <class C>
@@ -60,6 +61,7 @@ cudaError_t op_coz(uint32_t n, const uint8_t *qx, const uint8_t *qy, const uint8
     return cudaGetLastError();
 }
 
+// window tables (registered keys; P-384 keys grouped inside a launch)
 template <class C, int W>
 cudaError_t op_kt_build(const uint32_t *nkeys_ptr, uint32_t cap, const uint32_t *keylist, const uint8_t *qx, const uint8_t *qy,
                         uint32_t *bases, uint32_t *hs, uint32_t *ztop, uint32_t *pref, uint32_t *ktab, uint8_t *keyflags, cudaStream_t st) {
@@ -67,12 +69,12 @@ cudaError_t op_kt_build(const uint32_t *nkeys_ptr, uint32_t cap, const uint32_t 
     const unsigned kb = (cap + 63) / 64;
     const unsigned wb = (unsigned)(((size_t)cap * KT::NWIN + 63) / 64);
     static const int bases_variant = getenv("SBV_KT_BASES") ? atoi(getenv("SBV_KT_BASES")) : 0;  // A/B: 1 = one thread per key (inlined), 2 = (out of line)
-    if (bases_variant == 2) k_kt_bases<C, W, false><<<kb, 64, 0, st>>>(nkeys_ptr, cap, keylist, qx, qy, bases, keyflags);
-    else if (bases_variant == 1) k_kt_bases<C, W, true><<<kb, 64, 0, st>>>(nkeys_ptr, cap, keylist, qx, qy, bases, keyflags);
-    else k_kt_bases4<C, W><<<(unsigned)(((size_t)cap * 4 + 127) / 128), 128, 0, st>>>(nkeys_ptr, cap, keylist, qx, qy, bases, keyflags);
+    if (bases_variant == 2) k_kt_bases<C, KT, false><<<kb, 64, 0, st>>>(nkeys_ptr, cap, keylist, qx, qy, bases, keyflags);
+    else if (bases_variant == 1) k_kt_bases<C, KT, true><<<kb, 64, 0, st>>>(nkeys_ptr, cap, keylist, qx, qy, bases, keyflags);
+    else k_kt_bases4<C, KT><<<(unsigned)(((size_t)cap * 4 + 127) / 128), 128, 0, st>>>(nkeys_ptr, cap, keylist, qx, qy, bases, keyflags);
     k_kt_fill<C, W><<<wb, 64, 0, st>>>(nkeys_ptr, cap, bases, keyflags, hs, ztop, ktab);
-    k_kt_inv<C, W><<<kb, 64, 0, st>>>(nkeys_ptr, cap, keyflags, ztop, pref);
-    k_kt_final<C, W><<<wb, 64, 0, st>>>(nkeys_ptr, cap, bases, keyflags, hs, ztop, ktab);
+    k_kt_inv<C, KT><<<kb, 64, 0, st>>>(nkeys_ptr, cap, keyflags, ztop, pref);
+    k_kt_final<C, KT><<<wb, 64, 0, st>>>(nkeys_ptr, cap, bases, keyflags, hs, ztop, ktab);
     return cudaGetLastError();
 }
 
@@ -100,10 +102,37 @@ cudaError_t op_kt_verify(int reg, int warp, uint32_t n, const uint32_t *slot, co
     return cudaGetLastError();
 }
 
-template <class C, int W>
+// comb tables (P-256 keys grouped inside a launch)
+template <class C>
+cudaError_t op_comb_build(const uint32_t *nkeys_ptr, uint32_t cap, const uint32_t *keylist, const uint8_t *qx, const uint8_t *qy,
+                          uint32_t *bases, uint32_t *hs, uint32_t *ztop, uint32_t *pref, uint32_t *ktab, uint8_t *keyflags, cudaStream_t st) {
+    using CT = CombTab<C>;
+    const unsigned kb = (cap + 63) / 64;
+    const unsigned cb = (unsigned)(((size_t)cap * CT::NCHAIN + 63) / 64);
+    k_kt_bases4<C, CT><<<(unsigned)(((size_t)cap * 4 + 127) / 128), 128, 0, st>>>(nkeys_ptr, cap, keylist, qx, qy, bases, keyflags);
+    k_comb_affine<C><<<kb, 64, 0, st>>>(nkeys_ptr, cap, keyflags, bases, pref);
+    k_comb_fill<C><<<cb, 64, 0, st>>>(nkeys_ptr, cap, bases, keyflags, hs, ztop, ktab);
+    k_kt_inv<C, CT><<<kb, 64, 0, st>>>(nkeys_ptr, cap, keyflags, ztop, pref);
+    k_kt_final<C, CT><<<cb, 64, 0, st>>>(nkeys_ptr, cap, bases, keyflags, hs, ztop, ktab);
+    return cudaGetLastError();
+}
+
+template <class C>
+cudaError_t op_comb_verify(int reg, int warp, uint32_t n, const uint32_t *slot, const int32_t *kidmap, uint32_t n_slots,
+                           const uint8_t *keyflags, const uint8_t *r, const uint32_t *uw, const uint8_t *flags, const uint32_t *gtab,
+                           const uint32_t *ktab, uint8_t *ok, const uint32_t *list, const uint32_t *count, const uint32_t *gacc, cudaStream_t st) {
+    constexpr int BLOCK = 64;
+    (void)slot; (void)n_slots;
+    if (reg || warp || !list || !count) return cudaErrorInvalidValue;  // comb tables serve the grouped items of a launch only
+    k_verify_comb<C, BLOCK, Cfg<C>::COMB_MINB, Cfg<C>::COMB_INL><<<(n + BLOCK - 1) / BLOCK, BLOCK, 0, st>>>(
+        n, kidmap, keyflags, r, uw, flags, reinterpret_cast<const uint4 *>(gtab), reinterpret_cast<const uint4 *>(ktab), ok, list, count, gacc);
+    return cudaGetLastError();
+}
+
+template <class C, class KT>
 constexpr KtGeom kt_geom() {
-    using KS = KtSizes<C, W>;
-    return KtGeom{W, KS::KT::NWIN, KS::KT::ENT, KS::bases_words(1), KS::hs_words(1), KS::ztop_words(1), KS::ktab_words(1)};
+    using KS = KtSizes<C, KT>;
+    return KtGeom{KS::bases_words(1), KS::hs_words(1), KS::ztop_words(1), KS::ktab_words(1)};
 }
 
 }  // namespace sbv

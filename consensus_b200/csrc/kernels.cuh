@@ -10,8 +10,10 @@
 //                        thread: on-curve check, 4-bit signed window over a common-Z table of Q (shared memory,
 //                        bank = lane, + coalesced global scratch), 256 doublings interleaved with 65 additions, 16
 //                        comb additions for u1*G with the next gather in flight, final X == r*Z^2 comparison
-//   k_verify_kt          FIXED-BASE path for keys that have a per-key table (keygroup.cuh: built on the fly for keys
-//                        that repeat inside a batch, or once per registration for sbv_set_keys): no doublings,
+//   k_verify_comb        FIXED-BASE path for P-256 keys that repeat inside a batch (comb table of the key, keygroup.cuh
+//                        builds it on the fly): 32 comb additions and 15 doublings for u2*Q, then u1*G
+//   k_verify_kt          FIXED-BASE path over a window table: registered keys (sbv_set_keys, 8-bit windows, built once
+//                        per key set) and P-384 keys that repeat inside a batch (5-bit windows): no doublings,
 //                        NWIN(W) signed-window additions for u2*Q + the comb additions for u1*G
 //   k_verify_kt_warp     the same, ONE SIGNATURE PER WARP (small batches: lanes add their table points,
 //                        shuffle-tree reduction)
@@ -389,14 +391,52 @@ __global__ void __launch_bounds__(BLOCK, MINB) k_verify_coz(uint32_t n, const ui
 }
 
 // ------------------------------------------------------------------------------------------------
-// Fixed-base path: per-key table KT[kid][win][e-1] = e * 2^(W*win) * Q_kid for e = 1..2^(W-1), affine Montgomery
-// form (keygroup.cuh builds it).  u2*Q = sum over the NWIN Booth digits of u2: no doublings at all.
+// Per-key tables (keygroup.cuh builds both kinds).  The builder sees a table as NBASE bases 2^(STEP*i) * Q (a chain of
+// doublings) and NCHAIN chains of ENT entries, the entries of a chain sharing one chain of Z ratios.
+//
+// Window table (registered keys; P-384 keys grouped inside a launch): KT[kid][win][e-1] = e * 2^(W*win) * Q_kid for e = 1..2^(W-1), affine Montgomery
+// form.  u2*Q = sum over the NWIN Booth digits of u2: no doublings at all.
 template <int BITS, int W>
 struct KeyTab {
     static constexpr int NWIN = Windows<BITS, W>::COUNT;
     static constexpr int ENT = Windows<BITS, W>::ENTRIES;
+    static constexpr int NBASE = NWIN, STEP = W, NCHAIN = NWIN;
     static constexpr size_t POINTS = (size_t)NWIN * ENT;  // affine points per key
 };
+
+// Comb table (P-256 keys grouped inside a launch; Lim–Lee, Hankerson–Menezes–Vanstone Alg. 3.44): 16 bases P_c = 2^(SPACING*c) * Q
+// in BLOCKS = 2 blocks of TEETH = 8; a scalar is read as 16 rows of SPACING bits (row c = bits [SPACING*c, SPACING*(c+1))),
+// and column j of the rows of block b is the mask m of entry T_b[m] = sum of P_(8b+t) over the set bits t of m.  u2*Q then
+// takes SPACING - 1 doublings and 2 * SPACING additions (P-256: 15 and 32, P-384: 23 and 48).
+// Layout: chain (b, hi) holds the 16 entries m = 16*hi + g in Gray-code order of the low nibble g (the order the builder
+// walks them), so T_b[m] is slot (16*b + hi)*16 + k with gray(k) = g; the slot of m = 0 (hi = 0, k = 0) is never read.
+template <class C>
+struct CombTab {
+    static constexpr int TEETH = 8, BLOCKS = 2, NBASE = TEETH * BLOCKS;
+    static constexpr int SPACING = 32 * C::N / NBASE;       // 16 for P-256, 24 for P-384
+    static constexpr int STEP = SPACING;
+    static constexpr int NCHAIN = BLOCKS * 16, ENT = 16;  // (block, high nibble) x low nibble
+    static constexpr size_t POINTS = (size_t)NCHAIN * ENT;  // 512 affine points per key: 32 KiB (P-256), 48 KiB (P-384)
+    static_assert(SPACING * NBASE == 32 * C::N, "the rows cover the scalar exactly");
+    SBV_DEV static uint32_t slot(int b, uint32_t m) {
+        const uint32_t g = m & 15u;
+        return ((uint32_t)b * 16u + (m >> 4)) * 16u + (g ^ (g >> 1) ^ (g >> 2) ^ (g >> 3));  // inverse Gray code of g
+    }
+};
+
+// column j of block b of u2's comb: bit t = bit SPACING*(8b + t) + j of u2
+template <class C>
+SBV_DEV uint32_t comb_mask_u2(const uint32_t *__restrict__ uw, uint32_t n, uint32_t idx, int b, int j) {
+    using CT = CombTab<C>;
+    const uint32_t *u2 = uw + (size_t)C::N * n + idx;
+    uint32_t m = 0;
+#pragma unroll
+    for (int t = 0; t < CT::TEETH; t++) {
+        const int pos = CT::SPACING * (CT::TEETH * b + t) + j;
+        m |= ((__ldg(u2 + (size_t)(pos >> 5) * n) >> (pos & 31)) & 1u) << t;
+    }
+    return m;
+}
 
 // Inl<C>: the same curve with the field multiplications inlined at every call site instead of called out of line —
 // no argument marshalling and free scheduling across multiplications, at ~3 KB of code per site.  Only for loops
@@ -410,7 +450,8 @@ template <class C, bool INL> struct PickArith { using type = C; };
 template <class C> struct PickArith<C, true> { using type = Inl<C>; };
 
 // k_gpart — the u1*G half of a fixed-base verification on its own: needs only the scalars, so the grouped pipeline runs
-// it while the per-key tables are still being built; k_verify_kt<…, GSPLIT> then starts from the stored point.
+// it while the per-key tables are still being built; k_verify_comb (k_verify_kt<…, REG = false>) then closes with (starts
+// from) the stored point.
 // gacc: [3N][n] words (X, Y, Z of item idx at column idx).
 template <class C, int BLOCK, int MINB>
 __global__ void __launch_bounds__(BLOCK, MINB) k_gpart(uint32_t n, const uint32_t *__restrict__ uw, const uint4 *__restrict__ gtab,
@@ -507,6 +548,89 @@ __global__ void __launch_bounds__(BLOCK, MINB) k_verify_kt(uint32_t n, const uin
     }
     Jac<C> fin;
     mp_copy<N>(fin.X, acc.X); mp_copy<N>(fin.Y, acc.Y); mp_copy<N>(fin.Z, acc.Z);
+    ok_out[idx] = final_check<C>(fin, r_be, idx) ? 1 : 0;
+}
+
+// k_verify_comb — keys grouped inside a launch: the key of item list[t] is kidmap[list[t]] (>= 0 for every listed item),
+// its table a CombTab.  u2*Q column by column from the top: a doubling (none before the first column), then one table
+// addition per block; then u1*G, after the last doubling: one general addition of k_gpart's point when gacc != NULL,
+// else the GWINS comb additions from G's table.
+// One inlined addition site and one doubling site in one loop: the addition hands its exceptional case (accumulator ==
+// entry) to the doubling site (pt_add_m<…, DEFER>) instead of carrying its own copy of the doubling, and the next table
+// entry (a random 64-byte gather) is in flight while the current one is added.  The additions stay complete: the key
+// entries cannot meet the accumulator (its scalar and theirs are distinct multiples below n), but the G entries can.
+template <class C, int BLOCK, int MINB, bool INL>
+__global__ void __launch_bounds__(BLOCK, MINB) k_verify_comb(uint32_t n, const int32_t *__restrict__ kidmap, const uint8_t *__restrict__ keyflags,
+                                                              const uint8_t *__restrict__ r_be, const uint32_t *__restrict__ uw,
+                                                              const uint8_t *__restrict__ flags, const uint4 *__restrict__ gtab,
+                                                              const uint4 *__restrict__ ktab, uint8_t *__restrict__ ok_out,
+                                                              const uint32_t *__restrict__ list, const uint32_t *__restrict__ count,
+                                                              const uint32_t *__restrict__ gacc) {
+    using A = typename PickArith<C, INL>::type;  // arithmetic policy of the loop
+    constexpr int N = C::N;
+    constexpr int EU4 = 2 * N / 4;  // uint4 per table entry
+    using CT = CombTab<C>;
+    constexpr int KADD = CT::SPACING * CT::BLOCKS;  // key additions
+    const int TOTAL = gacc ? KADD : KADD + C::GWINS;
+    const uint32_t t = blockIdx.x * BLOCK + threadIdx.x;
+    if (t >= __ldg(count)) return;
+    const uint32_t idx = __ldg(list + t);
+    const int32_t kid = kidmap[idx];
+    const bool good = flags[idx] != 0 && kid >= 0 && keyflags[kid < 0 ? 0 : kid] != 0;
+    if (!good) { ok_out[idx] = 0; return; }
+    const uint4 *kt = ktab + (size_t)kid * CT::POINTS * EU4;
+    uint32_t one[N];
+    C::get_one(one);
+    Jac<A> acc;
+    mp_copy<N>(acc.X, one);
+    mp_copy<N>(acc.Y, one);
+#pragma unroll
+    for (int i = 0; i < N; i++) acc.Z[i] = 0;
+    // step s < KADD: column SPACING-1 - s/2, block s%2 of u2's comb; s >= KADD: comb digit s - KADD of u1 into G's table
+    auto fetch = [&](int s, uint32_t (&x)[N], uint32_t (&y)[N], bool &skip) {
+        if (s < KADD) {
+            const int b = s & 1;
+            const uint32_t m = comb_mask_u2<C>(uw, n, idx, b, CT::SPACING - 1 - (s >> 1));
+            load_affine<C>(x, y, kt + (size_t)CT::slot(b, m) * EU4);
+            skip = m == 0;
+        } else {
+            const int g = s - KADD;
+            const uint32_t d = comb_digit_u1<C>(uw, n, idx, g);
+            load_affine<C>(x, y, gtab + (((size_t)g << C::GW) + d) * EU4);
+            skip = d == 0;
+        }
+    };
+    uint32_t cx[N], cy[N];
+    bool cskip;
+    fetch(0, cx, cy, cskip);
+    int s = 0, dbl = 0;  // dbl: doublings due before the addition of step s
+#pragma unroll 1
+    while (s < TOTAL || dbl) {
+        if (dbl) {
+            pt_double<A>(acc);
+            dbl--;
+            continue;
+        }
+        uint32_t nx[N], ny[N];
+        bool nskip = true;
+        if (s + 1 < TOTAL) fetch(s + 1, nx, ny, nskip);
+        dbl = pt_add_m<A, 1, true>(acc, cx, cy, one, one, one, false, cskip) ? 1 : 0;  // acc == entry: the sum is 2 * acc
+        s++;
+        if (s < KADD && (s & 1) == 0) dbl++;  // next column
+        if (s < TOTAL) { mp_copy<N>(cx, nx); mp_copy<N>(cy, ny); cskip = nskip; }
+    }
+    Jac<C> fin;
+    mp_copy<N>(fin.X, acc.X); mp_copy<N>(fin.Y, acc.Y); mp_copy<N>(fin.Z, acc.Z);
+    if (gacc) {  // the closing general addition (out-of-line multiplications: once per signature, outside the loop)
+        Jac<C> g;
+#pragma unroll
+        for (int i = 0; i < N; i++) {
+            g.X[i] = __ldg(gacc + (size_t)i * n + idx);
+            g.Y[i] = __ldg(gacc + (size_t)(N + i) * n + idx);
+            g.Z[i] = __ldg(gacc + (size_t)(2 * N + i) * n + idx);
+        }
+        pt_add<C, false>(fin, g.X, g.Y, g.Z, false, mp_is_zero<N>(g.Z));
+    }
     ok_out[idx] = final_check<C>(fin, r_be, idx) ? 1 : 0;
 }
 

@@ -9,17 +9,21 @@
 //                 full-key compare on collision): rep[i] = first item with the same key; warp-aggregated count
 //   k_kg_assign   representatives whose key occurs >= T times (and while table slots last) get a dense key id
 //   k_kg_route    items are appended to the fixed-base list (their key has a table) or to the generic list
-//   k_kt_bases4   four lanes per key: validate the key, B_w = 2^(W*w) * Q for all windows — a chain of doublings whose
-//                 independent multiplications run on different lanes (k_kt_bases: the one-thread-per-key form)
-//   k_kt_fill     one thread per (key, window): e*B_w for e = 1..2^(W-1) with co-Z additions (5M+2S each — the
-//                 chain of Z ratios that comes with them is exactly what the inversion needs)
-//   k_kt_inv      one thread per key: ONE field inversion for all windows of the key (Montgomery's trick across
-//                 the windows' top Z's)
-//   k_kt_final    one thread per (key, window): back-substitute the Z ratios, convert to affine, in place
+//   k_kt_bases4   four lanes per key: validate the key, the bases B_i = 2^(STEP*i) * Q of its table — a chain of
+//                 doublings whose independent multiplications run on different lanes (k_kt_bases: one thread per key)
+//   k_comb_affine one thread per key (comb): the 16 bases to affine with one inversion
+//   k_comb_fill   one thread per (key, chain) (comb): the 16 entries of a chain, one mixed addition per Gray-code step
+//   k_kt_fill     one thread per (key, window) (window table): e*B_w for e = 1..2^(W-1) with co-Z additions (5M+2S
+//                 each — the chain of Z ratios that comes with them is exactly what the inversion needs)
+//   k_kt_inv      one thread per key: ONE field inversion for all chains of the key (Montgomery's trick across
+//                 the chains' top Z's)
+//   k_kt_final    one thread per (key, chain): back-substitute the Z ratios, convert to affine, in place
 //
-// The table feeds k_verify_kt (kernels.cuh).  sbv_set_keys uses the same builder once per registration.
-// Cost per key (P-256, W = 5: 52 windows x 16 entries): 255 doublings + 832 x ~12 multiplications + one inversion
-// ~ 4 generic verifications; a fixed-base verification is ~4.5x cheaper than a generic one, so T = 16 pays.
+// Keys grouped inside a launch get a comb table (CombTab, kernels.cuh), read by k_verify_comb: P-256: 240 doublings +
+// 512 mixed additions (~11 multiplications) + 512 conversions (~6) + two inversions per key ~ 3.5 generic verifications;
+// a comb verification (15 doublings + 32 additions + the u1*G half) is ~5x cheaper than a generic one, so T = 16 pays.
+// Registered keys (sbv_set_keys) get a window table (KeyTab, W = 8), read by k_verify_kt: built once per key set, so
+// its verifications are the ones to make cheapest — no doublings at all.
 #pragma once
 #include "kernels.cuh"
 
@@ -125,21 +129,21 @@ static __global__ void __launch_bounds__(256) k_kg_route(uint32_t n, const uint3
 // ---- table construction -------------------------------------------------------------------------------------
 // Scratch layout (cap = key capacity of the buffers; lanes of a warp are consecutive keys, so every access below
 // is coalesced):
-//   bases [win][3N words][cap]              Jacobian B_win = 2^(W*win) * Q
-//   hs    [win][e = 2..ENT][N words][cap]   Z ratios of the co-Z chain: Z_e = Z_{e-1} * H_e  (H_2 = 2*Y_B, Z_1 = Z_B)
-//   ztop  [win][N words][cap]               Z_ENT of the window; k_kt_inv overwrites it with its inverse
-//   ktab  [kid][win][e-1][2N words]         Jacobian X, Y from k_kt_fill; affine x, y after k_kt_final
+//   bases [i][3N words][cap]                Jacobian B_i = 2^(STEP*i) * Q (the comb's are made affine in place)
+//   hs    [win][e = 2..ENT][N words][cap]   Z ratios along chain win: Z_e = Z_{e-1} * H_e  (window: H_2 = 2*Y_B, Z_1 = Z_B)
+//   ztop  [win][N words][cap]               Z_ENT of the chain; k_kt_inv overwrites it with its inverse
+//   pref  [win][N words][cap]               prefix products of the inversions
+//   ktab  [kid][win][e-1][2N words]         Jacobian X, Y from the fill kernel; affine x, y after k_kt_final
 
 // nkeys_ptr: device counter (clamped to cap) — the grid is sized for the worst case and surplus threads leave.
 // key k is item keylist[k] of (qx_be, qy_be); for registered keys keylist is the identity over the key array.
 // INL: the eight multiplications of the doubling inlined (one site, ~25 KB): this kernel is a single dependent chain per
 // thread on an otherwise idle SM sub-partition, so what counts is how well independent multiplications interleave.
-template <class C, int W, bool INL>
+template <class C, class KT, bool INL>
 __global__ void __launch_bounds__(64) k_kt_bases(const uint32_t *__restrict__ nkeys_ptr, uint32_t cap, const uint32_t *__restrict__ keylist,
                                                  const uint8_t *__restrict__ qx_be, const uint8_t *__restrict__ qy_be,
                                                  uint32_t *__restrict__ bases, uint8_t *__restrict__ keyflags) {
     constexpr int N = C::N;
-    using KT = KeyTab<32 * N, W>;
     const uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
     uint32_t nkeys = __ldg(nkeys_ptr);
     if (nkeys > cap) nkeys = cap;
@@ -152,10 +156,10 @@ __global__ void __launch_bounds__(64) k_kt_bases(const uint32_t *__restrict__ nk
     if (!good) return;  // no table: every item of this key rejects (k_verify_kt checks the flag)
     C::get_one(B.Z);
 #pragma unroll 1
-    for (int win = 0; win < KT::NWIN; win++) {
+    for (int win = 0; win < KT::NBASE; win++) {
         if (win) {
 #pragma unroll 1
-            for (int d = 0; d < W; d++) pt_double<A>(B);
+            for (int d = 0; d < KT::STEP; d++) pt_double<A>(B);
         }
         uint32_t *o = bases + (size_t)win * 3 * N * cap + k;
 #pragma unroll
@@ -171,12 +175,11 @@ __global__ void __launch_bounds__(64) k_kt_bases(const uint32_t *__restrict__ nk
 //   level 4   lane 0: alpha*(beta4 - X3)
 // with six 8-word quad broadcasts per doubling (bb, beta4, 8Y^4, and the new X, Y, Z).  The kernel is one dependent
 // chain on an otherwise idle sub-partition, so halving the number of dependent multiplications halves its duration.
-template <class C, int W>
+template <class C, class KT>
 __global__ void __launch_bounds__(128) k_kt_bases4(const uint32_t *__restrict__ nkeys_ptr, uint32_t cap, const uint32_t *__restrict__ keylist,
                                                    const uint8_t *__restrict__ qx_be, const uint8_t *__restrict__ qy_be,
                                                    uint32_t *__restrict__ bases, uint8_t *__restrict__ keyflags) {
     constexpr int N = C::N;
-    using KT = KeyTab<32 * N, W>;
     const uint32_t gt = blockIdx.x * blockDim.x + threadIdx.x;
     const uint32_t k = gt >> 2, role = gt & 3;
     uint32_t nkeys = __ldg(nkeys_ptr);
@@ -194,10 +197,10 @@ __global__ void __launch_bounds__(128) k_kt_bases4(const uint32_t *__restrict__ 
         for (int i = 0; i < N; i++) v[i] = __shfl_sync(qmask, v[i], qbase + src);
     };
 #pragma unroll 1
-    for (int win = 0; win < KT::NWIN; win++) {
+    for (int win = 0; win < KT::NBASE; win++) {
         if (win) {
 #pragma unroll 1
-            for (int d = 0; d < W; d++) {
+            for (int d = 0; d < KT::STEP; d++) {
                 uint32_t s[N], a[N], b[N], r1[N], r2[N], r3[N], r4[N], t1[N], t2[N];
                 C::fadd(s, Y, Y);
                 // level 1: delta | bb | Z3 | (delta)
@@ -327,12 +330,11 @@ __global__ void __launch_bounds__(64) k_kt_fill(const uint32_t *__restrict__ nke
     for (int i = 0; i < N; i++) zp[(size_t)i * cap] = zacc[i];
 }
 
-// ztop[win] <- 1 / ztop[win] for all windows of a key with one inversion
-template <class C, int W>
+// ztop[win] <- 1 / ztop[win] for all chains of a key with one inversion
+template <class C, class KT>
 __global__ void __launch_bounds__(64) k_kt_inv(const uint32_t *__restrict__ nkeys_ptr, uint32_t cap, const uint8_t *__restrict__ keyflags,
                                                uint32_t *__restrict__ ztop, uint32_t *__restrict__ pref) {
     constexpr int N = C::N;
-    using KT = KeyTab<32 * N, W>;
     const uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
     uint32_t nkeys = __ldg(nkeys_ptr);
     if (nkeys > cap) nkeys = cap;
@@ -340,7 +342,7 @@ __global__ void __launch_bounds__(64) k_kt_inv(const uint32_t *__restrict__ nkey
     uint32_t run[N];
     C::get_one(run);
 #pragma unroll 1
-    for (int win = 0; win < KT::NWIN; win++) {
+    for (int win = 0; win < KT::NCHAIN; win++) {
         uint32_t z[N];
         const uint32_t *zp = ztop + (size_t)win * N * cap + k;
         uint32_t *pp = pref + (size_t)win * N * cap + k;
@@ -351,7 +353,7 @@ __global__ void __launch_bounds__(64) k_kt_inv(const uint32_t *__restrict__ nkey
     uint32_t inv[N];
     p_inv<C>(inv, run);  // binary extended GCD: this thread is alone on its chain, the dependent length is what counts
 #pragma unroll 1
-    for (int win = KT::NWIN - 1; win >= 0; win--) {
+    for (int win = KT::NCHAIN - 1; win >= 0; win--) {
         uint32_t z[N], pv[N], zi[N];
         uint32_t *zp = ztop + (size_t)win * N * cap + k;
         const uint32_t *pp = pref + (size_t)win * N * cap + k;
@@ -364,16 +366,15 @@ __global__ void __launch_bounds__(64) k_kt_inv(const uint32_t *__restrict__ nkey
     }
 }
 
-template <class C, int W>
+template <class C, class KT>
 __global__ void __launch_bounds__(64) k_kt_final(const uint32_t *__restrict__ nkeys_ptr, uint32_t cap, const uint32_t *__restrict__ bases,
                                                  const uint8_t *__restrict__ keyflags, const uint32_t *__restrict__ hs,
                                                  const uint32_t *__restrict__ ztop, uint32_t *__restrict__ ktab) {
     constexpr int N = C::N;
-    using KT = KeyTab<32 * N, W>;
     const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
     uint32_t nkeys = __ldg(nkeys_ptr);
     if (nkeys > cap) nkeys = cap;
-    if (t >= nkeys * KT::NWIN) return;
+    if (t >= nkeys * KT::NCHAIN) return;
     const uint32_t k = t % nkeys, win = t / nkeys;
     if (!keyflags[k]) return;
     uint32_t zi[N];  // 1 / Z_e, walking e = ENT .. 1
@@ -382,7 +383,7 @@ __global__ void __launch_bounds__(64) k_kt_final(const uint32_t *__restrict__ nk
 #pragma unroll
         for (int i = 0; i < N; i++) zi[i] = zp[(size_t)i * cap];
     }
-    uint32_t *out = ktab + ((size_t)k * KT::NWIN + win) * KT::ENT * 2 * N;
+    uint32_t *out = ktab + ((size_t)k * KT::NCHAIN + win) * KT::ENT * 2 * N;
     // entry e-1 and its Z ratio are loaded before entry e is converted and stored (independent addresses: the loads
     // overlap the six multiplications)
     uint32_t x[N], y[N], h[N];
@@ -417,13 +418,141 @@ __global__ void __launch_bounds__(64) k_kt_final(const uint32_t *__restrict__ nk
     (void)bases;
 }
 
-// words of scratch the builder needs for `cap` keys
-template <class C, int W>
+// ---- comb tables (CombTab, kernels.cuh) -------------------------------------------------------------------------
+// k_kt_bases4<C, CombTab<C>> leaves the 16 bases P_c = 2^(SPACING*c) * Q in Jacobian form; k_comb_affine makes them
+// affine, k_comb_fill walks the 32 chains, and k_kt_inv / k_kt_final finish the table as they do a window table.
+
+// bases -> affine (x, y in place of X, Y) with ONE inversion per key (Montgomery's trick over the 16 Z's; pref: prefix
+// products, [c][N words][cap])
+template <class C>
+__global__ void __launch_bounds__(64) k_comb_affine(const uint32_t *__restrict__ nkeys_ptr, uint32_t cap, const uint8_t *__restrict__ keyflags,
+                                                    uint32_t *__restrict__ bases, uint32_t *__restrict__ pref) {
+    constexpr int N = C::N;
+    using CT = CombTab<C>;
+    const uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
+    uint32_t nkeys = __ldg(nkeys_ptr);
+    if (nkeys > cap) nkeys = cap;
+    if (k >= nkeys || !keyflags[k]) return;
+    uint32_t run[N];
+    C::get_one(run);
+#pragma unroll 1
+    for (int c = 0; c < CT::NBASE; c++) {
+        uint32_t z[N];
+        const uint32_t *zp = bases + ((size_t)c * 3 + 2) * N * cap + k;
+        uint32_t *pp = pref + (size_t)c * N * cap + k;
+#pragma unroll
+        for (int i = 0; i < N; i++) { z[i] = zp[(size_t)i * cap]; pp[(size_t)i * cap] = run[i]; }
+        C::fmul(run, run, z);
+    }
+    uint32_t inv[N];
+    p_inv<C>(inv, run);
+#pragma unroll 1
+    for (int c = CT::NBASE - 1; c >= 0; c--) {
+        uint32_t *o = bases + (size_t)c * 3 * N * cap + k;
+        const uint32_t *pp = pref + (size_t)c * N * cap + k;
+        uint32_t x[N], y[N], z[N], pv[N], zi[N], z2[N], z3[N];
+#pragma unroll
+        for (int i = 0; i < N; i++) { x[i] = o[(size_t)i * cap]; y[i] = o[(size_t)(N + i) * cap]; z[i] = o[(size_t)(2 * N + i) * cap]; pv[i] = pp[(size_t)i * cap]; }
+        C::fmul(zi, inv, pv);
+        C::fmul(inv, inv, z);
+        C::fsqr(z2, zi);
+        C::fmul(z3, z2, zi);
+        C::fmul(x, x, z2);
+        C::fmul(y, y, z3);
+#pragma unroll
+        for (int i = 0; i < N; i++) { o[(size_t)i * cap] = x[i]; o[(size_t)(N + i) * cap] = y[i]; }
+    }
+}
+
+// One thread per (key, chain), chain = (block b, high nibble hi): slot 0 = the sum of the high teeth of hi, then the 15
+// Gray codes of the low nibble, one mixed addition of +-P_(8b+t) per step (t = the bit the step flips).  Records what
+// k_kt_final needs: Jacobian X, Y of every slot in ktab, the Z ratio H of every step in hs, the last Z in ztop.
+// The chain of hi = 0 starts at infinity: its first step is a copy of P_(8b) (Z = 1, H = 1), and its slot 0 (m = 0,
+// never read) is left as (0, 0).
+// No exceptional case arises: every point on a chain is s*Q with s a sum of distinct powers 2^(SPACING*c), so
+// 0 < s < 2^(15*SPACING + 1) <= 2^361 < n, and Q has prime order n.  An addition of +P_t (t not in the sum) meets the
+// accumulator only if s = 2^(SPACING*t) (impossible: distinct binary expansions) or s + 2^(SPACING*t) = n (too small);
+// an addition of -P_t (t in the sum) only if s = -2^(SPACING*t) mod n (too small) or the sum becomes empty — and a Gray
+// walk never returns to 0, while the chains with hi != 0 keep their high teeth.
+template <class C>
+__global__ void __launch_bounds__(64) k_comb_fill(const uint32_t *__restrict__ nkeys_ptr, uint32_t cap, const uint32_t *__restrict__ bases,
+                                                  const uint8_t *__restrict__ keyflags, uint32_t *__restrict__ hs,
+                                                  uint32_t *__restrict__ ztop, uint32_t *__restrict__ ktab) {
+    constexpr int N = C::N;
+    using CT = CombTab<C>;
+    const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
+    uint32_t nkeys = __ldg(nkeys_ptr);
+    if (nkeys > cap) nkeys = cap;
+    if (t >= nkeys * CT::NCHAIN) return;
+    const uint32_t k = t % nkeys, ch = t / nkeys;
+    if (!keyflags[k]) return;
+    const int b = (int)(ch >> 4), hi = (int)(ch & 15);
+    auto base = [&](int c, uint32_t (&x)[N], uint32_t (&y)[N]) {
+        const uint32_t *o = bases + (size_t)c * 3 * N * cap + k;
+#pragma unroll
+        for (int i = 0; i < N; i++) { x[i] = o[(size_t)i * cap]; y[i] = o[(size_t)(N + i) * cap]; }
+    };
+    uint32_t *out = ktab + ((size_t)k * CT::NCHAIN + ch) * CT::ENT * 2 * N;
+    auto store = [&](int slot, const uint32_t (&x)[N], const uint32_t (&y)[N], const uint32_t (&h)[N]) {
+        uint32_t *o = out + (size_t)slot * 2 * N;
+#pragma unroll
+        for (int i = 0; i < N; i++) { o[i] = x[i]; o[N + i] = y[i]; }
+        if (slot) {
+            uint32_t *hp = hs + ((size_t)ch * (CT::ENT - 1) + (slot - 1)) * N * cap + k;
+#pragma unroll
+            for (int i = 0; i < N; i++) hp[(size_t)i * cap] = h[i];
+        }
+    };
+    Jac<C> P;
+    uint32_t x[N], y[N], h[N];
+    C::get_one(P.Z);
+    C::get_one(h);
+    int first;  // first slot the Gray walk produces
+    if (hi == 0) {
+        uint32_t zero[N];
+#pragma unroll
+        for (int i = 0; i < N; i++) zero[i] = 0;
+        store(0, zero, zero, h);
+        base(CT::TEETH * b, P.X, P.Y);
+        store(1, P.X, P.Y, h);
+        first = 2;
+    } else {
+        bool empty = true;
+#pragma unroll 1
+        for (int i = 0; i < 4; i++) {
+            if (!((hi >> i) & 1)) continue;
+            base(CT::TEETH * b + 4 + i, x, y);
+            if (empty) { mp_copy<N>(P.X, x); mp_copy<N>(P.Y, y); empty = false; }
+            else pt_madd_table<C>(P, x, y, h);
+        }
+        store(0, P.X, P.Y, h);
+        first = 1;
+    }
+#pragma unroll 1
+    for (int kk = first; kk < CT::ENT; kk++) {
+        const int tooth = __ffs(kk) - 1;                           // gray(kk - 1) -> gray(kk) flips this bit
+        base(CT::TEETH * b + tooth, x, y);
+        if (!(((kk ^ (kk >> 1)) >> tooth) & 1)) {                  // the bit goes off: subtract
+            uint32_t zero[N];
+#pragma unroll
+            for (int i = 0; i < N; i++) zero[i] = 0;
+            C::fsub(y, zero, y);
+        }
+        pt_madd_table<C>(P, x, y, h);
+        store(kk, P.X, P.Y, h);
+    }
+    uint32_t *zp = ztop + (size_t)ch * N * cap + k;
+#pragma unroll
+    for (int i = 0; i < N; i++) zp[(size_t)i * cap] = P.Z[i];
+}
+
+// words of scratch the builder needs for `cap` keys (KT: KeyTab or CombTab)
+template <class C, class KT_>
 struct KtSizes {
-    using KT = KeyTab<32 * C::N, W>;
-    static constexpr size_t bases_words(size_t cap) { return (size_t)KT::NWIN * 3 * C::N * cap; }
-    static constexpr size_t hs_words(size_t cap) { return (size_t)KT::NWIN * (KT::ENT - 1) * C::N * cap; }
-    static constexpr size_t ztop_words(size_t cap) { return (size_t)KT::NWIN * C::N * cap; }
+    using KT = KT_;
+    static constexpr size_t bases_words(size_t cap) { return (size_t)KT::NBASE * 3 * C::N * cap; }
+    static constexpr size_t hs_words(size_t cap) { return (size_t)KT::NCHAIN * (KT::ENT - 1) * C::N * cap; }
+    static constexpr size_t ztop_words(size_t cap) { return (size_t)KT::NCHAIN * C::N * cap; }
     static constexpr size_t ktab_words(size_t cap) { return KT::POINTS * 2 * C::N * cap; }
 };
 

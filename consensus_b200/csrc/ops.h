@@ -1,22 +1,22 @@
 // ops.h — per-curve kernel launchers behind plain function pointers, so that the host pipeline (pipeline.cu) is
 // written once and the heavy kernel templates are compiled in parallel, one translation unit per group
-// (inst_<curve>_{prep,coz,kt5,kt8}.cu).
+// (inst_<curve>_{prep,coz,comb|kt5,kt8}.cu).
 #pragma once
 #include <cuda_runtime.h>
 #include <stddef.h>
 #include <stdint.h>
 
-struct KtGeom {           // geometry of a per-key table for one window width
-    int W, nwin, ent;     // window bits, windows, entries per window
-    size_t bases_words, hs_words, ztop_words, ktab_words;  // per key
+struct KtGeom {  // words per key of a per-key table and of its construction scratch
+    size_t bases_words, hs_words, ztop_words, ktab_words;
 };
 
 struct KtOps {
     KtGeom geom;
-    // the four table-construction kernels, enqueued back to back on st
+    // the table-construction kernels, enqueued back to back on st
     cudaError_t (*build)(const uint32_t *nkeys_ptr, uint32_t cap, const uint32_t *keylist, const uint8_t *qx, const uint8_t *qy,
                          uint32_t *bases, uint32_t *hs, uint32_t *ztop, uint32_t *pref, uint32_t *ktab, uint8_t *keyflags, cudaStream_t st);
     // fixed-base verification; reg: keys by slot (registered) or by item (grouped); warp: one signature per warp
+    // (registered only)
     cudaError_t (*verify)(int reg, int warp, uint32_t n, const uint32_t *slot, const int32_t *kidmap, uint32_t n_slots,
                           const uint8_t *keyflags, const uint8_t *r, const uint32_t *uw, const uint8_t *flags, const uint32_t *gtab,
                           const uint32_t *ktab, uint8_t *ok, const uint32_t *list, const uint32_t *count, const uint32_t *gacc, cudaStream_t st);
@@ -40,7 +40,8 @@ struct CurveOps {
     cudaError_t (*gpart)(uint32_t n, const uint32_t *uw, const uint32_t *gtab, uint32_t *gacc, cudaStream_t st);
     cudaError_t (*coz)(uint32_t n, const uint8_t *qx, const uint8_t *qy, const uint8_t *r, const uint32_t *uw, const uint8_t *flags,
                        const uint32_t *gtab, uint32_t *tscr, uint8_t *ok, const uint32_t *list, const uint32_t *count, cudaStream_t st);
-    const KtOps *kt5, *kt8;
+    // keys grouped inside a launch (P-256: comb tables; P-384: 5-bit window tables) / registered keys (8-bit windows)
+    const KtOps *grouped, *kt8;
 };
 
 #define SBV_COZ_DECL(NAME)                                                                                                          \
@@ -49,5 +50,5 @@ struct CurveOps {
 SBV_COZ_DECL(sbv_coz_p256);
 SBV_COZ_DECL(sbv_coz_p384);
 extern const CurveOps sbv_ops_p256, sbv_ops_p384;
-extern const KtOps sbv_kt5_p256, sbv_kt8_p256, sbv_kt5_p384, sbv_kt8_p384;
+extern const KtOps sbv_comb_p256, sbv_kt8_p256, sbv_kt5_p384, sbv_kt8_p384;
 inline const CurveOps &sbv_ops(int curve) { return curve == 0 ? sbv_ops_p256 : sbv_ops_p384; }

@@ -2,12 +2,12 @@
 //
 // Keys-per-item batch (sbv_verify_batch*, sbv_hash_verify_batch, sbv_verify_mixed):
 //
-//   st     memsets  k_kg_insert  k_kg_assign  k_kg_route ─┬─ k_prep ───────────────┬─ (wait tables) k_verify_kt ─ (wait generic) ─ done
-//   s_tab                                                 └─ k_kt_bases  k_kt_fill  k_kt_inv  k_kt_final ─┘
-//   s_gen                                                                          └─ k_verify_coz (keys without a table) ─┘
+//   st     memsets  k_kg_insert  k_kg_assign  k_kg_route ─┬─ k_prep ─ k_gpart ───────────────────────────────────┬─ (wait tables) k_verify_comb ─ (wait generic) ─ done
+//   s_tab                                                 └─ k_kt_bases4  k_comb_affine  k_comb_fill  k_kt_inv  k_kt_final ─┘
+//   s_gen                                                                          └─ k_verify_coz (keys without a table) ──────────────────────┘
 //
-// Keys that occur at least `group_threshold` times in the batch get a fixed-base table built on the spot (keygroup.cuh)
-// and their signatures take the doubling-free kernel; the rest take the generic kernel.  The scalar preparation
+// Keys that occur at least `group_threshold` times in the batch get a fixed-base table built on the spot (keygroup.cuh: a
+// comb for P-256, 5-bit windows for P-384) and their signatures take the fixed-base kernel; the rest take the generic kernel.  The scalar preparation
 // (latency-bound: one inversion chain) runs beside the table construction (latency-bound: one doubling chain).
 // Registered keys (sbv_set_keys) skip the grouping: their tables were built at registration.
 #include "engine.h"
@@ -161,7 +161,7 @@ int sbv_launch_verify_begin(sbv_engine *e, Dev &d, uint8_t curve, size_t n, cons
     if (n == 0) return 0;
     if (chunks < 1 || chunks > SBV_MAX_CHUNKS) return sbv_fail(e, SBV_ERR_ARG, "bad chunk count %d", chunks);
     const CurveOps &ops = sbv_ops(curve);
-    const KtOps *kt = ops.kt5;
+    const KtOps *kt = ops.grouped;
     const uint32_t nn = (uint32_t)n;
     const uint32_t T = e->group_threshold > 0 ? (uint32_t)e->group_threshold : 0;
     const bool grouping = T > 0 && n >= T && n >= (size_t)e->group_min_batch && e->group_max_keys > 0;
@@ -187,7 +187,7 @@ int sbv_launch_verify_begin(sbv_engine *e, Dev &d, uint8_t curve, size_t n, cons
     CU(e, cudaStreamWaitEvent(w->s_tab, w->ev_group, 0));
     CU(e, kt->build(counters + 0, (uint32_t)kcap, w->keylist, d_qx, d_qy, w->bases, w->hs, w->ztop, w->pref, w->ktab, w->keyflags, w->s_tab));
     CU(e, cudaEventRecord(w->ev_tab, w->s_tab));
-    e->launches += chunks == 1 ? 7 : 6;
+    e->launches += (chunks == 1 ? 3 : 2) + (curve == 0 ? 5 : 4);  // grouping + table construction
     return 0;
 }
 
@@ -200,7 +200,7 @@ int sbv_launch_verify_chunk(sbv_engine *e, Dev &d, const VerifyLaunch &vl, int c
     Dev::Scratch *w = vl.w;
     if (vl.chunks <= 1 || c < 0 || c >= vl.chunks || lo + cn > vl.n) return sbv_fail(e, SBV_ERR_ARG, "bad chunk");
     const CurveOps &ops = sbv_ops(vl.curve);
-    const KtOps *kt = ops.kt5;
+    const KtOps *kt = ops.grouped;
     const size_t N = (size_t)ops.N, L = (size_t)ops.bytes;
     const uint32_t nn = (uint32_t)cn;
     const uint32_t *gtab = d.gtab[vl.curve];
@@ -268,7 +268,7 @@ int sbv_launch_verify_finish(sbv_engine *e, Dev &d, const VerifyLaunch &vl, cons
     if (vl.n == 0) return 0;
     if (vl.chunks != 1) return sbv_fail(e, SBV_ERR_ARG, "chunked launch finished in one piece");
     const CurveOps &ops = sbv_ops(vl.curve);
-    const KtOps *kt = ops.kt5;
+    const KtOps *kt = ops.grouped;
     Dev::Scratch *w = vl.w;
     cudaEvent_t *ev = vl.ev;
     const uint32_t nn = (uint32_t)vl.n;
@@ -327,8 +327,8 @@ void sbv_keys_free(Dev &d) {
 }
 
 // Consenter keys are configuration (they change only with a reconfiguration, i.e. a new VerificationSequence —
-// /root/reference/pkg/api/dependencies.go:65-66): one table per key with 8-bit signed windows, built by the same
-// four kernels the on-the-fly path uses (a few milliseconds for a thousand keys).
+// /root/reference/pkg/api/dependencies.go:65-66): one table per key with 8-bit signed windows, built by the doubling,
+// inversion and conversion kernels the on-the-fly path uses (a few milliseconds for a thousand keys).
 int sbv_keys_build(sbv_engine *e, Dev &d) {
     CU(e, cudaSetDevice(d.ordinal));
     CU(e, cudaDeviceSynchronize());  // no launch on any lane may still read the old tables

@@ -6,6 +6,7 @@
 #include <stdlib.h>
 #include <string.h>
 #include <thread>
+#include <type_traits>
 #include <vector>
 
 #include "../../consensus_b200/csrc/hostsim.h"
@@ -90,35 +91,51 @@ static void run_grid_lockstep(unsigned blocks, unsigned threads, F &&body) {
         }
 }
 
-// per-key tables of `nkeys` keys (key k = item k of qx / qy), built by the product's four kernels; four != 0: the doubling
-// chain by k_kt_bases4 (four lanes per key, in lockstep), else by the one-thread-per-key k_kt_bases.  ktab_out: the final
-// affine tables (KtSizes::ktab_words(nkeys) words), flags_out: nkeys validity flags.
-template <class C, int W>
-static void tables_t(uint32_t nkeys, const uint8_t *qx, const uint8_t *qy, int four, uint32_t *ktab_out, uint8_t *flags_out) {
-    using KS = KtSizes<C, W>;
-    using KT = KeyTab<32 * C::N, W>;
-    const size_t cap = nkeys;
-    std::vector<uint32_t> bases(KS::bases_words(cap)), hs(KS::hs_words(cap)), ztop(KS::ztop_words(cap)), pref(KS::ztop_words(cap)), ktab(KS::ktab_words(cap), 0);
-    std::vector<uint8_t> kflags(cap, 0);
-    uint32_t cnt = nkeys;
-    if (four) run_grid_lockstep((unsigned)((cap * 4 + 127) / 128), 128, [&] { k_kt_bases4<C, W>(&cnt, (uint32_t)cap, nullptr, qx, qy, bases.data(), kflags.data()); });
-    else run_grid((unsigned)((cap + 63) / 64), 64, [&] { k_kt_bases<C, W, true>(&cnt, (uint32_t)cap, nullptr, qx, qy, bases.data(), kflags.data()); });
-    run_grid((unsigned)((cap * KT::NWIN + 63) / 64), 64, [&] { k_kt_fill<C, W>(&cnt, (uint32_t)cap, bases.data(), kflags.data(), hs.data(), ztop.data(), ktab.data()); });
-    run_grid((unsigned)((cap + 63) / 64), 64, [&] { k_kt_inv<C, W>(&cnt, (uint32_t)cap, kflags.data(), ztop.data(), pref.data()); });
-    run_grid((unsigned)((cap * KT::NWIN + 63) / 64), 64, [&] { k_kt_final<C, W>(&cnt, (uint32_t)cap, bases.data(), kflags.data(), hs.data(), ztop.data(), ktab.data()); });
-    memcpy(ktab_out, ktab.data(), ktab.size() * 4);
-    memcpy(flags_out, kflags.data(), cap);
+// the product's construction kernels for a window table (KT = KeyTab) or a comb table (KT = CombTab) of up to `cap` keys,
+// *cnt of them, key k = item keylist[k] of qx / qy (keylist NULL: item k).  four != 0: the doubling chain by k_kt_bases4
+// (four lanes per key, in lockstep), else by the one-thread-per-key k_kt_bases.  ktab: KtSizes::ktab_words(cap) words of
+// final affine tables, kflags: cap validity flags.
+template <class C, class KT>
+static void build_t(const uint32_t *cnt, uint32_t cap, const uint32_t *keylist, const uint8_t *qx, const uint8_t *qy, int four, uint32_t *ktab,
+                    uint8_t *kflags) {
+    using KS = KtSizes<C, KT>;
+    std::vector<uint32_t> bases(KS::bases_words(cap)), hs(KS::hs_words(cap)), ztop(KS::ztop_words(cap)), pref(KS::ztop_words(cap));
+    const unsigned kb = (cap + 63) / 64, cb = (unsigned)(((size_t)cap * KT::NCHAIN + 63) / 64);
+    if (four) run_grid_lockstep((unsigned)(((size_t)cap * 4 + 127) / 128), 128, [&] { k_kt_bases4<C, KT>(cnt, cap, keylist, qx, qy, bases.data(), kflags); });
+    else run_grid(kb, 64, [&] { k_kt_bases<C, KT, true>(cnt, cap, keylist, qx, qy, bases.data(), kflags); });
+    if constexpr (std::is_same<KT, CombTab<C>>::value) {
+        run_grid(kb, 64, [&] { k_comb_affine<C>(cnt, cap, kflags, bases.data(), pref.data()); });
+        run_grid(cb, 64, [&] { k_comb_fill<C>(cnt, cap, bases.data(), kflags, hs.data(), ztop.data(), ktab); });
+    } else {
+        run_grid(cb, 64, [&] { k_kt_fill<C, KT::STEP>(cnt, cap, bases.data(), kflags, hs.data(), ztop.data(), ktab); });
+    }
+    run_grid(kb, 64, [&] { k_kt_inv<C, KT>(cnt, cap, kflags, ztop.data(), pref.data()); });
+    run_grid(cb, 64, [&] { k_kt_final<C, KT>(cnt, cap, bases.data(), kflags, hs.data(), ztop.data(), ktab); });
 }
 
-extern "C" size_t hs_ktab_words(int curve, int w8, size_t nkeys) {
-    if (curve == 0) return w8 ? KtSizes<P256, 8>::ktab_words(nkeys) : KtSizes<P256, 5>::ktab_words(nkeys);
-    return w8 ? KtSizes<P384, 8>::ktab_words(nkeys) : KtSizes<P384, 5>::ktab_words(nkeys);
+template <class C, class KT>
+static void tables_t(uint32_t nkeys, const uint8_t *qx, const uint8_t *qy, int four, uint32_t *ktab_out, uint8_t *flags_out) {
+    std::vector<uint32_t> ktab(KtSizes<C, KT>::ktab_words(nkeys), 0);
+    std::vector<uint8_t> kflags(nkeys, 0);
+    build_t<C, KT>(&nkeys, nkeys, nullptr, qx, qy, four, ktab.data(), kflags.data());
+    memcpy(ktab_out, ktab.data(), ktab.size() * 4);
+    memcpy(flags_out, kflags.data(), nkeys);
 }
-extern "C" int hs_tables(int curve, int w8, size_t nkeys, const uint8_t *qx, const uint8_t *qy, int four, uint32_t *ktab_out, uint8_t *flags_out) {
-    if (curve == 0 && !w8) tables_t<P256, 5>((uint32_t)nkeys, qx, qy, four, ktab_out, flags_out);
-    else if (curve == 0) tables_t<P256, 8>((uint32_t)nkeys, qx, qy, four, ktab_out, flags_out);
-    else if (!w8) tables_t<P384, 5>((uint32_t)nkeys, qx, qy, four, ktab_out, flags_out);
-    else tables_t<P384, 8>((uint32_t)nkeys, qx, qy, four, ktab_out, flags_out);
+
+// kind: 0 = 5-bit windows, 1 = 8-bit windows, 2 = comb (P-256 only, as in the product)
+extern "C" size_t hs_ktab_words(int curve, int kind, size_t nkeys) {
+    if (curve == 0) return kind == 2 ? KtSizes<P256, CombTab<P256>>::ktab_words(nkeys)
+                         : kind ? KtSizes<P256, KeyTab<256, 8>>::ktab_words(nkeys) : KtSizes<P256, KeyTab<256, 5>>::ktab_words(nkeys);
+    return kind == 2 ? 0 : kind ? KtSizes<P384, KeyTab<384, 8>>::ktab_words(nkeys) : KtSizes<P384, KeyTab<384, 5>>::ktab_words(nkeys);
+}
+extern "C" int hs_tables(int curve, int kind, size_t nkeys, const uint8_t *qx, const uint8_t *qy, int four, uint32_t *ktab_out, uint8_t *flags_out) {
+    const uint32_t k = (uint32_t)nkeys;
+    if (curve == 0 && kind == 2) tables_t<P256, CombTab<P256>>(k, qx, qy, four, ktab_out, flags_out);
+    else if (curve == 0 && kind == 1) tables_t<P256, KeyTab<256, 8>>(k, qx, qy, four, ktab_out, flags_out);
+    else if (curve == 0) tables_t<P256, KeyTab<256, 5>>(k, qx, qy, four, ktab_out, flags_out);
+    else if (kind == 2) return -1;
+    else if (kind == 1) tables_t<P384, KeyTab<384, 8>>(k, qx, qy, four, ktab_out, flags_out);
+    else tables_t<P384, KeyTab<384, 5>>(k, qx, qy, four, ktab_out, flags_out);
     return 0;
 }
 
@@ -153,10 +170,10 @@ template <class C>
 static void registered_t(uint32_t n, uint32_t nkeys, const uint8_t *kx, const uint8_t *ky, const uint32_t *slot, const uint8_t *r, const uint8_t *s,
                          const uint8_t *dig, uint32_t dlen, const uint4 *gtab, int warp, uint8_t *ok) {
     constexpr int N = C::N, S = 8, W = 8;
-    using KS = KtSizes<C, W>;
-    std::vector<uint32_t> ktab(KS::ktab_words(nkeys));
+    using KT = KeyTab<32 * N, W>;
+    std::vector<uint32_t> ktab(KtSizes<C, KT>::ktab_words(nkeys));
     std::vector<uint8_t> kflags(nkeys);
-    tables_t<C, W>(nkeys, kx, ky, 0, ktab.data(), kflags.data());
+    tables_t<C, KT>(nkeys, kx, ky, 0, ktab.data(), kflags.data());
     std::vector<int32_t> s2l(nkeys);
     for (uint32_t i = 0; i < nkeys; i++) s2l[i] = (int32_t)i;
     std::vector<uint32_t> uw((size_t)2 * N * n);
@@ -195,14 +212,13 @@ static void verify_coz_t(uint32_t n, const uint8_t *r, const uint8_t *s, const u
     });
 }
 
-// grouped path: k_prep, key grouping, table construction, k_verify_kt for repeated keys + k_verify_coz for the rest
-template <class C, int W>
+// grouped path: k_prep, key grouping, table construction and the fixed-base kernel for repeated keys (P-256: comb tables and
+// k_verify_comb; P-384: 5-bit window tables and k_verify_kt, as in the product), k_verify_coz for the rest
+template <class C>
 static void verify_grouped_t(uint32_t n, const uint8_t *r, const uint8_t *s, const uint8_t *qx, const uint8_t *qy, const uint8_t *dig,
                              uint32_t dlen, const uint4 *gtab, uint32_t threshold, uint32_t max_keys, uint8_t *ok, uint32_t *stats,
                              uint32_t chunk = 0) {
     constexpr int N = C::N, S = 8;
-    using KS = KtSizes<C, W>;
-    using KT = KeyTab<32 * N, W>;
     std::vector<uint32_t> uw((size_t)2 * N * n);
     std::vector<uint8_t> flags(n);
     std::vector<uint32_t> tscr((size_t)12 * N * n);
@@ -215,12 +231,20 @@ static void verify_grouped_t(uint32_t n, const uint8_t *r, const uint8_t *s, con
     run_grid((n + 255) / 256, 256, [&] { k_kg_assign(n, rep.data(), kcnt.data(), threshold, max_keys, keyid.data(), keylist.data(), counters.data()); });
     if (!chunk) run_grid((n + 255) / 256, 256, [&] { k_kg_route(n, rep.data(), keyid.data(), item_kid.data(), klist.data(), glist.data(), counters.data()); });
     const size_t cap = max_keys ? max_keys : 1;
-    std::vector<uint32_t> bases(KS::bases_words(cap)), hs(KS::hs_words(cap)), ztop(KS::ztop_words(cap)), pref(KS::ztop_words(cap)), ktab(KS::ktab_words(cap));
+    constexpr bool comb = std::is_same<C, P256>::value;
+    using KT = typename std::conditional<comb, CombTab<C>, KeyTab<32 * N, 5>>::type;
+    std::vector<uint32_t> ktab(KtSizes<C, KT>::ktab_words(cap));
     std::vector<uint8_t> kflags(cap, 0);
-    run_grid((unsigned)((cap + 63) / 64), 64, [&] { k_kt_bases<C, W, true>(counters.data(), (uint32_t)cap, keylist.data(), qx, qy, bases.data(), kflags.data()); });
-    run_grid((unsigned)((cap * KT::NWIN + 63) / 64), 64, [&] { k_kt_fill<C, W>(counters.data(), (uint32_t)cap, bases.data(), kflags.data(), hs.data(), ztop.data(), ktab.data()); });
-    run_grid((unsigned)((cap + 63) / 64), 64, [&] { k_kt_inv<C, W>(counters.data(), (uint32_t)cap, kflags.data(), ztop.data(), pref.data()); });
-    run_grid((unsigned)((cap * KT::NWIN + 63) / 64), 64, [&] { k_kt_final<C, W>(counters.data(), (uint32_t)cap, bases.data(), kflags.data(), hs.data(), ztop.data(), ktab.data()); });
+    build_t<C, KT>(counters.data(), (uint32_t)cap, keylist.data(), qx, qy, 0, ktab.data(), kflags.data());
+    const uint4 *k4 = reinterpret_cast<const uint4 *>(ktab.data());
+    // the fixed-base kernel over items list[0 .. *count) of a batch of nb items
+    auto fixed_base = [&](uint32_t nb, const int32_t *kid, const uint8_t *rb, const uint32_t *uwb, const uint8_t *fl, uint8_t *okb, const uint32_t *list,
+                          const uint32_t *count, const uint32_t *ga) {
+        run_grid((nb + 63) / 64, 64, [&] {
+            if constexpr (comb) k_verify_comb<C, 64, 1, false>(nb, kid, kflags.data(), rb, uwb, fl, gtab, k4, okb, list, count, ga);
+            else k_verify_kt<C, 5, 64, 1, false, false>(nb, nullptr, kid, 0, kflags.data(), rb, uwb, fl, gtab, k4, okb, list, count, ga);
+        });
+    };
     const bool gsplit = (threshold & 1) == 0;  // exercise both forms: even thresholds take the split u1*G path
     std::vector<uint32_t> gacc((size_t)3 * N * n);
     if (chunk) {
@@ -239,20 +263,14 @@ static void verify_grouped_t(uint32_t n, const uint8_t *r, const uint8_t *s, con
             run_grid((cn + 255) / 256, 256, [&] { k_kg_route(cn, rep.data() + lo, keyid.data(), item_kid.data() + lo, klist.data() + lo, glist.data() + lo, cc.data()); });
             run_grid((cn + 63) / 64, 64, [&] { k_verify_coz<C, 64, 1>(cn, qx + lo * L, qy + lo * L, rc, uwc, flc, gtab, tsc, ok + lo, glist.data() + lo, cc.data() + 2); });
             if (gsplit) run_grid((cn + 63) / 64, 64, [&] { k_gpart<C, 64, 1>(cn, uwc, gtab, gac); });
-            run_grid((cn + 63) / 64, 64, [&] {
-                k_verify_kt<C, W, 64, 1, false, false>(cn, nullptr, item_kid.data() + lo, 0, kflags.data(), rc, uwc, flc, gtab,
-                                                reinterpret_cast<const uint4 *>(ktab.data()), ok + lo, klist.data() + lo, cc.data() + 1, gsplit ? gac : nullptr);
-            });
+            fixed_base(cn, item_kid.data() + lo, rc, uwc, flc, ok + lo, klist.data() + lo, cc.data() + 1, gsplit ? gac : nullptr);
             kt_total += cc[1]; gen_total += cc[2];
         }
         if (stats) { stats[0] = counters[0]; stats[1] = kt_total; stats[2] = gen_total; }
         return;
     }
     if (gsplit) run_grid((n + 63) / 64, 64, [&] { k_gpart<C, 64, 1>(n, uw.data(), gtab, gacc.data()); });
-    run_grid((n + 63) / 64, 64, [&] {
-        k_verify_kt<C, W, 64, 1, false, false>(n, nullptr, item_kid.data(), 0, kflags.data(), r, uw.data(), flags.data(), gtab,
-                                        reinterpret_cast<const uint4 *>(ktab.data()), ok, klist.data(), counters.data() + 1, gsplit ? gacc.data() : nullptr);
-    });
+    fixed_base(n, item_kid.data(), r, uw.data(), flags.data(), ok, klist.data(), counters.data() + 1, gsplit ? gacc.data() : nullptr);
     run_grid((n + 63) / 64, 64, [&] {
         k_verify_coz<C, 64, 1>(n, qx, qy, r, uw.data(), flags.data(), gtab, tscr.data(), ok, glist.data(), counters.data() + 2);
     });
@@ -275,8 +293,8 @@ static const uint4 *gtab_for(int idx) {
 // the same with the second half run chunk by chunk (chunk = items per chunk), as a chunked host-buffer call does
 extern "C" int hs_verify_chunked(int curve, size_t n, const uint8_t *r, const uint8_t *s, const uint8_t *qx, const uint8_t *qy, const uint8_t *dig,
                       uint32_t dlen, uint32_t threshold, uint32_t max_keys, uint32_t chunk, uint8_t *ok, uint32_t *stats) {
-    if (curve == 0) verify_grouped_t<P256, 5>((uint32_t)n, r, s, qx, qy, dig, dlen, gtab_for<P256>(0), threshold, max_keys, ok, stats, chunk);
-    else verify_grouped_t<P384, 5>((uint32_t)n, r, s, qx, qy, dig, dlen, gtab_for<P384>(1), threshold, max_keys, ok, stats, chunk);
+    if (curve == 0) verify_grouped_t<P256>((uint32_t)n, r, s, qx, qy, dig, dlen, gtab_for<P256>(0), threshold, max_keys, ok, stats, chunk);
+    else verify_grouped_t<P384>((uint32_t)n, r, s, qx, qy, dig, dlen, gtab_for<P384>(1), threshold, max_keys, ok, stats, chunk);
     return 0;
 }
 
@@ -290,8 +308,8 @@ extern "C" int hs_verify(int curve, size_t n, const uint8_t *r, const uint8_t *s
 // grouped (fixed-base for repeated keys) path; stats = {keys found, items on the fixed-base path, items on the generic path}
 extern "C" int hs_verify_grouped(int curve, size_t n, const uint8_t *r, const uint8_t *s, const uint8_t *qx, const uint8_t *qy, const uint8_t *dig,
                       uint32_t dlen, uint32_t threshold, uint32_t max_keys, uint8_t *ok, uint32_t *stats) {
-    if (curve == 0) verify_grouped_t<P256, 5>((uint32_t)n, r, s, qx, qy, dig, dlen, gtab_for<P256>(0), threshold, max_keys, ok, stats);
-    else verify_grouped_t<P384, 5>((uint32_t)n, r, s, qx, qy, dig, dlen, gtab_for<P384>(1), threshold, max_keys, ok, stats);
+    if (curve == 0) verify_grouped_t<P256>((uint32_t)n, r, s, qx, qy, dig, dlen, gtab_for<P256>(0), threshold, max_keys, ok, stats);
+    else verify_grouped_t<P384>((uint32_t)n, r, s, qx, qy, dig, dlen, gtab_for<P384>(1), threshold, max_keys, ok, stats);
     return 0;
 }
 
