@@ -386,8 +386,7 @@ int stage_and_verify(sbv_engine *e, Dev &d, int lane, uint8_t curve, size_t lo, 
         if (hashing && cn && (rc = sbv_launch_sha256(e, cn, ln.d_msgs, ln.d_off + clo, base, ln.d_dig + clo * 32, ln.d_perm + clo, ln.stream)))
             return abandon(rc);
         std::lock_guard<std::mutex> lk(e->mu);
-        if (chunks == 1) rc = sbv_launch_verify_finish(e, d, vl, ln.d_r, ln.d_s, ln.d_dig, dlen, ln.d_ok, ln.stream);
-        else rc = sbv_launch_verify_chunk(e, d, vl, c, clo, cn, c == chunks - 1, ln.d_r, ln.d_s, ln.d_dig, dlen, ln.d_ok, ln.stream);
+        rc = sbv_launch_verify_chunk(e, d, vl, c, clo, cn, c == chunks - 1, ln.d_r, ln.d_s, ln.d_dig, dlen, ln.d_ok, ln.stream);
         if (rc) { sbv_launch_verify_abort(vl, ln.stream); return rc; }
     }
     if (so_out) *so_out = so;
@@ -409,10 +408,7 @@ int sbv_create(const int *device_ordinals, int n_devices, sbv_engine **out) {
     e->group_threshold = env_int("SBV_GROUP_THRESHOLD", 16);
     e->group_max_keys = env_int("SBV_GROUP_MAX_KEYS", 8192);
     e->group_min_batch = env_int("SBV_GROUP_MIN_BATCH", 0);
-    e->gsplit = env_int("SBV_GSPLIT", 1) != 0;
     e->chunk_items = env_int("SBV_CHUNK_ITEMS", 262144);
-    e->gather_hi = env_int("SBV_GATHER_PRIORITY", 1) != 0;
-    e->tab_hi = env_int("SBV_TAB_PRIORITY", 1) != 0;
     {
         // per-engine hash seed: an adversary who picks the keys of a batch cannot aim at the probe sequence
         uint64_t t = (uint64_t)(uintptr_t)e;
@@ -573,13 +569,11 @@ int sbv_comm_init_rank(sbv_engine *e, const uint8_t *id128, int nranks, int rank
     void *comm = nullptr;
     NC(e, g_nccl.comm_init_rank(&comm, nranks, id, rank));
     sbv_engine::ChannelHi hi;
-    if (e->gather_hi) {
-        int lo_p = 0, hi_p = 0;
-        CU(e, cudaDeviceGetStreamPriorityRange(&lo_p, &hi_p));
-        CU(e, cudaStreamCreateWithPriority(&hi.st, cudaStreamNonBlocking, hi_p));
-        CU(e, cudaEventCreateWithFlags(&hi.in, cudaEventDisableTiming));
-        CU(e, cudaEventCreateWithFlags(&hi.out, cudaEventDisableTiming));
-    }
+    int lo_p = 0, hi_p = 0;
+    CU(e, cudaDeviceGetStreamPriorityRange(&lo_p, &hi_p));
+    CU(e, cudaStreamCreateWithPriority(&hi.st, cudaStreamNonBlocking, hi_p));
+    CU(e, cudaEventCreateWithFlags(&hi.in, cudaEventDisableTiming));
+    CU(e, cudaEventCreateWithFlags(&hi.out, cudaEventDisableTiming));
     std::lock_guard<std::mutex> lk(e->mu);
     e->rank_comms.push_back(comm);
     e->rank_hi.push_back(hi);
@@ -601,7 +595,7 @@ int sbv_gather_verdicts_device(sbv_engine *e, int channel, const uint8_t *d_ok, 
     const size_t wp = (n + 31) / 32;
     uint32_t *mine = d_mask_all + wp * (size_t)e->rank;
     if (e->nranks > 1 && (channel < 0 || channel >= (int)e->rank_comms.size())) return fail(e, SBV_ERR_NCCL, "no such channel: call sbv_comm_init_rank first");
-    const bool fork = e->nranks > 1 && e->rank_hi[channel].st;
+    const bool fork = e->nranks > 1;
     cudaStream_t gs = st;
     if (fork) {  // the exchange runs on the channel's high-priority stream, between two events on the caller's stream
         const sbv_engine::ChannelHi &hi = e->rank_hi[channel];
@@ -612,9 +606,9 @@ int sbv_gather_verdicts_device(sbv_engine *e, int channel, const uint8_t *d_ok, 
     k_pack_bits<<<(uint32_t)((n + 255) / 256), 256, 0, gs>>>((uint32_t)n, d_ok, mine);
     e->launches += 1;
     CU(e, cudaGetLastError());
-    if (e->nranks > 1) NC(e, g_nccl.all_gather(mine, d_mask_all, wp, NCCL_UINT32, e->rank_comms[channel], gs));
     if (fork) {
         const sbv_engine::ChannelHi &hi = e->rank_hi[channel];
+        NC(e, g_nccl.all_gather(mine, d_mask_all, wp, NCCL_UINT32, e->rank_comms[channel], gs));
         CU(e, cudaEventRecord(hi.out, gs));
         CU(e, cudaStreamWaitEvent(st, hi.out, 0));
     }

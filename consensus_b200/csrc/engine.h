@@ -18,35 +18,40 @@ constexpr int SBV_LANES = 6;    // concurrent host-buffer calls per engine
 constexpr int SBV_SCRATCH = 8;  // scratch sets per device (> SBV_LANES + 1: a launch may be held open per lane)
 constexpr int SBV_MAX_CHUNKS = 32;  // a large host-buffer batch is uploaded and verified in at most this many chunks
 
+// A device buffer with the bytes allocated for it; reads as a T *.
+struct DevBuf {
+    void *p = nullptr;
+    size_t bytes = 0;
+};
+template <class T>
+struct DevArray : DevBuf {
+    operator T *() const { return static_cast<T *>(p); }
+};
+
 struct Dev {
     int ordinal = 0;
     cudaStream_t stream = nullptr;
     uint32_t *gtab[2] = {nullptr, nullptr};
     // Per-launch workspace of the verify pipeline.  A launch takes the next set and first waits for the event of
     // that set's previous user, so launches on different streams overlap without sharing mutable state.
+    // The buffers are sized, grown and freed from one list (pipeline.cu: each_buffer).
     struct Scratch {
-        size_t cap = 0;   // items
-        size_t kcap = 0;  // keys with a table per launch
-        uint32_t *uw = nullptr;     // k_prep output: u1, u2 word-major [2N][cap]
-        uint8_t *flags = nullptr;   // r, s range verdicts
-        uint32_t *tscr = nullptr;   // k_verify_coz per-signature scratch: 12N words, word-major
-        uint32_t *gacc = nullptr;   // k_gpart -> k_verify_kt: u1*G of every item (Jacobian, 3N words, word-major)
+        DevArray<uint32_t> uw;      // k_prep output: u1, u2 word-major [2N][n]
+        DevArray<uint8_t> flags;    // r, s range verdicts
+        DevArray<uint32_t> tscr;    // k_verify_coz per-signature scratch: 12N words, word-major
+        DevArray<uint32_t> gacc;    // k_gpart -> fixed-base kernel: u1*G of every item (Jacobian, 3N words, word-major)
         // key grouping
         uint32_t hsize = 0;
-        uint32_t *htab = nullptr, *rep = nullptr, *keylist = nullptr, *klist = nullptr, *glist = nullptr;
-        uint32_t *zeroed = nullptr;  // one memset: counters[4], kcnt[n], then counters[4] per chunk of a chunked launch
-        int32_t *keyid = nullptr, *item_kid = nullptr;
+        DevArray<uint32_t> htab, rep, keylist, klist, glist;
+        DevArray<uint32_t> zeroed;  // one memset: counters[4], kcnt[n], then counters[4] per chunk
+        DevArray<int32_t> keyid, item_kid;
         // per-key tables of the launch
-        uint32_t *bases = nullptr, *hs = nullptr, *ztop = nullptr, *pref = nullptr, *ktab = nullptr;
-        uint8_t *keyflags = nullptr;
+        DevArray<uint32_t> bases, hs, ztop, pref, ktab;
+        DevArray<uint8_t> keyflags;
         cudaStream_t s_tab = nullptr, s_gen = nullptr;  // table construction / generic kernel run beside the main stream
         cudaEvent_t done = nullptr, ev_group = nullptr, ev_prep = nullptr, ev_tab = nullptr, ev_gen = nullptr;
         bool used = false;
         bool open = false;  // taken by a launch whose second half has not been enqueued yet
-        struct Caps {  // bytes allocated per buffer
-            size_t uw = 0, flags = 0, tscr = 0, gacc = 0, htab = 0, rep = 0, keylist = 0, klist = 0, glist = 0, zeroed = 0, keyid = 0, item_kid = 0, bases = 0,
-                   hs = 0, ztop = 0, pref = 0, ktab = 0, keyflags = 0;
-        } caps;
     } ws[SBV_SCRATCH];
     unsigned ws_next = 0;
     // Per-call lanes of the host-buffer entry points: own stream, input/verdict buffers and pinned staging, so that
@@ -96,7 +101,6 @@ struct sbv_engine {
     int group_max_keys = 8192;     // table slots per launch (SBV_GROUP_MAX_KEYS)
     int group_min_batch = 0;       // launches smaller than this skip the grouping (SBV_GROUP_MIN_BATCH)
     int chunk_items = 262144;      // host-buffer shards of >= this many items are uploaded and verified in >= 2 chunks of nominally this size (SBV_CHUNK_ITEMS; 0 = never)
-    bool gsplit = true;            // u1*G in its own kernel beside the table construction (SBV_GSPLIT=0: inside the fixed-base kernel)
     uint32_t hash_seed = 0x9e3779b9u;
     bool profiling = false;
     // NCCL (loaded lazily with dlopen so single-device, single-rank users never touch it)
@@ -106,12 +110,9 @@ struct sbv_engine {
     // collectives of a channel must be issued in the same order on every rank, so concurrent host threads take one each.
     std::vector<void *> rank_comms;
     // per channel: a high-priority stream for the pack + all-gather of a step (fork / join with two events), so that the
-    // exchange is dispatched ahead of the pending blocks of other lanes' verification kernels (SBV_GATHER_PRIORITY)
+    // exchange is dispatched ahead of the pending blocks of other lanes' verification kernels
     struct ChannelHi { cudaStream_t st = nullptr; cudaEvent_t in = nullptr, out = nullptr; };
     std::vector<ChannelHi> rank_hi;
-    bool gather_hi = true;
-    bool tab_hi = true;            // table-construction side streams at high priority: their few, latency-bound blocks are dispatched ahead of
-                                   // the pending blocks of other launches' verification kernels (SBV_TAB_PRIORITY=0: e2e 72.9 -> 76 M/s with it)
     int rank = 0, nranks = 1;
     // key registry
     uint64_t verification_seq = 0;
@@ -150,7 +151,7 @@ struct VerifyLaunch {
     size_t n = 0;
     uint8_t curve = 0;
     bool grouping = false;
-    int chunks = 1;   // > 1: the second half comes chunk by chunk (sbv_launch_verify_chunk)
+    int chunks = 1;   // the second half comes in this many chunks (sbv_launch_verify_chunk)
 };
 
 // ---- pipeline.cu: the verify pipelines (device pointers in, verdict bytes out; enqueue only, no sync) ----
@@ -160,12 +161,10 @@ int sbv_launch_verify(sbv_engine *e, Dev &d, uint8_t curve, size_t n, const uint
 int sbv_launch_verify_begin(sbv_engine *e, Dev &d, uint8_t curve, size_t n, const uint8_t *d_qx, const uint8_t *d_qy, cudaStream_t st, VerifyLaunch *vl,
                             int chunks = 1);
 void sbv_launch_verify_abort(const VerifyLaunch &vl, cudaStream_t st);  // hand the scratch set back after a fault between the halves
-// second half for items [lo, lo + cn) of a launch begun with chunks > 1 (the pointers are those of the WHOLE batch);
-// `last` closes the launch
+// second half for items [lo, lo + cn) of chunk c (the pointers are those of the WHOLE batch; a launch of one chunk has
+// c = 0, lo = 0, cn = n); `last` closes the launch
 int sbv_launch_verify_chunk(sbv_engine *e, Dev &d, const VerifyLaunch &vl, int c, size_t lo, size_t cn, bool last, const uint8_t *d_r, const uint8_t *d_s,
                             const uint8_t *d_dig, uint32_t dlen, uint8_t *d_ok, cudaStream_t st);
-int sbv_launch_verify_finish(sbv_engine *e, Dev &d, const VerifyLaunch &vl, const uint8_t *d_r, const uint8_t *d_s, const uint8_t *d_dig, uint32_t dlen,
-                             uint8_t *d_ok, cudaStream_t st);
 // registered keys (sbv_set_keys)
 int sbv_launch_keyed(sbv_engine *e, Dev &d, uint8_t curve, size_t n, const uint32_t *d_slot, const uint8_t *d_r, const uint8_t *d_s,
                      const uint8_t *d_dig, uint32_t dlen, uint8_t *d_ok, cudaStream_t st);

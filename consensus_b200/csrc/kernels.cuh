@@ -10,8 +10,9 @@
 //                        thread: on-curve check, 4-bit signed window over a common-Z table of Q (shared memory,
 //                        bank = lane, + coalesced global scratch), 256 doublings interleaved with 65 additions, 16
 //                        comb additions for u1*G with the next gather in flight, final X == r*Z^2 comparison
+//   k_gpart              u1*G alone, for the items of keys that repeat inside a batch
 //   k_verify_comb        FIXED-BASE path for P-256 keys that repeat inside a batch (comb table of the key, keygroup.cuh
-//                        builds it on the fly): 32 comb additions and 15 doublings for u2*Q, then u1*G
+//                        builds it on the fly): 32 comb additions and 15 doublings for u2*Q, then k_gpart's u1*G
 //   k_verify_kt          FIXED-BASE path over a window table: registered keys (sbv_set_keys, 8-bit windows, built once
 //                        per key set) and P-384 keys that repeat inside a batch (5-bit windows): no doublings,
 //                        NWIN(W) signed-window additions for u2*Q + the comb additions for u1*G
@@ -553,16 +554,14 @@ __global__ void __launch_bounds__(BLOCK, MINB) k_verify_kt(uint32_t n, const uin
 
 // k_verify_comb — keys grouped inside a launch: the key of item list[t] is kidmap[list[t]] (>= 0 for every listed item),
 // its table a CombTab.  u2*Q column by column from the top: a doubling (none before the first column), then one table
-// addition per block; then u1*G, after the last doubling: one general addition of k_gpart's point when gacc != NULL,
-// else the GWINS comb additions from G's table.
+// addition per block; then u1*G, after the last doubling: one general addition of k_gpart's point (gacc).
 // One inlined addition site and one doubling site in one loop: the addition hands its exceptional case (accumulator ==
 // entry) to the doubling site (pt_add_m<…, DEFER>) instead of carrying its own copy of the doubling, and the next table
-// entry (a random 64-byte gather) is in flight while the current one is added.  The additions stay complete: the key
-// entries cannot meet the accumulator (its scalar and theirs are distinct multiples below n), but the G entries can.
+// entry (a random 64-byte gather) is in flight while the current one is added.  The additions stay complete.
 template <class C, int BLOCK, int MINB, bool INL>
 __global__ void __launch_bounds__(BLOCK, MINB) k_verify_comb(uint32_t n, const int32_t *__restrict__ kidmap, const uint8_t *__restrict__ keyflags,
                                                               const uint8_t *__restrict__ r_be, const uint32_t *__restrict__ uw,
-                                                              const uint8_t *__restrict__ flags, const uint4 *__restrict__ gtab,
+                                                              const uint8_t *__restrict__ flags,
                                                               const uint4 *__restrict__ ktab, uint8_t *__restrict__ ok_out,
                                                               const uint32_t *__restrict__ list, const uint32_t *__restrict__ count,
                                                               const uint32_t *__restrict__ gacc) {
@@ -571,7 +570,6 @@ __global__ void __launch_bounds__(BLOCK, MINB) k_verify_comb(uint32_t n, const i
     constexpr int EU4 = 2 * N / 4;  // uint4 per table entry
     using CT = CombTab<C>;
     constexpr int KADD = CT::SPACING * CT::BLOCKS;  // key additions
-    const int TOTAL = gacc ? KADD : KADD + C::GWINS;
     const uint32_t t = blockIdx.x * BLOCK + threadIdx.x;
     if (t >= __ldg(count)) return;
     const uint32_t idx = __ldg(list + t);
@@ -586,26 +584,19 @@ __global__ void __launch_bounds__(BLOCK, MINB) k_verify_comb(uint32_t n, const i
     mp_copy<N>(acc.Y, one);
 #pragma unroll
     for (int i = 0; i < N; i++) acc.Z[i] = 0;
-    // step s < KADD: column SPACING-1 - s/2, block s%2 of u2's comb; s >= KADD: comb digit s - KADD of u1 into G's table
+    // step s: column SPACING-1 - s/2, block s%2 of u2's comb
     auto fetch = [&](int s, uint32_t (&x)[N], uint32_t (&y)[N], bool &skip) {
-        if (s < KADD) {
-            const int b = s & 1;
-            const uint32_t m = comb_mask_u2<C>(uw, n, idx, b, CT::SPACING - 1 - (s >> 1));
-            load_affine<C>(x, y, kt + (size_t)CT::slot(b, m) * EU4);
-            skip = m == 0;
-        } else {
-            const int g = s - KADD;
-            const uint32_t d = comb_digit_u1<C>(uw, n, idx, g);
-            load_affine<C>(x, y, gtab + (((size_t)g << C::GW) + d) * EU4);
-            skip = d == 0;
-        }
+        const int b = s & 1;
+        const uint32_t m = comb_mask_u2<C>(uw, n, idx, b, CT::SPACING - 1 - (s >> 1));
+        load_affine<C>(x, y, kt + (size_t)CT::slot(b, m) * EU4);
+        skip = m == 0;
     };
     uint32_t cx[N], cy[N];
     bool cskip;
     fetch(0, cx, cy, cskip);
     int s = 0, dbl = 0;  // dbl: doublings due before the addition of step s
 #pragma unroll 1
-    while (s < TOTAL || dbl) {
+    while (s < KADD || dbl) {
         if (dbl) {
             pt_double<A>(acc);
             dbl--;
@@ -613,15 +604,15 @@ __global__ void __launch_bounds__(BLOCK, MINB) k_verify_comb(uint32_t n, const i
         }
         uint32_t nx[N], ny[N];
         bool nskip = true;
-        if (s + 1 < TOTAL) fetch(s + 1, nx, ny, nskip);
+        if (s + 1 < KADD) fetch(s + 1, nx, ny, nskip);
         dbl = pt_add_m<A, 1, true>(acc, cx, cy, one, one, one, false, cskip) ? 1 : 0;  // acc == entry: the sum is 2 * acc
         s++;
         if (s < KADD && (s & 1) == 0) dbl++;  // next column
-        if (s < TOTAL) { mp_copy<N>(cx, nx); mp_copy<N>(cy, ny); cskip = nskip; }
+        if (s < KADD) { mp_copy<N>(cx, nx); mp_copy<N>(cy, ny); cskip = nskip; }
     }
     Jac<C> fin;
     mp_copy<N>(fin.X, acc.X); mp_copy<N>(fin.Y, acc.Y); mp_copy<N>(fin.Z, acc.Z);
-    if (gacc) {  // the closing general addition (out-of-line multiplications: once per signature, outside the loop)
+    {  // the closing general addition (out-of-line multiplications: once per signature, outside the loop)
         Jac<C> g;
 #pragma unroll
         for (int i = 0; i < N; i++) {

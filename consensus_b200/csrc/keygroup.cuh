@@ -10,7 +10,8 @@
 //   k_kg_assign   representatives whose key occurs >= T times (and while table slots last) get a dense key id
 //   k_kg_route    items are appended to the fixed-base list (their key has a table) or to the generic list
 //   k_kt_bases4   four lanes per key: validate the key, the bases B_i = 2^(STEP*i) * Q of its table — a chain of
-//                 doublings whose independent multiplications run on different lanes (k_kt_bases: one thread per key)
+//                 doublings whose independent multiplications run on different lanes (k_kt_bases, one thread per key,
+//                 is its reference in the CPU simulation)
 //   k_comb_affine one thread per key (comb): the 16 bases to affine with one inversion
 //   k_comb_fill   one thread per (key, chain) (comb): the 16 entries of a chain, one mixed addition per Gray-code step
 //   k_kt_fill     one thread per (key, window) (window table): e*B_w for e = 1..2^(W-1) with co-Z additions (5M+2S
@@ -137,9 +138,8 @@ static __global__ void __launch_bounds__(256) k_kg_route(uint32_t n, const uint3
 
 // nkeys_ptr: device counter (clamped to cap) — the grid is sized for the worst case and surplus threads leave.
 // key k is item keylist[k] of (qx_be, qy_be); for registered keys keylist is the identity over the key array.
-// INL: the eight multiplications of the doubling inlined (one site, ~25 KB): this kernel is a single dependent chain per
-// thread on an otherwise idle SM sub-partition, so what counts is how well independent multiplications interleave.
-template <class C, class KT, bool INL>
+// One thread per key: the reference for k_kt_bases4 in the CPU simulation (tools/hostsim); libsbv.so launches k_kt_bases4.
+template <class C, class KT>
 __global__ void __launch_bounds__(64) k_kt_bases(const uint32_t *__restrict__ nkeys_ptr, uint32_t cap, const uint32_t *__restrict__ keylist,
                                                  const uint8_t *__restrict__ qx_be, const uint8_t *__restrict__ qy_be,
                                                  uint32_t *__restrict__ bases, uint8_t *__restrict__ keyflags) {
@@ -149,8 +149,7 @@ __global__ void __launch_bounds__(64) k_kt_bases(const uint32_t *__restrict__ nk
     if (nkeys > cap) nkeys = cap;
     if (k >= nkeys) return;
     const uint32_t item = keylist ? keylist[k] : k;
-    using A = typename PickArith<C, INL>::type;
-    Jac<A> B;
+    Jac<C> B;
     const bool good = load_key<C>(B.X, B.Y, qx_be, qy_be, item);
     keyflags[k] = good ? 1 : 0;
     if (!good) return;  // no table: every item of this key rejects (k_verify_kt checks the flag)
@@ -159,7 +158,7 @@ __global__ void __launch_bounds__(64) k_kt_bases(const uint32_t *__restrict__ nk
     for (int win = 0; win < KT::NBASE; win++) {
         if (win) {
 #pragma unroll 1
-            for (int d = 0; d < KT::STEP; d++) pt_double<A>(B);
+            for (int d = 0; d < KT::STEP; d++) pt_double<C>(B);
         }
         uint32_t *o = bases + (size_t)win * 3 * N * cap + k;
 #pragma unroll

@@ -2,17 +2,58 @@
 //
 // Keys-per-item batch (sbv_verify_batch*, sbv_hash_verify_batch, sbv_verify_mixed):
 //
-//   st     memsets  k_kg_insert  k_kg_assign  k_kg_route ─┬─ k_prep ─ k_gpart ───────────────────────────────────┬─ (wait tables) k_verify_comb ─ (wait generic) ─ done
-//   s_tab                                                 └─ k_kt_bases4  k_comb_affine  k_comb_fill  k_kt_inv  k_kt_final ─┘
-//   s_gen                                                                          └─ k_verify_coz (keys without a table) ──────────────────────┘
+//   st     memsets  k_kg_insert  k_kg_assign ─┬─ k_prep  k_kg_route ─┬─ k_gpart ──────────────────────────────────┬─ (wait tables) k_verify_comb ─ (wait generic) ─ done
+//   s_tab                                     └─ k_kt_bases4  k_comb_affine  k_comb_fill  k_kt_inv  k_kt_final ─┘
+//   s_gen                                                             └─ k_verify_coz (keys without a table) ──────────────────────────────────┘
 //
 // Keys that occur at least `group_threshold` times in the batch get a fixed-base table built on the spot (keygroup.cuh: a
 // comb for P-256, 5-bit windows for P-384) and their signatures take the fixed-base kernel; the rest take the generic kernel.  The scalar preparation
 // (latency-bound: one inversion chain) runs beside the table construction (latency-bound: one doubling chain).
+// A large host-buffer batch runs the part after the table fork chunk by chunk, as its chunks arrive.
 // Registered keys (sbv_set_keys) skip the grouping: their tables were built at registration.
 #include "engine.h"
 
 namespace {
+
+uint32_t hash_slots(size_t n) {  // open-addressing table of the key grouping: a power of two >= 2n
+    uint32_t h = 1;
+    while (h < 2 * n) h <<= 1;
+    return h;
+}
+
+// A launch of n items of a curve with N words per coordinate, kcap keys of which get a table with geometry q
+struct ScratchDims {
+    size_t N = 0, n = 0, kcap = 0;
+    KtGeom q{};
+};
+
+// Every per-launch buffer of scratch set x, once: visit(buffer, need, alloc) with the bytes the launch uses (need) and
+// the bytes to allocate when the buffer must grow (alloc: headroom, so that a slowly growing batch size does not
+// reallocate every call).
+template <class V>
+void each_buffer(Dev::Scratch &x, const ScratchDims &s, V &&visit) {
+    const size_t N = s.N, n = s.n, k = s.kcap, ni = n + n / 8 + 1024, kc = k + k / 8 + 16;
+    const bool g = k > 0;
+    const KtGeom &q = s.q;
+    visit(x.uw, 2 * N * n * 4, 2 * N * ni * 4);
+    visit(x.flags, n, ni);
+    visit(x.tscr, 12 * N * n * 4, 12 * N * ni * 4);
+    visit(x.gacc, g ? 3 * N * n * 4 : 0, 3 * N * ni * 4);
+    visit(x.htab, g ? (size_t)hash_slots(n) * 4 : 0, (size_t)hash_slots(ni) * 4);
+    visit(x.rep, g ? n * 4 : 0, ni * 4);
+    visit(x.klist, g ? n * 4 : 0, ni * 4);
+    visit(x.glist, g ? n * 4 : 0, ni * 4);
+    visit(x.zeroed, g ? (n + 4 + 4 * SBV_MAX_CHUNKS) * 4 : 0, (ni + 4 + 4 * SBV_MAX_CHUNKS) * 4);
+    visit(x.keyid, g ? n * 4 : 0, ni * 4);
+    visit(x.item_kid, g ? n * 4 : 0, ni * 4);
+    visit(x.keylist, k * 4, kc * 4);
+    visit(x.keyflags, k, kc);
+    visit(x.bases, q.bases_words * k * 4, q.bases_words * kc * 4);
+    visit(x.hs, q.hs_words * k * 4, q.hs_words * kc * 4);
+    visit(x.ztop, q.ztop_words * k * 4, q.ztop_words * kc * 4);
+    visit(x.pref, q.ztop_words * k * 4, q.ztop_words * kc * 4);
+    visit(x.ktab, q.ktab_words * k * 4, q.ktab_words * kc * 4);
+}
 
 // Takes the next scratch set of device d for a launch on stream st: waits (on the stream) for the set's previous user
 // and grows the buffers to n items / kcap keys of curve `ops` (growth drains the previous user on the host first).
@@ -23,10 +64,13 @@ int take_scratch(sbv_engine *e, Dev &d, const CurveOps &ops, const KtOps *kt, si
     for (int tries = 0; tries < SBV_SCRATCH && d.ws[idx].open; tries++) idx = (int)(d.ws_next++ % SBV_SCRATCH);
     if (d.ws[idx].open) return sbv_fail(e, SBV_ERR_ARG, "no free scratch set (more launches held open than lanes?)");
     Dev::Scratch &w = d.ws[idx];
-    Dev::Scratch::Caps &c = w.caps;
     if (!w.done) {
         // The events and side streams of EVERY set are created now: a set first taken in the middle of a steady stream of
         // launches would otherwise stop to create streams there (measured: 2 - 40 ms at the head of a timed region).
+        // The table-construction stream runs at high priority: its few, latency-bound blocks are dispatched ahead of the
+        // pending blocks of other launches' verification kernels.
+        int lo_p = 0, hi_p = 0;
+        CU(e, cudaDeviceGetStreamPriorityRange(&lo_p, &hi_p));
         for (int j = 0; j < SBV_SCRATCH; j++) {
             Dev::Scratch &x = d.ws[j];
             if (x.done) continue;
@@ -35,50 +79,13 @@ int take_scratch(sbv_engine *e, Dev &d, const CurveOps &ops, const KtOps *kt, si
             CU(e, cudaEventCreateWithFlags(&x.ev_prep, cudaEventDisableTiming));
             CU(e, cudaEventCreateWithFlags(&x.ev_tab, cudaEventDisableTiming));
             CU(e, cudaEventCreateWithFlags(&x.ev_gen, cudaEventDisableTiming));
-            if (e->tab_hi) {
-                int lo_p = 0, hi_p = 0;
-                CU(e, cudaDeviceGetStreamPriorityRange(&lo_p, &hi_p));
-                CU(e, cudaStreamCreateWithPriority(&x.s_tab, cudaStreamNonBlocking, hi_p));
-            } else {
-                CU(e, cudaStreamCreateWithFlags(&x.s_tab, cudaStreamNonBlocking));
-            }
+            CU(e, cudaStreamCreateWithPriority(&x.s_tab, cudaStreamNonBlocking, hi_p));
             CU(e, cudaStreamCreateWithFlags(&x.s_gen, cudaStreamNonBlocking));
         }
     }
-    const size_t N = (size_t)ops.N;
-    uint32_t hsize = 1;
-    while (hsize < 2 * n) hsize <<= 1;
-    struct Need { void **p; size_t *cap; size_t need, alloc; };
-    // `need` = bytes this launch uses; `alloc` = bytes to allocate when the buffer must grow (headroom so that a slowly
-    // growing batch size does not reallocate every call)
-    const size_t ni = n + n / 8 + 1024, kc = kcap + kcap / 8 + 16;
-    uint32_t hs2 = 1;
-    while (hs2 < 2 * ni) hs2 <<= 1;
-    const bool g = kcap > 0, t = g && kt;
-    const KtGeom z{};
-    const KtGeom &q = t ? kt->geom : z;
-    Need needs[] = {
-        {(void **)&w.uw, &c.uw, 2 * N * n * 4, 2 * N * ni * 4},
-        {(void **)&w.flags, &c.flags, n, ni},
-        {(void **)&w.tscr, &c.tscr, 12 * N * n * 4, 12 * N * ni * 4},
-        {(void **)&w.gacc, &c.gacc, g ? 3 * N * n * 4 : 0, 3 * N * ni * 4},
-        {(void **)&w.htab, &c.htab, g ? (size_t)hsize * 4 : 0, (size_t)hs2 * 4},
-        {(void **)&w.rep, &c.rep, g ? n * 4 : 0, ni * 4},
-        {(void **)&w.klist, &c.klist, g ? n * 4 : 0, ni * 4},
-        {(void **)&w.glist, &c.glist, g ? n * 4 : 0, ni * 4},
-        {(void **)&w.zeroed, &c.zeroed, g ? (n + 4 + 4 * SBV_MAX_CHUNKS) * 4 : 0, (ni + 4 + 4 * SBV_MAX_CHUNKS) * 4},
-        {(void **)&w.keyid, &c.keyid, g ? n * 4 : 0, ni * 4},
-        {(void **)&w.item_kid, &c.item_kid, g ? n * 4 : 0, ni * 4},
-        {(void **)&w.keylist, &c.keylist, t ? kcap * 4 : 0, kc * 4},
-        {(void **)&w.keyflags, &c.keyflags, t ? kcap : 0, kc},
-        {(void **)&w.bases, &c.bases, q.bases_words * kcap * 4, q.bases_words * kc * 4},
-        {(void **)&w.hs, &c.hs, q.hs_words * kcap * 4, q.hs_words * kc * 4},
-        {(void **)&w.ztop, &c.ztop, q.ztop_words * kcap * 4, q.ztop_words * kc * 4},
-        {(void **)&w.pref, &c.pref, q.ztop_words * kcap * 4, q.ztop_words * kc * 4},
-        {(void **)&w.ktab, &c.ktab, q.ktab_words * kcap * 4, q.ktab_words * kc * 4},
-    };
+    const ScratchDims dims{(size_t)ops.N, n, kcap, kt ? kt->geom : KtGeom{}};
     bool grows = false;
-    for (const Need &nd : needs) grows = grows || nd.need > *nd.cap;
+    each_buffer(w, dims, [&](DevBuf &b, size_t need, size_t) { grows = grows || need > b.bytes; });
     if (grows) {
         // Grow EVERY scratch set of the device now, not just this one: otherwise the first launch on each of the other sets
         // would stop to allocate in the middle of a steady stream of launches (cudaMalloc of hundreds of MB synchronises).
@@ -86,27 +93,18 @@ int take_scratch(sbv_engine *e, Dev &d, const CurveOps &ops, const KtOps *kt, si
             Dev::Scratch &x = d.ws[j];
             if (x.open && &x != &w) continue;  // held by a launch between its halves: it grows when it is next taken
             if (x.used && x.done) CU(e, cudaEventSynchronize(x.done));  // nothing may still be using the buffers we are about to free
-            Dev::Scratch::Caps &cx = x.caps;
-            struct Slot { void **p; size_t *cap; };
-            const Slot slots[] = {
-                {(void **)&x.uw, &cx.uw}, {(void **)&x.flags, &cx.flags}, {(void **)&x.tscr, &cx.tscr}, {(void **)&x.gacc, &cx.gacc},
-                {(void **)&x.htab, &cx.htab}, {(void **)&x.rep, &cx.rep}, {(void **)&x.klist, &cx.klist}, {(void **)&x.glist, &cx.glist},
-                {(void **)&x.zeroed, &cx.zeroed}, {(void **)&x.keyid, &cx.keyid}, {(void **)&x.item_kid, &cx.item_kid}, {(void **)&x.keylist, &cx.keylist},
-                {(void **)&x.keyflags, &cx.keyflags}, {(void **)&x.bases, &cx.bases}, {(void **)&x.hs, &cx.hs}, {(void **)&x.ztop, &cx.ztop},
-                {(void **)&x.pref, &cx.pref}, {(void **)&x.ktab, &cx.ktab},
-            };
-            static_assert(sizeof(slots) / sizeof(slots[0]) == sizeof(needs) / sizeof(needs[0]), "one slot per buffer");
-            for (size_t q = 0; q < sizeof(slots) / sizeof(slots[0]); q++) {
-                if (needs[q].need <= *slots[q].cap) continue;
-                if (*slots[q].p) cudaFree(*slots[q].p);
-                *slots[q].p = nullptr;
-                *slots[q].cap = 0;
-                CU(e, cudaMalloc(slots[q].p, needs[q].alloc));
-                *slots[q].cap = needs[q].alloc;
-            }
+            cudaError_t err = cudaSuccess;
+            each_buffer(x, dims, [&](DevBuf &b, size_t need, size_t alloc) {
+                if (err != cudaSuccess || need <= b.bytes) return;
+                if (b.p) cudaFree(b.p);
+                b = DevBuf{};
+                err = cudaMalloc(&b.p, alloc);
+                if (err == cudaSuccess) b.bytes = alloc;
+            });
+            CU(e, err);
         }
     }
-    w.hsize = hsize;
+    w.hsize = hash_slots(n);
     if (w.used) CU(e, cudaStreamWaitEvent(st, w.done, 0));
     w.used = true;
     *out = &w;
@@ -130,8 +128,7 @@ cudaEvent_t *prof_take(sbv_engine *e, Dev &d) {
 
 void sbv_scratch_free(Dev &d) {
     for (auto &w : d.ws) {
-        void *ptrs[] = {w.uw, w.flags, w.tscr, w.gacc, w.htab, w.rep, w.keylist, w.klist, w.glist, w.zeroed, w.keyid, w.item_kid, w.bases, w.hs, w.ztop, w.pref, w.ktab, w.keyflags};
-        for (void *p : ptrs) if (p) cudaFree(p);
+        each_buffer(w, ScratchDims{}, [](DevBuf &b, size_t, size_t) { if (b.p) cudaFree(b.p); });
         cudaEvent_t evs[] = {w.done, w.ev_group, w.ev_prep, w.ev_tab, w.ev_gen};
         for (cudaEvent_t ev : evs) if (ev) cudaEventDestroy(ev);
         if (w.s_tab) cudaStreamDestroy(w.s_tab);
@@ -154,7 +151,8 @@ int sbv_init_gtables(sbv_engine *e, Dev &d) {
 // The keys-per-item pipeline in two halves, so that a host-buffer call can upload the keys first and let the grouping
 // and the table construction (the latency-bound part) run while the rest of the batch is still on its way:
 //   begin : scratch set, key grouping on st, table construction on the set's side stream   (needs qx, qy)
-//   finish: k_prep, generic kernel on the second side stream, fixed-base kernel, join       (needs r, s, digest)
+//   chunk : k_prep, routing, generic kernel on the second side stream, k_gpart, fixed-base kernel, join
+//           (needs r, s, digest), once per chunk of the batch
 int sbv_launch_verify_begin(sbv_engine *e, Dev &d, uint8_t curve, size_t n, const uint8_t *d_qx, const uint8_t *d_qy, cudaStream_t st,
                             VerifyLaunch *vl, int chunks) {
     *vl = VerifyLaunch{};
@@ -173,39 +171,40 @@ int sbv_launch_verify_begin(sbv_engine *e, Dev &d, uint8_t curve, size_t n, cons
     }
     Dev::Scratch *w = nullptr;
     if (int rc = take_scratch(e, d, ops, grouping ? kt : nullptr, n, kcap, st, &w)) return rc;
-    w->open = true;  // until sbv_launch_verify_finish records the set's `done` event
+    w->open = true;  // until the last chunk records the set's `done` event
     vl->w = w; vl->curve = curve; vl->n = n; vl->grouping = grouping; vl->d_qx = d_qx; vl->d_qy = d_qy; vl->chunks = chunks;
     vl->ev = prof_take(e, d);
     if (vl->ev) CU(e, cudaEventRecord(vl->ev[0], st));
     if (!grouping) return 0;
     uint32_t *counters = w->zeroed, *kcnt = w->zeroed + 4;
     CU(e, cudaMemsetAsync(w->htab, 0xff, (size_t)w->hsize * 4, st));
-    CU(e, cudaMemsetAsync(w->zeroed, 0, (n + 4 + (chunks > 1 ? 4 * chunks : 0)) * 4, st));
-    CU(e, ops.group(nn, d_qx, d_qy, e->hash_seed, w->hsize - 1, w->htab, w->rep, kcnt, T, (uint32_t)kcap, w->keyid, w->keylist, w->item_kid, w->klist,
-                    w->glist, counters, chunks == 1, st));
+    CU(e, cudaMemsetAsync(w->zeroed, 0, (n + 4 + 4 * (size_t)chunks) * 4, st));
+    CU(e, ops.group(nn, d_qx, d_qy, e->hash_seed, w->hsize - 1, w->htab, w->rep, kcnt, T, (uint32_t)kcap, w->keyid, w->keylist, counters, st));
     CU(e, cudaEventRecord(w->ev_group, st));
     CU(e, cudaStreamWaitEvent(w->s_tab, w->ev_group, 0));
     CU(e, kt->build(counters + 0, (uint32_t)kcap, w->keylist, d_qx, d_qy, w->bases, w->hs, w->ztop, w->pref, w->ktab, w->keyflags, w->s_tab));
     CU(e, cudaEventRecord(w->ev_tab, w->s_tab));
-    e->launches += (chunks == 1 ? 3 : 2) + (curve == 0 ? 5 : 4);  // grouping + table construction
+    e->launches += 2 + (curve == 0 ? 5 : 4);  // grouping + table construction
     return 0;
 }
 
-// One chunk of a chunked launch: the items [lo, lo + cn) are a batch of their own as far as the per-item arrays go (every one
+// One chunk of a launch: the items [lo, lo + cn) are a batch of their own as far as the per-item arrays go (every one
 // of them is word-major with the batch size as its stride, so the chunk's slice is the contiguous block at `words per item *
 // lo`); what the chunks share is the grouping (hash table, rep, key ids) and the key tables.
 int sbv_launch_verify_chunk(sbv_engine *e, Dev &d, const VerifyLaunch &vl, int c, size_t lo, size_t cn, bool last, const uint8_t *d_r, const uint8_t *d_s,
                             const uint8_t *d_dig, uint32_t dlen, uint8_t *d_ok, cudaStream_t st) {
     if (vl.n == 0) return 0;
     Dev::Scratch *w = vl.w;
-    if (vl.chunks <= 1 || c < 0 || c >= vl.chunks || lo + cn > vl.n) return sbv_fail(e, SBV_ERR_ARG, "bad chunk");
+    if (c < 0 || c >= vl.chunks || lo + cn > vl.n) return sbv_fail(e, SBV_ERR_ARG, "bad chunk");
     const CurveOps &ops = sbv_ops(vl.curve);
-    const KtOps *kt = ops.grouped;
+    const GroupedKtOps *kt = ops.grouped;
     const size_t N = (size_t)ops.N, L = (size_t)ops.bytes;
     const uint32_t nn = (uint32_t)cn;
     const uint32_t *gtab = d.gtab[vl.curve];
-    cudaEvent_t *ev = last ? vl.ev : nullptr;  // the profile of a chunked launch is that of its last chunk (nothing of the first half overlaps it)
-    if (ev) CU(e, cudaEventRecord(ev[0], st));
+    // The profile of a launch is that of its last chunk.  A chunked launch starts it again there (nothing of the first
+    // half overlaps the last chunk); a launch of one chunk keeps the start of its first half, so the grouping counts as prep.
+    cudaEvent_t *ev = last ? vl.ev : nullptr;
+    if (ev && vl.chunks > 1) CU(e, cudaEventRecord(ev[0], st));
     uint32_t *uw = w->uw + 2 * N * lo, *tscr = w->tscr + 12 * N * lo;
     uint8_t *flags = w->flags + lo;
     const uint8_t *r = d_r + lo * L;
@@ -213,9 +212,8 @@ int sbv_launch_verify_chunk(sbv_engine *e, Dev &d, const VerifyLaunch &vl, int c
         CU(e, ops.prep(nn, r, d_s + lo * L, d_dig + lo * dlen, dlen, uw, flags, st));
         e->launches += 1;
     }
-    if (ev) CU(e, cudaEventRecord(ev[1], st));
     if (!vl.grouping) {
-        if (ev) { CU(e, cudaEventRecord(ev[4], st)); CU(e, cudaEventRecord(ev[2], st)); }
+        if (ev) { CU(e, cudaEventRecord(ev[1], st)); CU(e, cudaEventRecord(ev[4], st)); CU(e, cudaEventRecord(ev[2], st)); }
         if (cn) {
             CU(e, ops.coz(nn, vl.d_qx + lo * L, vl.d_qy + lo * L, r, uw, flags, gtab, tscr, d_ok + lo, nullptr, nullptr, st));
             e->launches += 1;
@@ -223,28 +221,24 @@ int sbv_launch_verify_chunk(sbv_engine *e, Dev &d, const VerifyLaunch &vl, int c
         if (ev) CU(e, cudaEventRecord(ev[3], st));
     } else if (cn) {
         uint32_t *cc = w->zeroed + 4 + vl.n + 4 * (size_t)c;   // this chunk's counters (zeroed by the first half)
-        uint32_t *klist = w->klist + lo, *glist = w->glist + lo;
+        uint32_t *klist = w->klist + lo, *glist = w->glist + lo, *gacc = w->gacc + 3 * N * lo;
         CU(e, ops.route(nn, w->rep + lo, w->keyid, w->item_kid + lo, klist, glist, cc, st));
+        if (ev) CU(e, cudaEventRecord(ev[1], st));
         CU(e, cudaEventRecord(w->ev_prep, st));
         CU(e, cudaStreamWaitEvent(w->s_gen, w->ev_prep, 0));
         CU(e, ops.coz(nn, vl.d_qx + lo * L, vl.d_qy + lo * L, r, uw, flags, gtab, tscr, d_ok + lo, glist, cc + 2, w->s_gen));
         CU(e, cudaEventRecord(w->ev_gen, w->s_gen));
-        const uint32_t *gacc = nullptr;
-        if (e->gsplit) {
-            uint32_t *ga = w->gacc + 3 * N * lo;
-            CU(e, ops.gpart(nn, uw, gtab, ga, st));
-            gacc = ga;
-            e->launches += 1;
-        }
+        // the u1*G half needs no table: it runs while the tables are still being built
+        CU(e, ops.gpart(nn, uw, gtab, gacc, st));
         if (ev) CU(e, cudaEventRecord(ev[4], st));
         if (c == 0) CU(e, cudaStreamWaitEvent(st, w->ev_tab, 0));
         if (ev) CU(e, cudaEventRecord(ev[2], st));
-        CU(e, kt->verify(0, 0, nn, nullptr, w->item_kid + lo, 0, w->keyflags, r, uw, flags, gtab, w->ktab, d_ok + lo, klist, cc + 1, gacc, st));
+        CU(e, kt->verify(nn, w->item_kid + lo, w->keyflags, r, uw, flags, gtab, w->ktab, d_ok + lo, klist, cc + 1, gacc, st));
         if (ev) CU(e, cudaEventRecord(ev[3], st));
         CU(e, cudaStreamWaitEvent(st, w->ev_gen, 0));
-        e->launches += 3;
+        e->launches += 4;
     } else if (ev) {
-        CU(e, cudaEventRecord(ev[4], st)); CU(e, cudaEventRecord(ev[2], st)); CU(e, cudaEventRecord(ev[3], st));
+        CU(e, cudaEventRecord(ev[1], st)); CU(e, cudaEventRecord(ev[4], st)); CU(e, cudaEventRecord(ev[2], st)); CU(e, cudaEventRecord(ev[3], st));
     }
     if (last) {
         CU(e, cudaEventRecord(w->done, st));
@@ -263,56 +257,11 @@ void sbv_launch_verify_abort(const VerifyLaunch &vl, cudaStream_t st) {
     w->open = false;
 }
 
-int sbv_launch_verify_finish(sbv_engine *e, Dev &d, const VerifyLaunch &vl, const uint8_t *d_r, const uint8_t *d_s, const uint8_t *d_dig,
-                             uint32_t dlen, uint8_t *d_ok, cudaStream_t st) {
-    if (vl.n == 0) return 0;
-    if (vl.chunks != 1) return sbv_fail(e, SBV_ERR_ARG, "chunked launch finished in one piece");
-    const CurveOps &ops = sbv_ops(vl.curve);
-    const KtOps *kt = ops.grouped;
-    Dev::Scratch *w = vl.w;
-    cudaEvent_t *ev = vl.ev;
-    const uint32_t nn = (uint32_t)vl.n;
-    const uint32_t *gtab = d.gtab[vl.curve];
-    CU(e, ops.prep(nn, d_r, d_s, d_dig, dlen, w->uw, w->flags, st));
-    if (!vl.grouping) {
-        if (ev) { CU(e, cudaEventRecord(ev[1], st)); CU(e, cudaEventRecord(ev[4], st)); CU(e, cudaEventRecord(ev[2], st)); }
-        CU(e, ops.coz(nn, vl.d_qx, vl.d_qy, d_r, w->uw, w->flags, gtab, w->tscr, d_ok, nullptr, nullptr, st));
-        if (ev) CU(e, cudaEventRecord(ev[3], st));
-        CU(e, cudaEventRecord(w->done, st));
-        w->open = false;
-        e->launches += 2;
-        return 0;
-    }
-    uint32_t *counters = w->zeroed;
-    CU(e, cudaEventRecord(w->ev_prep, st));
-    if (ev) CU(e, cudaEventRecord(ev[1], st));
-    CU(e, cudaStreamWaitEvent(w->s_gen, w->ev_prep, 0));
-    CU(e, ops.coz(nn, vl.d_qx, vl.d_qy, d_r, w->uw, w->flags, gtab, w->tscr, d_ok, w->glist, counters + 2, w->s_gen));
-    CU(e, cudaEventRecord(w->ev_gen, w->s_gen));
-    // the u1*G half needs no table: it runs while the tables are still being built
-    const uint32_t *gacc = nullptr;
-    if (e->gsplit) {
-        CU(e, ops.gpart(nn, w->uw, gtab, w->gacc, st));
-        gacc = w->gacc;
-        e->launches += 1;
-    }
-    if (ev) CU(e, cudaEventRecord(ev[4], st));  // == ev[1] without the split
-    CU(e, cudaStreamWaitEvent(st, w->ev_tab, 0));
-    if (ev) CU(e, cudaEventRecord(ev[2], st));
-    CU(e, kt->verify(0, 0, nn, nullptr, w->item_kid, 0, w->keyflags, d_r, w->uw, w->flags, gtab, w->ktab, d_ok, w->klist, counters + 1, gacc, st));
-    if (ev) CU(e, cudaEventRecord(ev[3], st));
-    CU(e, cudaStreamWaitEvent(st, w->ev_gen, 0));
-    CU(e, cudaEventRecord(w->done, st));
-    w->open = false;
-    e->launches += 3;
-    return 0;
-}
-
 int sbv_launch_verify(sbv_engine *e, Dev &d, uint8_t curve, size_t n, const uint8_t *d_r, const uint8_t *d_s, const uint8_t *d_qx,
                       const uint8_t *d_qy, const uint8_t *d_dig, uint32_t dlen, uint8_t *d_ok, cudaStream_t st) {
     VerifyLaunch vl;
     if (int rc = sbv_launch_verify_begin(e, d, curve, n, d_qx, d_qy, st, &vl)) return rc;
-    return sbv_launch_verify_finish(e, d, vl, d_r, d_s, d_dig, dlen, d_ok, st);
+    return sbv_launch_verify_chunk(e, d, vl, 0, 0, n, true, d_r, d_s, d_dig, dlen, d_ok, st);
 }
 
 // ---- registered keys ----------------------------------------------------------------------------------------
@@ -387,7 +336,7 @@ int sbv_launch_keyed(sbv_engine *e, Dev &d, uint8_t curve, size_t n, const uint3
         return 0;
     }
     const CurveOps &ops = sbv_ops(curve);
-    const KtOps *kt = ops.kt8;
+    const RegisteredKtOps *kt = ops.kt8;
     const uint32_t nn = (uint32_t)n;
     Dev::Scratch *w = nullptr;
     if (int rc = take_scratch(e, d, ops, nullptr, n, 0, st, &w)) return rc;
@@ -396,8 +345,8 @@ int sbv_launch_keyed(sbv_engine *e, Dev &d, uint8_t curve, size_t n, const uint3
     CU(e, ops.prep(nn, d_r, d_s, d_dig, dlen, w->uw, w->flags, st));
     if (ev) { CU(e, cudaEventRecord(ev[1], st)); CU(e, cudaEventRecord(ev[4], st)); CU(e, cudaEventRecord(ev[2], st)); }
     const int warp = nn <= (uint32_t)e->keyed_warp_limit ? 1 : 0;  // small batch: one signature per warp (latency path)
-    CU(e, kt->verify(1, warp, nn, d_slot, d.slot2local[curve], d.n_slots, d.keyflags[curve], d_r, w->uw, w->flags, d.gtab[curve], d.ktab[curve], d_ok,
-                     nullptr, nullptr, nullptr, st));
+    CU(e, kt->verify(nn, d_slot, d.slot2local[curve], d.n_slots, d.keyflags[curve], d_r, w->uw, w->flags, d.gtab[curve], d.ktab[curve], d_ok, warp,
+                     st));
     if (ev) CU(e, cudaEventRecord(ev[3], st));
     CU(e, cudaEventRecord(w->done, st));
     e->launches += 2;

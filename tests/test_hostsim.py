@@ -169,7 +169,7 @@ def test_verify_chunked_second_half(hs, curve, n, K, thr, chunk):
     """The second half of the pipeline run chunk by chunk (what a chunked host-buffer call enqueues, csrc/pipeline.cu:
     sbv_launch_verify_chunk): shared grouping and key tables, per-chunk routing with chunk-local indices, every per-item
     array addressed as the contiguous slice of the chunk — same verdicts and the same split between the two paths as
-    the one-piece launch, for chunk sizes that do not divide the batch, with and without the split u1*G kernel."""
+    the launch of one chunk, for chunk sizes that do not divide the batch, with odd and even thresholds."""
     cv = oracle.P256 if curve == 0 else oracle.P384
     b = corpus.make_batch(cv, n=n, K=K, seed=25 + chunk, corrupt_rate=3)
     want = oracle.verify_batch(cv, b["r"], b["s"], b["qx"], b["qy"], b["digest"])
@@ -206,9 +206,10 @@ def _crafted(curve, cases):
 
 @pytest.mark.parametrize("curve,thr", [(0, 1), (0, 2), (1, 2)])
 def test_exceptional_points_on_the_fixed_base_path(hs, curve, thr):
-    """Every key gets a table (threshold 1 / 2: with the u1*G half inside the fixed-base kernel and in k_gpart) and the
-    scalars are chosen so that the running sum meets the next table entry (doubling inside a mixed addition), its
-    negative (infinity in the middle), or ends at infinity (must reject)."""
+    """Every key gets a table (threshold 1 / 2) and the scalars are chosen so that the running sum meets the next table
+    entry (doubling inside a mixed addition), its negative (infinity in the middle), or ends at infinity (must reject).
+    u1*G comes from k_gpart: where it meets the accumulator, that is the closing general addition of k_verify_comb (P-256)
+    or the first window addition of k_verify_kt (P-384)."""
     c = ref.CURVES[curve]
     n = c.n
     ks = [1, 2, 3, n - 1, 5, 2**8 + 1] if curve == 0 else [1, 3, n - 2]

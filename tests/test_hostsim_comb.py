@@ -64,8 +64,8 @@ def test_comb_entries_match_python_integers(hs, curve):
 
 
 def _comb_cases(curve):
-    """(u1, u2, k) for Q = k*G, chosen for the comb's order: u2*Q column by column from the top, then u1*G (G's 16-bit comb
-    digits after the last doubling, or k_gpart's point in one closing addition)."""
+    """(u1, u2, k) for Q = k*G, chosen for the comb's order: u2*Q column by column from the top, then u1*G (k_gpart's point
+    in one closing addition)."""
     c = ref.CURVES[curve]
     n, L = c.n, c.size
     sp = 8 * L // 16
@@ -74,9 +74,9 @@ def _comb_cases(curve):
     for k in (1, 3, 2**70 + 9):
         kinv = pow(k, -1, n)
         for d in (5, 0xFFFF, 2**15 + 3):
-            cases.append((d, d * kinv % n, k))                               # u2*Q = the first G entry right after the doublings
-            cases.append((d, (n - d) * kinv % n, k))                         # ... its negative: infinity, then nothing: reject
-            cases.append((d + (7 << 16), (n - d) * kinv % n, k))             # infinity in the middle, then more G entries
+            cases.append((d, d * kinv % n, k))                               # u2*Q = u1*G = the first G entry: the closing addition doubles
+            cases.append((d, (n - d) * kinv % n, k))                         # ... its negative: infinity: reject
+            cases.append((d + (7 << 16), (n - d) * kinv % n, k))             # u1*G = -u2*Q + a second G entry
         for v in (7, 2**200 + 11, n - 5):
             cases.append((v * k % n, v, k))                                  # u1*G = u2*Q: the closing addition doubles
             cases.append(((n - v * k % n) % n, v, k))                        # u1*G = -u2*Q: R = infinity, reject
@@ -90,9 +90,9 @@ def _comb_cases(curve):
 
 @pytest.mark.parametrize("curve,thr", [(0, 1), (0, 2)])
 def test_comb_order_exceptional_points(hs, curve, thr):
-    """Every key gets a comb table (threshold 1: u1*G's comb additions follow the last doubling inside k_verify_comb;
-    threshold 2: k_gpart's point closes with one general addition): the oracle's verdicts when the accumulator meets
-    +-the first G entry right after the doublings, when u2's masks are all ones or all zero, and when u1*G = +-u2*Q."""
+    """Every key gets a comb table (threshold 1 / 2) and k_gpart's point closes with one general addition: the oracle's
+    verdicts when u1*G = +-u2*Q (the closing addition doubles or reaches infinity) or u1*G + u2*Q is one G comb entry,
+    and when u2's masks are all ones or all zero."""
     b = _crafted(curve, _comb_cases(curve))
     want = oracle.verify_batch(curve, b["r"], b["s"], b["qx"], b["qy"], b["digest"])
     assert 0 < int(want.sum()) < want.size

@@ -102,7 +102,7 @@ static void build_t(const uint32_t *cnt, uint32_t cap, const uint32_t *keylist, 
     std::vector<uint32_t> bases(KS::bases_words(cap)), hs(KS::hs_words(cap)), ztop(KS::ztop_words(cap)), pref(KS::ztop_words(cap));
     const unsigned kb = (cap + 63) / 64, cb = (unsigned)(((size_t)cap * KT::NCHAIN + 63) / 64);
     if (four) run_grid_lockstep((unsigned)(((size_t)cap * 4 + 127) / 128), 128, [&] { k_kt_bases4<C, KT>(cnt, cap, keylist, qx, qy, bases.data(), kflags); });
-    else run_grid(kb, 64, [&] { k_kt_bases<C, KT, true>(cnt, cap, keylist, qx, qy, bases.data(), kflags); });
+    else run_grid(kb, 64, [&] { k_kt_bases<C, KT>(cnt, cap, keylist, qx, qy, bases.data(), kflags); });
     if constexpr (std::is_same<KT, CombTab<C>>::value) {
         run_grid(kb, 64, [&] { k_comb_affine<C>(cnt, cap, kflags, bases.data(), pref.data()); });
         run_grid(cb, 64, [&] { k_comb_fill<C>(cnt, cap, bases.data(), kflags, hs.data(), ztop.data(), ktab); });
@@ -213,7 +213,11 @@ static void verify_coz_t(uint32_t n, const uint8_t *r, const uint8_t *s, const u
 }
 
 // grouped path: k_prep, key grouping, table construction and the fixed-base kernel for repeated keys (P-256: comb tables and
-// k_verify_comb; P-384: 5-bit window tables and k_verify_kt, as in the product), k_verify_coz for the rest
+// k_verify_comb; P-384: 5-bit window tables and k_verify_kt, as in the product), k_verify_coz for the rest.  The second half
+// runs chunk by chunk (chunk = items per chunk; 0: the whole batch as one chunk), as sbv_launch_verify_chunk
+// (csrc/pipeline.cu) enqueues it: the items [lo, lo + cn) are a batch of their own for every per-item array (word-major,
+// stride = the chunk's size, base = words per item * lo); the grouping (rep, keyid) and the key tables are shared; routing
+// is per chunk, chunk-local indices, the chunk's own counters.
 template <class C>
 static void verify_grouped_t(uint32_t n, const uint8_t *r, const uint8_t *s, const uint8_t *qx, const uint8_t *qy, const uint8_t *dig,
                              uint32_t dlen, const uint4 *gtab, uint32_t threshold, uint32_t max_keys, uint8_t *ok, uint32_t *stats,
@@ -222,14 +226,12 @@ static void verify_grouped_t(uint32_t n, const uint8_t *r, const uint8_t *s, con
     std::vector<uint32_t> uw((size_t)2 * N * n);
     std::vector<uint8_t> flags(n);
     std::vector<uint32_t> tscr((size_t)12 * N * n);
-    if (!chunk) run_grid(((n + S - 1) / S + 127) / 128, 128, [&] { k_prep<C, S>(n, r, s, dig, dlen, uw.data(), flags.data()); });
     uint32_t hsize = 1;
     while (hsize < 2 * n) hsize <<= 1;
     std::vector<uint32_t> htab(hsize, KG_EMPTY), rep(n), kcnt(n, 0), keylist(max_keys ? max_keys : 1), klist(n), glist(n), counters(4, 0);
     std::vector<int32_t> keyid(n), item_kid(n);
     run_grid((n + 255) / 256, 256, [&] { k_kg_insert<C>(n, qx, qy, 0x1234567u, hsize - 1, htab.data(), rep.data(), kcnt.data()); });
     run_grid((n + 255) / 256, 256, [&] { k_kg_assign(n, rep.data(), kcnt.data(), threshold, max_keys, keyid.data(), keylist.data(), counters.data()); });
-    if (!chunk) run_grid((n + 255) / 256, 256, [&] { k_kg_route(n, rep.data(), keyid.data(), item_kid.data(), klist.data(), glist.data(), counters.data()); });
     const size_t cap = max_keys ? max_keys : 1;
     constexpr bool comb = std::is_same<C, P256>::value;
     using KT = typename std::conditional<comb, CombTab<C>, KeyTab<32 * N, 5>>::type;
@@ -237,44 +239,29 @@ static void verify_grouped_t(uint32_t n, const uint8_t *r, const uint8_t *s, con
     std::vector<uint8_t> kflags(cap, 0);
     build_t<C, KT>(counters.data(), (uint32_t)cap, keylist.data(), qx, qy, 0, ktab.data(), kflags.data());
     const uint4 *k4 = reinterpret_cast<const uint4 *>(ktab.data());
-    // the fixed-base kernel over items list[0 .. *count) of a batch of nb items
-    auto fixed_base = [&](uint32_t nb, const int32_t *kid, const uint8_t *rb, const uint32_t *uwb, const uint8_t *fl, uint8_t *okb, const uint32_t *list,
-                          const uint32_t *count, const uint32_t *ga) {
-        run_grid((nb + 63) / 64, 64, [&] {
-            if constexpr (comb) k_verify_comb<C, 64, 1, false>(nb, kid, kflags.data(), rb, uwb, fl, gtab, k4, okb, list, count, ga);
-            else k_verify_kt<C, 5, 64, 1, false, false>(nb, nullptr, kid, 0, kflags.data(), rb, uwb, fl, gtab, k4, okb, list, count, ga);
-        });
-    };
-    const bool gsplit = (threshold & 1) == 0;  // exercise both forms: even thresholds take the split u1*G path
     std::vector<uint32_t> gacc((size_t)3 * N * n);
-    if (chunk) {
-        // The second half chunk by chunk, as sbv_launch_verify_chunk (csrc/pipeline.cu) enqueues it: the items [lo, lo + cn) are a
-        // batch of their own for every per-item array (word-major, stride = the chunk's size, base = words per item * lo); the
-        // grouping (rep, keyid) and the key tables are shared; routing is per chunk, chunk-local indices, the chunk's own counters.
-        const size_t L = C::BYTES;
-        uint32_t kt_total = 0, gen_total = 0;
-        for (uint32_t lo = 0; lo < n; lo += chunk) {
-            const uint32_t cn = n - lo < chunk ? n - lo : chunk;
-            std::vector<uint32_t> cc(4, 0);
-            uint32_t *uwc = uw.data() + (size_t)2 * N * lo, *tsc = tscr.data() + (size_t)12 * N * lo, *gac = gacc.data() + (size_t)3 * N * lo;
-            uint8_t *flc = flags.data() + lo;
-            const uint8_t *rc = r + lo * L;
-            run_grid(((cn + S - 1) / S + 127) / 128, 128, [&] { k_prep<C, S>(cn, rc, s + lo * L, dig + (size_t)lo * dlen, dlen, uwc, flc); });
-            run_grid((cn + 255) / 256, 256, [&] { k_kg_route(cn, rep.data() + lo, keyid.data(), item_kid.data() + lo, klist.data() + lo, glist.data() + lo, cc.data()); });
-            run_grid((cn + 63) / 64, 64, [&] { k_verify_coz<C, 64, 1>(cn, qx + lo * L, qy + lo * L, rc, uwc, flc, gtab, tsc, ok + lo, glist.data() + lo, cc.data() + 2); });
-            if (gsplit) run_grid((cn + 63) / 64, 64, [&] { k_gpart<C, 64, 1>(cn, uwc, gtab, gac); });
-            fixed_base(cn, item_kid.data() + lo, rc, uwc, flc, ok + lo, klist.data() + lo, cc.data() + 1, gsplit ? gac : nullptr);
-            kt_total += cc[1]; gen_total += cc[2];
-        }
-        if (stats) { stats[0] = counters[0]; stats[1] = kt_total; stats[2] = gen_total; }
-        return;
+    const size_t L = C::BYTES;
+    const uint32_t per = chunk ? chunk : n;
+    uint32_t kt_total = 0, gen_total = 0;
+    for (uint32_t lo = 0; lo < n; lo += per) {
+        const uint32_t cn = n - lo < per ? n - lo : per;
+        std::vector<uint32_t> cc(4, 0);
+        uint32_t *uwc = uw.data() + (size_t)2 * N * lo, *tsc = tscr.data() + (size_t)12 * N * lo, *gac = gacc.data() + (size_t)3 * N * lo;
+        uint8_t *flc = flags.data() + lo;
+        const uint8_t *rc = r + lo * L;
+        const int32_t *kid = item_kid.data() + lo;
+        const uint32_t *kl = klist.data() + lo;
+        run_grid(((cn + S - 1) / S + 127) / 128, 128, [&] { k_prep<C, S>(cn, rc, s + lo * L, dig + (size_t)lo * dlen, dlen, uwc, flc); });
+        run_grid((cn + 255) / 256, 256, [&] { k_kg_route(cn, rep.data() + lo, keyid.data(), item_kid.data() + lo, klist.data() + lo, glist.data() + lo, cc.data()); });
+        run_grid((cn + 63) / 64, 64, [&] { k_verify_coz<C, 64, 1>(cn, qx + lo * L, qy + lo * L, rc, uwc, flc, gtab, tsc, ok + lo, glist.data() + lo, cc.data() + 2); });
+        run_grid((cn + 63) / 64, 64, [&] { k_gpart<C, 64, 1>(cn, uwc, gtab, gac); });
+        run_grid((cn + 63) / 64, 64, [&] {
+            if constexpr (comb) k_verify_comb<C, 64, 1, false>(cn, kid, kflags.data(), rc, uwc, flc, k4, ok + lo, kl, cc.data() + 1, gac);
+            else k_verify_kt<C, 5, 64, 1, false, false>(cn, nullptr, kid, 0, kflags.data(), rc, uwc, flc, gtab, k4, ok + lo, kl, cc.data() + 1, gac);
+        });
+        kt_total += cc[1]; gen_total += cc[2];
     }
-    if (gsplit) run_grid((n + 63) / 64, 64, [&] { k_gpart<C, 64, 1>(n, uw.data(), gtab, gacc.data()); });
-    fixed_base(n, item_kid.data(), r, uw.data(), flags.data(), ok, klist.data(), counters.data() + 1, gsplit ? gacc.data() : nullptr);
-    run_grid((n + 63) / 64, 64, [&] {
-        k_verify_coz<C, 64, 1>(n, qx, qy, r, uw.data(), flags.data(), gtab, tscr.data(), ok, glist.data(), counters.data() + 2);
-    });
-    if (stats) { stats[0] = counters[0]; stats[1] = counters[1]; stats[2] = counters[2]; }
+    if (stats) { stats[0] = counters[0]; stats[1] = kt_total; stats[2] = gen_total; }
 }
 
 static std::vector<uint32_t> g_gtab[2];
