@@ -1,14 +1,23 @@
 // debug_ops.cuh — arithmetic-layer test operations shared by the GPU test hook (debug.cu, sbv_debug_op) and the
 // CPU host simulation of the same headers (tools/hostsim).  Test infrastructure; not part of include/sbv.h.
 // Operands are little-endian 32-bit limb arrays, 2N limbs per slot (unused limbs zero).
+//
+// op & 0xff: 0 fmul, 1 fadd, 2 fsub, 3 nmul, 4 f_inv, 5 doubling, 6 general add, 7 mixed add, 8 n_inv, 9 fsqr, 10 p_inv.
+// Flags: DEBUG_INL runs the op with the inlined field multiplications of Inl<C> (the fixed-base kernels' arithmetic);
+// DEBUG_NEG / DEBUG_SKIP are the `neg` / `skip` arguments of the additions (ops 6, 7).  For ops 5-7 an accumulator
+// given as (0, 0) is the point at infinity (Z = 0).
 #pragma once
 #include "kernels.cuh"
 
 namespace sbv {
 
+constexpr int DEBUG_INL = 0x100, DEBUG_NEG = 0x200, DEBUG_SKIP = 0x400;
+
 template <class C>
 SBV_DEV void debug_op_item(int op, uint32_t i, const uint32_t *__restrict__ a, const uint32_t *__restrict__ b, uint32_t *__restrict__ out) {
     constexpr int N = C::N;
+    const bool neg = (op & DEBUG_NEG) != 0, skip = (op & DEBUG_SKIP) != 0;
+    op &= 0xff;
     uint32_t x[N], y[N], u[N], v[N], r0[N], r1[N];
     for (int k = 0; k < N; k++) { x[k] = a[i * 2 * N + k]; y[k] = a[i * 2 * N + N + k]; u[k] = b[i * 2 * N + k]; v[k] = b[i * 2 * N + N + k]; r0[k] = 0; r1[k] = 0; }
     uint32_t rr[N], one[N], plain1[N];
@@ -25,7 +34,9 @@ SBV_DEV void debug_op_item(int op, uint32_t i, const uint32_t *__restrict__ a, c
     else if (op >= 5 && op <= 7) {
         // affine plain (x,y) [+ (u,v)] -> Montgomery Jacobian -> op -> affine plain
         Jac<C> P;
+        const bool inf = mp_is_zero<N>(x) && mp_is_zero<N>(y);
         C::fmul(P.X, x, rr); C::fmul(P.Y, y, rr); mp_copy<N>(P.Z, one);
+        if (inf) { mp_copy<N>(P.X, one); mp_copy<N>(P.Y, one); for (int k = 0; k < N; k++) P.Z[k] = 0; }
         uint32_t um[N], vm[N];
         C::fmul(um, u, rr); C::fmul(vm, v, rr);
         if (op == 5) pt_double<C>(P);
@@ -36,8 +47,8 @@ SBV_DEV void debug_op_item(int op, uint32_t i, const uint32_t *__restrict__ a, c
             C::fsqr(z2, z); C::fmul(z3, z2, z);
             C::fmul(um, um, z2); C::fmul(vm, vm, z3);
             pt_double<C>(P);  // make Z1 non-trivial as well: P = 2*(x,y)
-            pt_add<C, false>(P, um, vm, z, false, false);
-        } else pt_add<C, true>(P, um, vm, one, false, false);
+            pt_add<C, false>(P, um, vm, z, neg, skip);
+        } else pt_add<C, true>(P, um, vm, one, neg, skip);
         if (mp_is_zero<N>(P.Z)) { for (int k = 0; k < N; k++) { r0[k] = 0; r1[k] = 0; } }
         else {
             uint32_t zi[N], zi2[N], zi3[N];
@@ -48,6 +59,13 @@ SBV_DEV void debug_op_item(int op, uint32_t i, const uint32_t *__restrict__ a, c
         }
     }
     for (int k = 0; k < N; k++) { out[i * 2 * N + k] = r0[k]; out[i * 2 * N + N + k] = r1[k]; }
+}
+
+// DEBUG_INL selects the arithmetic policy; the other bits go to debug_op_item
+template <class C>
+SBV_DEV void debug_op_dispatch(int op, uint32_t i, const uint32_t *__restrict__ a, const uint32_t *__restrict__ b, uint32_t *__restrict__ out) {
+    if (op & DEBUG_INL) debug_op_item<Inl<C>>(op & ~DEBUG_INL, i, a, b, out);
+    else debug_op_item<C>(op, i, a, b, out);
 }
 
 }  // namespace sbv

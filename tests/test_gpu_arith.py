@@ -5,6 +5,7 @@ import ctypes as C
 import numpy as np
 import pytest
 
+import edges
 from oracle import ecdsa_ref as ref
 
 pytestmark = pytest.mark.gpu
@@ -44,40 +45,29 @@ def _run(eng, curve, op, a, b):
     return _ints(out, N)
 
 
-def _edge_values(m, rng, count):
-    vals = [0, 1, 2, m - 1, m - 2, (m - 1) // 2, (1 << 32) - 1, 1 << 32, (1 << 64) - 1, (1 << 96), (1 << 224) % m, m >> 1,
-            0xFFFFFFFF00000000FFFFFFFF00000000FFFFFFFF00000000FFFFFFFF00000000 % m]
-    vals += [int.from_bytes(rng.bytes(48), "big") % m for _ in range(count)]
-    return vals
-
-
 @pytest.mark.parametrize("curve", [0, 1])
 def test_field_ops(eng, curve):
+    """The CPU simulation's cases (edges.montgomery_cases) on the device, out of line and with the inlined multiplications
+    of Inl<C> (k_verify_comb, the P-256 k_verify_kt): edge values, operands that put P256::redc / P384::redc /
+    mont_reduce_sos on each side of the final subtraction, operands in [m, R); then the inverses."""
     c = ref.CURVES[curve]
     N = c.size // 4
     R = 1 << (32 * N)
     rng = np.random.default_rng(curve + 1)
-    for m, mulop in [(c.p, 0), (c.n, 3)]:
-        xs = _edge_values(m, rng, 300)
-        ys = list(reversed(_edge_values(m, rng, 300)))
+    for label, op, xs, ys, want in edges.montgomery_cases(curve, rng, 300):
         a = [(x, 0) for x in xs]; b = [(y, 0) for y in ys]
-        Rinv = pow(R, -1, m)
-        got = _run(eng, curve, mulop, a, b)
-        assert [g[0] for g in got] == [x * y * Rinv % m for x, y in zip(xs, ys)]
-        if m == c.p:
-            assert [g[0] for g in _run(eng, curve, 9, a, b)] == [x * x * Rinv % m for x in xs]
-            assert [g[0] for g in _run(eng, curve, 1, a, b)] == [(x + y) % m for x, y in zip(xs, ys)]
-            assert [g[0] for g in _run(eng, curve, 2, a, b)] == [(x - y) % m for x, y in zip(xs, ys)]
+        for flag in (0, edges.INL):
+            assert [g[0] for g in _run(eng, curve, op | flag, a, b)] == want, (label, op | flag)
     # inverses (Montgomery in/out): inv(aR) = a^-1 R
-    xs = [v for v in _edge_values(c.p, rng, 20) if v]
+    xs = [v for v in edges.edge_values(c.p, rng, 20) if v]
     got = _run(eng, curve, 4, [(x * R % c.p, 0) for x in xs], [(0, 0)] * len(xs))
     assert [g[0] for g in got] == [pow(x, -1, c.p) * R % c.p for x in xs]
-    xs = [v for v in _edge_values(c.p, rng, 600) if v] + [pow(2, k, c.p) for k in (1, 31, 32, 33, 64, 96, 128, 224, 255, 256, 300)]
+    xs = [v for v in edges.edge_values(c.p, rng, 600) if v] + [pow(2, k, c.p) for k in (1, 31, 32, 33, 64, 96, 128, 224, 255, 256, 300)]
     got = _run(eng, curve, 10, [(x * R % c.p, 0) for x in xs], [(0, 0)] * len(xs))   # binary-GCD field inverse (table construction)
     assert [g[0] for g in got] == [pow(x, -1, c.p) * R % c.p for x in xs]
     # scalar-field inverse (binary extended GCD): many random values plus powers of two and their
     # neighbours, which exercise long runs of trailing zeros (tz = 31 passes, zero low words)
-    xs = [v for v in _edge_values(c.n, rng, 1500) if v]
+    xs = [v for v in edges.edge_values(c.n, rng, 1500) if v]
     xs += [pow(2, k, c.n) for k in (1, 31, 32, 33, 63, 64, 65, 96, 128, 255, 256, 300, 383)]
     xs += [(pow(2, k, c.n) * pow(R, -1, c.n)) % c.n for k in (32, 64, 96, 200)]   # residue itself a power of two
     xs += [(c.n - pow(2, k, c.n)) % c.n for k in (1, 32, 64, 128)]
@@ -88,16 +78,11 @@ def test_field_ops(eng, curve):
 
 @pytest.mark.parametrize("curve", [0, 1])
 def test_group_law(eng, curve):
+    """Doubling, mixed add (P == Q: the doubling branch; P == -Q: infinity -> (0, 0)) and general add 2P + Q with
+    non-trivial Z on both sides, each with the neg / skip flags of the verification loops and from an accumulator at
+    infinity, out of line and inlined."""
     c = ref.CURVES[curve]
-    G = (c.gx, c.gy)
     ks = [1, 2, 3, 4, 5, 7, 8, 255, 256, c.n - 1, c.n - 2, 2**100 + 3, 0xDEADBEEF]
-    pts = [ref.scalar_mult(c, k, G) for k in ks]
-    # doubling
-    assert _run(eng, curve, 5, pts, pts) == [ref._add(c, P, P) for P in pts]
-    # mixed add P + Q incl. P == Q (doubling branch) and P == -Q (infinity -> (0,0))
-    pairs = [(P, Q) for P in pts for Q in pts]
-    want = [ref._add(c, P, Q) or (0, 0) for P, Q in pairs]
-    assert _run(eng, curve, 7, [p for p, _ in pairs], [q for _, q in pairs]) == want
-    # general add 2P + Q with non-trivial Z on both sides, incl. 2P == Q and 2P == -Q
-    want = [ref._add(c, ref._add(c, P, P), Q) or (0, 0) for P, Q in pairs]
-    assert _run(eng, curve, 6, [p for p, _ in pairs], [q for _, q in pairs]) == want
+    for op, a, b, want in edges.group_cases(curve, ks):
+        for flag in (0, edges.INL):
+            assert _run(eng, curve, op | flag, a, b) == want, op | flag

@@ -5,6 +5,7 @@ import hashlib
 import numpy as np
 import pytest
 
+import edges
 import oracle
 from oracle import P256, P384, corpus
 from oracle import ecdsa_ref as ref
@@ -51,34 +52,6 @@ def test_empty_batch(eng):
     assert eng.verify_batch(P256, z, z, z, z, z).size == 0
 
 
-def _crafted(curve, cases):
-    """cases: list of (u1, u2, k) -> signature (r, s, e) on Q = k*G with s = 1 (so u1 = e, u2 = r is
-    impossible to force); instead choose s freely: pick u1,u2, R = u1 G + u2 Q, r = R.x mod n,
-    s = r/u2, e = u1*s.  Exercises exceptional points inside the double-scalar multiplication."""
-    c = ref.CURVES[curve]
-    L = c.size
-    rows = []
-    for u1, u2, k in cases:
-        Q = ref.scalar_mult(c, k % c.n, (c.gx, c.gy))
-        R = ref._add(c, ref.scalar_mult(c, u1 % c.n, (c.gx, c.gy)), ref.scalar_mult(c, u2 % c.n, Q))
-        if R is None or u2 % c.n == 0:
-            r = 1  # R = infinity must reject whatever r is; keep it well-formed
-            s = 1
-            e = u1 % c.n
-            if u2 % c.n:
-                s = r * pow(u2, -1, c.n) % c.n
-                e = u1 * s % c.n
-        else:
-            r = R[0] % c.n
-            if r == 0:
-                continue
-            s = r * pow(u2, -1, c.n) % c.n
-            e = u1 * s % c.n
-        rows.append((r, s, Q[0], Q[1], e))
-    f = lambda j: np.stack([_be(row[j], L) for row in rows])
-    return f(0), f(1), f(2), f(3), f(4)
-
-
 @pytest.mark.parametrize("curve", [P256, P384])
 def test_exceptional_points_inside_the_scalar_multiplication(eng, curve):
     c = ref.CURVES[curve]
@@ -88,9 +61,9 @@ def test_exceptional_points_inside_the_scalar_multiplication(eng, curve):
         for u1, u2 in [(1, 1), (k, 1), (n - k, 1), (k, n - 1), (2, n - 1), (1, 2), (7, 3), (2**255, 2**255), (n - 1, n - 1),
                        (k * 5 % n, 5), (n - (k * 5 % n), 5), (2**64, 2**64), (0x1111, 0x1111), (16, 1), (1, 16), (0, 1), (0, 77)]:
             cases.append((u1, u2, k))
-    r, s, qx, qy, e = _crafted(curve, cases)
-    want = oracle.verify_batch(curve, r, s, qx, qy, e)
-    got = eng.verify_batch(curve, r, s, qx, qy, e)
+    b = edges.crafted(curve, cases)
+    want = oracle.verify_batch(curve, b["r"], b["s"], b["qx"], b["qy"], b["digest"])
+    got = eng.verify_batch(curve, b["r"], b["s"], b["qx"], b["qy"], b["digest"])
     assert want.tolist() == got.tolist()
     assert 0 < want.sum() < want.size  # both accept and reject (R = infinity) cases present
 

@@ -11,6 +11,7 @@ import subprocess
 import numpy as np
 import pytest
 
+import edges
 import oracle
 from oracle import corpus
 from oracle import ecdsa_ref as ref
@@ -47,44 +48,26 @@ def _run(hs, curve, op, a, b):
     return _ints(out, N)
 
 
-def _edge_values(m, rng, count):
-    F = (1 << 32) - 1
-    vals = [0, 1, 2, m - 1, m - 2, (m - 1) // 2, F, 1 << 32, (1 << 64) - 1, 1 << 96, (1 << 224) % m, m >> 1,
-            0xFFFFFFFF00000000FFFFFFFF00000000FFFFFFFF00000000FFFFFFFF00000000 % m, ((1 << 96) - 1), (m - (1 << 96)) % m,
-            (m - (1 << 192)) % m, ((1 << 256) - 1) % m, ((1 << 255) + 12345) % m]
-    vals += [int.from_bytes(rng.bytes(48), "big") % m for _ in range(count)]
-    # values with long runs of ones / zeros in single limbs: carry-chain stress
-    for _ in range(count // 4):
-        v = 0
-        for k in range(12):
-            v |= int(rng.choice([0, F, 1, F - 1, 0x80000000, int(rng.integers(0, F))])) << (32 * k)
-        vals.append(v % m)
-    return vals
-
-
 @pytest.mark.parametrize("curve", [0, 1])
 def test_field_ops(hs, curve):
+    """Montgomery products (out of line and, with edges.INL, inlined as Inl<C> runs them), field additions and the
+    inverses against Python integers: edge values, operands on both sides of each reduction's final subtraction, and
+    operands in [m, R)."""
     c = ref.CURVES[curve]
     N = c.size // 4
     R = 1 << (32 * N)
     rng = np.random.default_rng(curve + 11)
-    for m, mulop in [(c.p, 0), (c.n, 3)]:
-        xs = _edge_values(m, rng, 1500)
-        ys = list(reversed(_edge_values(m, rng, 1500)))
+    for label, op, xs, ys, want in edges.montgomery_cases(curve, rng, 1500):
         a = [(x, 0) for x in xs]; b = [(y, 0) for y in ys]
-        Rinv = pow(R, -1, m)
-        assert [g[0] for g in _run(hs, curve, mulop, a, b)] == [x * y * Rinv % m for x, y in zip(xs, ys)]
-        if m == c.p:
-            assert [g[0] for g in _run(hs, curve, 9, a, b)] == [x * x * Rinv % m for x in xs]
-            assert [g[0] for g in _run(hs, curve, 1, a, b)] == [(x + y) % m for x, y in zip(xs, ys)]
-            assert [g[0] for g in _run(hs, curve, 2, a, b)] == [(x - y) % m for x, y in zip(xs, ys)]
-    xs = [v for v in _edge_values(c.p, rng, 10) if v]
+        for flag in (0, edges.INL):
+            assert [g[0] for g in _run(hs, curve, op | flag, a, b)] == want, (label, op | flag)
+    xs = [v for v in edges.edge_values(c.p, rng, 10) if v]
     got = _run(hs, curve, 4, [(x * R % c.p, 0) for x in xs], [(0, 0)] * len(xs))
     assert [g[0] for g in got] == [pow(x, -1, c.p) * R % c.p for x in xs]
-    xs = [v for v in _edge_values(c.p, rng, 300) if v] + [pow(2, k, c.p) for k in (1, 31, 32, 33, 64, 96, 128, 224, 255, 256, 300)]
+    xs = [v for v in edges.edge_values(c.p, rng, 300) if v] + [pow(2, k, c.p) for k in (1, 31, 32, 33, 64, 96, 128, 224, 255, 256, 300)]
     got = _run(hs, curve, 10, [(x * R % c.p, 0) for x in xs], [(0, 0)] * len(xs))   # binary-GCD field inverse
     assert [g[0] for g in got] == [pow(x, -1, c.p) * R % c.p for x in xs]
-    xs = [v for v in _edge_values(c.n, rng, 200) if v]
+    xs = [v for v in edges.edge_values(c.n, rng, 200) if v]
     xs += [pow(2, k, c.n) for k in (1, 31, 32, 33, 63, 64, 65, 96, 128, 255, 256, 300, 383)]
     got = _run(hs, curve, 8, [(x * R % c.n, 0) for x in xs], [(0, 0)] * len(xs))
     assert [g[0] for g in got] == [pow(x, -1, c.n) * R % c.n for x in xs]
@@ -92,16 +75,12 @@ def test_field_ops(hs, curve):
 
 @pytest.mark.parametrize("curve", [0, 1])
 def test_group_law(hs, curve):
+    """Doubling, mixed and general addition (with neg / skip, from an accumulator at infinity), out of line and inlined."""
     c = ref.CURVES[curve]
-    G = (c.gx, c.gy)
     ks = [1, 2, 3, 4, 5, 7, 8, 255, c.n - 1, c.n - 2, 2**100 + 3]
-    pts = [ref.scalar_mult(c, k, G) for k in ks]
-    assert _run(hs, curve, 5, pts, pts) == [ref._add(c, P, P) for P in pts]
-    pairs = [(P, Q) for P in pts for Q in pts]
-    want = [ref._add(c, P, Q) or (0, 0) for P, Q in pairs]
-    assert _run(hs, curve, 7, [p for p, _ in pairs], [q for _, q in pairs]) == want
-    want = [ref._add(c, ref._add(c, P, P), Q) or (0, 0) for P, Q in pairs]
-    assert _run(hs, curve, 6, [p for p, _ in pairs], [q for _, q in pairs]) == want
+    for op, a, b, want in edges.group_cases(curve, ks):
+        for flag in (0, edges.INL):
+            assert _run(hs, curve, op | flag, a, b) == want, op | flag
 
 
 def _p8(a):
@@ -184,47 +163,63 @@ def test_verify_chunked_second_half(hs, curve, n, K, thr, chunk):
     assert list(stats) == list(st_whole) and int(stats[1]) > 0
 
 
-def _crafted(curve, cases):
-    """(u1, u2, k) -> a signature on Q = k*G whose verification computes exactly u1*G + u2*Q (s = r/u2, e = u1*s):
-    places exceptional points (doubling, P + (-P), infinity in the middle or at the end) inside the scalar multiplication."""
-    c = ref.CURVES[curve]
-    L = c.size
-    rows = []
-    for u1, u2, k in cases:
-        Q = ref.scalar_mult(c, k % c.n, (c.gx, c.gy))
-        R = ref._add(c, ref.scalar_mult(c, u1 % c.n, (c.gx, c.gy)), ref.scalar_mult(c, u2 % c.n, Q))
-        if u2 % c.n == 0:
-            continue
-        r = 1 if R is None else R[0] % c.n
-        if r == 0:
-            continue
-        s = r * pow(u2, -1, c.n) % c.n
-        rows.append((r, s, Q[0], Q[1], u1 * s % c.n))
-    f = lambda j: np.stack([np.frombuffer(int(row[j]).to_bytes(L, "big"), np.uint8) for row in rows])
-    return {"r": f(0), "s": f(1), "qx": f(2), "qy": f(3), "digest": f(4)}
-
-
 @pytest.mark.parametrize("curve,thr", [(0, 1), (0, 2), (1, 2)])
 def test_exceptional_points_on_the_fixed_base_path(hs, curve, thr):
     """Every key gets a table (threshold 1 / 2) and the scalars are chosen so that the running sum meets the next table
     entry (doubling inside a mixed addition), its negative (infinity in the middle), or ends at infinity (must reject).
     u1*G comes from k_gpart: where it meets the accumulator, that is the closing general addition of k_verify_comb (P-256)
     or the first window addition of k_verify_kt (P-384)."""
-    c = ref.CURVES[curve]
-    n = c.n
-    ks = [1, 2, 3, n - 1, 5, 2**8 + 1] if curve == 0 else [1, 3, n - 2]
-    cases = []
-    for k in ks:
-        for u1, u2 in [(1, 1), (k, 1), (n - k, 1), (k, n - 1), (2, n - 1), (1, 2), (7, 3), (2**255, 2**255), (n - 1, n - 1), (k * 5 % n, 5),
-                       (n - (k * 5 % n), 5), (k * 16 % n, 16), (n - (k * 16 % n), 16), (k * 33 % n, 33), (2**64, 2**64), (16, 1), (1, 16),
-                       (0, 1), (0, 77), ((k << 5) % n, 32), (n - ((k << 5) % n), 32)]:
-            cases.append((u1, u2, k))
-    b = _crafted(curve, cases)
+    b = edges.crafted(curve, edges.fixed_base_cases(curve))
     want = oracle.verify_batch(curve, b["r"], b["s"], b["qx"], b["qy"], b["digest"])
     assert 0 < int(want.sum()) < want.size
     got, stats = _verify(hs, curve, b, grouped=(thr, 64))
     assert int(stats[2]) == 0                                   # nothing on the generic path
     assert np.array_equal(got, want), np.nonzero(got != want)[0][:10]
+
+
+def _registered(hs, curve, b, warp):
+    """b's rows through hs_verify_registered: one slot per distinct key"""
+    L = b["qx"].shape[1]
+    kxy = np.concatenate([b["qx"], b["qy"]], axis=1)
+    keys, slot = np.unique(kxy, axis=0, return_inverse=True)
+    slot = np.ascontiguousarray(slot.reshape(-1), dtype=np.uint32)
+    kx, ky = np.ascontiguousarray(keys[:, :L]), np.ascontiguousarray(keys[:, L:])
+    n = slot.size
+    f = [np.ascontiguousarray(b[k]) for k in ("r", "s", "digest")]
+    ok = np.full(n, 7, np.uint8)
+    assert hs.hs_verify_registered(C.c_int(curve), C.c_size_t(n), C.c_size_t(len(keys)), _p8(kx), _p8(ky), slot.ctypes.data_as(C.POINTER(C.c_uint32)),
+                                   _p8(f[0]), _p8(f[1]), _p8(f[2]), C.c_uint32(f[2].size // n), C.c_int(warp), _p8(ok)) == 0
+    return ok
+
+
+def _every_simulated_path(hs, curve, b):
+    want = oracle.verify_batch(curve, b["r"], b["s"], b["qx"], b["qy"], b["digest"])
+    assert np.array_equal(want, b["want"])
+    assert np.array_equal(_verify(hs, curve, b), want), "generic"
+    got, stats = _verify(hs, curve, b, grouped=(1, 64))
+    assert int(stats[2]) == 0 and np.array_equal(got, want), "grouped"
+    for warp in (0, 1):
+        assert np.array_equal(_registered(hs, curve, b, warp), want), ("registered", warp)
+
+
+@pytest.mark.parametrize("curve", [0, 1])
+def test_r_plus_n_accepts_when_R_x_is_at_least_n(hs, curve):
+    """R.x in [n, p): r = R.x - n must be accepted (final_check compares X with (r + n) * Z^2), r = R.x (out of range) and
+    r + 1 rejected — on the generic, grouped and registered thread / warp kernels."""
+    b = edges.big_x_signatures(curve, 3, seed=7 + curve)
+    assert all(x >= ref.CURVES[curve].n for x in b["rx"]) and 0 < b["want"].sum() < b["want"].size
+    _every_simulated_path(hs, curve, b)
+
+
+@pytest.mark.parametrize("curve,dlen", [(0, 32), (0, 48), (0, 20), (1, 64), (1, 48), (1, 28)])
+def test_digests_at_least_n_and_of_other_lengths(hs, curve, dlen):
+    """e from the leftmost min(dlen, BYTES) digest bytes, also when that is >= n or the digest is longer than the field:
+    the same verdicts on every simulated path, and a bit flipped past the first BYTES bytes changes nothing."""
+    b = edges.wide_digest_signatures(curve, dlen, 4, seed=dlen + curve)
+    c = ref.CURVES[curve]
+    assert (dlen < c.size) or any(e >= c.n for e in b["e"])
+    assert 0 < b["want"].sum() < b["want"].size
+    _every_simulated_path(hs, curve, b)
 
 
 def _tables(hs, curve, w8, kxy, four):

@@ -6,10 +6,11 @@ import ctypes as C
 import numpy as np
 import pytest
 
+import edges
 import oracle
 from oracle import corpus
 from oracle import ecdsa_ref as ref
-from test_hostsim import _crafted, _p8, _verify, hs  # noqa: F401  (hs: the simulation library fixture)
+from test_hostsim import _p8, _verify, hs  # noqa: F401  (hs: the simulation library fixture)
 
 COMB = 2  # hs_tables / hs_ktab_words: table kind of the comb
 
@@ -63,37 +64,12 @@ def test_comb_entries_match_python_integers(hs, curve):
                 assert (val(e[0]), val(e[1])) == (P[0] * Rm % c.p, P[1] * Rm % c.p), (key, blk, m)
 
 
-def _comb_cases(curve):
-    """(u1, u2, k) for Q = k*G, chosen for the comb's order: u2*Q column by column from the top, then u1*G (k_gpart's point
-    in one closing addition)."""
-    c = ref.CURVES[curve]
-    n, L = c.n, c.size
-    sp = 8 * L // 16
-    ones_col = lambda j: sum(1 << (sp * r + j) for r in range(16))          # column j all ones: both masks 255
-    cases = []
-    for k in (1, 3, 2**70 + 9):
-        kinv = pow(k, -1, n)
-        for d in (5, 0xFFFF, 2**15 + 3):
-            cases.append((d, d * kinv % n, k))                               # u2*Q = u1*G = the first G entry: the closing addition doubles
-            cases.append((d, (n - d) * kinv % n, k))                         # ... its negative: infinity: reject
-            cases.append((d + (7 << 16), (n - d) * kinv % n, k))             # u1*G = -u2*Q + a second G entry
-        for v in (7, 2**200 + 11, n - 5):
-            cases.append((v * k % n, v, k))                                  # u1*G = u2*Q: the closing addition doubles
-            cases.append(((n - v * k % n) % n, v, k))                        # u1*G = -u2*Q: R = infinity, reject
-        for u2 in ((1 << (sp * 8)) - 1,                                      # block 0 masks all ones, block 1 all zero
-                   ((1 << (8 * L)) - 1) ^ ((1 << (sp * 8)) - 1),             # the other way round (mod n)
-                   n - 1, ones_col(0), ones_col(sp - 1), ones_col(0) | ones_col(sp - 1), (1 << sp) - 1, 1 << (8 * L - 1)):
-            cases.append((12345, u2 % n, k))
-            cases.append((u2 * k % n, u2 % n, k))
-    return cases
-
-
 @pytest.mark.parametrize("curve,thr", [(0, 1), (0, 2)])
 def test_comb_order_exceptional_points(hs, curve, thr):
     """Every key gets a comb table (threshold 1 / 2) and k_gpart's point closes with one general addition: the oracle's
     verdicts when u1*G = +-u2*Q (the closing addition doubles or reaches infinity) or u1*G + u2*Q is one G comb entry,
     and when u2's masks are all ones or all zero."""
-    b = _crafted(curve, _comb_cases(curve))
+    b = edges.crafted(curve, edges.comb_cases(curve))
     want = oracle.verify_batch(curve, b["r"], b["s"], b["qx"], b["qy"], b["digest"])
     assert 0 < int(want.sum()) < want.size
     got, stats = _verify(hs, curve, b, grouped=(thr, 64))

@@ -66,8 +66,8 @@ static void run_grid(unsigned blocks, unsigned threads, F &&body) {
 
 extern "C" int hs_debug_op(int curve, int op, size_t n, const uint32_t *a, const uint32_t *b, uint32_t *out) {
     for (size_t i = 0; i < n; i++) {
-        if (curve == 0) debug_op_item<P256>(op, (uint32_t)i, a, b, out);
-        else debug_op_item<P384>(op, (uint32_t)i, a, b, out);
+        if (curve == 0) debug_op_dispatch<P256>(op, (uint32_t)i, a, b, out);
+        else debug_op_dispatch<P384>(op, (uint32_t)i, a, b, out);
     }
     return 0;
 }
