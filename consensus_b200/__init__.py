@@ -24,7 +24,7 @@ SYMBOLS = [
     "sbv_probe_mad_rate", "sbv_profile_enable", "sbv_profile_read", "sbv_verify_registered",
     "sbv_verify_registered_device", "sbv_hash_verify_registered", "sbv_prepare_quorum", "sbv_verify_quorum",
     "sbv_comm_unique_id", "sbv_comm_init_rank", "sbv_comm_ranks", "sbv_gather_verdicts_device", "sbv_gather_words_device",
-    "sbv_verify_batch_ranked", "sbv_host_alloc", "sbv_host_free",
+    "sbv_verify_batch_ranked", "sbv_host_alloc", "sbv_host_free", "sbv_ed25519_verify_batch",
 ]
 
 
@@ -221,6 +221,26 @@ class Engine:
                                                     off.ctypes.data_as(C.POINTER(C.c_uint64)), _p8(r), _p8(s), _p8(qx), _p8(qy),
                                                     _p8(dig) if want_digest else None, _p8(ok)), "sbv_hash_verify_batch")
         return (ok, dig) if want_digest else ok
+
+    def ed25519_verify_batch(self, msgs, off, sig, pub, out=None) -> np.ndarray:
+        """Ed25519 (Go crypto/ed25519.Verify): msgs concatenated with off[n+1] byte offsets, sig = n x 64 bytes (R || S),
+        pub = n x 32 bytes.  Returns the n verdict bytes (into `out` if given)."""
+        msgs = _u8(msgs if len(msgs) else np.zeros(1, np.uint8))
+        off = np.ascontiguousarray(off, dtype=np.uint64)
+        sig, pub = _u8(sig), _u8(pub)
+        n = off.size - 1
+        if sig.size != 64 * n or pub.size != 32 * n:
+            raise ValueError("sig must hold 64 bytes and pub 32 bytes per message")
+        ok = out if out is not None else np.zeros(n, np.uint8)
+        self._check(self._lib.sbv_ed25519_verify_batch(self._h, C.c_size_t(n), _p8(msgs), off.ctypes.data_as(C.POINTER(C.c_uint64)),
+                                                       _p8(sig), _p8(pub), _p8(ok)), "sbv_ed25519_verify_batch")
+        return ok
+
+    def ed25519_verify_batch_ptr(self, n, msgs, off, sig, pub, ok):
+        """Raw host pointers (ints) — used with pinned buffers."""
+        vp = C.c_void_p
+        self._check(self._lib.sbv_ed25519_verify_batch(self._h, C.c_size_t(n), vp(msgs), vp(off), vp(sig), vp(pub), vp(ok)),
+                    "sbv_ed25519_verify_batch")
 
     def verify_mixed(self, curve_tag, r48, s48, qx48, qy48, digest32) -> np.ndarray:
         curve_tag, r48, s48, qx48, qy48, digest32 = map(_u8, (curve_tag, r48, s48, qx48, qy48, digest32))

@@ -1,5 +1,8 @@
+#include <vector>
+
 #include "engine.h"
 #include "debug_ops.cuh"
+#include "ed25519_debug.cuh"
 using namespace sbv;
 // debug.cu — arithmetic-layer test hooks (used only by tests/; not part of include/sbv.h).
 // Operands are little-endian 32-bit limb arrays, 2N limbs per slot (unused limbs zero).
@@ -29,6 +32,70 @@ extern "C" int sbv_debug_op(sbv_engine *e, uint8_t curve, int op, size_t n, cons
     CU(e, cudaGetLastError());
     CU(e, cudaMemcpyAsync(out, dout, bytes, cudaMemcpyDeviceToHost, d.stream));
     CU(e, cudaStreamSynchronize(d.stream));
+    return SBV_OK;
+}
+
+namespace {
+__global__ void k_debug_ed25519(int op, uint32_t n, const uint32_t *__restrict__ in, uint32_t *__restrict__ out) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    ed_debug_dispatch(op, i, in, out);
+}
+}  // namespace
+
+// Ed25519 arithmetic on device 0: op and the 24-word slots of in / out as in ed25519_debug.cuh.
+extern "C" int sbv_debug_ed25519(sbv_engine *e, int op, size_t n, const uint32_t *in, uint32_t *out) {
+    if (!e || op < ED_DBG_MUL || op > ED_DBG_REDUCE || !in || !out) return SBV_ERR_ARG;
+    if (n == 0) return SBV_OK;
+    std::lock_guard<std::mutex> lk(e->mu);
+    Dev &d = e->devs[0];
+    CU(e, cudaSetDevice(d.ordinal));
+    const size_t bytes = n * ED_DEBUG_WORDS * 4;
+    int rc = sbv_ensure_scratch(e, d, 2 * bytes + 1024);
+    if (rc) return rc;
+    uint32_t *din = (uint32_t *)d.d_scratch, *dout = din + n * ED_DEBUG_WORDS;
+    CU(e, cudaMemcpyAsync(din, in, bytes, cudaMemcpyHostToDevice, d.stream));
+    k_debug_ed25519<<<(uint32_t)((n + 63) / 64), 64, 0, d.stream>>>(op, (uint32_t)n, din, dout);
+    CU(e, cudaGetLastError());
+    CU(e, cudaMemcpyAsync(out, dout, bytes, cudaMemcpyDeviceToHost, d.stream));
+    CU(e, cudaStreamSynchronize(d.stream));
+    return SBV_OK;
+}
+
+// The production SHA-512 kernel of Ed25519 on device 0: dig_out = the 64-byte digests of R || A || M (as SHA-512 outputs
+// them), k_out = the 8 little-endian limbs of k = digest mod L per item.  msg_off are offsets into msgs (off[0] may be > 0).
+extern "C" int sbv_debug_ed25519_sha512(sbv_engine *e, size_t n, const uint8_t *msgs, const uint64_t *msg_off, const uint8_t *sig,
+                                        const uint8_t *pub, uint8_t *dig_out, uint32_t *k_out) {
+    if (!e || !msgs || !msg_off || !sig || !pub || !dig_out || !k_out) return SBV_ERR_ARG;
+    if (n == 0) return SBV_OK;
+    std::lock_guard<std::mutex> lk(e->mu);
+    Dev &d = e->devs[0];
+    CU(e, cudaSetDevice(d.ordinal));
+    const size_t mb = (msg_off[n] + 16 + 255) & ~(size_t)255, ob = ((n + 1) * 8 + 255) & ~(size_t)255;
+    const size_t need = mb + ob + n * 64 + n * 32 + n * 64 + n * 32;
+    int rc = sbv_ensure_scratch(e, d, need + 1024);
+    if (rc) return rc;
+    uint8_t *p = d.d_scratch;
+    uint8_t *dm = p; p += mb;
+    uint64_t *doff = (uint64_t *)p; p += ob;
+    uint8_t *dsig = p; p += n * 64;
+    uint8_t *dpub = p; p += n * 32;
+    uint32_t *ddig = (uint32_t *)p; p += n * 64;
+    uint32_t *dk = (uint32_t *)p;
+    CU(e, cudaMemcpyAsync(dm, msgs, msg_off[n], cudaMemcpyHostToDevice, d.stream));
+    CU(e, cudaMemcpyAsync(doff, msg_off, (n + 1) * 8, cudaMemcpyHostToDevice, d.stream));
+    CU(e, cudaMemcpyAsync(dsig, sig, n * 64, cudaMemcpyHostToDevice, d.stream));
+    CU(e, cudaMemcpyAsync(dpub, pub, n * 32, cudaMemcpyHostToDevice, d.stream));
+    if ((rc = sbv_launch_ed_sha512_digest(e, n, dm, doff, dsig, dpub, dk, ddig, d.stream))) return rc;
+    std::vector<uint32_t> dig(n * 16), kw(n * 8);
+    CU(e, cudaMemcpyAsync(dig.data(), ddig, n * 64, cudaMemcpyDeviceToHost, d.stream));
+    CU(e, cudaMemcpyAsync(kw.data(), dk, n * 32, cudaMemcpyDeviceToHost, d.stream));
+    CU(e, cudaStreamSynchronize(d.stream));
+    for (size_t i = 0; i < n; i++) {
+        for (int w = 0; w < 16; w++)  // digest limbs are little-endian: back to bytes
+            for (int b = 0; b < 4; b++) dig_out[i * 64 + 4 * w + b] = (uint8_t)(dig[i * 16 + w] >> (8 * b));
+        for (int w = 0; w < 8; w++) k_out[i * 8 + w] = kw[(size_t)w * n + i];
+    }
     return SBV_OK;
 }
 

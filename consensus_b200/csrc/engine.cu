@@ -154,9 +154,8 @@ int sbv_lane_ensure_aux(sbv_engine *e, Dev::Lane &ln, size_t bytes) {
     ln.aux_cap = cap;
     return 0;
 }
-int sbv_launch_sha256(sbv_engine *e, size_t n, const uint8_t *d_msgs, const uint64_t *d_off, uint64_t base, uint8_t *d_digest, uint32_t *d_perm,
-                      cudaStream_t st) {
-    const uint32_t *perm = nullptr;
+int sbv_launch_length_sort(sbv_engine *e, size_t n, const uint64_t *d_off, uint32_t *d_perm, cudaStream_t st, const uint32_t **perm) {
+    *perm = nullptr;
     if (d_perm && n >= 2048) {  // sort by block count so that a warp's 32 messages have equal length
         uint32_t *hist = d_perm + n, *start = hist + SHA_BINS, *cursor = start + SHA_BINS;
         CU(e, cudaMemsetAsync(hist, 0, SHA_BINS * sizeof(uint32_t), st));
@@ -164,8 +163,15 @@ int sbv_launch_sha256(sbv_engine *e, size_t n, const uint8_t *d_msgs, const uint
         k_sha_scan<<<1, SHA_BINS, 0, st>>>(hist, start, cursor);
         k_sha_scatter<<<(uint32_t)((n + 255) / 256), 256, 0, st>>>((uint32_t)n, d_off, start, cursor, d_perm);
         e->launches += 3;
-        perm = d_perm;
+        *perm = d_perm;
     }
+    return 0;
+}
+int sbv_launch_sha256(sbv_engine *e, size_t n, const uint8_t *d_msgs, const uint64_t *d_off, uint64_t base, uint8_t *d_digest, uint32_t *d_perm,
+                      cudaStream_t st) {
+    const uint32_t *perm = nullptr;
+    int rc = sbv_launch_length_sort(e, n, d_off, d_perm, st, &perm);
+    if (rc) return rc;
     k_sha256<<<(uint32_t)((n + 127) / 128), 128, 0, st>>>((uint32_t)n, d_msgs, d_off, base, d_digest, perm);
     e->launches += 1;
     CU(e, cudaGetLastError());
@@ -459,7 +465,7 @@ void sbv_destroy(sbv_engine *e) {
     }
     for (Dev &d : e->devs) {
         cudaSetDevice(d.ordinal);
-        void *ptrs[] = {d.gtab[0], d.gtab[1], d.d_scratch};
+        void *ptrs[] = {d.gtab[0], d.gtab[1], d.ed_btab, d.d_scratch};
         for (void *p : ptrs) if (p) cudaFree(p);
         sbv_scratch_free(d);
         sbv_keys_free(d);

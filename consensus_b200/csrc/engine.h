@@ -32,6 +32,7 @@ struct Dev {
     int ordinal = 0;
     cudaStream_t stream = nullptr;
     uint32_t *gtab[2] = {nullptr, nullptr};
+    uint32_t *ed_btab = nullptr;  // fixed-base table of the Ed25519 base point, built on the device's first Ed25519 call
     // Per-launch workspace of the verify pipeline.  A launch takes the next set and first waits for the event of
     // that set's previous user, so launches on different streams overlap without sharing mutable state.
     // The buffers are sized, grown and freed from one list (pipeline.cu: each_buffer).
@@ -172,6 +173,14 @@ int sbv_init_gtables(sbv_engine *e, Dev &d);
 int sbv_keys_build(sbv_engine *e, Dev &d);  // (re)builds the per-key tables of the registry
 void sbv_keys_free(Dev &d);
 void sbv_scratch_free(Dev &d);
+// ---- inst_ed25519.cu: Ed25519 (enqueue only, no sync) ----
+int sbv_ed_btab_ensure(sbv_engine *e, Dev &d);  // caller holds e->mu and has set the device
+// k = SHA-512(R || A || M) mod L into d_k (word-major, 8n words), then the verdicts into d_ok.  d_sig: 64n bytes (R || S),
+// d_pub: 32n bytes, d_perm: n + 3072 words of scratch.  The table of B must exist (sbv_ed_btab_ensure).
+int sbv_launch_ed25519(sbv_engine *e, Dev &d, size_t n, const uint8_t *d_msgs, const uint64_t *d_off, uint64_t base, const uint8_t *d_sig,
+                       const uint8_t *d_pub, uint32_t *d_k, uint32_t *d_perm, uint8_t *d_ok, cudaStream_t st);
+int sbv_launch_ed_sha512_digest(sbv_engine *e, size_t n, const uint8_t *d_msgs, const uint64_t *d_off, const uint8_t *d_sig, const uint8_t *d_pub,
+                                uint32_t *d_k, uint32_t *d_dig, cudaStream_t st);
 
 // ---- engine.cu helpers shared with the other translation units ----
 int sbv_lane_acquire(sbv_engine *e);            // blocks until a lane index is free; returns it
@@ -182,6 +191,8 @@ int sbv_lane_ensure_aux(sbv_engine *e, Dev::Lane &ln, size_t bytes);
 // d_perm: n + 3072 words of scratch (may be null: no length sort)
 int sbv_launch_sha256(sbv_engine *e, size_t n, const uint8_t *d_msgs, const uint64_t *d_off, uint64_t base, uint8_t *d_digest, uint32_t *d_perm,
                       cudaStream_t st);
+// the block-count sort of the SHA-256 launch on its own: *perm = the permutation in d_perm, or nullptr below 2048 items
+int sbv_launch_length_sort(sbv_engine *e, size_t n, const uint64_t *d_off, uint32_t *d_perm, cudaStream_t st, const uint32_t **perm);
 int sbv_lane_h2d(sbv_engine *e, Dev::Lane &ln, void *dst, const void *src, size_t bytes, size_t &stage_off, cudaStream_t st = nullptr);
 int sbv_ensure_scratch(sbv_engine *e, Dev &d, size_t bytes);
 

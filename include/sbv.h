@@ -102,6 +102,16 @@ int sbv_hash_verify_batch(sbv_engine *e, uint8_t curve, size_t n, const uint8_t 
 int sbv_verify_mixed(sbv_engine *e, size_t n, const uint8_t *curve_tag, const uint8_t *r48, const uint8_t *s48,
                      const uint8_t *qx48, const uint8_t *qy48, const uint8_t *digest32, uint8_t *ok);
 
+/* Ed25519 verify over raw messages, for a Verifier whose keys are crypto/ed25519 keys (VerifyConsenterSig /
+ * VerifySignature / VerifyRequest, dependencies.go:58-64).  msgs concatenated with msg_off[n+1] byte offsets (msgs may
+ * be NULL when every message is empty); sig = 64n bytes (R || S), pub = 32n bytes, both as RFC 8032 encodes them.
+ * Accept set = Go crypto/ed25519.Verify (pure Ed25519, no context): S < L; A decodes as edwards25519 Point.SetBytes does
+ * (y >= p reduced, "-0" accepted, no subgroup check); k = SHA-512(R || A || M) mod L over the caller's bytes; accept iff
+ * the canonical encoding of [S]B - [k]A equals R byte for byte (cofactorless; each signature on its own).  Messages are
+ * hashed on the device.  The first call on an engine builds a 384 KiB table of B on every device. */
+int sbv_ed25519_verify_batch(sbv_engine *e, size_t n, const uint8_t *msgs, const uint64_t *msg_off, const uint8_t *sig,
+                             const uint8_t *pub, uint8_t *ok);
+
 /* Distinct-signer quorum count per consensus instance (processCommits, view.go:519-551).
  * Votes are given in arrival order.  A vote is registered iff signer == sender and sender !=
  * self_id[instance] and the sender has no earlier registered vote in the instance

@@ -28,11 +28,15 @@ import (
 	"github.com/hyperledger-labs/SmartBFT/pkg/types"
 )
 
-// item is one unit of engine work: verify (r, s) under registry slot `slot` over SHA-256(msg).
+// item is one unit of engine work: verify (r, s) under registry slot `slot` over SHA-256(msg), or, when ed is set,
+// the Ed25519 signature edSig under the key edPub over msg (crypto/ed25519.Verify).
 type item struct {
-	r, s [32]byte
-	slot uint32
-	msg  []byte
+	r, s  [32]byte
+	slot  uint32
+	msg   []byte
+	ed    bool
+	edPub [32]byte
+	edSig [64]byte
 }
 
 // Verifier implements api.Verifier.
@@ -45,6 +49,8 @@ type Verifier struct {
 	slots      map[[64]byte]uint32 // key -> slot
 	consenters map[uint64]uint32
 	clients    map[string]uint32
+	edKeys     map[uint64][32]byte // consenters with crypto/ed25519 keys: verified by sbv_ed25519_verify_batch
+	edClients  map[string][32]byte // clients with crypto/ed25519 keys
 	dirty      bool
 
 	pool sync.Pool // *pinned: one block of page-locked memory per in-flight batch
@@ -62,7 +68,8 @@ func New(devices []int) (*Verifier, error) {
 	if rc := C.sbv_create(&ords[0], C.int(len(devices)), &eng); rc != 0 {
 		return nil, fmt.Errorf("sbv_create failed: %d (there is no CPU fallback)", int(rc))
 	}
-	v := &Verifier{eng: eng, slots: map[[64]byte]uint32{}, consenters: map[uint64]uint32{}, clients: map[string]uint32{}}
+	v := &Verifier{eng: eng, slots: map[[64]byte]uint32{}, consenters: map[uint64]uint32{}, clients: map[string]uint32{},
+		edKeys: map[uint64][32]byte{}, edClients: map[string][32]byte{}}
 	v.pool.New = func() interface{} { return &pinned{} }
 	v.agg = newAggregator(v.engineBatch, 200*time.Microsecond, 65536)
 	return v, nil
@@ -88,11 +95,41 @@ func (v *Verifier) slotOf(xy [64]byte) uint32 { // v.mu held
 	return s
 }
 
-func (v *Verifier) SetConsenterKey(id uint64, xy [64]byte) { v.mu.Lock(); v.consenters[id] = v.slotOf(xy); v.mu.Unlock() }
-func (v *Verifier) SetClientKey(c string, xy [64]byte)     { v.mu.Lock(); v.clients[c] = v.slotOf(xy); v.mu.Unlock() }
-func (v *Verifier) SetVerificationSequence(s uint64)        { v.mu.Lock(); v.verSeq = s; v.mu.Unlock() }
+// A consenter or client holds one key: setting a key of one type removes any key of the other type it held, so a
+// signature is never checked under a key the configuration no longer gives it.
+func (v *Verifier) SetConsenterKey(id uint64, xy [64]byte) {
+	v.mu.Lock()
+	v.consenters[id] = v.slotOf(xy)
+	delete(v.edKeys, id)
+	v.mu.Unlock()
+}
+func (v *Verifier) SetClientKey(c string, xy [64]byte) {
+	v.mu.Lock()
+	v.clients[c] = v.slotOf(xy)
+	delete(v.edClients, c)
+	v.mu.Unlock()
+}
+func (v *Verifier) SetVerificationSequence(s uint64) { v.mu.Lock(); v.verSeq = s; v.mu.Unlock() }
 
-// ResetKeys drops every registered key. Keys change only with a reconfiguration, i.e. a new verification
+// SetConsenterEd25519Key: consenter `id` signs with crypto/ed25519 (an Ed25519 identity, as Fabric 3 allows next to
+// ECDSA ones). Its signatures are 64 raw bytes R || S over the message itself (no prehash).
+func (v *Verifier) SetConsenterEd25519Key(id uint64, pub [32]byte) {
+	v.mu.Lock()
+	v.edKeys[id] = pub
+	delete(v.consenters, id)
+	v.mu.Unlock()
+}
+
+// SetClientEd25519Key: client `c` signs its requests with crypto/ed25519; the signature field of its requests is the
+// 64-byte R || S over the signed bytes of the request.
+func (v *Verifier) SetClientEd25519Key(c string, pub [32]byte) {
+	v.mu.Lock()
+	v.edClients[c] = pub
+	delete(v.clients, c)
+	v.mu.Unlock()
+}
+
+// ResetKeys drops every key, ECDSA and Ed25519, of consenters and clients. Keys change only with a reconfiguration, i.e. a new verification
 // sequence (dependencies.go:65-66): the application calls ResetKeys, re-registers the new configuration's keys
 // and bumps the sequence, so rotated keys do not pile up in HBM (264 KiB per key and GPU). Client keys of high
 // cardinality should not be registered at all: sbv_hash_verify_batch takes the key with every item and groups
@@ -101,6 +138,7 @@ func (v *Verifier) ResetKeys() {
 	v.mu.Lock()
 	v.registry, v.slots = nil, map[[64]byte]uint32{}
 	v.consenters, v.clients = map[uint64]uint32{}, map[string]uint32{}
+	v.edKeys, v.edClients = map[uint64][32]byte{}, map[string][32]byte{}
 	v.dirty = true
 	v.mu.Unlock()
 }
@@ -155,10 +193,70 @@ func (b *pinned) reserve(n int) []byte {
 	return unsafe.Slice((*byte)(b.p), b.cap)[:n]
 }
 
-// engineBatch is the one cgo crossing: SHA-256 of every message and ECDSA verification against the
-// registered keys, both on the GPU. The batch is marshalled straight into pinned memory (one block per
-// in-flight batch, pooled): r | s | slot | off | msgs.
+// engineBatch dispatches an aggregated batch by key type: the ECDSA items in one sbv_hash_verify_registered call,
+// the Ed25519 items in one sbv_ed25519_verify_batch call; verdicts come back in the items' order.
 func (v *Verifier) engineBatch(items []item) []byte {
+	var ec, ed []item
+	var ecAt, edAt []int
+	for i := range items {
+		if items[i].ed {
+			ed, edAt = append(ed, items[i]), append(edAt, i)
+		} else {
+			ec, ecAt = append(ec, items[i]), append(ecAt, i)
+		}
+	}
+	ok := make([]byte, len(items))
+	if len(ec) > 0 {
+		for j, o := range v.ecdsaBatch(ec) {
+			ok[ecAt[j]] = o
+		}
+	}
+	if len(ed) > 0 {
+		for j, o := range v.ed25519Batch(ed) {
+			ok[edAt[j]] = o
+		}
+	}
+	return ok
+}
+
+// ed25519Batch: SHA-512(R || A || M) and the Ed25519 equation of every item on the GPU. Marshalled into pinned
+// memory: sig (64n) | pub (32n) | off | msgs.
+func (v *Verifier) ed25519Batch(items []item) []byte {
+	n := len(items)
+	ok := make([]byte, n)
+	total := 0
+	for i := range items {
+		total += len(items[i].msg)
+	}
+	oPub := 64 * n
+	oOff := oPub + 32*n
+	oMsgs := oOff + 8*(n+1)
+	pb := v.pool.Get().(*pinned)
+	defer v.pool.Put(pb)
+	buf := pb.reserve(oMsgs + total + 16)
+	pos := 0
+	binary.LittleEndian.PutUint64(buf[oOff:], 0)
+	for i := range items {
+		copy(buf[64*i:], items[i].edSig[:])
+		copy(buf[oPub+32*i:], items[i].edPub[:])
+		copy(buf[oMsgs+pos:], items[i].msg)
+		pos += len(items[i].msg)
+		binary.LittleEndian.PutUint64(buf[oOff+8*(i+1):], uint64(pos))
+	}
+	base := uintptr(pb.p)
+	rc := C.sbv_ed25519_verify_batch(v.eng, C.size_t(n), (*C.uint8_t)(unsafe.Pointer(base+uintptr(oMsgs))),
+		(*C.uint64_t)(unsafe.Pointer(base+uintptr(oOff))), (*C.uint8_t)(unsafe.Pointer(base)),
+		(*C.uint8_t)(unsafe.Pointer(base+uintptr(oPub))), (*C.uint8_t)(unsafe.Pointer(&ok[0])))
+	if rc != 0 {
+		v.fault("sbv_ed25519_verify_batch", rc)
+	}
+	return ok
+}
+
+// ecdsaBatch: SHA-256 of every message and ECDSA verification against the registered keys, both on the GPU.
+// The batch is marshalled straight into pinned memory (one block per in-flight batch, pooled):
+// r | s | slot | off | msgs.
+func (v *Verifier) ecdsaBatch(items []item) []byte {
 	v.syncRegistry()
 	n := len(items)
 	ok := make([]byte, n)
@@ -247,7 +345,16 @@ func parseDER(sig []byte) (r, s [32]byte, ok bool) {
 func (v *Verifier) consenterItem(sig types.Signature) (item, error) {
 	v.mu.RLock()
 	slot, known := v.consenters[sig.ID]
+	edPub, isEd := v.edKeys[sig.ID]
 	v.mu.RUnlock()
+	if isEd {
+		if len(sig.Value) != 64 { // crypto/ed25519.Verify rejects any other length
+			return item{}, fmt.Errorf("malformed signature from %d", sig.ID)
+		}
+		it := item{ed: true, edPub: edPub, msg: sig.Msg}
+		copy(it.edSig[:], sig.Value)
+		return it, nil
+	}
 	if !known {
 		return item{}, fmt.Errorf("unknown consenter %d", sig.ID)
 	}
@@ -318,7 +425,7 @@ func (v *Verifier) VerifySignature(sig types.Signature) error {
 	return nil
 }
 
-// request := u16be siglen || sig(DER) || u32be clen || client || u32be ilen || id || payload
+// request := u16be siglen || sig (DER, or R || S for an Ed25519 client) || u32be clen || client || u32be ilen || id || payload
 func (v *Verifier) requestItem(val []byte) (item, types.RequestInfo, error) {
 	if len(val) < 2 {
 		return item{}, types.RequestInfo{}, errors.New("malformed request")
@@ -348,7 +455,17 @@ func (v *Verifier) requestItem(val []byte) (item, types.RequestInfo, error) {
 	}
 	v.mu.RLock()
 	slot, known := v.clients[client]
+	edPub, isEd := v.edClients[client]
 	v.mu.RUnlock()
+	info := types.RequestInfo{ClientID: client, ID: id}
+	if isEd {
+		if len(sig) != 64 { // crypto/ed25519.Verify rejects any other length
+			return item{}, types.RequestInfo{}, errors.New("malformed request signature")
+		}
+		it := item{ed: true, edPub: edPub, msg: signed}
+		copy(it.edSig[:], sig)
+		return it, info, nil
+	}
 	if !known {
 		return item{}, types.RequestInfo{}, fmt.Errorf("unknown client %s", client)
 	}
@@ -356,7 +473,7 @@ func (v *Verifier) requestItem(val []byte) (item, types.RequestInfo, error) {
 	if !ok {
 		return item{}, types.RequestInfo{}, errors.New("malformed request signature")
 	}
-	return item{r: r, s: s, slot: slot, msg: signed}, types.RequestInfo{ClientID: client, ID: id}, nil
+	return item{r: r, s: s, slot: slot, msg: signed}, info, nil
 }
 
 // VerifyRequest — dependencies.go:58-59 (controller.go:239, 742-745; requestpool.go:335-354).

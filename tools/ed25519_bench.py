@@ -1,0 +1,119 @@
+"""Ed25519 throughput of sbv_ed25519_verify_batch through the C ABI, with the OpenSSL CPU arm measured in the same run.
+
+    python tools/ed25519_bench.py [--n 65536] [--keys 1024] [--msg-len 256] [--steps 20] [--warmup 5]
+
+Inputs live in pinned host memory (sbv_host_alloc); each timed call uploads them, hashes, verifies and returns the
+verdicts.  Kernel times of k_ed_sha512 and k_ed_verify come from a separate torch.profiler run.  Prints one JSON line;
+the verdicts of every timed call are checked against the oracle.
+"""
+from __future__ import annotations
+
+import argparse
+import ctypes as C
+import json
+import os
+import subprocess
+import sys
+import time
+
+import numpy as np
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+
+
+def power_limit_w():
+    try:
+        out = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader,nounits", "-i", "0"],
+                             capture_output=True, text=True, timeout=30).stdout.strip()
+        return float(out.splitlines()[0])
+    except (OSError, ValueError, IndexError, subprocess.SubprocessError):
+        return None
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--n", type=int, default=65536)
+    ap.add_argument("--keys", type=int, default=1024)
+    ap.add_argument("--msg-len", type=int, default=256)
+    ap.add_argument("--steps", type=int, default=20)
+    ap.add_argument("--warmup", type=int, default=5)
+    args = ap.parse_args()
+
+    import torch
+
+    import consensus_b200 as sbv
+    import oracle_ed25519 as oe
+    from oracle_ed25519 import corpus
+
+    c = corpus.make_corpus(args.n, seed=2024, n_keys=args.keys, fixed_len=args.msg_len, crafted_max=64)
+    want = oe.verify_batch(c["msgs"], c["off"], c["sig"], c["pub"])
+    lib = sbv.load_library()
+    lib.sbv_host_alloc.restype = C.c_void_p
+    eng = sbv.Engine(devices=[0])
+    bufs = []
+
+    def pinned(a):
+        a = np.ascontiguousarray(a).view(np.uint8).reshape(-1)
+        ptr = lib.sbv_host_alloc(C.c_size_t(a.nbytes))
+        if not ptr:
+            raise sbv.EngineFault("sbv_host_alloc failed")
+        bufs.append(ptr)
+        np.ctypeslib.as_array((C.c_uint8 * a.nbytes).from_address(ptr))[:] = a
+        return ptr
+
+    n = args.n
+    m, o, s, p, ok = pinned(c["msgs"]), pinned(c["off"]), pinned(c["sig"]), pinned(c["pub"]), pinned(np.zeros(n, np.uint8))
+    okv = np.ctypeslib.as_array((C.c_uint8 * n).from_address(ok))
+    try:
+        for _ in range(args.warmup):
+            eng.ed25519_verify_batch_ptr(n, m, o, s, p, ok)
+        times, verdicts_ok = [], True
+        for _ in range(args.steps):
+            okv[:] = 2
+            t0 = time.perf_counter()
+            eng.ed25519_verify_batch_ptr(n, m, o, s, p, ok)
+            times.append(time.perf_counter() - t0)
+            verdicts_ok &= bool(np.array_equal(okv, want))
+        from torch.profiler import ProfilerActivity, profile
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            for _ in range(3):
+                eng.ed25519_verify_batch_ptr(n, m, o, s, p, ok)
+            torch.cuda.synchronize()
+        kern = {}
+        for ev in prof.key_averages():
+            for name in ("k_ed_sha512", "k_ed_verify"):
+                if name in ev.key:
+                    t = getattr(ev, "device_time", None) or getattr(ev, "cuda_time", 0.0)  # average µs per call
+                    kern[name + "_us"] = round(float(t), 1)
+        verdicts_ok &= bool(np.array_equal(okv, want))
+    finally:
+        eng.close()
+        for ptr in bufs:
+            lib.sbv_host_free(C.c_void_p(ptr))
+    cores = oe.ncores()
+    cpu_s, cpu_ok = oe.bench_verify(c["msgs"], c["off"], c["sig"], c["pub"], nthreads=cores)
+    med = float(np.median(times))
+    props = torch.cuda.get_device_properties(0)
+    res = {
+        "metric": "ed25519_verifies_per_s",
+        "value": n / med,
+        "unit": "verifies/s",
+        "n": n, "keys": args.keys, "msg_len": args.msg_len, "steps": args.steps, "warmup": args.warmup,
+        "median_call_ms": med * 1e3,
+        "best_call_ms": min(times) * 1e3,
+        **kern,
+        "cpu_openssl_verifies_per_s": n / cpu_s,
+        "cpu_cores": cores,
+        "gpu_over_cpu": (n / med) / (n / cpu_s),
+        "accepts": int(want.sum()),
+        "verdicts_match_oracle": bool(verdicts_ok and np.array_equal(cpu_ok, want)),
+        "device": props.name,
+        "power_limit_w": power_limit_w(),
+    }
+    print(json.dumps(res))
+    return 0 if res["verdicts_match_oracle"] else 1
+
+
+if __name__ == "__main__":
+    sys.exit(main())

@@ -17,6 +17,9 @@ namespace sbv { uint32_t tab[1 << 18]; }
 #include "../../consensus_b200/csrc/keygroup.cuh"
 #include "../../consensus_b200/csrc/sha256.cuh"
 #include "../../consensus_b200/csrc/quorum.cuh"
+#include "../../consensus_b200/csrc/ed25519_debug.cuh"
+#include "../../consensus_b200/csrc/sha512.cuh"
+#include "../../consensus_b200/csrc/ed25519_verify.cuh"
 
 using namespace sbv;
 
@@ -300,3 +303,37 @@ extern "C" int hs_verify_grouped(int curve, size_t n, const uint8_t *r, const ui
     return 0;
 }
 
+
+// ---- Ed25519 (ed25519.cuh, sha512.cuh, ed25519_verify.cuh) ----
+// field / decode / mod-L operations of ed25519_debug.cuh, 24-word slots
+extern "C" int hs_ed25519_op(int op, size_t n, const uint32_t *in, uint32_t *out) {
+    for (size_t i = 0; i < n; i++) ed_debug_dispatch(op, (uint32_t)i, in, out);
+    return 0;
+}
+// k_ed_sha512 over a ragged batch (perm: optional processing order): k word-major [8][n], and the 16 digest limbs per item
+extern "C" int hs_ed25519_sha512(size_t n, const uint8_t *msgs, const uint64_t *off, uint64_t base, const uint8_t *sig, const uint8_t *pub,
+                                 const uint32_t *perm, uint32_t *k_out, uint32_t *dig_out) {
+    run_grid((unsigned)((n + 127) / 128), 128, [&] { k_ed_sha512((uint32_t)n, sig, pub, msgs, off, base, k_out, perm, dig_out); });
+    return 0;
+}
+static std::vector<uint32_t> &ed_btab_host() {
+    static std::vector<uint32_t> t;
+    if (t.empty()) {
+        t.resize(ED_BTAB_WORDS);
+        run_grid((ED_BWINS * ED_BENT + 63) / 64, 64, [&] { k_ed_btab_init(t.data()); });
+    }
+    return t;
+}
+// the fixed-base table of B as k_ed_btab_init builds it
+extern "C" int hs_ed25519_btab(uint32_t *out) {
+    memcpy(out, ed_btab_host().data(), ED_BTAB_WORDS * 4);
+    return 0;
+}
+// the whole pipeline of sbv_ed25519_verify_batch on one device: k_ed_sha512, then k_ed_verify with blocks of 32 threads
+extern "C" int hs_ed25519_verify(size_t n, const uint8_t *msgs, const uint64_t *off, const uint8_t *sig, const uint8_t *pub, uint8_t *ok) {
+    std::vector<uint32_t> k(8 * n + 8);
+    run_grid((unsigned)((n + 127) / 128), 128, [&] { k_ed_sha512((uint32_t)n, sig, pub, msgs, off, 0, k.data(), nullptr, nullptr); });
+    const uint4 *bt = reinterpret_cast<const uint4 *>(ed_btab_host().data());
+    run_grid((unsigned)((n + 31) / 32), 32, [&] { k_ed_verify<32>((uint32_t)n, sig, pub, k.data(), bt, ok); });
+    return 0;
+}
