@@ -181,6 +181,11 @@ int sbv_launch_ed25519(sbv_engine *e, Dev &d, size_t n, const uint8_t *d_msgs, c
                        const uint8_t *d_pub, uint32_t *d_k, uint32_t *d_perm, uint8_t *d_ok, cudaStream_t st);
 int sbv_launch_ed_sha512_digest(sbv_engine *e, size_t n, const uint8_t *d_msgs, const uint64_t *d_off, const uint8_t *d_sig, const uint8_t *d_pub,
                                 uint32_t *d_k, uint32_t *d_dig, cudaStream_t st);
+// test hook: k_ed_verify with the caller's k (word-major [8][n], every k < L); the table of B must exist
+int sbv_launch_ed_verify_k(sbv_engine *e, Dev &d, size_t n, const uint8_t *d_sig, const uint8_t *d_pub, const uint32_t *d_k, uint8_t *d_ok,
+                           cudaStream_t st);
+// shape of the table of B (ed25519_verify.cuh: ED_BWINS x ED_BENT entries of ED_BWORDS words; checked in inst_ed25519.cu)
+constexpr size_t SBV_ED_BTAB_ENTRIES = 32 * 128, SBV_ED_BTAB_ENTRY_WORDS = 24;
 
 // ---- engine.cu helpers shared with the other translation units ----
 int sbv_lane_acquire(sbv_engine *e);            // blocks until a lane index is free; returns it

@@ -9,6 +9,7 @@ namespace {
 constexpr int ED_BLOCK = 32;  // 32 KiB of shared memory per block (the 1A..8A tables): no opt-in attribute needed
 constexpr size_t ED_SMEM = (size_t)8 * 4 * 8 * 4 * ED_BLOCK;
 }  // namespace
+static_assert(SBV_ED_BTAB_ENTRIES == (size_t)ED_BWINS * ED_BENT && SBV_ED_BTAB_ENTRY_WORDS == ED_BWORDS, "engine.h: table of B");
 
 // The fixed-base table of B, built on the first Ed25519 call of each device.  Caller holds e->mu and has set the device.
 // The build is synchronised before the pointer is published, so a verification on any stream sees a finished table.
@@ -45,6 +46,17 @@ int sbv_launch_ed25519(sbv_engine *e, Dev &d, size_t n, const uint8_t *d_msgs, c
 int sbv_launch_ed_sha512_digest(sbv_engine *e, size_t n, const uint8_t *d_msgs, const uint64_t *d_off, const uint8_t *d_sig, const uint8_t *d_pub,
                                 uint32_t *d_k, uint32_t *d_dig, cudaStream_t st) {
     k_ed_sha512<<<(uint32_t)((n + 127) / 128), 128, 0, st>>>((uint32_t)n, d_sig, d_pub, d_msgs, d_off, 0, d_k, nullptr, d_dig);
+    e->launches += 1;
+    CU(e, cudaGetLastError());
+    return 0;
+}
+
+// test hook (debug.cu): the production verification kernel with the caller's k (word-major, every k < L) in place of
+// SHA-512's.  The table of B must exist (sbv_ed_btab_ensure).
+int sbv_launch_ed_verify_k(sbv_engine *e, Dev &d, size_t n, const uint8_t *d_sig, const uint8_t *d_pub, const uint32_t *d_k, uint8_t *d_ok,
+                           cudaStream_t st) {
+    k_ed_verify<ED_BLOCK><<<(uint32_t)((n + ED_BLOCK - 1) / ED_BLOCK), ED_BLOCK, ED_SMEM, st>>>(
+        (uint32_t)n, d_sig, d_pub, d_k, reinterpret_cast<const uint4 *>(d.ed_btab), d_ok);
     e->launches += 1;
     CU(e, cudaGetLastError());
     return 0;

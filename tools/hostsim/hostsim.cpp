@@ -337,3 +337,18 @@ extern "C" int hs_ed25519_verify(size_t n, const uint8_t *msgs, const uint64_t *
     run_grid((unsigned)((n + 31) / 32), 32, [&] { k_ed_verify<32>((uint32_t)n, sig, pub, k.data(), bt, ok); });
     return 0;
 }
+// k_ed_verify alone with the caller's k (8 little-endian limbs per item, each < L; -1 otherwise), as
+// sbv_debug_ed25519_verify_k runs it on the device
+extern "C" int hs_ed25519_verify_k(size_t n, const uint8_t *sig, const uint8_t *pub, const uint32_t *k_in, uint8_t *ok) {
+    uint32_t Lm[8];
+    ed_order(Lm);
+    std::vector<uint32_t> k(8 * n + 8);
+    for (size_t i = 0; i < n; i++) {
+        uint32_t ki[8];
+        for (int w = 0; w < 8; w++) k[(size_t)w * n + i] = ki[w] = k_in[i * 8 + w];
+        if (!mp_lt<8>(ki, Lm)) return -1;
+    }
+    const uint4 *bt = reinterpret_cast<const uint4 *>(ed_btab_host().data());
+    run_grid((unsigned)((n + 31) / 32), 32, [&] { k_ed_verify<32>((uint32_t)n, sig, pub, k.data(), bt, ok); });
+    return 0;
+}
