@@ -25,6 +25,7 @@ SYMBOLS = [
     "sbv_verify_registered_device", "sbv_hash_verify_registered", "sbv_prepare_quorum", "sbv_verify_quorum",
     "sbv_comm_unique_id", "sbv_comm_init_rank", "sbv_comm_ranks", "sbv_gather_verdicts_device", "sbv_gather_words_device",
     "sbv_verify_batch_ranked", "sbv_host_alloc", "sbv_host_free", "sbv_ed25519_verify_batch",
+    "sbv_ed25519_set_keys", "sbv_ed25519_verify_registered",
 ]
 
 
@@ -241,6 +242,37 @@ class Engine:
         vp = C.c_void_p
         self._check(self._lib.sbv_ed25519_verify_batch(self._h, C.c_size_t(n), vp(msgs), vp(off), vp(sig), vp(pub), vp(ok)),
                     "sbv_ed25519_verify_batch")
+
+    def ed25519_set_keys(self, pub):
+        """Replaces the Ed25519 key registry: slot i = the 32-byte encoding pub[i] (n x 32 bytes; n = 0 empties it) and
+        builds a 384 KiB fixed-base table per decodable key on every device."""
+        pub = _u8(pub)
+        if pub.size % 32:
+            raise ValueError("pub must hold 32 bytes per key")
+        n = pub.size // 32
+        self._check(self._lib.sbv_ed25519_set_keys(self._h, C.c_size_t(n), _p8(pub) if n else None), "sbv_ed25519_set_keys")
+
+    def ed25519_verify_registered(self, msgs, off, key_slot, sig, out=None) -> np.ndarray:
+        """Ed25519 with the key of item i taken from registry slot key_slot[i] (ed25519_set_keys): msgs concatenated with
+        off[n+1] byte offsets, sig = n x 64 bytes (R || S).  Returns the n verdict bytes (into `out` if given)."""
+        msgs = _u8(msgs if len(msgs) else np.zeros(1, np.uint8))
+        off = np.ascontiguousarray(off, dtype=np.uint64)
+        key_slot = np.ascontiguousarray(key_slot, dtype=np.uint32)
+        sig = _u8(sig)
+        n = off.size - 1
+        if sig.size != 64 * n or key_slot.size != n:
+            raise ValueError("sig must hold 64 bytes and key_slot one slot per message")
+        ok = out if out is not None else np.zeros(n, np.uint8)
+        self._check(self._lib.sbv_ed25519_verify_registered(self._h, C.c_size_t(n), _p8(msgs), off.ctypes.data_as(C.POINTER(C.c_uint64)),
+                                                            key_slot.ctypes.data_as(C.POINTER(C.c_uint32)), _p8(sig), _p8(ok)),
+                    "sbv_ed25519_verify_registered")
+        return ok
+
+    def ed25519_verify_registered_ptr(self, n, msgs, off, key_slot, sig, ok):
+        """Raw host pointers (ints) — used with pinned buffers."""
+        vp = C.c_void_p
+        self._check(self._lib.sbv_ed25519_verify_registered(self._h, C.c_size_t(n), vp(msgs), vp(off), vp(key_slot), vp(sig), vp(ok)),
+                    "sbv_ed25519_verify_registered")
 
     def verify_mixed(self, curve_tag, r48, s48, qx48, qy48, digest32) -> np.ndarray:
         curve_tag, r48, s48, qx48, qy48, digest32 = map(_u8, (curve_tag, r48, s48, qx48, qy48, digest32))

@@ -164,3 +164,57 @@ extern "C" int sbv_debug_ed25519_verify_k(sbv_engine *e, size_t n, const uint8_t
     CU(e, cudaStreamSynchronize(d.stream));
     return SBV_OK;
 }
+
+// Copies entries [first, first + count) of the table of registry slot `slot` on device 0 (sbv_ed25519_set_keys: entry
+// win * 128 + j - 1 is j * 256^win * A as y + x, y - x, 2dxy, 24 limbs).  SBV_ERR_ARG for an unknown slot, a key that does
+// not decode or a range outside the table.
+extern "C" int sbv_debug_ed25519_ktab(sbv_engine *e, uint32_t slot, size_t first, size_t count, uint32_t *out) {
+    if (!e || !out || first > SBV_ED_BTAB_ENTRIES || count > SBV_ED_BTAB_ENTRIES - first) return SBV_ERR_ARG;
+    std::lock_guard<std::mutex> lk(e->mu);
+    Dev &d = e->devs[0];
+    if (slot >= d.ed_n_slots) return SBV_ERR_ARG;
+    CU(e, cudaSetDevice(d.ordinal));
+    int32_t loc = -1;
+    CU(e, cudaMemcpy(&loc, d.ed_slot2local + slot, sizeof loc, cudaMemcpyDeviceToHost));
+    if (loc < 0) return SBV_ERR_ARG;
+    const size_t words = SBV_ED_BTAB_ENTRY_WORDS, per_key = SBV_ED_BTAB_ENTRIES * words;
+    CU(e, cudaMemcpyAsync(out, d.ed_ktab + (size_t)loc * per_key + first * words, count * words * 4, cudaMemcpyDeviceToHost, d.stream));
+    CU(e, cudaStreamSynchronize(d.stream));
+    return SBV_OK;
+}
+
+// The production registered-key kernel (k_ed_verify_keyed) on device 0 with the caller's k in place of SHA-512(R || A || M)
+// mod L: k = 8 little-endian limbs per item, each < L (SBV_ERR_ARG otherwise), key_slot = registry slots, sig = R || S.
+extern "C" int sbv_debug_ed25519_verify_registered_k(sbv_engine *e, size_t n, const uint32_t *key_slot, const uint8_t *sig, const uint32_t *k,
+                                                     uint8_t *ok) {
+    if (!e || !key_slot || !sig || !k || !ok || n > UINT32_MAX) return SBV_ERR_ARG;
+    static const uint32_t L[8] = {0x5cf5d3ed, 0x5812631a, 0xa2f79cd6, 0x14def9de, 0, 0, 0, 0x10000000};
+    for (size_t i = 0; i < n; i++) {
+        int w = 7;
+        while (w > 0 && k[i * 8 + w] == L[w]) w--;
+        if (k[i * 8 + w] >= L[w]) return SBV_ERR_ARG;
+    }
+    if (n == 0) return SBV_OK;
+    std::lock_guard<std::mutex> lk(e->mu);
+    Dev &d = e->devs[0];
+    CU(e, cudaSetDevice(d.ordinal));
+    int rc = sbv_ed_btab_ensure(e, d);
+    if (rc) return rc;
+    const size_t okb = (n + 255) & ~(size_t)255;
+    if ((rc = sbv_ensure_scratch(e, d, n * 64 + n * 4 + n * 32 + okb + 1024))) return rc;
+    uint8_t *p = d.d_scratch;
+    uint8_t *dsig = p; p += n * 64;
+    uint32_t *dk = (uint32_t *)p; p += n * 32;
+    uint32_t *dslot = (uint32_t *)p; p += (n * 4 + 15) & ~(size_t)15;
+    uint8_t *dok = p;
+    std::vector<uint32_t> kw(n * 8);
+    for (size_t i = 0; i < n; i++)
+        for (int w = 0; w < 8; w++) kw[(size_t)w * n + i] = k[i * 8 + w];
+    CU(e, cudaMemcpyAsync(dsig, sig, n * 64, cudaMemcpyHostToDevice, d.stream));
+    CU(e, cudaMemcpyAsync(dk, kw.data(), n * 32, cudaMemcpyHostToDevice, d.stream));
+    CU(e, cudaMemcpyAsync(dslot, key_slot, n * 4, cudaMemcpyHostToDevice, d.stream));
+    if ((rc = sbv_launch_ed_verify_registered_k(e, d, n, dslot, dsig, dk, dok, d.stream))) return rc;
+    CU(e, cudaMemcpyAsync(ok, dok, n, cudaMemcpyDeviceToHost, d.stream));
+    CU(e, cudaStreamSynchronize(d.stream));
+    return SBV_OK;
+}

@@ -376,6 +376,13 @@ SBV_DEV int ed_digit8(const uint8_t *__restrict__ s, int win) {
     const uint32_t prev = win ? (uint32_t)(__ldg(s + win - 1) >> 7) : 0u;
     return (int)(w & 127u) - (int)(w & 128u) + (int)prev;
 }
+// 8-bit Booth digit `win` of a word-major scalar k[w * n + idx] (k < L, so window 31 carries nothing out), in [-128, 128]
+SBV_DEV int ed_digit8w(const uint32_t *__restrict__ k, uint32_t n, uint32_t idx, int win) {
+    const uint32_t w = (__ldg(k + (size_t)(win >> 2) * n + idx) >> (8 * (win & 3))) & 255u;
+    const int pos = 8 * win - 1;
+    const uint32_t prev = win ? (__ldg(k + (size_t)(pos >> 5) * n + idx) >> (pos & 31)) & 1u : 0u;
+    return (int)(w & 127u) - (int)(w & 128u) + (int)prev;
+}
 
 static __device__ __noinline__ EdFe ed_fmul_call(EdFe a, EdFe b) {
     EdFe r;

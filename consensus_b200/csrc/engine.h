@@ -8,6 +8,7 @@
 #include <cstdint>
 #include <condition_variable>
 #include <mutex>
+#include <shared_mutex>
 #include <string>
 #include <vector>
 
@@ -84,6 +85,12 @@ struct Dev {
     uint8_t *keyflags[2] = {nullptr, nullptr};
     int32_t *slot2local[2] = {nullptr, nullptr};
     uint32_t n_slots = 0, n_local[2] = {0, 0};
+    // registered Ed25519 keys (sbv_ed25519_set_keys): the registered bytes of every slot (32 each), slot -> table index
+    // (-1: the key does not decode) and one fixed-base table per decodable key (ed25519_keyed.cuh)
+    uint8_t *ed_kpub = nullptr;
+    int32_t *ed_slot2local = nullptr;
+    uint32_t *ed_ktab = nullptr;
+    uint32_t ed_n_slots = 0, ed_n_local = 0;
     // profiling: event quadruples per verify launch (start, after prep, before / after the dominant kernel)
     std::vector<cudaEvent_t> prof_events;
     size_t prof_used = 0;
@@ -93,6 +100,9 @@ struct sbv_engine {
     std::vector<Dev> devs;
     std::mutex mu;       // kernel enqueue + workspace growth
     std::mutex err_mu;   // last-error string
+    // the Ed25519 registry: sbv_ed25519_set_keys holds it exclusively, sbv_ed25519_verify_registered shared for the
+    // enqueue of all its shards, so every shard of one call reads the same registry (taken before mu, never inside it)
+    std::shared_mutex ed_reg_mu;
     std::condition_variable lane_cv;
     bool lane_busy[SBV_LANES] = {};
     std::string err;
@@ -184,6 +194,17 @@ int sbv_launch_ed_sha512_digest(sbv_engine *e, size_t n, const uint8_t *d_msgs, 
 // test hook: k_ed_verify with the caller's k (word-major [8][n], every k < L); the table of B must exist
 int sbv_launch_ed_verify_k(sbv_engine *e, Dev &d, size_t n, const uint8_t *d_sig, const uint8_t *d_pub, const uint32_t *d_k, uint8_t *d_ok,
                            cudaStream_t st);
+// registered Ed25519 keys.  sbv_ed_keys_build: caller holds e->mu; waits for the device to drain, frees the old registry of
+// device d and builds one from the n keys of pub (host, 32 bytes each); a fault leaves d's registry empty.
+int sbv_ed_keys_build(sbv_engine *e, Dev &d, size_t n, const uint8_t *pub);
+void sbv_ed_keys_free(Dev &d);
+// k_ed_key_gather (registered bytes of each item's slot into d_pub, 32n bytes), SHA-512 into d_k, then k_ed_verify_keyed.
+// Caller holds e->mu (the registry is read at enqueue time); the table of B must exist.
+int sbv_launch_ed25519_registered(sbv_engine *e, Dev &d, size_t n, const uint8_t *d_msgs, const uint64_t *d_off, uint64_t base, const uint32_t *d_slot,
+                                  const uint8_t *d_sig, uint8_t *d_pub, uint32_t *d_k, uint32_t *d_perm, uint8_t *d_ok, cudaStream_t st);
+// test hook: k_ed_verify_keyed with the caller's k (word-major [8][n], every k < L); caller holds e->mu
+int sbv_launch_ed_verify_registered_k(sbv_engine *e, Dev &d, size_t n, const uint32_t *d_slot, const uint8_t *d_sig, const uint32_t *d_k, uint8_t *d_ok,
+                                      cudaStream_t st);
 // shape of the table of B (ed25519_verify.cuh: ED_BWINS x ED_BENT entries of ED_BWORDS words; checked in inst_ed25519.cu)
 constexpr size_t SBV_ED_BTAB_ENTRIES = 32 * 128, SBV_ED_BTAB_ENTRY_WORDS = 24;
 

@@ -112,6 +112,20 @@ int sbv_verify_mixed(sbv_engine *e, size_t n, const uint8_t *curve_tag, const ui
 int sbv_ed25519_verify_batch(sbv_engine *e, size_t n, const uint8_t *msgs, const uint64_t *msg_off, const uint8_t *sig,
                              const uint8_t *pub, uint8_t *ok);
 
+/* Ed25519 key registry.  Consenter and client keys are configuration: they change only with a reconfiguration
+ * (api.Verifier, dependencies.go:58-66).  sbv_ed25519_set_keys replaces the registry: slot i = the 32-byte encoding
+ * pub[32i..32i+32); n = 0 empties it.  On every device it builds a fixed-base table per decodable key (8-bit signed
+ * windows: 32 x 128 affine points = 384 KiB per key per device).  It waits for the launches that may still read the old
+ * tables.  Independent of sbv_set_keys: neither call touches the other's registry.  A fault leaves the registry empty. */
+int sbv_ed25519_set_keys(sbv_engine *e, size_t n, const uint8_t *pub);
+/* sbv_ed25519_verify_batch with the key of item i taken from registry slot key_slot[i].  Same accept set: k hashes the
+ * 32 bytes registered in the slot, not a re-encoding; a slot >= n, a registered key that does not decode and an empty
+ * registry reject.  [k]A is fixed-base (32 additions, no doublings and no key decoding).  Every shard of one call, on
+ * every device, reads the same registry: a concurrent sbv_ed25519_set_keys waits until the calls already enqueueing have
+ * enqueued all their shards (and then for their kernels), and calls that start after it see the new registry. */
+int sbv_ed25519_verify_registered(sbv_engine *e, size_t n, const uint8_t *msgs, const uint64_t *msg_off,
+                                  const uint32_t *key_slot, const uint8_t *sig, uint8_t *ok);
+
 /* Distinct-signer quorum count per consensus instance (processCommits, view.go:519-551).
  * Votes are given in arrival order.  A vote is registered iff signer == sender and sender !=
  * self_id[instance] and the sender has no earlier registered vote in the instance

@@ -29,13 +29,12 @@ import (
 )
 
 // item is one unit of engine work: verify (r, s) under registry slot `slot` over SHA-256(msg), or, when ed is set,
-// the Ed25519 signature edSig under the key edPub over msg (crypto/ed25519.Verify).
+// the Ed25519 signature edSig under slot `slot` of the Ed25519 registry over msg (crypto/ed25519.Verify).
 type item struct {
 	r, s  [32]byte
 	slot  uint32
 	msg   []byte
 	ed    bool
-	edPub [32]byte
 	edSig [64]byte
 }
 
@@ -49,9 +48,12 @@ type Verifier struct {
 	slots      map[[64]byte]uint32 // key -> slot
 	consenters map[uint64]uint32
 	clients    map[string]uint32
-	edKeys     map[uint64][32]byte // consenters with crypto/ed25519 keys: verified by sbv_ed25519_verify_batch
-	edClients  map[string][32]byte // clients with crypto/ed25519 keys
-	dirty      bool
+	edRegistry [][32]byte          // Ed25519 slot -> key, as the consenter or client registered it
+	edSlots    map[[32]byte]uint32 // Ed25519 key -> slot
+	edKeys     map[uint64]uint32   // consenters with crypto/ed25519 keys: their Ed25519 slot
+	edClients  map[string]uint32   // clients with crypto/ed25519 keys: their Ed25519 slot
+	dirty      bool                // the ECDSA registry differs from the engine's
+	edDirty    bool                // the Ed25519 registry differs from the engine's
 
 	pool sync.Pool // *pinned: one block of page-locked memory per in-flight batch
 
@@ -69,7 +71,7 @@ func New(devices []int) (*Verifier, error) {
 		return nil, fmt.Errorf("sbv_create failed: %d (there is no CPU fallback)", int(rc))
 	}
 	v := &Verifier{eng: eng, slots: map[[64]byte]uint32{}, consenters: map[uint64]uint32{}, clients: map[string]uint32{},
-		edKeys: map[uint64][32]byte{}, edClients: map[string][32]byte{}}
+		edSlots: map[[32]byte]uint32{}, edKeys: map[uint64]uint32{}, edClients: map[string]uint32{}}
 	v.pool.New = func() interface{} { return &pinned{} }
 	v.agg = newAggregator(v.engineBatch, 200*time.Microsecond, 65536)
 	return v, nil
@@ -95,6 +97,17 @@ func (v *Verifier) slotOf(xy [64]byte) uint32 { // v.mu held
 	return s
 }
 
+func (v *Verifier) edSlotOf(pub [32]byte) uint32 { // v.mu held
+	if s, ok := v.edSlots[pub]; ok {
+		return s
+	}
+	s := uint32(len(v.edRegistry))
+	v.edRegistry = append(v.edRegistry, pub)
+	v.edSlots[pub] = s
+	v.edDirty = true
+	return s
+}
+
 // A consenter or client holds one key: setting a key of one type removes any key of the other type it held, so a
 // signature is never checked under a key the configuration no longer gives it.
 func (v *Verifier) SetConsenterKey(id uint64, xy [64]byte) {
@@ -115,38 +128,54 @@ func (v *Verifier) SetVerificationSequence(s uint64) { v.mu.Lock(); v.verSeq = s
 // ECDSA ones). Its signatures are 64 raw bytes R || S over the message itself (no prehash).
 func (v *Verifier) SetConsenterEd25519Key(id uint64, pub [32]byte) {
 	v.mu.Lock()
-	v.edKeys[id] = pub
+	v.edKeys[id] = v.edSlotOf(pub)
 	delete(v.consenters, id)
 	v.mu.Unlock()
 }
 
 // SetClientEd25519Key: client `c` signs its requests with crypto/ed25519; the signature field of its requests is the
-// 64-byte R || S over the signed bytes of the request.
+// 64-byte R || S over the signed bytes of the request. The key is registered: a key the registry has not seen yet makes
+// the next flush rebuild the Ed25519 registry (see ResetKeys for the cost).
 func (v *Verifier) SetClientEd25519Key(c string, pub [32]byte) {
 	v.mu.Lock()
-	v.edClients[c] = pub
+	v.edClients[c] = v.edSlotOf(pub)
 	delete(v.clients, c)
 	v.mu.Unlock()
 }
 
 // ResetKeys drops every key, ECDSA and Ed25519, of consenters and clients. Keys change only with a reconfiguration, i.e. a new verification
 // sequence (dependencies.go:65-66): the application calls ResetKeys, re-registers the new configuration's keys
-// and bumps the sequence, so rotated keys do not pile up in HBM (264 KiB per key and GPU). Client keys of high
-// cardinality should not be registered at all: sbv_hash_verify_batch takes the key with every item and groups
-// the repeated ones on the device.
+// and bumps the sequence, so rotated keys do not pile up in HBM (264 KiB per P-256 key and 384 KiB per Ed25519 key,
+// per GPU). ECDSA client keys of high cardinality should not be registered at all: sbv_hash_verify_batch takes the
+// key with every item and groups the repeated ones on the device. Ed25519 client keys are always registered
+// (SetClientEd25519Key): each new key costs 384 KiB per GPU and makes the next flush rebuild every Ed25519 table
+// (about 8 ms per thousand keys), so a deployment whose Ed25519 clients come and go between reconfigurations should
+// verify their requests with sbv_ed25519_verify_batch instead.
 func (v *Verifier) ResetKeys() {
 	v.mu.Lock()
 	v.registry, v.slots = nil, map[[64]byte]uint32{}
 	v.consenters, v.clients = map[uint64]uint32{}, map[string]uint32{}
-	v.edKeys, v.edClients = map[uint64][32]byte{}, map[string][32]byte{}
-	v.dirty = true
+	v.edRegistry, v.edSlots = nil, map[[32]byte]uint32{}
+	v.edKeys, v.edClients = map[uint64]uint32{}, map[string]uint32{}
+	v.dirty, v.edDirty = true, true
 	v.mu.Unlock()
 }
 
-// syncRegistry pushes the key registry to the engine (sbv_set_keys builds one comb table per key).
+// syncRegistry pushes the key registries that changed to the engine (sbv_set_keys builds one comb table per ECDSA
+// key, sbv_ed25519_set_keys one fixed-base table per Ed25519 key).
 func (v *Verifier) syncRegistry() {
 	v.mu.Lock()
 	defer v.mu.Unlock()
+	if v.edDirty {
+		var pub *C.uint8_t
+		if len(v.edRegistry) > 0 {
+			pub = (*C.uint8_t)(unsafe.Pointer(&v.edRegistry[0][0]))
+		}
+		if rc := C.sbv_ed25519_set_keys(v.eng, C.size_t(len(v.edRegistry)), pub); rc != 0 {
+			v.fault("sbv_ed25519_set_keys", rc)
+		}
+		v.edDirty = false
+	}
 	if !v.dirty {
 		return
 	}
@@ -194,7 +223,7 @@ func (b *pinned) reserve(n int) []byte {
 }
 
 // engineBatch dispatches an aggregated batch by key type: the ECDSA items in one sbv_hash_verify_registered call,
-// the Ed25519 items in one sbv_ed25519_verify_batch call; verdicts come back in the items' order.
+// the Ed25519 items in one sbv_ed25519_verify_registered call; verdicts come back in the items' order.
 func (v *Verifier) engineBatch(items []item) []byte {
 	var ec, ed []item
 	var ecAt, edAt []int
@@ -219,17 +248,18 @@ func (v *Verifier) engineBatch(items []item) []byte {
 	return ok
 }
 
-// ed25519Batch: SHA-512(R || A || M) and the Ed25519 equation of every item on the GPU. Marshalled into pinned
-// memory: sig (64n) | pub (32n) | off | msgs.
+// ed25519Batch: SHA-512(R || A || M) over the registered bytes of each item's key and the Ed25519 equation over the
+// key's fixed-base table, both on the GPU. Marshalled into pinned memory: sig (64n) | slot (4n) | off | msgs.
 func (v *Verifier) ed25519Batch(items []item) []byte {
+	v.syncRegistry()
 	n := len(items)
 	ok := make([]byte, n)
 	total := 0
 	for i := range items {
 		total += len(items[i].msg)
 	}
-	oPub := 64 * n
-	oOff := oPub + 32*n
+	oSlot := 64 * n
+	oOff := (oSlot + 4*n + 7) &^ 7
 	oMsgs := oOff + 8*(n+1)
 	pb := v.pool.Get().(*pinned)
 	defer v.pool.Put(pb)
@@ -238,17 +268,17 @@ func (v *Verifier) ed25519Batch(items []item) []byte {
 	binary.LittleEndian.PutUint64(buf[oOff:], 0)
 	for i := range items {
 		copy(buf[64*i:], items[i].edSig[:])
-		copy(buf[oPub+32*i:], items[i].edPub[:])
+		binary.LittleEndian.PutUint32(buf[oSlot+4*i:], items[i].slot)
 		copy(buf[oMsgs+pos:], items[i].msg)
 		pos += len(items[i].msg)
 		binary.LittleEndian.PutUint64(buf[oOff+8*(i+1):], uint64(pos))
 	}
 	base := uintptr(pb.p)
-	rc := C.sbv_ed25519_verify_batch(v.eng, C.size_t(n), (*C.uint8_t)(unsafe.Pointer(base+uintptr(oMsgs))),
-		(*C.uint64_t)(unsafe.Pointer(base+uintptr(oOff))), (*C.uint8_t)(unsafe.Pointer(base)),
-		(*C.uint8_t)(unsafe.Pointer(base+uintptr(oPub))), (*C.uint8_t)(unsafe.Pointer(&ok[0])))
+	rc := C.sbv_ed25519_verify_registered(v.eng, C.size_t(n), (*C.uint8_t)(unsafe.Pointer(base+uintptr(oMsgs))),
+		(*C.uint64_t)(unsafe.Pointer(base+uintptr(oOff))), (*C.uint32_t)(unsafe.Pointer(base+uintptr(oSlot))),
+		(*C.uint8_t)(unsafe.Pointer(base)), (*C.uint8_t)(unsafe.Pointer(&ok[0])))
 	if rc != 0 {
-		v.fault("sbv_ed25519_verify_batch", rc)
+		v.fault("sbv_ed25519_verify_registered", rc)
 	}
 	return ok
 }
@@ -345,13 +375,13 @@ func parseDER(sig []byte) (r, s [32]byte, ok bool) {
 func (v *Verifier) consenterItem(sig types.Signature) (item, error) {
 	v.mu.RLock()
 	slot, known := v.consenters[sig.ID]
-	edPub, isEd := v.edKeys[sig.ID]
+	edSlot, isEd := v.edKeys[sig.ID]
 	v.mu.RUnlock()
 	if isEd {
 		if len(sig.Value) != 64 { // crypto/ed25519.Verify rejects any other length
 			return item{}, fmt.Errorf("malformed signature from %d", sig.ID)
 		}
-		it := item{ed: true, edPub: edPub, msg: sig.Msg}
+		it := item{ed: true, slot: edSlot, msg: sig.Msg}
 		copy(it.edSig[:], sig.Value)
 		return it, nil
 	}
@@ -455,14 +485,14 @@ func (v *Verifier) requestItem(val []byte) (item, types.RequestInfo, error) {
 	}
 	v.mu.RLock()
 	slot, known := v.clients[client]
-	edPub, isEd := v.edClients[client]
+	edSlot, isEd := v.edClients[client]
 	v.mu.RUnlock()
 	info := types.RequestInfo{ClientID: client, ID: id}
 	if isEd {
 		if len(sig) != 64 { // crypto/ed25519.Verify rejects any other length
 			return item{}, types.RequestInfo{}, errors.New("malformed request signature")
 		}
-		it := item{ed: true, edPub: edPub, msg: signed}
+		it := item{ed: true, slot: edSlot, msg: signed}
 		copy(it.edSig[:], sig)
 		return it, info, nil
 	}

@@ -1,10 +1,13 @@
-"""Ed25519 throughput of sbv_ed25519_verify_batch through the C ABI, with the OpenSSL CPU arm measured in the same run.
+"""Ed25519 throughput through the C ABI: sbv_ed25519_verify_batch (keys per item) and sbv_ed25519_verify_registered (the
+corpus's distinct keys registered with sbv_ed25519_set_keys, items by slot), timed in the same run and alternated step by
+step, with the OpenSSL CPU arm measured in the same run.
 
     python tools/ed25519_bench.py [--n 65536] [--keys 1024] [--msg-len 256] [--steps 20] [--warmup 5]
 
 Inputs live in pinned host memory (sbv_host_alloc); each timed call uploads them, hashes, verifies and returns the
-verdicts.  Kernel times of k_ed_sha512 and k_ed_verify come from a separate torch.profiler run.  Prints one JSON line;
-the verdicts of every timed call are checked against the oracle.
+verdicts.  Kernel times of k_ed_sha512, k_ed_verify, k_ed_key_gather and k_ed_verify_keyed come from a separate
+torch.profiler run; sbv_ed25519_set_keys is timed on its first and second call.  Prints one JSON line; the verdicts of
+every timed call are checked against the oracle.
 """
 from __future__ import annotations
 
@@ -12,6 +15,7 @@ import argparse
 import ctypes as C
 import json
 import os
+import re
 import subprocess
 import sys
 import time
@@ -63,27 +67,40 @@ def main():
         return ptr
 
     n = args.n
+    keys, slot = np.unique(c["pub"], axis=0, return_inverse=True)
+    slot = slot.reshape(-1).astype(np.uint32)
     m, o, s, p, ok = pinned(c["msgs"]), pinned(c["off"]), pinned(c["sig"]), pinned(c["pub"]), pinned(np.zeros(n, np.uint8))
+    sl = pinned(slot)
     okv = np.ctypeslib.as_array((C.c_uint8 * n).from_address(ok))
     try:
-        for _ in range(args.warmup):
-            eng.ed25519_verify_batch_ptr(n, m, o, s, p, ok)
-        times, verdicts_ok = [], True
-        for _ in range(args.steps):
-            okv[:] = 2
+        set_keys_ms = []
+        for _ in range(2):  # the first call on a fresh engine also loads the kernels; the second replaces a full registry
             t0 = time.perf_counter()
-            eng.ed25519_verify_batch_ptr(n, m, o, s, p, ok)
-            times.append(time.perf_counter() - t0)
-            verdicts_ok &= bool(np.array_equal(okv, want))
+            eng.ed25519_set_keys(keys)
+            set_keys_ms.append((time.perf_counter() - t0) * 1e3)
+        arms = {"per_item": lambda: eng.ed25519_verify_batch_ptr(n, m, o, s, p, ok),
+                "registered": lambda: eng.ed25519_verify_registered_ptr(n, m, o, sl, s, ok)}
+        for _ in range(args.warmup):
+            for f in arms.values():
+                f()
+        times, verdicts_ok = {a: [] for a in arms}, True
+        for step in range(args.steps):
+            for a in (("per_item", "registered") if step % 2 == 0 else ("registered", "per_item")):
+                okv[:] = 2
+                t0 = time.perf_counter()
+                arms[a]()
+                times[a].append(time.perf_counter() - t0)
+                verdicts_ok &= bool(np.array_equal(okv, want))
         from torch.profiler import ProfilerActivity, profile
         with profile(activities=[ProfilerActivity.CUDA]) as prof:
             for _ in range(3):
-                eng.ed25519_verify_batch_ptr(n, m, o, s, p, ok)
+                for f in arms.values():
+                    f()
             torch.cuda.synchronize()
         kern = {}
         for ev in prof.key_averages():
-            for name in ("k_ed_sha512", "k_ed_verify"):
-                if name in ev.key:
+            for name in ("k_ed_sha512", "k_ed_verify", "k_ed_key_gather", "k_ed_verify_keyed"):
+                if re.search(r"\b" + name + r"\b", ev.key):
                     t = getattr(ev, "device_time", None) or getattr(ev, "cuda_time", 0.0)  # average µs per call
                     kern[name + "_us"] = round(float(t), 1)
         verdicts_ok &= bool(np.array_equal(okv, want))
@@ -93,7 +110,8 @@ def main():
             lib.sbv_host_free(C.c_void_p(ptr))
     cores = oe.ncores()
     cpu_s, cpu_ok = oe.bench_verify(c["msgs"], c["off"], c["sig"], c["pub"], nthreads=cores)
-    med = float(np.median(times))
+    med = float(np.median(times["per_item"]))
+    med_reg = float(np.median(times["registered"]))
     props = torch.cuda.get_device_properties(0)
     res = {
         "metric": "ed25519_verifies_per_s",
@@ -101,7 +119,13 @@ def main():
         "unit": "verifies/s",
         "n": n, "keys": args.keys, "msg_len": args.msg_len, "steps": args.steps, "warmup": args.warmup,
         "median_call_ms": med * 1e3,
-        "best_call_ms": min(times) * 1e3,
+        "best_call_ms": min(times["per_item"]) * 1e3,
+        "registered_verifies_per_s": n / med_reg,
+        "registered_median_call_ms": med_reg * 1e3,
+        "registered_best_call_ms": min(times["registered"]) * 1e3,
+        "registered_keys": int(keys.shape[0]),
+        "set_keys_first_ms": round(set_keys_ms[0], 2),
+        "set_keys_second_ms": round(set_keys_ms[1], 2),
         **kern,
         "cpu_openssl_verifies_per_s": n / cpu_s,
         "cpu_cores": cores,

@@ -3,6 +3,7 @@
 // big integers and with the oracle, so limb-level mistakes are caught without a GPU.  Not linked into libsbv.so.
 #define SBV_HOSTSIM 1
 #include <stdint.h>
+#include <algorithm>
 #include <stdlib.h>
 #include <string.h>
 #include <thread>
@@ -20,6 +21,7 @@ namespace sbv { uint32_t tab[1 << 18]; }
 #include "../../consensus_b200/csrc/ed25519_debug.cuh"
 #include "../../consensus_b200/csrc/sha512.cuh"
 #include "../../consensus_b200/csrc/ed25519_verify.cuh"
+#include "../../consensus_b200/csrc/ed25519_keyed.cuh"
 
 using namespace sbv;
 
@@ -350,5 +352,78 @@ extern "C" int hs_ed25519_verify_k(size_t n, const uint8_t *sig, const uint8_t *
     }
     const uint4 *bt = reinterpret_cast<const uint4 *>(ed_btab_host().data());
     run_grid((unsigned)((n + 31) / 32), 32, [&] { k_ed_verify<32>((uint32_t)n, sig, pub, k.data(), bt, ok); });
+    return 0;
+}
+
+// ---- registered Ed25519 keys (ed25519_keyed.cuh) ----
+// The registry of sbv_ed25519_set_keys, built by the same kernels: the registered bytes of every slot, slot -> table
+// (-1: the key does not decode) and one table per decodable key.
+static struct {
+    std::vector<uint4> pub;  // 2 per slot (16-byte aligned, as cudaMalloc gives it)
+    std::vector<int32_t> slot2local;
+    std::vector<uint32_t> ktab;
+    uint32_t n = 0;
+} g_edk;
+
+// chunk: keys per k_ed_ktab_build launch, as ed_keys_fill (inst_ed25519.cu) splits them; 0 = ED_KBUILD_MAX
+extern "C" int hs_ed25519_set_keys(size_t n, const uint8_t *pub, uint32_t chunk) {
+    g_edk.pub.assign(2 * n + 2, uint4{0, 0, 0, 0});
+    if (n) memcpy(g_edk.pub.data(), pub, n * 32);
+    const uint8_t *kp = reinterpret_cast<const uint8_t *>(g_edk.pub.data());
+    std::vector<uint32_t> xy(16 * n + 16);
+    std::vector<uint8_t> flag(n + 1);
+    run_grid((unsigned)((n + 63) / 64), 64, [&] { k_ed_kdecode((uint32_t)n, kp, xy.data(), flag.data()); });
+    g_edk.slot2local.assign(n + 1, -1);
+    std::vector<uint32_t> slot_of;
+    for (size_t i = 0; i < n; i++)
+        if (flag[i]) { g_edk.slot2local[i] = (int32_t)slot_of.size(); slot_of.push_back((uint32_t)i); }
+    const uint32_t cnt = (uint32_t)slot_of.size();
+    g_edk.ktab.assign((size_t)cnt * ED_KTAB_WORDS + 4, 0);
+    const uint32_t per = std::min(cnt, chunk ? chunk : ED_KBUILD_MAX);
+    std::vector<uint32_t> pref((size_t)per * ED_BWINS * ED_BENT * 8 + 1);
+    for (uint32_t c0 = 0; c0 < cnt; c0 += per) {
+        const uint32_t cc = std::min(per, cnt - c0);
+        run_grid((cc * ED_BWINS + 63) / 64, 64,
+                 [&] { k_ed_ktab_build(cc, slot_of.data() + c0, xy.data(), g_edk.ktab.data() + (size_t)c0 * ED_KTAB_WORDS, pref.data()); });
+    }
+    g_edk.n = (uint32_t)n;
+    return 0;
+}
+// the whole table (32 x 128 entries of 24 words) of a registered slot; -1 for an unknown slot or a key that does not decode
+extern "C" int hs_ed25519_ktab(uint32_t slot, uint32_t *out) {
+    if (slot >= g_edk.n || g_edk.slot2local[slot] < 0) return -1;
+    memcpy(out, g_edk.ktab.data() + (size_t)g_edk.slot2local[slot] * ED_KTAB_WORDS, ED_KTAB_WORDS * 4);
+    return 0;
+}
+static void ed_verify_keyed_host(size_t n, const uint32_t *key_slot, const uint8_t *sig, const uint32_t *k, uint8_t *ok) {
+    const uint4 *bt = reinterpret_cast<const uint4 *>(ed_btab_host().data());
+    const uint4 *kt = reinterpret_cast<const uint4 *>(g_edk.ktab.data());
+    run_grid((unsigned)((n + 127) / 128), 128,
+             [&] { k_ed_verify_keyed<128>((uint32_t)n, sig, key_slot, g_edk.n, g_edk.slot2local.data(), kt, k, bt, ok); });
+}
+// the pipeline of sbv_ed25519_verify_registered on one device: k_ed_key_gather, k_ed_sha512, k_ed_verify_keyed
+extern "C" int hs_ed25519_verify_registered(size_t n, const uint8_t *msgs, const uint64_t *off, const uint32_t *key_slot, const uint8_t *sig,
+                                            uint8_t *ok) {
+    std::vector<uint4> pub(2 * n + 2);
+    run_grid((unsigned)((2 * n + 255) / 256), 256,
+             [&] { k_ed_key_gather((uint32_t)n, key_slot, g_edk.n, g_edk.pub.data(), pub.data()); });
+    std::vector<uint32_t> k(8 * n + 8);
+    const uint8_t *pb = reinterpret_cast<const uint8_t *>(pub.data());
+    run_grid((unsigned)((n + 127) / 128), 128, [&] { k_ed_sha512((uint32_t)n, sig, pb, msgs, off, 0, k.data(), nullptr, nullptr); });
+    ed_verify_keyed_host(n, key_slot, sig, k.data(), ok);
+    return 0;
+}
+// k_ed_verify_keyed alone with the caller's k (8 little-endian limbs per item, each < L; -1 otherwise), as
+// sbv_debug_ed25519_verify_registered_k runs it on the device
+extern "C" int hs_ed25519_verify_registered_k(size_t n, const uint32_t *key_slot, const uint8_t *sig, const uint32_t *k_in, uint8_t *ok) {
+    uint32_t Lm[8];
+    ed_order(Lm);
+    std::vector<uint32_t> k(8 * n + 8);
+    for (size_t i = 0; i < n; i++) {
+        uint32_t ki[8];
+        for (int w = 0; w < 8; w++) k[(size_t)w * n + i] = ki[w] = k_in[i * 8 + w];
+        if (!mp_lt<8>(ki, Lm)) return -1;
+    }
+    ed_verify_keyed_host(n, key_slot, sig, k.data(), ok);
     return 0;
 }
