@@ -25,7 +25,7 @@ SYMBOLS = [
     "sbv_verify_registered_device", "sbv_hash_verify_registered", "sbv_prepare_quorum", "sbv_verify_quorum",
     "sbv_comm_unique_id", "sbv_comm_init_rank", "sbv_comm_ranks", "sbv_gather_verdicts_device", "sbv_gather_words_device",
     "sbv_verify_batch_ranked", "sbv_host_alloc", "sbv_host_free", "sbv_ed25519_verify_batch",
-    "sbv_ed25519_set_keys", "sbv_ed25519_verify_registered",
+    "sbv_ed25519_set_keys", "sbv_ed25519_verify_registered", "sbv_ed25519_verify_quorum",
 ]
 
 
@@ -273,6 +273,44 @@ class Engine:
         vp = C.c_void_p
         self._check(self._lib.sbv_ed25519_verify_registered(self._h, C.c_size_t(n), vp(msgs), vp(off), vp(key_slot), vp(sig), vp(ok)),
                     "sbv_ed25519_verify_registered")
+
+    def ed25519_verify_quorum(self, msgs, off, key_slot, sig, instance, sender, signer, digest_match, n_instances, threshold,
+                              self_id=None):
+        """Ed25519 commit votes against registered keys (ed25519_set_keys): signatures verified, verdicts counted on the
+        device.  msgs concatenated with off[n+1] byte offsets, sig = n x 64 bytes (R || S), votes grouped by
+        non-decreasing instance.  Returns (ok, valid_count, reached)."""
+        msgs = _u8(msgs if len(msgs) else np.zeros(1, np.uint8))
+        off = np.ascontiguousarray(off, dtype=np.uint64)
+        key_slot = np.ascontiguousarray(key_slot, dtype=np.uint32)
+        instance = np.ascontiguousarray(instance, dtype=np.uint32)
+        sender = np.ascontiguousarray(sender, dtype=np.uint16)
+        signer = np.ascontiguousarray(signer, dtype=np.uint16)
+        sig, digest_match = _u8(sig), _u8(digest_match)
+        n = instance.size
+        if off.size != n + 1 or sig.size != 64 * n or key_slot.size != n or sender.size != n or signer.size != n or digest_match.size != n:
+            raise ValueError("off must hold n + 1 offsets, sig 64 bytes and every other column one entry per vote")
+        ok = np.zeros(n, np.uint8)
+        cnt = np.zeros(n_instances, np.uint32)
+        reached = np.zeros(n_instances, np.uint8)
+        sid = None
+        if self_id is not None:
+            self_id = np.ascontiguousarray(self_id, dtype=np.uint16)
+            sid = self_id.ctypes.data_as(C.POINTER(C.c_uint16))
+        u16 = lambda a: a.ctypes.data_as(C.POINTER(C.c_uint16))
+        u32 = lambda a: a.ctypes.data_as(C.POINTER(C.c_uint32))
+        self._check(self._lib.sbv_ed25519_verify_quorum(self._h, C.c_size_t(n), _p8(msgs), off.ctypes.data_as(C.POINTER(C.c_uint64)), u32(key_slot),
+                                                        _p8(sig), u32(instance), u16(sender), u16(signer), _p8(digest_match),
+                                                        C.c_size_t(n_instances), sid, C.c_uint32(threshold), _p8(ok), u32(cnt), _p8(reached)),
+                    "sbv_ed25519_verify_quorum")
+        return ok, cnt, reached
+
+    def ed25519_verify_quorum_ptr(self, n, msgs, off, key_slot, sig, instance, sender, signer, digest_match, n_instances, self_id, threshold,
+                                  ok, valid_count, reached):
+        """Raw host pointers (ints; self_id may be None) — used with pinned buffers."""
+        vp = C.c_void_p
+        self._check(self._lib.sbv_ed25519_verify_quorum(self._h, C.c_size_t(n), vp(msgs), vp(off), vp(key_slot), vp(sig), vp(instance), vp(sender),
+                                                        vp(signer), vp(digest_match), C.c_size_t(n_instances), vp(self_id), C.c_uint32(threshold),
+                                                        vp(ok), vp(valid_count), vp(reached)), "sbv_ed25519_verify_quorum")
 
     def verify_mixed(self, curve_tag, r48, s48, qx48, qy48, digest32) -> np.ndarray:
         curve_tag, r48, s48, qx48, qy48, digest32 = map(_u8, (curve_tag, r48, s48, qx48, qy48, digest32))

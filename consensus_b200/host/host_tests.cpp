@@ -423,6 +423,104 @@ static void TestGpuVerifierEndToEnd() {
     EC_KEY_free(ck.k);
 }
 
+// Ed25519 commits from the wire (marshal.hpp, CommitBatch::Ed25519): three instances with the Byzantine cases of the
+// CommitBatch block above, plus a Commit without a Signature, a 63-byte Value, an unknown signer and a Signer beyond 16
+// bits.  Without a GPU only the decoding rules are checked: which votes are inert and which are registered with a
+// rejecting row.  On the GPU one sbv_ed25519_verify_quorum call is compared vote by vote with the VoteSet restatement.
+static bool g_gpu = false;  // `host_tests gpu`
+static void TestEd25519CommitBatch() {
+    std::map<uint64_t, TestEdKey> keys;
+    for (uint64_t id = 1; id <= 16; id++) keys[id] = makeEdKey();
+    auto slot_of = [](uint64_t signer) { return signer >= 1 && signer <= 16 ? (int)signer - 1 : -1; };
+    int q, f; computeQuorum(16, q, f);
+    Proposal last{{9}, {8}, ViewMetadata{0, 7, 0}.Marshal(), 1};
+    std::vector<Proposal> props3 = {fixtureProposal(), last, Proposal{{7, 7}, {1}, ViewMetadata{2, 9, 1}.Marshal(), 1}};
+    Bytes aux = PreparesFrom{{2, 3}}.Marshal();
+    struct WireVote { uint16_t sender; Bytes wire; std::optional<Vote> seen; EdCommit want; };  // seen: what the reference receives
+    std::vector<std::vector<WireVote>> all(props3.size());
+    for (size_t pi = 0; pi < props3.size(); pi++) {
+        const Proposal &pp = props3[pi];
+        for (uint64_t id = 2; id <= 16; id++) {
+            Signature sg = signProposalEd25519(id, keys[id], pp, aux);
+            uint64_t sender = id, signer = id;
+            std::string dig = pp.Digest();
+            EdCommit want = EdCommit::Verify;
+            if (pi == 0 && id == 4) sg.Value[9] ^= 2;                                        // bad signature
+            if (pi == 0 && id == 5) { sg.Value.resize(63); want = EdCommit::Rejecting; }     // 63-byte Value: registered, rejects
+            if (pi == 1 && id == 7) dig = fixtureWrongProposal().Digest();                   // wrong digest
+            if (pi == 1 && id == 9) signer = 10;                                             // signer != sender
+            if (pi == 1 && id == 13) { sender = signer = 99; want = EdCommit::Rejecting; }   // unknown signer: registered, rejects
+            if (pi == 2 && id == 12) sender = 11;                                            // second vote of sender 11
+            if (pi == 2 && id >= 3 && id <= 8) sg.Value[11] ^= 1;                            // six bad signatures: quorum fails
+            if (pi == 2 && id == 14) { signer = 70000; want = EdCommit::Inert; }             // Signer beyond the 16-bit column
+            Vote vt = commitFrom(sender, signer, dig);
+            vt.commit->Sig = ProtoSignature{signer, sg.Value, sg.Msg};
+            if (pi == 0 && id == 15) { vt.commit->Sig.reset(); want = EdCommit::Inert; }     // no Signature
+            Bytes wire = MarshalCommit(*vt.commit);
+            std::optional<Vote> seen = vt;
+            if (pi == 0 && id == 16) { wire.resize(wire.size() - 3); seen.reset(); want = EdCommit::Inert; }  // truncated on the wire
+            all[pi].push_back({(uint16_t)sender, wire, seen, want});
+        }
+    }
+    // the decoding rules
+    size_t n_inert = 0, n_rejecting = 0;
+    for (auto &votes : all)
+        for (auto &w : votes) {
+            CommitView c;
+            uint32_t slot = 0;
+            const EdCommit k = decode_ed25519_commit(w.wire.data(), w.wire.size(), slot_of, c, slot);
+            CHECK(k == w.want);
+            CHECK((k == EdCommit::Verify) == (slot != ED25519_NO_SLOT));
+            if (k == EdCommit::Verify) CHECK(slot == c.Signer - 1 && c.value_len == 64);
+            n_inert += k == EdCommit::Inert;
+            n_rejecting += k == EdCommit::Rejecting;
+        }
+    CHECK(n_inert == 3 && n_rejecting == 2);
+    if (!g_gpu) return;
+
+    sbv_engine *e = nullptr;
+    CHECK(sbv_create(nullptr, 1, &e) == SBV_OK);
+    if (!e) return;
+    Bytes reg(16 * 32);
+    for (uint64_t id = 1; id <= 16; id++) memcpy(&reg[32 * (id - 1)], keys[id].pub, 32);
+    CHECK(sbv_ed25519_set_keys(e, 16, reg.data()) == SBV_OK);
+    std::vector<uint8_t> okv, reached; std::vector<uint32_t> cnt;
+    {
+        CommitBatch batch(CommitBatch::Ed25519);
+        for (size_t pi = 0; pi < props3.size(); pi++) {
+            batch.begin_instance(props3[pi].Digest(), 1);
+            for (auto &w : all[pi]) batch.add_wire_commit(w.sender, w.wire.data(), w.wire.size(), slot_of);
+        }
+        CHECK(batch.size() == 45 && batch.instances() == 3 && batch.malformed().size() == 3 && batch.rejected().size() == 2);
+        batch.verify_and_count(e, q - 1, okv, cnt, reached);
+    }
+    size_t i = 0;
+    for (size_t pi = 0; pi < props3.size(); pi++) {
+        VoteSet set(acceptCommits);
+        int valid = 0;
+        for (auto &w : all[pi]) {
+            const size_t at = i++;
+            bool sig_ok = false;
+            if (w.seen && w.seen->commit->Sig) {
+                const ProtoSignature &ps = *w.seen->commit->Sig;
+                sig_ok = ps.Signer >= 1 && ps.Signer <= 16 && verifyEd25519(keys[ps.Signer].pub, ps.Value, ps.Msg);
+            }
+            CHECK(okv[at] == (w.want == EdCommit::Verify && sig_ok ? 1 : 0));  // inert and rejecting rows reject
+            if (!w.seen || w.seen->sender == 1) continue;
+            size_t before = set.votes().size();
+            set.registerVote(w.seen->sender, *w.seen);
+            if (set.votes().size() == before) continue;
+            if (w.seen->commit->Digest == props3[pi].Digest() && sig_ok) valid++;
+        }
+        CHECK((int)cnt[pi] == valid);
+        CHECK(reached[pi] == (valid >= q - 1 ? 1 : 0));
+    }
+    CHECK(reached[0] == 1 && reached[1] == 1 && reached[2] == 0);
+    CHECK(cnt[0] == 11 && cnt[1] == 12 && cnt[2] == 7);
+    sbv_destroy(e);
+    for (auto &kv : keys) EVP_PKEY_free(kv.second.k);
+}
+
 int main(int argc, char **argv) {
     std::string mode = argc > 1 ? argv[1] : "cpu";
     RUN(TestProposalDigestFixtures);
@@ -438,6 +536,8 @@ int main(int argc, char **argv) {
     RUN(TestControllerLeaderRequestHandling);
     RUN(TestAggregatorCoalesces);
     if (mode == "gpu") RUN(TestGpuVerifierEndToEnd);
+    g_gpu = mode == "gpu";
+    RUN(TestEd25519CommitBatch);
     printf("%d checks, %d failures\n", g_checks, g_fail);
     return g_fail ? 1 : 0;
 }

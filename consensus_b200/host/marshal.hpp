@@ -10,6 +10,10 @@
 // digest_match for the quorum stage.  Decoding a vote writes straight into those arrays — the DER signature is parsed
 // into its r, s rows, Signature.Msg is appended to the message blob — so the engine DMAs from where the decoder wrote
 // and no intermediate copy exists.
+//
+// An Ed25519 batch (CommitBatch::Ed25519) takes Commits whose Signature.Value is a raw 64-byte Ed25519 signature: the r and
+// s columns together hold one 64-byte row (R || S) per vote, the slots index the engine's Ed25519 registry
+// (sbv_ed25519_set_keys), and verify_and_count makes one sbv_ed25519_verify_quorum call.
 #pragma once
 #include "verifier.hpp"
 #include "callsites.hpp"
@@ -117,12 +121,31 @@ inline bool parse_der_sig_span(const uint8_t *sig, size_t n, uint8_t *r, uint8_t
     return parse_der_sig(tmp, r, s);
 }
 
+// How a wire Commit enters an Ed25519 batch, by the reference's registration rule (acceptCommits, view.go:161-171, then
+// registerVote, util.go:130-143).  Only a Commit the reference would never register is Inert: undecodable bytes, no
+// Signature, or a Signer that does not fit the 16-bit column.  Any other Commit is registered and burns its sender's
+// slot; it is Rejecting when its Value is not exactly 64 bytes (crypto/ed25519.Verify rejects any other length) or its
+// signer has no slot, and its row then carries ED25519_NO_SLOT, which rejects on the device.
+enum class EdCommit { Inert, Rejecting, Verify };
+constexpr uint32_t ED25519_NO_SLOT = 0xffffffffu;
+template <class SlotOf>
+inline EdCommit decode_ed25519_commit(const uint8_t *wire, size_t len, SlotOf &&slot_of, CommitView &c, uint32_t &slot) {
+    slot = ED25519_NO_SLOT;
+    if (!DecodeCommit(wire, len, c) || !c.has_sig || c.Signer > 0xffff) return EdCommit::Inert;
+    const int s = slot_of(c.Signer);
+    if (c.value_len != 64 || s < 0) return EdCommit::Rejecting;
+    slot = (uint32_t)s;
+    return EdCommit::Verify;
+}
+
 // One batch of commit votes (many instances = consensus sequences in flight, or many views during catch-up).
 class CommitBatch {
   public:
+    enum Scheme { EcdsaP256, Ed25519 };
+    explicit CommitBatch(Scheme scheme = EcdsaP256) : ed25519_(scheme == Ed25519) {}
     size_t size() const { return n_; }
     size_t instances() const { return n_inst_; }
-    void clear() { n_ = 0; msg_bytes_ = 0; n_inst_ = 0; malformed_.clear(); }
+    void clear() { n_ = 0; msg_bytes_ = 0; n_inst_ = 0; malformed_.clear(); rejected_.clear(); }
 
     // Starts the votes of the next instance: `expected_digest` is proposal.Digest() (64 hex chars, view.go:524)
     // and `self` the local node id (its own vote never reaches the vote set).
@@ -133,9 +156,10 @@ class CommitBatch {
         return (uint32_t)n_inst_++;
     }
     // Decodes one wire Commit received from `sender` and appends it to the current instance.  `slot_of(signer)` maps
-    // the claimed signer to its slot of the engine's key registry (sbv_set_keys), < 0 when unknown.
+    // the claimed signer to its slot of the engine's key registry (sbv_set_keys, or sbv_ed25519_set_keys for an Ed25519
+    // batch), < 0 when unknown.
     // Malformed input never throws: the vote is recorded as one that cannot count (the reference drops such votes:
-    // view.go:161-171, 839-842).
+    // view.go:161-171, 839-842).  An Ed25519 batch follows decode_ed25519_commit instead.
     template <class SlotOf>
     void add_wire_commit(uint16_t sender, const uint8_t *wire, size_t len, SlotOf &&slot_of) {
         grow(n_ + 1);
@@ -143,6 +167,23 @@ class CommitBatch {
         inst()[i] = (uint32_t)(n_inst_ - 1);
         snd()[i] = sender;
         CommitView c;
+        if (ed25519_) {
+            uint32_t slot = ED25519_NO_SLOT;
+            const EdCommit k = n_inst_ > 0 ? decode_ed25519_commit(wire, len, slot_of, c, slot) : EdCommit::Inert;
+            uint8_t *row = r() + 64 * i;
+            slt()[i] = slot;
+            if (k == EdCommit::Verify) memcpy(row, c.value, 64);
+            else memset(row, 0, 64);
+            if (k == EdCommit::Inert) {  // signer != sender keeps it out of the vote set
+                sig()[i] = (uint16_t)(sender + 1); dm()[i] = 0;
+                off()[i + 1] = msg_bytes_;
+                malformed_.push_back(i);
+                return;
+            }
+            if (k == EdCommit::Rejecting) rejected_.push_back(i);
+            append_registered(i, c);
+            return;
+        }
         bool ok = n_inst_ > 0 && DecodeCommit(wire, len, c) && c.has_sig && c.Signer <= 0xffff;
         int slot = ok ? slot_of(c.Signer) : -1;
         ok = ok && slot >= 0 && parse_der_sig_span(c.value, c.value_len, r() + 32 * i, s() + 32 * i);
@@ -153,28 +194,40 @@ class CommitBatch {
             malformed_.push_back(i);
             return;
         }
-        sig()[i] = (uint16_t)c.Signer;
         slt()[i] = (uint32_t)slot;
-        dm()[i] = (c.digest_len == expected_.size() && memcmp(c.digest, expected_.data(), c.digest_len) == 0) ? 1 : 0;
-        msgs_.reserve(msg_bytes_ + c.msg_len + 16, msg_bytes_);
-        if (c.msg_len) memcpy(msgs_.p + msg_bytes_, c.msg, c.msg_len);
-        msg_bytes_ += c.msg_len;
-        off()[i + 1] = msg_bytes_;
+        append_registered(i, c);
     }
     // Verifies every signature (SHA-256 of Signature.Msg on the device, registered keys) and counts the valid distinct
     // foreign votes per instance.  ok / count / reached are sized by the call.
+    // An Ed25519 batch makes one sbv_ed25519_verify_quorum call (Signature.Msg hashed with SHA-512 on the device).
     void verify_and_count(sbv_engine *e, uint32_t threshold, std::vector<uint8_t> &ok, std::vector<uint32_t> &count, std::vector<uint8_t> &reached) {
         ok.assign(n_, 0); count.assign(n_inst_, 0); reached.assign(n_inst_, 0);
         if (n_ == 0 || n_inst_ == 0) return;
+        if (ed25519_) {
+            if (sbv_ed25519_verify_quorum(e, n_, msgs_.p, off(), slt(), r(), inst(), snd(), sig(), dm(), n_inst_, (const uint16_t *)self_.p, threshold,
+                                          ok.data(), count.data(), reached.data()) != SBV_OK)
+                throw EngineFault(std::string("sbv_ed25519_verify_quorum: ") + sbv_last_error(e));
+            return;
+        }
         if (sbv_hash_verify_registered(e, SBV_P256, n_, msgs_.p ? msgs_.p : (const uint8_t *)"", off(), slt(), r(), s(), ok.data()) != SBV_OK)
             throw EngineFault(std::string("sbv_hash_verify_registered: ") + sbv_last_error(e));
         if (sbv_quorum(e, n_, inst(), snd(), sig(), dm(), ok.data(), n_inst_, (const uint16_t *)self_.p, threshold, count.data(), reached.data()) != SBV_OK)
             throw EngineFault(std::string("sbv_quorum: ") + sbv_last_error(e));
     }
     const std::vector<size_t> &malformed() const { return malformed_; }
+    const std::vector<size_t> &rejected() const { return rejected_; }  // Ed25519: registered votes with a rejecting row
     const uint8_t *r_rows() const { return cols_.p; }
 
   private:
+    // signer, digest match and message of a vote that enters the vote set
+    void append_registered(size_t i, const CommitView &c) {
+        sig()[i] = (uint16_t)c.Signer;
+        dm()[i] = (c.digest_len == expected_.size() && memcmp(c.digest, expected_.data(), c.digest_len) == 0) ? 1 : 0;
+        msgs_.reserve(msg_bytes_ + c.msg_len + 16, msg_bytes_);
+        if (c.msg_len) memcpy(msgs_.p + msg_bytes_, c.msg, c.msg_len);
+        msg_bytes_ += c.msg_len;
+        off()[i + 1] = msg_bytes_;
+    }
     // column block (one pinned allocation): r, s, off, slot, instance, sender, signer, digest_match
     static constexpr size_t ROW = 32 + 32 + 8 + 4 + 4 + 2 + 2 + 1;
     void grow(size_t n) {
@@ -187,7 +240,7 @@ class CommitBatch {
                                 64 * capn + 8 * (capn + 1) + 8 * capn, 64 * capn + 8 * (capn + 1) + 10 * capn, 64 * capn + 8 * (capn + 1) + 12 * capn};
             return base + o[k];
         };
-        const size_t w[] = {32, 32, 8, 4, 4, 2, 2, 1};
+        const size_t w[] = {ed25519_ ? (size_t)64 : 32, ed25519_ ? (size_t)0 : 32, 8, 4, 4, 2, 2, 1};  // Ed25519: one 64-byte row over r and s
         if (cols_.p)
             for (int k = 0; k < 8; k++) memcpy(at(nb.p, nc, k), at(cols_.p, cap_, k), w[k] * (n_ + (k == 2 ? 1 : 0)));
         else
@@ -213,7 +266,8 @@ class CommitBatch {
     PinnedBuf cols_, msgs_, self_;
     size_t cap_ = 0, n_ = 0, msg_bytes_ = 0, n_inst_ = 0;
     std::string expected_;
-    std::vector<size_t> malformed_;
+    std::vector<size_t> malformed_, rejected_;
+    bool ed25519_ = false;
 };
 
 }  // namespace sbft

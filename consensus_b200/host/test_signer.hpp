@@ -5,6 +5,7 @@
 #include <openssl/bn.h>
 #include <openssl/ec.h>
 #include <openssl/ecdsa.h>
+#include <openssl/evp.h>
 #include <openssl/obj_mac.h>
 
 #include "callsites.hpp"
@@ -38,6 +39,45 @@ inline Signature signProposal(uint64_t id, const TestKey &k, const Proposal &p, 
     return s;
 }
 
+
+// Ed25519 consenter keys (OpenSSL EVP_PKEY_ED25519): Value = the raw 64-byte signature (R || S) over Signature.Msg.
+struct TestEdKey { EVP_PKEY *k; uint8_t pub[32]; };
+inline TestEdKey makeEdKey() {
+    TestEdKey t{nullptr, {}};
+    EVP_PKEY_CTX *ctx = EVP_PKEY_CTX_new_id(EVP_PKEY_ED25519, nullptr);
+    EVP_PKEY_keygen_init(ctx);
+    EVP_PKEY_keygen(ctx, &t.k);
+    EVP_PKEY_CTX_free(ctx);
+    size_t len = 32;
+    EVP_PKEY_get_raw_public_key(t.k, t.pub, &len);
+    return t;
+}
+inline Bytes signEd25519(const TestEdKey &k, const Bytes &msg) {
+    Bytes sig(64);
+    size_t len = 64;
+    EVP_MD_CTX *ctx = EVP_MD_CTX_new();
+    EVP_DigestSignInit(ctx, nullptr, nullptr, nullptr, k.k);
+    EVP_DigestSign(ctx, sig.data(), &len, msg.data(), msg.size());
+    EVP_MD_CTX_free(ctx);
+    return sig;
+}
+// crypto/ed25519.Verify for the keys and signatures of the tests: a Value of any length other than 64 rejects
+inline bool verifyEd25519(const uint8_t pub[32], const Bytes &sig, const Bytes &msg) {
+    if (sig.size() != 64) return false;
+    EVP_PKEY *k = EVP_PKEY_new_raw_public_key(EVP_PKEY_ED25519, nullptr, pub, 32);
+    if (!k) return false;
+    EVP_MD_CTX *ctx = EVP_MD_CTX_new();
+    bool ok = EVP_DigestVerifyInit(ctx, nullptr, nullptr, nullptr, k) == 1 && EVP_DigestVerify(ctx, sig.data(), 64, msg.data(), msg.size()) == 1;
+    EVP_MD_CTX_free(ctx);
+    EVP_PKEY_free(k);
+    return ok;
+}
+inline Signature signProposalEd25519(uint64_t id, const TestEdKey &k, const Proposal &p, const Bytes &aux) {
+    Signature s; s.ID = id;
+    s.Msg = p.DigestRaw(); s.Msg.insert(s.Msg.end(), aux.begin(), aux.end());
+    s.Value = signEd25519(k, s.Msg);
+    return s;
+}
 
 // One CPU ECDSA verification per call — the shape of a Go application calling crypto/ecdsa from
 // VerifyConsenterSig / VerifyRequest (stand-in: OpenSSL ECDSA_verify; no Go toolchain here).

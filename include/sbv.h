@@ -154,6 +154,22 @@ int sbv_verify_quorum(sbv_engine *e, uint8_t curve, size_t n_votes, const uint8_
                       const uint16_t *sender, const uint16_t *signer, const uint8_t *digest_match, size_t n_instances,
                       const uint16_t *self_id, uint32_t threshold, uint8_t *ok, uint32_t *valid_count, uint8_t *reached);
 
+/* sbv_verify_quorum for consenters with registered Ed25519 keys (verifyVote + processCommits, view.go:519-551, 827-849;
+ * voteSet, util.go:130-143).  ok[i] = the verdict of sbv_ed25519_verify_registered for vote i: key from registry slot
+ * key_slot[i], message msgs[msg_off[i]..msg_off[i+1]) hashed on the device (msgs may be NULL when every message is empty),
+ * sig = 64 bytes per vote (R || S); a slot >= n, a registered key that does not decode and an empty registry reject.
+ * valid_count / reached = sbv_quorum over those verdicts, with the same vote rules, self_id (NULL = no self filter) and
+ * threshold (the caller passes Quorum-1).  The verdicts stay on the device.  Votes must be grouped by instance with
+ * non-decreasing instance ids, in arrival order inside an instance.  A multi-device engine shards BY INSTANCE, as
+ * sbv_verify_quorum does, and every shard of one call reads the same registry (as in sbv_ed25519_verify_registered).
+ * Shards are uploaded whole: unlike the ECDSA calls, large Ed25519 shards are not uploaded in chunks.
+ * Outputs: ok[n_votes], valid_count[n_instances], reached[n_instances]; n_instances == 0 does nothing. */
+int sbv_ed25519_verify_quorum(sbv_engine *e, size_t n_votes, const uint8_t *msgs, const uint64_t *msg_off,
+                              const uint32_t *key_slot, const uint8_t *sig, const uint32_t *instance,
+                              const uint16_t *sender, const uint16_t *signer, const uint8_t *digest_match,
+                              size_t n_instances, const uint16_t *self_id, uint32_t threshold, uint8_t *ok,
+                              uint32_t *valid_count, uint8_t *reached);
+
 /* computeQuorum(n) -> (q, f), internal/bft/util.go:183-187. */
 void sbv_compute_quorum(uint64_t n, uint32_t *q, uint32_t *f);
 
