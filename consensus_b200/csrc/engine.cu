@@ -21,6 +21,7 @@
 #include "engine.h"
 #include "sha256.cuh"
 #include "quorum.cuh"
+#include "shards.h"
 
 using namespace sbv;
 
@@ -244,69 +245,6 @@ int nccl_load(sbv_engine *e) {
             return fail(e, SBV_ERR_NCCL, "%s failed: %s", #call, g_nccl.err_string ? g_nccl.err_string(_r) : "?"); \
     } while (0)
 
-struct Shard { size_t lo, n; };
-Shard shard_of(size_t n, int g, int G) {
-    size_t lo = n * g / G, hi = n * (g + 1) / G;
-    return {lo, hi - lo};
-}
-
-// Multi-device epilogue: every device packs its shard's verdict bytes into a bitmask (k_pack_bits), one ncclAllGather
-// (in place, on each device's lane stream, right behind its verify kernel) assembles the whole mask on every device,
-// and device 0 returns it to the host in a single n/8-byte copy into the lane's pinned mirror.  Shards are padded to a
-// common word count, so device g's words start at g * words_per.  `extra_words` more words per device travel in the
-// same collective (the quorum path appends its `reached` bits).
-size_t words_per_shard(size_t n, int G) { return (((n + G - 1) / G) + 31) / 32; }
-
-int gather_verdicts(sbv_engine *e, size_t n, int lane, size_t extra_words) {
-    const int G = (int)e->devs.size();
-    const size_t wp = words_per_shard(n, G) + extra_words;
-    for (int g = 0; g < G; g++) {
-        Dev &d = e->devs[g];
-        CU(e, cudaSetDevice(d.ordinal));
-        Dev::Lane &ln = d.lanes[lane];
-        int rc = sbv_lane_ensure_aux(e, ln, wp * G * 4);
-        if (rc) return rc;
-    }
-    for (int g = 0; g < G; g++) {
-        Dev &d = e->devs[g];
-        CU(e, cudaSetDevice(d.ordinal));
-        Shard sh = shard_of(n, g, G);
-        Dev::Lane &ln = d.lanes[lane];
-        uint32_t *mine = (uint32_t *)ln.d_aux + wp * g;
-        CU(e, cudaMemsetAsync(mine, 0, (wp - extra_words) * 4, ln.stream));
-        if (sh.n) {
-            k_pack_bits<<<(uint32_t)((sh.n + 255) / 256), 256, 0, ln.stream>>>((uint32_t)sh.n, ln.d_ok, mine);
-            e->launches += 1;
-            CU(e, cudaGetLastError());
-        }
-    }
-    {
-        std::lock_guard<std::mutex> lk(e->mu);  // collectives of one communicator set must be issued in one order
-        NC(e, g_nccl.group_start());
-        for (int g = 0; g < G; g++) {
-            Dev &d = e->devs[g];
-            uint32_t *buf = (uint32_t *)d.lanes[lane].d_aux;
-            NC(e, g_nccl.all_gather(buf + wp * g, buf, wp, NCCL_UINT32, e->nccl_comms[g], d.lanes[lane].stream));
-        }
-        NC(e, g_nccl.group_end());
-    }
-    Dev &d0 = e->devs[0];
-    CU(e, cudaSetDevice(d0.ordinal));
-    CU(e, cudaMemcpyAsync(d0.lanes[lane].h_aux, d0.lanes[lane].d_aux, wp * G * 4, cudaMemcpyDeviceToHost, d0.lanes[lane].stream));
-    return 0;
-}
-
-void unpack_verdicts(sbv_engine *e, size_t n, int lane, size_t extra_words, uint8_t *ok_host) {
-    const int G = (int)e->devs.size();
-    const size_t wp = words_per_shard(n, G) + extra_words;
-    const uint32_t *words = (const uint32_t *)e->devs[0].lanes[lane].h_aux;
-    for (int g = 0; g < G; g++) {
-        Shard sh = shard_of(n, g, G);
-        const uint32_t *w = words + wp * g;
-        for (size_t i = 0; i < sh.n; i++) ok_host[sh.lo + i] = (w[i >> 5] >> (i & 31)) & 1u;
-    }
-}
-
 int sync_lane(sbv_engine *e, int lane) {
     for (Dev &d : e->devs) {
         if (!d.lanes[lane].stream) continue;
@@ -314,6 +252,54 @@ int sync_lane(sbv_engine *e, int lane) {
         CU(e, cudaStreamSynchronize(d.lanes[lane].stream));
     }
     return 0;
+}
+
+// The verdicts of sbv_verify_batch and of the commit-vote calls leave the devices in two steps.  shard_out runs on device
+// g's lane stream behind its verdicts d_ok (s.vr[g].n bytes) and reached flags d_rch (s.ir[g].n bytes, if there are
+// instances).  A single device copies them to the host directly.  Several pack them (k_pack_bits) into device g's slot of
+// its gather buffer gbuf (s.wp() * G words); then gather_unpack issues one grouped ncclAllGather (in place, on the lane
+// streams), copies the whole buffer from device 0 into the lane's pinned mirror, drains the lane and unpacks on the host.
+int shard_out(sbv_engine *e, Dev::Lane &ln, const Shards &s, int g, uint32_t *gbuf, const uint8_t *d_ok, const uint8_t *d_rch, uint8_t *ok,
+              uint8_t *reached) {
+    const size_t nv = s.vr[g].n, ni = s.ir.empty() ? 0 : s.ir[g].n;
+    if (s.vr.size() == 1) {
+        if (nv) CU(e, cudaMemcpyAsync(ok, d_ok, nv, cudaMemcpyDeviceToHost, ln.stream));
+        if (ni) CU(e, cudaMemcpyAsync(reached, d_rch, ni, cudaMemcpyDeviceToHost, ln.stream));
+        return 0;
+    }
+    uint32_t *mine = gbuf + s.wp() * g;
+    CU(e, cudaMemsetAsync(mine, 0, s.wp() * 4, ln.stream));
+    if (nv) {  // a grid of zero blocks is an invalid configuration
+        k_pack_bits<<<(uint32_t)((nv + 255) / 256), 256, 0, ln.stream>>>((uint32_t)nv, d_ok, mine);
+        e->launches += 1;
+    }
+    if (ni) {
+        k_pack_bits<<<(uint32_t)((ni + 255) / 256), 256, 0, ln.stream>>>((uint32_t)ni, d_rch, mine + s.wv);
+        e->launches += 1;
+    }
+    CU(e, cudaGetLastError());
+    return 0;
+}
+
+int gather_unpack(sbv_engine *e, int lane, const Shards &s, const std::vector<uint32_t *> &gbuf, uint8_t *ok, uint8_t *reached) {
+    const int G = (int)s.vr.size();
+    const size_t wp = s.wp();
+    if (G > 1) {
+        {
+            std::lock_guard<std::mutex> lk(e->mu);  // collectives of one communicator set must be issued in one order
+            NC(e, g_nccl.group_start());
+            for (int g = 0; g < G; g++)
+                NC(e, g_nccl.all_gather(gbuf[g] + wp * g, gbuf[g], wp, NCCL_UINT32, e->nccl_comms[g], e->devs[g].lanes[lane].stream));
+            NC(e, g_nccl.group_end());
+        }
+        Dev &d0 = e->devs[0];
+        CU(e, cudaSetDevice(d0.ordinal));
+        CU(e, cudaMemcpyAsync(d0.lanes[lane].h_aux, gbuf[0], wp * G * 4, cudaMemcpyDeviceToHost, d0.lanes[lane].stream));
+    }
+    int rc = sync_lane(e, lane);
+    if (rc) return rc;
+    if (G > 1) unpack_shards(s, (const uint32_t *)e->devs[0].lanes[lane].h_aux, ok, reached);
+    return SBV_OK;
 }
 
 // One shard of a keys-per-item host-buffer call on device d's lane: what to verify and where it comes from.
@@ -528,28 +514,26 @@ int sbv_verify_batch(sbv_engine *e, uint8_t curve, size_t n, const uint8_t *r, c
     if (!r || !s || !qx || !qy || !digest || !ok) return fail(e, SBV_ERR_ARG, "null buffer");
     if (n > 0x7fffffffu) return fail(e, SBV_ERR_ARG, "n too large");
     const int G = (int)e->devs.size();
+    const Shards sh = batch_shards(n, G);
+    std::vector<uint32_t *> gbuf(G);
     // A call owns one lane (stream + buffers) on every device; the engine lock is held only while
     // kernels are enqueued, so other host threads overlap their copies and kernels with ours.
     LaneGuard guard(e);
     const int lane = guard.lane;
-    if (G == 1) {
-        Dev &d = e->devs[0];
-        int rc = stage_and_verify(e, d, lane, curve, 0, n, BatchSrc{r, s, qx, qy, digest, digest_len, nullptr, nullptr});
-        if (rc) return rc;
-        CU(e, cudaMemcpyAsync(ok, d.lanes[lane].d_ok, n, cudaMemcpyDeviceToHost, d.lanes[lane].stream));
-        return sync_lane(e, lane);
-    }
     for (int g = 0; g < G; g++) {
-        Shard sh = shard_of(n, g, G);
-        if (sh.n == 0) continue;
-        int rc = stage_and_verify(e, e->devs[g], lane, curve, sh.lo, sh.n, BatchSrc{r, s, qx, qy, digest, digest_len, nullptr, nullptr});
-        if (rc) return rc;
+        Dev &d = e->devs[g];
+        Dev::Lane &ln = d.lanes[lane];
+        const Range v = sh.vr[g];
+        int rc = 0;
+        if (v.n && (rc = stage_and_verify(e, d, lane, curve, v.lo, v.n, BatchSrc{r, s, qx, qy, digest, digest_len, nullptr, nullptr}))) return rc;
+        if (G > 1) {  // the aux area holds the gather buffer
+            CU(e, cudaSetDevice(d.ordinal));
+            if ((rc = sbv_lane_ensure_aux(e, ln, sh.wp() * G * 4))) return rc;
+            gbuf[g] = (uint32_t *)ln.d_aux;
+        }
+        if ((rc = shard_out(e, ln, sh, g, gbuf[g], ln.d_ok, nullptr, ok, nullptr))) return rc;
     }
-    int rc = gather_verdicts(e, n, lane, 0);
-    if (rc) return rc;
-    if ((rc = sync_lane(e, lane))) return rc;
-    unpack_verdicts(e, n, lane, 0, ok);
-    return SBV_OK;
+    return gather_unpack(e, lane, sh, gbuf, ok, nullptr);
 }
 
 // ---- one process per GPU: this engine is one rank of an N-rank job ------------------------------------------

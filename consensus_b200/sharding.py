@@ -4,15 +4,15 @@ Signatures are independent, so a batch shards into contiguous ranges with no dat
 quorum counting is independent per instance, so votes shard BY INSTANCE (all votes of an instance on
 one rank).  The only exchange is the final gather of the bit-packed verdict mask (n/8 bytes) and, for
 the quorum stream, of the per-instance reached bits — `ncclAllGather` over NVLink on a GPU box, gloo
-in the CPU tests.  Mirrors the device-level sharding inside libsbv.so (engine.cu: shard_of,
-gather_verdicts)."""
+in the CPU tests.  Mirrors the device-level sharding inside libsbv.so (csrc/shards.h: shard_range,
+quorum_shards, unpack_shards; engine.cu: shard_out, gather_unpack)."""
 from __future__ import annotations
 
 import numpy as np
 
 
 def shard_range(n: int, rank: int, world: int):
-    """Contiguous range [lo, hi) of rank `rank` — same rule as engine.cu shard_of()."""
+    """Contiguous range [lo, hi) of rank `rank` — same rule as shards.h shard_range()."""
     return n * rank // world, n * (rank + 1) // world
 
 

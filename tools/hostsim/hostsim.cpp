@@ -22,6 +22,7 @@ namespace sbv { uint32_t tab[1 << 18]; }
 #include "../../consensus_b200/csrc/sha512.cuh"
 #include "../../consensus_b200/csrc/ed25519_verify.cuh"
 #include "../../consensus_b200/csrc/ed25519_keyed.cuh"
+#include "../../consensus_b200/csrc/shards.h"
 
 using namespace sbv;
 
@@ -165,6 +166,29 @@ extern "C" int hs_quorum(size_t n_votes, const uint32_t *instance, const uint16_
 // k_pack_bits in lockstep (a warp ballot per 32 verdicts)
 extern "C" int hs_pack_bits(size_t n, const uint8_t *ok, uint32_t *mask) {
     run_grid_lockstep((unsigned)((n + 255) / 256), 256, [&] { k_pack_bits((uint32_t)n, ok, mask); });
+    return 0;
+}
+
+// the shards of a multi-device engine (shards.h, host code of libsbv itself): a plain batch of n items (votes == 0) or n
+// commit votes grouped by instance.  ranges: [G][4] = item lo, item count, instance lo, instance count; words = wv, wi.
+static Shards make_shards(int votes, size_t n, const uint32_t *instance, size_t n_instances, int G) {
+    return votes ? quorum_shards(n, instance, n_instances, G) : batch_shards(n, G);
+}
+extern "C" int hs_shards(int votes, size_t n, const uint32_t *instance, size_t n_instances, int G, size_t *ranges, size_t *words) {
+    const Shards s = make_shards(votes, n, instance, n_instances, G);
+    for (int g = 0; g < G; g++) {
+        const Range ir = s.ir.empty() ? Range{0, 0} : s.ir[g];
+        const size_t r[4] = {s.vr[g].lo, s.vr[g].n, ir.lo, ir.n};
+        memcpy(ranges + 4 * g, r, sizeof r);
+    }
+    words[0] = s.wv;
+    words[1] = s.wi;
+    return 0;
+}
+// the host unpack of the gathered words (G * (wv + wi) words) into verdict and reached bytes
+extern "C" int hs_unpack_shards(int votes, size_t n, const uint32_t *instance, size_t n_instances, int G, const uint32_t *gathered, uint8_t *ok,
+                                uint8_t *reached) {
+    unpack_shards(make_shards(votes, n, instance, n_instances, G), gathered, ok, reached);
     return 0;
 }
 
