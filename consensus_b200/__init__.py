@@ -14,7 +14,7 @@ import numpy as np
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libsbv.so")
 
-P256, P384 = 0, 1
+P256, P384, ED25519 = 0, 1, 2  # scheme tags of the mixed calls (the other calls take P256 / P384 only)
 FIELD_BYTES = {P256: 32, P384: 48}
 
 SYMBOLS = [
@@ -25,7 +25,8 @@ SYMBOLS = [
     "sbv_verify_registered_device", "sbv_hash_verify_registered", "sbv_prepare_quorum", "sbv_verify_quorum",
     "sbv_comm_unique_id", "sbv_comm_init_rank", "sbv_comm_ranks", "sbv_gather_verdicts_device", "sbv_gather_words_device",
     "sbv_verify_batch_ranked", "sbv_host_alloc", "sbv_host_free", "sbv_ed25519_verify_batch",
-    "sbv_ed25519_set_keys", "sbv_ed25519_verify_registered", "sbv_ed25519_verify_quorum",
+    "sbv_ed25519_set_keys", "sbv_ed25519_verify_registered", "sbv_ed25519_verify_quorum", "sbv_mixed_verify_registered",
+    "sbv_mixed_verify_quorum",
 ]
 
 
@@ -311,6 +312,69 @@ class Engine:
         self._check(self._lib.sbv_ed25519_verify_quorum(self._h, C.c_size_t(n), vp(msgs), vp(off), vp(key_slot), vp(sig), vp(instance), vp(sender),
                                                         vp(signer), vp(digest_match), C.c_size_t(n_instances), vp(self_id), C.c_uint32(threshold),
                                                         vp(ok), vp(valid_count), vp(reached)), "sbv_ed25519_verify_quorum")
+
+    def mixed_verify_registered(self, scheme, msgs, off, key_slot, sig96, out=None) -> np.ndarray:
+        """Registered-key items of any scheme in one call: scheme[i] in {P256, P384, ED25519}, msgs concatenated with off[n+1]
+        byte offsets, key_slot[i] a slot of the item's own registry (set_keys / ed25519_set_keys), sig96 = n x 96 bytes
+        (P-256 r || s in [0, 64), P-384 r || s, Ed25519 R || S in [0, 64)).  Returns the n verdict bytes (into `out` if given)."""
+        scheme = _u8(scheme)
+        msgs = _u8(msgs if len(msgs) else np.zeros(1, np.uint8))
+        off = np.ascontiguousarray(off, dtype=np.uint64)
+        key_slot = np.ascontiguousarray(key_slot, dtype=np.uint32)
+        sig96 = _u8(sig96)
+        n = off.size - 1
+        if scheme.size != n or sig96.size != 96 * n or key_slot.size != n:
+            raise ValueError("scheme and key_slot must hold one entry and sig96 96 bytes per message")
+        ok = out if out is not None else np.zeros(n, np.uint8)
+        self._check(self._lib.sbv_mixed_verify_registered(self._h, C.c_size_t(n), _p8(scheme), _p8(msgs), off.ctypes.data_as(C.POINTER(C.c_uint64)),
+                                                          key_slot.ctypes.data_as(C.POINTER(C.c_uint32)), _p8(sig96), _p8(ok)),
+                    "sbv_mixed_verify_registered")
+        return ok
+
+    def mixed_verify_registered_ptr(self, n, scheme, msgs, off, key_slot, sig96, ok):
+        """Raw host pointers (ints) — used with pinned buffers."""
+        vp = C.c_void_p
+        self._check(self._lib.sbv_mixed_verify_registered(self._h, C.c_size_t(n), vp(scheme), vp(msgs), vp(off), vp(key_slot), vp(sig96), vp(ok)),
+                    "sbv_mixed_verify_registered")
+
+    def mixed_verify_quorum(self, scheme, msgs, off, key_slot, sig96, instance, sender, signer, digest_match, n_instances, threshold,
+                            self_id=None):
+        """Commit votes of a mixed consenter set: the items of mixed_verify_registered, verified and counted on the device
+        (votes grouped by non-decreasing instance).  Returns (ok, valid_count, reached)."""
+        scheme = _u8(scheme)
+        msgs = _u8(msgs if len(msgs) else np.zeros(1, np.uint8))
+        off = np.ascontiguousarray(off, dtype=np.uint64)
+        key_slot = np.ascontiguousarray(key_slot, dtype=np.uint32)
+        instance = np.ascontiguousarray(instance, dtype=np.uint32)
+        sender = np.ascontiguousarray(sender, dtype=np.uint16)
+        signer = np.ascontiguousarray(signer, dtype=np.uint16)
+        sig96, digest_match = _u8(sig96), _u8(digest_match)
+        n = instance.size
+        if (off.size != n + 1 or scheme.size != n or sig96.size != 96 * n or key_slot.size != n or sender.size != n or signer.size != n
+                or digest_match.size != n):
+            raise ValueError("off must hold n + 1 offsets, sig96 96 bytes and every other column one entry per vote")
+        ok = np.zeros(n, np.uint8)
+        cnt = np.zeros(n_instances, np.uint32)
+        reached = np.zeros(n_instances, np.uint8)
+        sid = None
+        if self_id is not None:
+            self_id = np.ascontiguousarray(self_id, dtype=np.uint16)
+            sid = self_id.ctypes.data_as(C.POINTER(C.c_uint16))
+        u16 = lambda a: a.ctypes.data_as(C.POINTER(C.c_uint16))
+        u32 = lambda a: a.ctypes.data_as(C.POINTER(C.c_uint32))
+        self._check(self._lib.sbv_mixed_verify_quorum(self._h, C.c_size_t(n), _p8(scheme), _p8(msgs), off.ctypes.data_as(C.POINTER(C.c_uint64)),
+                                                      u32(key_slot), _p8(sig96), u32(instance), u16(sender), u16(signer), _p8(digest_match),
+                                                      C.c_size_t(n_instances), sid, C.c_uint32(threshold), _p8(ok), u32(cnt), _p8(reached)),
+                    "sbv_mixed_verify_quorum")
+        return ok, cnt, reached
+
+    def mixed_verify_quorum_ptr(self, n, scheme, msgs, off, key_slot, sig96, instance, sender, signer, digest_match, n_instances, self_id,
+                                threshold, ok, valid_count, reached):
+        """Raw host pointers (ints; self_id may be None) — used with pinned buffers."""
+        vp = C.c_void_p
+        self._check(self._lib.sbv_mixed_verify_quorum(self._h, C.c_size_t(n), vp(scheme), vp(msgs), vp(off), vp(key_slot), vp(sig96), vp(instance),
+                                                      vp(sender), vp(signer), vp(digest_match), C.c_size_t(n_instances), vp(self_id),
+                                                      C.c_uint32(threshold), vp(ok), vp(valid_count), vp(reached)), "sbv_mixed_verify_quorum")
 
     def verify_mixed(self, curve_tag, r48, s48, qx48, qy48, digest32) -> np.ndarray:
         curve_tag, r48, s48, qx48, qy48, digest32 = map(_u8, (curve_tag, r48, s48, qx48, qy48, digest32))

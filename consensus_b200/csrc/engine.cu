@@ -10,6 +10,7 @@
 #include <dlfcn.h>
 
 #include <algorithm>
+#include <array>
 #include <cstdarg>
 #include <cstdio>
 #include <cstdlib>
@@ -153,6 +154,25 @@ int sbv_lane_ensure_aux(sbv_engine *e, Dev::Lane &ln, size_t bytes) {
     CU(e, cudaMalloc(&ln.d_aux, cap));
     CU(e, cudaHostAlloc(&ln.h_aux, cap, cudaHostAllocPortable));
     ln.aux_cap = cap;
+    return 0;
+}
+int sbv_lane_stream2(sbv_engine *e, Dev::Lane &ln) {
+    if (ln.stream2) return 0;
+    CU(e, cudaStreamCreateWithFlags(&ln.stream2, cudaStreamNonBlocking));
+    CU(e, cudaEventCreateWithFlags(&ln.ev_a, cudaEventDisableTiming));
+    CU(e, cudaEventCreateWithFlags(&ln.ev_b, cudaEventDisableTiming));
+    return 0;
+}
+int sbv_lane_ensure_mix(sbv_engine *e, Dev::Lane &ln, size_t bytes) {
+    if (bytes <= ln.mix_cap) return 0;
+    CU(e, cudaStreamSynchronize(ln.stream));
+    if (ln.stream2) CU(e, cudaStreamSynchronize(ln.stream2));
+    if (ln.d_mix) cudaFree(ln.d_mix);
+    ln.d_mix = nullptr;
+    ln.mix_cap = 0;
+    const size_t cap = bytes + bytes / 8 + 4096;
+    CU(e, cudaMalloc(&ln.d_mix, cap));
+    ln.mix_cap = cap;
     return 0;
 }
 int sbv_launch_length_sort(sbv_engine *e, size_t n, const uint64_t *d_off, uint32_t *d_perm, cudaStream_t st, const uint32_t **perm) {
@@ -335,11 +355,7 @@ int stage_and_verify(sbv_engine *e, Dev &d, int lane, uint8_t curve, size_t lo, 
     if (hashing && (rc = sbv_lane_ensure_msgs(e, ln, bytes + 16, cnt + 1))) return rc;
     cudaStream_t up = ln.stream;   // the stream the rest of the batch is uploaded on
     if (chunks > 1) {
-        if (!ln.stream2) {
-            CU(e, cudaStreamCreateWithFlags(&ln.stream2, cudaStreamNonBlocking));
-            CU(e, cudaEventCreateWithFlags(&ln.ev_a, cudaEventDisableTiming));
-            CU(e, cudaEventCreateWithFlags(&ln.ev_b, cudaEventDisableTiming));
-        }
+        if (int rc2 = sbv_lane_stream2(e, ln)) return rc2;
         for (int c = 0; c < chunks; c++)
             if (!ln.ev_chunk[c]) CU(e, cudaEventCreateWithFlags(&ln.ev_chunk[c], cudaEventDisableTiming));
         up = ln.stream2;
@@ -457,7 +473,7 @@ void sbv_destroy(sbv_engine *e) {
         sbv_keys_free(d);
         sbv_ed_keys_free(d);
         for (auto &ln : d.lanes) {
-            void *lp[] = {ln.d_r, ln.d_s, ln.d_qx, ln.d_qy, ln.d_dig, ln.d_ok, ln.d_slot, ln.d_msgs, ln.d_off, ln.d_perm, ln.d_aux};
+            void *lp[] = {ln.d_r, ln.d_s, ln.d_qx, ln.d_qy, ln.d_dig, ln.d_ok, ln.d_slot, ln.d_msgs, ln.d_off, ln.d_perm, ln.d_aux, ln.d_mix};
             for (void *p : lp) if (p) cudaFree(p);
             if (ln.h_pin) cudaFreeHost(ln.h_pin);
             if (ln.h_aux) cudaFreeHost(ln.h_aux);

@@ -76,6 +76,9 @@ struct Dev {
         cudaStream_t stream2 = nullptr;
         cudaEvent_t ev_a = nullptr, ev_b = nullptr;
         cudaEvent_t ev_chunk[SBV_MAX_CHUNKS] = {};  // "chunk c has arrived" (recorded on stream2, the upload stream of a chunked call)
+        // device scratch of a mixed ECDSA / Ed25519 shard (inst_mixed.cu: sbv_mix_carve)
+        uint8_t *d_mix = nullptr;
+        size_t mix_cap = 0;
     } lanes[SBV_LANES];
     // generic scratch of the entry points that serialise on the engine lock
     uint8_t *d_scratch = nullptr;
@@ -205,6 +208,27 @@ int sbv_launch_ed25519_registered(sbv_engine *e, Dev &d, size_t n, const uint8_t
 // test hook: k_ed_verify_keyed with the caller's k (word-major [8][n], every k < L); caller holds e->mu
 int sbv_launch_ed_verify_registered_k(sbv_engine *e, Dev &d, size_t n, const uint32_t *d_slot, const uint8_t *d_sig, const uint32_t *d_k, uint8_t *d_ok,
                                       cudaStream_t st);
+// ---- inst_mixed.cu: mixed ECDSA / Ed25519 shards (mixed.cuh; family f = scheme tag f) ----
+// The device scratch of a shard of n items, m[f] of family f and `bytes` message bytes, carved from one buffer: the
+// uploaded tags, slots and 96-byte rows, the tile prefixes of the split, the shared message buffer of the three families,
+// and per family the compacted arrays and the scratch of its pipeline.
+struct MixBufs {
+    uint8_t *tag, *sig96;
+    uint32_t *slot_in, *tile_cnt;
+    uint64_t *tile_bytes;
+    uint8_t *blob;
+    uint32_t *idx[3], *slot[3], *perm[3];
+    uint8_t *r[3], *s[3], *ok[3], *dig[3], *pub[3];  // dig: SHA-256 digests (ECDSA) or k (Ed25519); pub: Ed25519 only
+    uint64_t *off[3];
+};
+// base == nullptr only sizes; returns the bytes the carve takes
+size_t sbv_mix_carve(uint8_t *base, size_t n, const uint32_t m[3], uint64_t bytes, MixBufs *out);
+// the split of a staged shard (b.tag, b.slot_in, b.sig96, messages at d_msgs with offsets d_off from base) into the families
+int sbv_launch_mix_split(sbv_engine *e, const MixBufs &b, size_t n, const uint32_t m[3], const uint8_t *d_msgs, const uint64_t *d_off, uint64_t base,
+                         cudaStream_t st);
+// the family verdicts b.ok[f] back into item order in d_ok
+int sbv_launch_mix_ok(sbv_engine *e, const MixBufs &b, size_t n, const uint32_t m[3], uint8_t *d_ok, cudaStream_t st);
+
 // shape of the table of B (ed25519_verify.cuh: ED_BWINS x ED_BENT entries of ED_BWORDS words; checked in inst_ed25519.cu)
 constexpr size_t SBV_ED_BTAB_ENTRIES = 32 * 128, SBV_ED_BTAB_ENTRY_WORDS = 24;
 
@@ -214,6 +238,8 @@ void sbv_lane_release(sbv_engine *e, int lane);
 int sbv_lane_ensure(sbv_engine *e, Dev &d, Dev::Lane &ln, size_t n, size_t pinned_bytes);
 int sbv_lane_ensure_msgs(sbv_engine *e, Dev::Lane &ln, size_t bytes, size_t n_off);
 int sbv_lane_ensure_aux(sbv_engine *e, Dev::Lane &ln, size_t bytes);
+int sbv_lane_ensure_mix(sbv_engine *e, Dev::Lane &ln, size_t bytes);
+int sbv_lane_stream2(sbv_engine *e, Dev::Lane &ln);  // creates the lane's second stream and its two events on first use
 // d_perm: n + 3072 words of scratch (may be null: no length sort)
 int sbv_launch_sha256(sbv_engine *e, size_t n, const uint8_t *d_msgs, const uint64_t *d_off, uint64_t base, uint8_t *d_digest, uint32_t *d_perm,
                       cudaStream_t st);

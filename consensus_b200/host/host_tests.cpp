@@ -521,6 +521,144 @@ static void TestEd25519CommitBatch() {
     for (auto &kv : keys) EVP_PKEY_free(kv.second.k);
 }
 
+// Commits of a mixed consenter set from the wire (marshal.hpp, CommitBatch::Mixed): consenters 1-7 hold P-256 keys, 8-9
+// P-384 keys and 10-16 Ed25519 keys.  Three instances with the Byzantine cases of TestEd25519CommitBatch, plus a DER
+// Value with a trailing byte, a 63-byte Ed25519 Value, a raw 64-byte Value from an ECDSA signer, a P-384 vote claiming an
+// Ed25519 signer and an unknown signer (all registered, rejecting), and the inert cases.  Without a GPU only the decoding
+// rules are checked; on the GPU one sbv_mixed_verify_quorum call is compared vote by vote with the VoteSet restatement.
+static void TestMixedCommitBatch() {
+    std::map<uint64_t, TestEcKey> ec;
+    std::map<uint64_t, TestEdKey> ed;
+    for (uint64_t id = 1; id <= 9; id++) ec[id] = makeEcKey(id <= 7 ? 32 : 48);
+    for (uint64_t id = 10; id <= 16; id++) ed[id] = makeEdKey();
+    auto key_of = [](uint64_t signer) -> MixedKey {
+        if (signer >= 1 && signer <= 9) return {(uint8_t)(signer <= 7 ? SBV_P256 : SBV_P384), (int)signer - 1};
+        if (signer >= 10 && signer <= 16) return {(uint8_t)SBV_ED25519, (int)signer - 10};
+        return {(uint8_t)SBV_ED25519, -1};
+    };
+    // crypto/ecdsa.VerifyASN1 or crypto/ed25519.Verify under the signer's own key
+    auto sig_valid = [&](uint64_t signer, const Bytes &val, const Bytes &msg) {
+        if (signer >= 1 && signer <= 9) return CpuVerifier::check(ec[signer].k, val, msg);
+        return signer >= 10 && signer <= 16 && verifyEd25519(ed[signer].pub, val, msg);
+    };
+    int q, f; computeQuorum(16, q, f);
+    Proposal last{{9}, {8}, ViewMetadata{0, 7, 0}.Marshal(), 1};
+    std::vector<Proposal> props3 = {fixtureProposal(), last, Proposal{{7, 7}, {1}, ViewMetadata{2, 9, 1}.Marshal(), 1}};
+    Bytes aux = PreparesFrom{{2, 3}}.Marshal();
+    struct WireVote { uint16_t sender; Bytes wire; std::optional<Vote> seen; EdCommit want; };
+    std::vector<std::vector<WireVote>> all(props3.size());
+    for (size_t pi = 0; pi < props3.size(); pi++) {
+        const Proposal &pp = props3[pi];
+        for (uint64_t id = 2; id <= 16; id++) {
+            Signature sg; sg.ID = id;
+            sg.Msg = pp.DigestRaw(); sg.Msg.insert(sg.Msg.end(), aux.begin(), aux.end());
+            sg.Value = id <= 9 ? signDerEc(ec[id].k, sg.Msg) : signEd25519(ed[id], sg.Msg);
+            uint64_t sender = id, signer = id;
+            std::string dig = pp.Digest();
+            EdCommit want = EdCommit::Verify;
+            if (pi == 0 && id == 4) sg.Value[9] ^= 2;                                        // bad P-256 signature
+            if (pi == 0 && id == 5) { sg.Value.push_back(0); want = EdCommit::Rejecting; }   // DER with a trailing byte
+            if (pi == 0 && id == 8) sg.Value[20] ^= 4;                                       // bad P-384 signature
+            if (pi == 0 && id == 11) { sg.Value.resize(63); want = EdCommit::Rejecting; }    // 63-byte Ed25519 Value
+            if (pi == 1 && id == 2) { sg.Value.assign(64, 0x30); want = EdCommit::Rejecting; }  // raw 64 bytes from a P-256 signer
+            if (pi == 1 && id == 7) dig = fixtureWrongProposal().Digest();                   // wrong digest
+            if (pi == 1 && id == 9) { signer = 10; want = EdCommit::Rejecting; }             // P-384 DER under an Ed25519 signer
+            if (pi == 1 && id == 13) { sender = signer = 99; want = EdCommit::Rejecting; }   // unknown signer
+            if (pi == 2 && id == 12) sender = 11;                                            // second vote of sender 11
+            if (pi == 2 && id >= 3 && id <= 8) sg.Value[11] ^= 1;                            // six bad signatures: quorum fails
+            if (pi == 2 && id == 14) { signer = 70000; want = EdCommit::Inert; }             // Signer beyond the 16-bit column
+            Vote vt = commitFrom(sender, signer, dig);
+            vt.commit->Sig = ProtoSignature{signer, sg.Value, sg.Msg};
+            if (pi == 0 && id == 15) { vt.commit->Sig.reset(); want = EdCommit::Inert; }     // no Signature
+            Bytes wire = MarshalCommit(*vt.commit);
+            std::optional<Vote> seen = vt;
+            if (pi == 0 && id == 16) { wire.resize(wire.size() - 3); seen.reset(); want = EdCommit::Inert; }  // truncated on the wire
+            all[pi].push_back({(uint16_t)sender, wire, seen, want});
+        }
+    }
+    // the decoding rules
+    size_t n_inert = 0, n_rejecting = 0;
+    for (auto &votes : all)
+        for (auto &w : votes) {
+            CommitView c;
+            uint8_t row[96], scheme = 0;
+            uint32_t slot = 0;
+            const EdCommit k = decode_mixed_commit(w.wire.data(), w.wire.size(), key_of, c, row, scheme, slot);
+            CHECK(k == w.want);
+            CHECK((k == EdCommit::Verify) == (slot != ED25519_NO_SLOT));
+            if (k == EdCommit::Verify) {
+                const MixedKey mk = key_of(c.Signer);
+                CHECK(scheme == mk.scheme && (int)slot == mk.slot);
+                if (scheme == SBV_ED25519) CHECK(c.value_len == 64 && memcmp(row, c.value, 64) == 0);
+                if (scheme == SBV_P256) {
+                    uint8_t r[32], s[32];
+                    CHECK(parse_der_sig_span(c.value, c.value_len, r, s) && memcmp(row, r, 32) == 0 && memcmp(row + 32, s, 32) == 0);
+                }
+                if (scheme == SBV_P384) CHECK(std::any_of(row + 48, row + 96, [](uint8_t b) { return b != 0; }));
+                if (scheme != SBV_P384) CHECK(std::all_of(row + 64, row + 96, [](uint8_t b) { return b == 0; }));
+            } else {
+                CHECK(std::all_of(row, row + 96, [](uint8_t b) { return b == 0; }));
+            }
+            n_inert += k == EdCommit::Inert;
+            n_rejecting += k == EdCommit::Rejecting;
+        }
+    CHECK(n_inert == 3 && n_rejecting == 5);
+    if (g_gpu) {
+        sbv_engine *e = nullptr;
+        CHECK(sbv_create(nullptr, 1, &e) == SBV_OK);
+        if (!e) return;
+        std::vector<uint64_t> ids(9);
+        std::vector<uint8_t> curves(9), xy(9 * 96);
+        for (uint64_t id = 1; id <= 9; id++) {
+            ids[id - 1] = id;
+            curves[id - 1] = id <= 7 ? SBV_P256 : SBV_P384;
+            memcpy(&xy[96 * (id - 1)], ec[id].xy96, 96);
+        }
+        CHECK(sbv_set_keys(e, 1, 9, ids.data(), curves.data(), xy.data()) == SBV_OK);
+        Bytes reg(7 * 32);
+        for (uint64_t id = 10; id <= 16; id++) memcpy(&reg[32 * (id - 10)], ed[id].pub, 32);
+        CHECK(sbv_ed25519_set_keys(e, 7, reg.data()) == SBV_OK);
+        std::vector<uint8_t> okv, reached; std::vector<uint32_t> cnt;
+        {
+            CommitBatch batch(CommitBatch::Mixed);
+            for (size_t pi = 0; pi < props3.size(); pi++) {
+                batch.begin_instance(props3[pi].Digest(), 1);
+                for (auto &w : all[pi]) batch.add_mixed_commit(w.sender, w.wire.data(), w.wire.size(), key_of);
+            }
+            CHECK(batch.size() == 45 && batch.instances() == 3 && batch.malformed().size() == 3 && batch.rejected().size() == 5);
+            batch.verify_and_count(e, q - 1, okv, cnt, reached);
+        }
+        size_t i = 0;
+        for (size_t pi = 0; pi < props3.size(); pi++) {
+            VoteSet set(acceptCommits);
+            int valid = 0;
+            for (auto &w : all[pi]) {
+                const size_t at = i++;
+                bool sig_ok = false;
+                if (w.seen && w.seen->commit->Sig) {
+                    const ProtoSignature &ps = *w.seen->commit->Sig;
+                    sig_ok = sig_valid(ps.Signer, ps.Value, ps.Msg);
+                }
+                CHECK(okv[at] == (w.want == EdCommit::Verify && sig_ok ? 1 : 0));  // inert and rejecting rows reject
+                if (!w.seen || w.seen->sender == 1) continue;
+                size_t before = set.votes().size();
+                set.registerVote(w.seen->sender, *w.seen);
+                if (set.votes().size() == before) continue;
+                if (w.seen->commit->Digest == props3[pi].Digest() && sig_ok && w.want == EdCommit::Verify) valid++;
+            }
+            CHECK((int)cnt[pi] == valid);
+            CHECK(reached[pi] == (valid >= q - 1 ? 1 : 0));
+        }
+        // instance 0: two bad signatures, two rejecting rows and two inert votes leave 9 < Q - 1; instance 1: a rejecting row,
+        // a wrong digest, a foreign signer and an unknown signer leave 11; instance 2 as in TestEd25519CommitBatch
+        CHECK(cnt[0] == 9 && cnt[1] == 11 && cnt[2] == 7);
+        CHECK(reached[0] == 0 && reached[1] == 1 && reached[2] == 0);
+        sbv_destroy(e);
+    }
+    for (auto &kv : ec) EC_KEY_free(kv.second.k);
+    for (auto &kv : ed) EVP_PKEY_free(kv.second.k);
+}
+
 int main(int argc, char **argv) {
     std::string mode = argc > 1 ? argv[1] : "cpu";
     RUN(TestProposalDigestFixtures);
@@ -538,6 +676,7 @@ int main(int argc, char **argv) {
     if (mode == "gpu") RUN(TestGpuVerifierEndToEnd);
     g_gpu = mode == "gpu";
     RUN(TestEd25519CommitBatch);
+    RUN(TestMixedCommitBatch);
     printf("%d checks, %d failures\n", g_checks, g_fail);
     return g_fail ? 1 : 0;
 }

@@ -14,6 +14,11 @@
 // An Ed25519 batch (CommitBatch::Ed25519) takes Commits whose Signature.Value is a raw 64-byte Ed25519 signature: the r and
 // s columns together hold one 64-byte row (R || S) per vote, the slots index the engine's Ed25519 registry
 // (sbv_ed25519_set_keys), and verify_and_count makes one sbv_ed25519_verify_quorum call.
+//
+// A mixed batch (CommitBatch::Mixed) takes Commits of a consenter set whose keys may be P-256, P-384 or Ed25519:
+// key_of(signer) gives the signer's scheme and its slot of that scheme's registry, each vote gets a scheme tag and one
+// 96-byte signature row (DER r, s parsed into r || s of the curve's width, or the raw R || S), and verify_and_count makes
+// one sbv_mixed_verify_quorum call.
 #pragma once
 #include "verifier.hpp"
 #include "callsites.hpp"
@@ -138,11 +143,69 @@ inline EdCommit decode_ed25519_commit(const uint8_t *wire, size_t len, SlotOf &&
     return EdCommit::Verify;
 }
 
+// Strict DER SEQUENCE{INTEGER r, INTEGER s} (crypto/ecdsa.VerifyASN1 rules) into r || s of width L each (32 for P-256,
+// 48 for P-384), right-aligned.
+inline bool parse_der_sig_width(const uint8_t *sig, size_t n, uint8_t *r, uint8_t *s, size_t L) {
+    auto rd_int = [L](const uint8_t *&p, const uint8_t *end, uint8_t *out) {
+        if (end - p < 2 || p[0] != 0x02) return false;
+        size_t len = p[1];
+        p += 2;
+        if ((len & 0x80) || len == 0 || (size_t)(end - p) < len) return false;
+        if (p[0] & 0x80) return false;
+        if (len > 1 && p[0] == 0 && !(p[1] & 0x80)) return false;
+        const uint8_t *v = p; size_t vl = len;
+        if (vl > 1 && v[0] == 0) { v++; vl--; }
+        if (vl > L) return false;
+        memset(out, 0, L); memcpy(out + L - vl, v, vl);
+        p += len;
+        return true;
+    };
+    const uint8_t *p = sig, *end = sig + n;
+    if (n < 2 || p[0] != 0x30) return false;
+    size_t len;
+    if (p[1] < 0x80) { len = p[1]; p += 2; }
+    else if (p[1] == 0x81) { if (n < 3 || p[2] < 0x80) return false; len = p[2]; p += 3; }
+    else return false;
+    if ((size_t)(end - p) != len) return false;
+    return rd_int(p, end, r) && rd_int(p, end, s) && p == end;
+}
+
+// A signer's key in a mixed consenter set: its scheme (SBV_P256, SBV_P384 or SBV_ED25519) and its slot of that
+// scheme's registry (sbv_set_keys or sbv_ed25519_set_keys); slot < 0: the signer has no key.
+struct MixedKey { uint8_t scheme; int slot; };
+
+// How a wire Commit enters a mixed batch, by the same registration rule as decode_ed25519_commit: Inert for undecodable
+// bytes, no Signature or a Signer beyond 16 bits; otherwise registered, and Rejecting when the signer has no key or its
+// Value does not parse for the signer's scheme (strict DER for ECDSA, exactly 64 bytes for Ed25519).  row: the vote's
+// 96-byte signature row, written for Verify and zeroed otherwise; scheme / slot: what the row is verified as (a rejecting
+// or inert vote carries SBV_ED25519 or its signer's scheme and ED25519_NO_SLOT, which rejects on the device).
+template <class KeyOf>
+inline EdCommit decode_mixed_commit(const uint8_t *wire, size_t len, KeyOf &&key_of, CommitView &c, uint8_t *row, uint8_t &scheme, uint32_t &slot) {
+    slot = ED25519_NO_SLOT;
+    scheme = SBV_ED25519;
+    memset(row, 0, 96);
+    if (!DecodeCommit(wire, len, c) || !c.has_sig || c.Signer > 0xffff) return EdCommit::Inert;
+    const MixedKey k = key_of(c.Signer);
+    if (k.slot < 0 || k.scheme > SBV_ED25519) return EdCommit::Rejecting;
+    scheme = k.scheme;
+    bool parsed;
+    if (k.scheme == SBV_ED25519) {
+        parsed = c.value_len == 64;
+        if (parsed) memcpy(row, c.value, 64);
+    } else {
+        const size_t L = k.scheme == SBV_P256 ? 32 : 48;
+        parsed = parse_der_sig_width(c.value, c.value_len, row, row + L, L);
+    }
+    if (!parsed) { memset(row, 0, 96); return EdCommit::Rejecting; }
+    slot = (uint32_t)k.slot;
+    return EdCommit::Verify;
+}
+
 // One batch of commit votes (many instances = consensus sequences in flight, or many views during catch-up).
 class CommitBatch {
   public:
-    enum Scheme { EcdsaP256, Ed25519 };
-    explicit CommitBatch(Scheme scheme = EcdsaP256) : ed25519_(scheme == Ed25519) {}
+    enum Scheme { EcdsaP256, Ed25519, Mixed };
+    explicit CommitBatch(Scheme scheme = EcdsaP256) : ed25519_(scheme == Ed25519), mixed_(scheme == Mixed) {}
     size_t size() const { return n_; }
     size_t instances() const { return n_inst_; }
     void clear() { n_ = 0; msg_bytes_ = 0; n_inst_ = 0; malformed_.clear(); rejected_.clear(); }
@@ -157,7 +220,7 @@ class CommitBatch {
     }
     // Decodes one wire Commit received from `sender` and appends it to the current instance.  `slot_of(signer)` maps
     // the claimed signer to its slot of the engine's key registry (sbv_set_keys, or sbv_ed25519_set_keys for an Ed25519
-    // batch), < 0 when unknown.
+    // batch), < 0 when unknown.  A mixed batch takes add_mixed_commit instead.
     // Malformed input never throws: the vote is recorded as one that cannot count (the reference drops such votes:
     // view.go:161-171, 839-842).  An Ed25519 batch follows decode_ed25519_commit instead.
     template <class SlotOf>
@@ -197,12 +260,45 @@ class CommitBatch {
         slt()[i] = (uint32_t)slot;
         append_registered(i, c);
     }
+    // The same for a mixed batch (CommitBatch::Mixed only): key_of(signer) -> MixedKey gives the signer's scheme and slot, and
+    // the vote follows decode_mixed_commit.
+    template <class KeyOf>
+    void add_mixed_commit(uint16_t sender, const uint8_t *wire, size_t len, KeyOf &&key_of) {
+        grow(n_ + 1);
+        const size_t i = n_++;
+        inst()[i] = (uint32_t)(n_inst_ - 1);
+        snd()[i] = sender;
+        CommitView c;
+        uint32_t slot = ED25519_NO_SLOT;
+        uint8_t scheme = SBV_ED25519;
+        uint8_t *row = rows_.p + 96 * i;
+        EdCommit k = EdCommit::Inert;
+        if (n_inst_ > 0) k = decode_mixed_commit(wire, len, key_of, c, row, scheme, slot);
+        else memset(row, 0, 96);
+        slt()[i] = slot;
+        tags_.p[i] = scheme;
+        if (k == EdCommit::Inert) {  // signer != sender keeps it out of the vote set
+            sig()[i] = (uint16_t)(sender + 1); dm()[i] = 0;
+            off()[i + 1] = msg_bytes_;
+            malformed_.push_back(i);
+            return;
+        }
+        if (k == EdCommit::Rejecting) rejected_.push_back(i);
+        append_registered(i, c);
+    }
     // Verifies every signature (SHA-256 of Signature.Msg on the device, registered keys) and counts the valid distinct
     // foreign votes per instance.  ok / count / reached are sized by the call.
-    // An Ed25519 batch makes one sbv_ed25519_verify_quorum call (Signature.Msg hashed with SHA-512 on the device).
+    // An Ed25519 batch makes one sbv_ed25519_verify_quorum call (Signature.Msg hashed with SHA-512 on the device), a mixed
+    // batch one sbv_mixed_verify_quorum call.
     void verify_and_count(sbv_engine *e, uint32_t threshold, std::vector<uint8_t> &ok, std::vector<uint32_t> &count, std::vector<uint8_t> &reached) {
         ok.assign(n_, 0); count.assign(n_inst_, 0); reached.assign(n_inst_, 0);
         if (n_ == 0 || n_inst_ == 0) return;
+        if (mixed_) {
+            if (sbv_mixed_verify_quorum(e, n_, tags_.p, msgs_.p, off(), slt(), rows_.p, inst(), snd(), sig(), dm(), n_inst_, (const uint16_t *)self_.p,
+                                        threshold, ok.data(), count.data(), reached.data()) != SBV_OK)
+                throw EngineFault(std::string("sbv_mixed_verify_quorum: ") + sbv_last_error(e));
+            return;
+        }
         if (ed25519_) {
             if (sbv_ed25519_verify_quorum(e, n_, msgs_.p, off(), slt(), r(), inst(), snd(), sig(), dm(), n_inst_, (const uint16_t *)self_.p, threshold,
                                           ok.data(), count.data(), reached.data()) != SBV_OK)
@@ -215,8 +311,10 @@ class CommitBatch {
             throw EngineFault(std::string("sbv_quorum: ") + sbv_last_error(e));
     }
     const std::vector<size_t> &malformed() const { return malformed_; }
-    const std::vector<size_t> &rejected() const { return rejected_; }  // Ed25519: registered votes with a rejecting row
+    const std::vector<size_t> &rejected() const { return rejected_; }  // Ed25519 / mixed: registered votes with a rejecting row
     const uint8_t *r_rows() const { return cols_.p; }
+    const uint8_t *mixed_rows() const { return rows_.p; }    // mixed: the 96-byte signature rows
+    const uint8_t *mixed_schemes() const { return tags_.p; }  // mixed: the scheme tag of every vote
 
   private:
     // signer, digest match and message of a vote that enters the vote set
@@ -246,6 +344,10 @@ class CommitBatch {
         else
             memset(at(nb.p, nc, 2), 0, 8);
         std::swap(cols_.p, nb.p); std::swap(cols_.cap, nb.cap);
+        if (mixed_) {  // the signature rows and scheme tags of a mixed batch live beside the column block
+            rows_.reserve(nc * 96, n_ * 96);
+            tags_.reserve(nc, n_);
+        }
         cap_ = nc;
     }
     uint8_t *col(int k) const {
@@ -263,11 +365,11 @@ class CommitBatch {
     uint16_t *sig() const { return (uint16_t *)col(6); }
     uint8_t *dm() const { return col(7); }
 
-    PinnedBuf cols_, msgs_, self_;
+    PinnedBuf cols_, msgs_, self_, rows_, tags_;
     size_t cap_ = 0, n_ = 0, msg_bytes_ = 0, n_inst_ = 0;
     std::string expected_;
     std::vector<size_t> malformed_, rejected_;
-    bool ed25519_ = false;
+    bool ed25519_ = false, mixed_ = false;
 };
 
 }  // namespace sbft

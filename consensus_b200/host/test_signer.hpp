@@ -40,6 +40,27 @@ inline Signature signProposal(uint64_t id, const TestKey &k, const Proposal &p, 
 }
 
 
+// An ECDSA key on P-256 (L = 32) or P-384 (L = 48); xy96 = X || Y in 48-byte slots, right-aligned, as sbv_set_keys takes
+// them.  signDerEc: DER ECDSA over SHA-256(msg), as signDer.
+struct TestEcKey { EC_KEY *k; uint8_t xy96[96]; };
+inline TestEcKey makeEcKey(int L) {
+    TestEcKey t{EC_KEY_new_by_curve_name(L == 32 ? NID_X9_62_prime256v1 : NID_secp384r1), {}};
+    EC_KEY_generate_key(t.k);
+    BIGNUM *x = BN_new(), *y = BN_new();
+    EC_POINT_get_affine_coordinates(EC_KEY_get0_group(t.k), EC_KEY_get0_public_key(t.k), x, y, nullptr);
+    BN_bn2binpad(x, t.xy96 + 48 - L, L); BN_bn2binpad(y, t.xy96 + 96 - L, L);
+    BN_free(x); BN_free(y);
+    return t;
+}
+inline Bytes signDerEc(EC_KEY *k, const Bytes &msg) {
+    Bytes dig = sha256(msg);
+    unsigned int len = ECDSA_size(k);
+    Bytes sig(len);
+    ECDSA_sign(0, dig.data(), 32, sig.data(), &len, k);
+    sig.resize(len);
+    return sig;
+}
+
 // Ed25519 consenter keys (OpenSSL EVP_PKEY_ED25519): Value = the raw 64-byte signature (R || S) over Signature.Msg.
 struct TestEdKey { EVP_PKEY *k; uint8_t pub[32]; };
 inline TestEdKey makeEdKey() {

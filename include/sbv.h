@@ -52,7 +52,9 @@ extern "C" {
 
 typedef struct sbv_engine sbv_engine;
 
-enum { SBV_P256 = 0, SBV_P384 = 1 };
+/* Scheme tags.  The calls that take a curve (or a curve tag per item) accept SBV_P256 and SBV_P384 only and return
+ * SBV_ERR_ARG for SBV_ED25519; only the sbv_mixed_* calls take all three. */
+enum { SBV_P256 = 0, SBV_P384 = 1, SBV_ED25519 = 2 };
 enum {
     SBV_OK = 0,
     SBV_ERR_ARG = -1,   /* bad argument */
@@ -169,6 +171,33 @@ int sbv_ed25519_verify_quorum(sbv_engine *e, size_t n_votes, const uint8_t *msgs
                               const uint16_t *sender, const uint16_t *signer, const uint8_t *digest_match,
                               size_t n_instances, const uint16_t *self_id, uint32_t threshold, uint8_t *ok,
                               uint32_t *valid_count, uint8_t *reached);
+
+/* Registered-key batch whose items may be of any scheme (a consenter or client set that mixes ECDSA and Ed25519 keys,
+ * e.g. while it moves from one to the other).  scheme[i] in {SBV_P256, SBV_P384, SBV_ED25519}; msgs concatenated with
+ * msg_off[n+1] byte offsets (msgs may be NULL when every message is empty); sig96 = one 96-byte row per item:
+ *   P-256    r || s, 32 bytes each, big-endian, in bytes [0, 64)
+ *   P-384    r || s, 48 bytes each, big-endian, filling the row
+ *   Ed25519  R || S as RFC 8032 encodes them, in bytes [0, 64)
+ * Bytes past the signature are ignored.  key_slot[i] indexes the registry of the item's own scheme: sbv_set_keys for
+ * ECDSA, sbv_ed25519_set_keys for Ed25519 (slot 3 of an ECDSA item and slot 3 of an Ed25519 item are different keys).
+ * ok[i] is byte for byte what the single-scheme call returns for item i: sbv_hash_verify_registered(scheme[i], ...)
+ * for ECDSA items, sbv_ed25519_verify_registered for Ed25519 items.  The shard of each device is uploaded once, whole,
+ * and split into the three families on the device; the ECDSA families run on the call's stream while the Ed25519 one
+ * runs beside them on its second stream, and the verdicts are put back in item order on the device.  A tag > 2 returns
+ * SBV_ERR_ARG with its index in sbv_last_error, before anything is written or launched.  Every shard of one call reads
+ * the same Ed25519 registry, as in sbv_ed25519_verify_registered. */
+int sbv_mixed_verify_registered(sbv_engine *e, size_t n, const uint8_t *scheme, const uint8_t *msgs, const uint64_t *msg_off,
+                                const uint32_t *key_slot, const uint8_t *sig96, uint8_t *ok);
+/* Commit votes of a mixed consenter set verified and counted in one call (verifyVote + processCommits,
+ * view.go:519-551, 827-849): ok = the verdicts of sbv_mixed_verify_registered, valid_count / reached = sbv_quorum over
+ * them, with the same vote rules, self_id (NULL = no self filter) and threshold.  The verdicts stay on the device.  Votes
+ * must be grouped by instance with non-decreasing instance ids; a multi-device engine shards BY INSTANCE, as
+ * sbv_verify_quorum does.  Outputs: ok[n_votes], valid_count[n_instances], reached[n_instances]; n_instances == 0 does
+ * nothing. */
+int sbv_mixed_verify_quorum(sbv_engine *e, size_t n_votes, const uint8_t *scheme, const uint8_t *msgs, const uint64_t *msg_off,
+                            const uint32_t *key_slot, const uint8_t *sig96, const uint32_t *instance, const uint16_t *sender,
+                            const uint16_t *signer, const uint8_t *digest_match, size_t n_instances, const uint16_t *self_id,
+                            uint32_t threshold, uint8_t *ok, uint32_t *valid_count, uint8_t *reached);
 
 /* computeQuorum(n) -> (q, f), internal/bft/util.go:183-187. */
 void sbv_compute_quorum(uint64_t n, uint32_t *q, uint32_t *f);

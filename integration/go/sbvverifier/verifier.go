@@ -222,71 +222,12 @@ func (b *pinned) reserve(n int) []byte {
 	return unsafe.Slice((*byte)(b.p), b.cap)[:n]
 }
 
-// engineBatch dispatches an aggregated batch by key type: the ECDSA items in one sbv_hash_verify_registered call,
-// the Ed25519 items in one sbv_ed25519_verify_registered call; verdicts come back in the items' order.
+// engineBatch verifies an aggregated batch in one sbv_mixed_verify_registered call, whatever keys its items hold: the
+// engine splits the items by scheme on the GPU, hashes each message there (SHA-256 for ECDSA, SHA-512(R || A || M) for
+// Ed25519) and verifies it against the item's registered key; verdicts come back in the items' order. The batch is
+// marshalled once, straight into pinned memory (one block per in-flight batch, pooled):
+// rows (96n: P-256 r || s or Ed25519 R || S in bytes [0, 64)) | slot (4n) | off (8(n+1)) | scheme (n) | msgs.
 func (v *Verifier) engineBatch(items []item) []byte {
-	var ec, ed []item
-	var ecAt, edAt []int
-	for i := range items {
-		if items[i].ed {
-			ed, edAt = append(ed, items[i]), append(edAt, i)
-		} else {
-			ec, ecAt = append(ec, items[i]), append(ecAt, i)
-		}
-	}
-	ok := make([]byte, len(items))
-	if len(ec) > 0 {
-		for j, o := range v.ecdsaBatch(ec) {
-			ok[ecAt[j]] = o
-		}
-	}
-	if len(ed) > 0 {
-		for j, o := range v.ed25519Batch(ed) {
-			ok[edAt[j]] = o
-		}
-	}
-	return ok
-}
-
-// ed25519Batch: SHA-512(R || A || M) over the registered bytes of each item's key and the Ed25519 equation over the
-// key's fixed-base table, both on the GPU. Marshalled into pinned memory: sig (64n) | slot (4n) | off | msgs.
-func (v *Verifier) ed25519Batch(items []item) []byte {
-	v.syncRegistry()
-	n := len(items)
-	ok := make([]byte, n)
-	total := 0
-	for i := range items {
-		total += len(items[i].msg)
-	}
-	oSlot := 64 * n
-	oOff := (oSlot + 4*n + 7) &^ 7
-	oMsgs := oOff + 8*(n+1)
-	pb := v.pool.Get().(*pinned)
-	defer v.pool.Put(pb)
-	buf := pb.reserve(oMsgs + total + 16)
-	pos := 0
-	binary.LittleEndian.PutUint64(buf[oOff:], 0)
-	for i := range items {
-		copy(buf[64*i:], items[i].edSig[:])
-		binary.LittleEndian.PutUint32(buf[oSlot+4*i:], items[i].slot)
-		copy(buf[oMsgs+pos:], items[i].msg)
-		pos += len(items[i].msg)
-		binary.LittleEndian.PutUint64(buf[oOff+8*(i+1):], uint64(pos))
-	}
-	base := uintptr(pb.p)
-	rc := C.sbv_ed25519_verify_registered(v.eng, C.size_t(n), (*C.uint8_t)(unsafe.Pointer(base+uintptr(oMsgs))),
-		(*C.uint64_t)(unsafe.Pointer(base+uintptr(oOff))), (*C.uint32_t)(unsafe.Pointer(base+uintptr(oSlot))),
-		(*C.uint8_t)(unsafe.Pointer(base)), (*C.uint8_t)(unsafe.Pointer(&ok[0])))
-	if rc != 0 {
-		v.fault("sbv_ed25519_verify_registered", rc)
-	}
-	return ok
-}
-
-// ecdsaBatch: SHA-256 of every message and ECDSA verification against the registered keys, both on the GPU.
-// The batch is marshalled straight into pinned memory (one block per in-flight batch, pooled):
-// r | s | slot | off | msgs.
-func (v *Verifier) ecdsaBatch(items []item) []byte {
 	v.syncRegistry()
 	n := len(items)
 	ok := make([]byte, n)
@@ -297,29 +238,36 @@ func (v *Verifier) ecdsaBatch(items []item) []byte {
 	for i := range items {
 		total += len(items[i].msg)
 	}
-	oS, oSlot := 32*n, 64*n
+	oSlot := 96 * n
 	oOff := (oSlot + 4*n + 7) &^ 7
-	oMsgs := oOff + 8*(n+1)
+	oScheme := oOff + 8*(n+1)
+	oMsgs := oScheme + n
 	pb := v.pool.Get().(*pinned)
 	defer v.pool.Put(pb)
 	buf := pb.reserve(oMsgs + total + 16)
 	pos := 0
 	binary.LittleEndian.PutUint64(buf[oOff:], 0)
 	for i := range items {
-		copy(buf[32*i:], items[i].r[:])
-		copy(buf[oS+32*i:], items[i].s[:])
+		row := buf[96*i : 96*i+96]
+		if items[i].ed {
+			copy(row, items[i].edSig[:])
+			buf[oScheme+i] = byte(C.SBV_ED25519)
+		} else {
+			copy(row, items[i].r[:])
+			copy(row[32:], items[i].s[:])
+			buf[oScheme+i] = byte(C.SBV_P256)
+		}
 		binary.LittleEndian.PutUint32(buf[oSlot+4*i:], items[i].slot)
 		copy(buf[oMsgs+pos:], items[i].msg)
 		pos += len(items[i].msg)
 		binary.LittleEndian.PutUint64(buf[oOff+8*(i+1):], uint64(pos))
 	}
 	base := uintptr(pb.p)
-	rc := C.sbv_hash_verify_registered(v.eng, C.SBV_P256, C.size_t(n),
+	rc := C.sbv_mixed_verify_registered(v.eng, C.size_t(n), (*C.uint8_t)(unsafe.Pointer(base+uintptr(oScheme))),
 		(*C.uint8_t)(unsafe.Pointer(base+uintptr(oMsgs))), (*C.uint64_t)(unsafe.Pointer(base+uintptr(oOff))),
-		(*C.uint32_t)(unsafe.Pointer(base+uintptr(oSlot))), (*C.uint8_t)(unsafe.Pointer(base)),
-		(*C.uint8_t)(unsafe.Pointer(base+uintptr(oS))), (*C.uint8_t)(unsafe.Pointer(&ok[0])))
+		(*C.uint32_t)(unsafe.Pointer(base+uintptr(oSlot))), (*C.uint8_t)(unsafe.Pointer(base)), (*C.uint8_t)(unsafe.Pointer(&ok[0])))
 	if rc != 0 {
-		v.fault("sbv_hash_verify_registered", rc)
+		v.fault("sbv_mixed_verify_registered", rc)
 	}
 	return ok
 }

@@ -23,6 +23,7 @@ namespace sbv { uint32_t tab[1 << 18]; }
 #include "../../consensus_b200/csrc/ed25519_verify.cuh"
 #include "../../consensus_b200/csrc/ed25519_keyed.cuh"
 #include "../../consensus_b200/csrc/shards.h"
+#include "../../consensus_b200/csrc/mixed.cuh"
 
 using namespace sbv;
 
@@ -449,5 +450,96 @@ extern "C" int hs_ed25519_verify_registered_k(size_t n, const uint32_t *key_slot
         if (!mp_lt<8>(ki, Lm)) return -1;
     }
     ed_verify_keyed_host(n, key_slot, sig, k.data(), ok);
+    return 0;
+}
+
+// ---- mixed ECDSA / Ed25519 shards (mixed.cuh) ----
+// The caller's arrays as the plan of a shard with m = {m0, m1, n - m0 - m1} items per family: idx, slot and ok hold the
+// three families one after the other (n entries each), off their m_f + 1 offsets one after the other (n + 3 entries);
+// r0 / s0 (32 B per item), r1 / s1 (48 B) and sig2 (64-byte rows) are per family; blob is the shared message buffer.
+static MixPlan hs_plan(size_t n, uint32_t m0, uint32_t m1, uint32_t *idx, uint32_t *slot, uint8_t *r0, uint8_t *s0, uint8_t *r1, uint8_t *s1,
+                       uint8_t *sig2, uint64_t *off, uint8_t *blob, uint8_t *ok) {
+    const uint32_t at[3] = {0, m0, m0 + m1};
+    MixPlan p;
+    for (int f = 0; f < MIX_FAMILIES; f++)
+        p.f[f] = MixFamily{idx ? idx + at[f] : nullptr, slot ? slot + at[f] : nullptr, f == 0 ? r0 : f == 1 ? r1 : sig2, f == 0 ? s0 : f == 1 ? s1 : nullptr,
+                           off ? off + at[f] + f : nullptr, ok ? ok + at[f] : nullptr};
+    p.blob = blob;
+    (void)n;
+    return p;
+}
+// k_mix_count, k_mix_scan (as one thread: the simulation has no block barrier) and k_mix_split over a shard whose offsets
+// are off_in[0..n]
+extern "C" int hs_mixed_split(size_t n, const uint8_t *tag, const uint32_t *slot_in, const uint8_t *sig96, const uint64_t *off_in, uint32_t m0, uint32_t m1,
+                              uint32_t *idx, uint32_t *slot, uint8_t *r0, uint8_t *s0, uint8_t *r1, uint8_t *s1, uint8_t *sig2, uint64_t *off_out) {
+    const MixPlan p = hs_plan(n, m0, m1, idx, slot, r0, s0, r1, s1, sig2, off_out, nullptr, nullptr);
+    const uint32_t nn = (uint32_t)n, ntiles = (uint32_t)((n + MIX_TILE - 1) / MIX_TILE);
+    std::vector<uint32_t> tc((size_t)MIX_FAMILIES * ntiles + 1);
+    std::vector<uint64_t> tb((size_t)MIX_FAMILIES * ntiles + 1);
+    run_grid((ntiles + 255) / 256, 256, [&] { k_mix_count(nn, tag, off_in, ntiles, tc.data(), tb.data()); });
+    run_grid(1, 1, [&] { k_mix_scan(ntiles, tc.data(), tb.data(), p); });
+    run_grid((ntiles + 255) / 256, 256, [&] { k_mix_split(nn, tag, slot_in, sig96, off_in, ntiles, tc.data(), tb.data(), p); });
+    return 0;
+}
+// k_mix_compact: the messages of src (offsets off_in from base; src readable 8 bytes past the last one) into blob at the
+// split's offsets
+extern "C" int hs_mixed_compact(size_t n, uint32_t m0, uint32_t m1, const uint8_t *src, const uint64_t *off_in, uint64_t base, const uint32_t *idx,
+                                const uint64_t *off_out, uint8_t *blob) {
+    const MixPlan p = hs_plan(n, m0, m1, const_cast<uint32_t *>(idx), nullptr, nullptr, nullptr, nullptr, nullptr, nullptr,
+                              const_cast<uint64_t *>(off_out), blob, nullptr);
+    run_grid((unsigned)((n * MIX_LANES + 255) / 256), 256, [&] { k_mix_compact((uint32_t)n, m0, m1, src, off_in, base, p); });
+    return 0;
+}
+// k_mix_ok: the family verdicts ok_fam (compacted order) back to item order
+extern "C" int hs_mixed_scatter(size_t n, uint32_t m0, uint32_t m1, const uint32_t *idx, const uint8_t *ok_fam, uint8_t *ok) {
+    const MixPlan p = hs_plan(n, m0, m1, const_cast<uint32_t *>(idx), nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr,
+                              const_cast<uint8_t *>(ok_fam));
+    run_grid((unsigned)((n + 255) / 256), 256, [&] { k_mix_ok((uint32_t)n, m0, m1, p, ok); });
+    return 0;
+}
+// The pipeline of sbv_mixed_verify_registered on one device: split, compaction, then per ECDSA family hs_sha256 and
+// hs_verify_registered against the keys of that curve in the ECDSA registry (nkeys keys: curve tags, X || Y in 48-byte
+// slots as sbv_set_keys takes them; a slot >= nkeys or of the other curve rejects), hs_ed25519_verify_registered against
+// the registry of hs_ed25519_set_keys for the Ed25519 family, and the scatter.  Tags must be <= 2.
+extern "C" int hs_mixed_verify_registered(size_t n, const uint8_t *tag, const uint8_t *msgs, const uint64_t *off, const uint32_t *slot_in,
+                                          const uint8_t *sig96, size_t nkeys, const uint8_t *key_curve, const uint8_t *key_xy, uint8_t *ok) {
+    uint32_t m[3] = {0, 0, 0};
+    for (size_t i = 0; i < n; i++) {
+        if (tag[i] > 2) return -1;
+        m[tag[i]]++;
+    }
+    const uint64_t base = off[0], bytes = off[n] - base;
+    std::vector<uint8_t> src(bytes + 16, 0);
+    if (bytes) memcpy(src.data(), msgs + base, bytes);
+    std::vector<uint32_t> idx(n + 1), slot(n + 1);
+    std::vector<uint8_t> r0(32 * m[0] + 1), s0(32 * m[0] + 1), r1(48 * m[1] + 1), s1(48 * m[1] + 1), sig2(64 * m[2] + 1), blob(bytes + 128, 0), okf(n + 1, 0);
+    std::vector<uint64_t> fo(n + 3);
+    hs_mixed_split(n, tag, slot_in, sig96, off, m[0], m[1], idx.data(), slot.data(), r0.data(), s0.data(), r1.data(), s1.data(), sig2.data(), fo.data());
+    hs_mixed_compact(n, m[0], m[1], src.data(), off, base, idx.data(), fo.data(), blob.data());
+    const uint32_t at[3] = {0, m[0], m[0] + m[1]};
+    for (int f = 0; f < 2; f++) {
+        if (!m[f]) continue;
+        const size_t L = f ? 48 : 32;
+        std::vector<uint8_t> dig(32 * m[f]), kx, ky;
+        hs_sha256(m[f], blob.data(), fo.data() + at[f] + f, 0, nullptr, dig.data());
+        std::vector<int64_t> local(nkeys, -1);
+        uint32_t nloc = 0;
+        for (size_t k = 0; k < nkeys; k++)
+            if (key_curve[k] == f) {
+                local[k] = nloc++;
+                kx.insert(kx.end(), key_xy + 96 * k + 48 - L, key_xy + 96 * k + 48);
+                ky.insert(ky.end(), key_xy + 96 * k + 96 - L, key_xy + 96 * k + 96);
+            }
+        if (!nloc) continue;  // no key of this curve: every item rejects (okf is zero)
+        std::vector<uint32_t> ls(m[f]);
+        for (uint32_t j = 0; j < m[f]; j++) {
+            const uint32_t s = slot[at[f] + j];
+            ls[j] = s < nkeys && local[s] >= 0 ? (uint32_t)local[s] : nloc;
+        }
+        hs_verify_registered(f, m[f], nloc, kx.data(), ky.data(), ls.data(), f ? r1.data() : r0.data(), f ? s1.data() : s0.data(), dig.data(), 32, 0,
+                             okf.data() + at[f]);
+    }
+    if (m[2]) hs_ed25519_verify_registered(m[2], blob.data(), fo.data() + at[2] + 2, slot.data() + at[2], sig2.data(), okf.data() + at[2]);
+    hs_mixed_scatter(n, m[0], m[1], idx.data(), okf.data(), ok);
     return 0;
 }
