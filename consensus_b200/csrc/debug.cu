@@ -183,6 +183,83 @@ extern "C" int sbv_debug_ed25519_ktab(sbv_engine *e, uint32_t slot, size_t first
     return SBV_OK;
 }
 
+// The comb tables of a keys-per-item launch of the n keys of pub (32 bytes each) on device 0, grouped with the engine's
+// settings (SBV_GROUP_THRESHOLD, SBV_GROUP_MAX_KEYS, SBV_GROUP_MIN_BATCH).  For each of the m query items items[q] < n:
+// status[q] = 0 and the key's table at out + q * 510 * 24 (entry b * 255 + mask - 1 = the sum of 2^(16 (8b + t)) * A over
+// the set bits t of mask, as y + x, y - x, 2dxy, 24 limbs); 1 when the key got no table (fewer items than the threshold,
+// table slots used up, or a launch that does not group); 2 when it got a table slot but does not decode.
+extern "C" int sbv_debug_ed25519_comb_tab(sbv_engine *e, size_t n, const uint8_t *pub, size_t m, const uint32_t *items, int32_t *status,
+                                          uint32_t *out) {
+    if (!e || !pub || (m && (!items || !status || !out)) || n > UINT32_MAX) return SBV_ERR_ARG;
+    for (size_t q = 0; q < m; q++)
+        if (items[q] >= n) return SBV_ERR_ARG;
+    if (n == 0) return SBV_OK;
+    std::lock_guard<std::mutex> lk(e->mu);
+    Dev &d = e->devs[0];
+    CU(e, cudaSetDevice(d.ordinal));
+    int rc = sbv_ensure_scratch(e, d, n * 32 + 1024);
+    if (rc) return rc;
+    CU(e, cudaMemcpyAsync(d.d_scratch, pub, n * 32, cudaMemcpyHostToDevice, d.stream));
+    Dev::Scratch *w = nullptr;
+    if ((rc = sbv_launch_ed_comb_tables(e, d, n, d.d_scratch, d.stream, &w))) return rc;
+    const size_t words = SBV_ED_COMB_ENTRIES * SBV_ED_BTAB_ENTRY_WORDS;
+    for (size_t q = 0; q < m && !rc; q++) {
+        status[q] = 1;
+        if (!w) continue;
+        uint32_t r = 0;
+        int32_t kid = -1;
+        uint8_t flag = 0;
+        cudaError_t st = cudaMemcpy(&r, (uint32_t *)w->rep + items[q], 4, cudaMemcpyDeviceToHost);
+        if (st == cudaSuccess) st = cudaMemcpy(&kid, (int32_t *)w->keyid + r, 4, cudaMemcpyDeviceToHost);
+        if (st == cudaSuccess && kid >= 0) st = cudaMemcpy(&flag, (uint8_t *)w->keyflags + kid, 1, cudaMemcpyDeviceToHost);
+        if (st == cudaSuccess && kid >= 0 && flag)
+            st = cudaMemcpy(out + q * words, (uint32_t *)w->ktab + (size_t)kid * words, words * 4, cudaMemcpyDeviceToHost);
+        if (st != cudaSuccess) rc = sbv_fail(e, SBV_ERR_CUDA, "sbv_debug_ed25519_comb_tab: %s", cudaGetErrorString(st));
+        else if (kid >= 0) status[q] = flag ? 0 : 2;
+    }
+    if (w) {
+        const cudaError_t st = cudaEventRecord(w->done, d.stream);
+        if (!rc && st != cudaSuccess) rc = sbv_fail(e, SBV_ERR_CUDA, "cudaEventRecord: %s", cudaGetErrorString(st));
+    }
+    return rc;
+}
+
+// The comb kernel of grouped keys (k_ed_verify_comb) on device 0 with the caller's k in place of SHA-512(R || A || M) mod
+// L: every distinct key of pub gets a comb table and every item takes the comb kernel.  k = 8 little-endian limbs per item,
+// each < L (SBV_ERR_ARG otherwise); sig = R || S (64 bytes), pub = 32 bytes per item.
+extern "C" int sbv_debug_ed25519_verify_comb_k(sbv_engine *e, size_t n, const uint8_t *sig, const uint8_t *pub, const uint32_t *k, uint8_t *ok) {
+    if (!e || !sig || !pub || !k || !ok || n > UINT32_MAX) return SBV_ERR_ARG;
+    static const uint32_t L[8] = {0x5cf5d3ed, 0x5812631a, 0xa2f79cd6, 0x14def9de, 0, 0, 0, 0x10000000};
+    for (size_t i = 0; i < n; i++) {
+        int w = 7;
+        while (w > 0 && k[i * 8 + w] == L[w]) w--;
+        if (k[i * 8 + w] >= L[w]) return SBV_ERR_ARG;
+    }
+    if (n == 0) return SBV_OK;
+    std::lock_guard<std::mutex> lk(e->mu);
+    Dev &d = e->devs[0];
+    CU(e, cudaSetDevice(d.ordinal));
+    int rc = sbv_ed_btab_ensure(e, d);
+    if (rc) return rc;
+    const size_t okb = (n + 255) & ~(size_t)255;
+    if ((rc = sbv_ensure_scratch(e, d, n * 64 + n * 32 + n * 32 + okb + 1024))) return rc;
+    uint8_t *p = d.d_scratch;
+    uint8_t *dsig = p; p += n * 64;
+    uint8_t *dpub = p; p += n * 32;
+    uint32_t *dk = (uint32_t *)p; p += n * 32;
+    uint8_t *dok = p;
+    std::vector<uint32_t> kw(n * 8);
+    for (size_t i = 0; i < n; i++)
+        for (int w = 0; w < 8; w++) kw[(size_t)w * n + i] = k[i * 8 + w];
+    CU(e, cudaMemcpyAsync(dsig, sig, n * 64, cudaMemcpyHostToDevice, d.stream));
+    CU(e, cudaMemcpyAsync(dpub, pub, n * 32, cudaMemcpyHostToDevice, d.stream));
+    CU(e, cudaMemcpyAsync(dk, kw.data(), n * 32, cudaMemcpyHostToDevice, d.stream));
+    if ((rc = sbv_launch_ed_verify_comb_k(e, d, n, dsig, dpub, dk, dok, d.stream))) return rc;
+    CU(e, cudaMemcpyAsync(ok, dok, n, cudaMemcpyDeviceToHost, d.stream));
+    CU(e, cudaStreamSynchronize(d.stream));
+    return SBV_OK;
+}
+
 // The production registered-key kernel (k_ed_verify_keyed) on device 0 with the caller's k in place of SHA-512(R || A || M)
 // mod L: k = 8 little-endian limbs per item, each < L (SBV_ERR_ARG otherwise), key_slot = registry slots, sig = R || S.
 extern "C" int sbv_debug_ed25519_verify_registered_k(sbv_engine *e, size_t n, const uint32_t *key_slot, const uint8_t *sig, const uint32_t *k,

@@ -66,14 +66,18 @@ SBV_DEV void ed_load32(uint32_t (&r)[8], const uint8_t *__restrict__ p) {
 // with bank = lane: 1 KiB per thread), 252 doublings and 64 additions; then [S]B with 8-bit signed windows from the
 // fixed-base table (32 additions, no doublings); one inversion to encode R'.
 // sig: 64 bytes per item (R || S); pub: 32 bytes per item; k: word-major [8][n].
+// list (optional): thread t verifies item list[t] for t < *count (the keys of a grouped launch that got no table);
+// NULL: item t < n.
 template <int BLOCK>
 __global__ void __launch_bounds__(BLOCK) k_ed_verify(uint32_t n, const uint8_t *__restrict__ sig, const uint8_t *__restrict__ pub,
                                                      const uint32_t *__restrict__ k, const uint4 *__restrict__ btab,
-                                                     uint8_t *__restrict__ ok_out) {
+                                                     uint8_t *__restrict__ ok_out, const uint32_t *__restrict__ list,
+                                                     const uint32_t *__restrict__ count) {
     extern __shared__ uint32_t tab[];  // [((e - 1) * 4 + coord) * 8 + limb][BLOCK], e = 1..8
     const uint32_t tid = threadIdx.x;
-    const uint32_t idx = blockIdx.x * BLOCK + tid;
-    if (idx >= n) return;  // the table is thread-private: no block-wide barrier anywhere
+    const uint32_t t = blockIdx.x * BLOCK + tid;
+    if (t >= (list ? __ldg(count) : n)) return;  // the table is thread-private: no block-wide barrier anywhere
+    const uint32_t idx = list ? __ldg(list + t) : t;
 #define TAB(e, c, w) tab[((((e) - 1) * 4 + (c)) * 8 + (w)) * BLOCK + tid]
     {
         uint32_t s[8];

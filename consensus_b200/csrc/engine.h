@@ -182,6 +182,9 @@ int sbv_launch_verify_chunk(sbv_engine *e, Dev &d, const VerifyLaunch &vl, int c
 // registered keys (sbv_set_keys)
 int sbv_launch_keyed(sbv_engine *e, Dev &d, uint8_t curve, size_t n, const uint32_t *d_slot, const uint8_t *d_r, const uint8_t *d_s,
                      const uint8_t *d_dig, uint32_t dlen, uint8_t *d_ok, cudaStream_t st);
+// the next scratch set of device d for a launch of n items (N words per coordinate; 0: none of the ECDSA per-item buffers)
+// with kcap keys of table geometry q (nullptr: no grouping); the launch must record the set's `done` event on st
+int sbv_take_scratch(sbv_engine *e, Dev &d, size_t N, const KtGeom *q, size_t n, size_t kcap, cudaStream_t st, Dev::Scratch **out);
 int sbv_init_gtables(sbv_engine *e, Dev &d);
 int sbv_keys_build(sbv_engine *e, Dev &d);  // (re)builds the per-key tables of the registry
 void sbv_keys_free(Dev &d);
@@ -189,9 +192,19 @@ void sbv_scratch_free(Dev &d);
 // ---- inst_ed25519.cu: Ed25519 (enqueue only, no sync) ----
 int sbv_ed_btab_ensure(sbv_engine *e, Dev &d);  // caller holds e->mu and has set the device
 // k = SHA-512(R || A || M) mod L into d_k (word-major, 8n words), then the verdicts into d_ok.  d_sig: 64n bytes (R || S),
-// d_pub: 32n bytes, d_perm: n + 3072 words of scratch.  The table of B must exist (sbv_ed_btab_ensure).
+// d_pub: 32n bytes, d_perm: n + 3072 words of scratch.  The table of B must exist (sbv_ed_btab_ensure).  Keys whose 32
+// bytes occur at least group_threshold times get a comb table built in the launch (ed25519_comb.cuh), over a scratch
+// set; caller holds e->mu.
 int sbv_launch_ed25519(sbv_engine *e, Dev &d, size_t n, const uint8_t *d_msgs, const uint64_t *d_off, uint64_t base, const uint8_t *d_sig,
                        const uint8_t *d_pub, uint32_t *d_k, uint32_t *d_perm, uint8_t *d_ok, cudaStream_t st);
+// test hooks (caller holds e->mu; the table of B must exist):
+// the grouping and comb tables of a keys-per-item launch of the n keys of d_pub with the engine's settings, finished
+// (synchronised) on return; *w = the scratch set holding them (rep, keyid, keyflags, ktab), or nullptr when the launch
+// would not group.  The caller records (*w)->done when it has read them.
+int sbv_launch_ed_comb_tables(sbv_engine *e, Dev &d, size_t n, const uint8_t *d_pub, cudaStream_t st, Dev::Scratch **w);
+// k_ed_verify_comb over every item with the caller's k (word-major [8][n], every k < L); every distinct key gets a table
+int sbv_launch_ed_verify_comb_k(sbv_engine *e, Dev &d, size_t n, const uint8_t *d_sig, const uint8_t *d_pub, const uint32_t *d_k, uint8_t *d_ok,
+                                cudaStream_t st);
 int sbv_launch_ed_sha512_digest(sbv_engine *e, size_t n, const uint8_t *d_msgs, const uint64_t *d_off, const uint8_t *d_sig, const uint8_t *d_pub,
                                 uint32_t *d_k, uint32_t *d_dig, cudaStream_t st);
 // test hook: k_ed_verify with the caller's k (word-major [8][n], every k < L); the table of B must exist
@@ -231,6 +244,8 @@ int sbv_launch_mix_ok(sbv_engine *e, const MixBufs &b, size_t n, const uint32_t 
 
 // shape of the table of B (ed25519_verify.cuh: ED_BWINS x ED_BENT entries of ED_BWORDS words; checked in inst_ed25519.cu)
 constexpr size_t SBV_ED_BTAB_ENTRIES = 32 * 128, SBV_ED_BTAB_ENTRY_WORDS = 24;
+// entries of a per-launch comb table (ed25519_comb.cuh: 2 blocks x 255 entries of 24 words; checked in inst_ed25519.cu)
+constexpr size_t SBV_ED_COMB_ENTRIES = 2 * 255;
 
 // ---- engine.cu helpers shared with the other translation units ----
 int sbv_lane_acquire(sbv_engine *e);            // blocks until a lane index is free; returns it

@@ -37,7 +37,7 @@ cudaError_t op_group(uint32_t n, const uint8_t *qx, const uint8_t *qy, uint32_t 
                      uint32_t *kcnt, uint32_t threshold, uint32_t max_keys, int32_t *keyid, uint32_t *keylist, uint32_t *counters,
                      cudaStream_t st) {
     const unsigned blocks = (n + 255) / 256;
-    k_kg_insert<C><<<blocks, 256, 0, st>>>(n, qx, qy, seed, hmask, htab, rep, kcnt);
+    k_kg_insert<<<blocks, 256, 0, st>>>(n, KgXY<C>{qx, qy}, seed, hmask, htab, rep, kcnt);
     k_kg_assign<<<blocks, 256, 0, st>>>(n, rep, kcnt, threshold, max_keys, keyid, keylist, counters);
     return cudaGetLastError();
 }

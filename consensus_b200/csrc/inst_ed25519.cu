@@ -1,10 +1,12 @@
-// inst_ed25519.cu — launchers of the Ed25519 kernels (sha512.cuh, ed25519_verify.cuh, ed25519_keyed.cuh) behind engine.h,
-// and the registry of registered Ed25519 keys.
+// inst_ed25519.cu — launchers of the Ed25519 kernels (sha512.cuh, ed25519_verify.cuh, ed25519_keyed.cuh,
+// ed25519_comb.cuh) behind engine.h, and the registry of registered Ed25519 keys.
 #include <vector>
 
 #include "engine.h"
+#include "ed25519_comb.cuh"
 #include "ed25519_keyed.cuh"
 #include "ed25519_verify.cuh"
+#include "keygroup.cuh"
 #include "sha512.cuh"
 
 using namespace sbv;
@@ -13,6 +15,7 @@ namespace {
 constexpr int ED_BLOCK = 32;  // 32 KiB of shared memory per block (the 1A..8A tables): no opt-in attribute needed
 constexpr size_t ED_SMEM = (size_t)8 * 4 * 8 * 4 * ED_BLOCK;
 constexpr int EDK_BLOCK = 128;  // k_ed_verify_keyed: no shared memory; see DESIGN.md §3 for registers and occupancy
+constexpr int EDC_BLOCK = 128;  // k_ed_verify_comb: likewise
 }  // namespace
 static_assert(SBV_ED_BTAB_ENTRIES == (size_t)ED_BWINS * ED_BENT && SBV_ED_BTAB_ENTRY_WORDS == ED_BWORDS, "engine.h: table of B");
 
@@ -34,17 +37,147 @@ int sbv_ed_btab_ensure(sbv_engine *e, Dev &d) {
     return 0;
 }
 
+// ---- keys per item ----
+// A keys-per-item launch (pipeline.cu draws the same for ECDSA):
+//
+//   st     memsets  k_kg_insert  k_kg_assign ─┬─ k_kg_route  length sort  k_ed_sha512 ─┬──────────── (wait tables) k_ed_verify_comb ─ (wait generic) ─ done
+//   s_tab                                     └─ k_edc_bases  k_edc_fill  k_edc_inv  k_edc_final ──┘
+//   s_gen                                                                              └─ k_ed_verify (keys without a table) ─────────────────┘
+//
+// Keys whose 32 bytes occur at least group_threshold times get a comb table (ed25519_comb.cuh) and their items take
+// k_ed_verify_comb; the table construction (latency-bound: one doubling chain per key) runs beside SHA-512.
+namespace {
+constexpr KtGeom ED_COMB_GEOM{EDC_BASES_WORDS, EDC_HS_WORDS, EDC_ZTOP_WORDS, EDC_TAB_WORDS};
+static_assert(SBV_ED_COMB_ENTRIES * SBV_ED_BTAB_ENTRY_WORDS == EDC_TAB_WORDS, "engine.h: comb table");
+
+// table slots of a launch of n items at threshold T, as the ECDSA launches count them; 0: the launch does not group
+size_t ed_group_cap(const sbv_engine *e, size_t n, uint32_t T) {
+    if (T == 0 || n < T || n < (size_t)e->group_min_batch || e->group_max_keys <= 0) return 0;
+    size_t kcap = n / T;
+    if (kcap > (size_t)e->group_max_keys) kcap = (size_t)e->group_max_keys;
+    return kcap ? kcap : 1;
+}
+
+// On st: the grouping of the n keys of d_pub (at most kcap of them with >= T items get a table slot) and the routing onto
+// w->klist / w->glist (counts at zeroed[1] / zeroed[2]); on w->s_tab: the comb tables, then w->ev_tab.
+int ed_group(sbv_engine *e, Dev::Scratch *w, size_t n, const uint8_t *d_pub, uint32_t T, size_t kcap, cudaStream_t st) {
+    const uint32_t nn = (uint32_t)n, cap = (uint32_t)kcap, blocks = (nn + 255) / 256;
+    uint32_t *counters = w->zeroed, *kcnt = w->zeroed + 4;
+    CU(e, cudaMemsetAsync(w->htab, 0xff, (size_t)w->hsize * 4, st));
+    CU(e, cudaMemsetAsync(w->zeroed, 0, (n + 4) * 4, st));
+    k_kg_insert<<<blocks, 256, 0, st>>>(nn, KgKey32{d_pub}, e->hash_seed, w->hsize - 1, w->htab, w->rep, kcnt);
+    k_kg_assign<<<blocks, 256, 0, st>>>(nn, w->rep, kcnt, T, cap, w->keyid, w->keylist, counters);
+    CU(e, cudaGetLastError());
+    CU(e, cudaEventRecord(w->ev_group, st));
+    CU(e, cudaStreamWaitEvent(w->s_tab, w->ev_group, 0));
+    const unsigned kb = (cap + 63) / 64, cb = (unsigned)(((size_t)cap * EDC_NCHAIN + 63) / 64);
+    k_edc_bases<<<kb, 64, 0, w->s_tab>>>(counters, cap, w->keylist, d_pub, w->bases, w->keyflags);
+    k_edc_fill<<<cb, 64, 0, w->s_tab>>>(counters, cap, w->bases, w->keyflags, w->hs, w->ztop, w->ktab);
+    k_edc_inv<<<kb, 64, 0, w->s_tab>>>(counters, cap, w->keyflags, w->ztop, w->pref);
+    k_edc_final<<<cb, 64, 0, w->s_tab>>>(counters, cap, w->keyflags, w->hs, w->ztop, w->ktab);
+    CU(e, cudaGetLastError());
+    CU(e, cudaEventRecord(w->ev_tab, w->s_tab));
+    k_kg_route<<<blocks, 256, 0, st>>>(nn, w->rep, w->keyid, w->item_kid, w->klist, w->glist, counters);
+    e->launches += 7;
+    CU(e, cudaGetLastError());
+    return 0;
+}
+
+// Hands the set back behind everything the launch enqueued on its side streams: on success and after a fault alike.
+int ed_close(sbv_engine *e, Dev::Scratch *w, cudaStream_t st, int rc) {
+    if (rc) cudaStreamWaitEvent(st, w->ev_tab, 0);  // a fault before the join: the tables may still be in flight
+    const cudaError_t a = cudaStreamWaitEvent(st, w->ev_gen, 0), b = cudaEventRecord(w->done, st);
+    if (rc) return rc;
+    CU(e, a);
+    CU(e, b);
+    return 0;
+}
+
+int ed_grouped(sbv_engine *e, Dev &d, Dev::Scratch *w, size_t n, const uint8_t *d_msgs, const uint64_t *d_off, uint64_t base, const uint8_t *d_sig,
+               const uint8_t *d_pub, uint32_t *d_k, uint32_t *d_perm, uint8_t *d_ok, uint32_t T, size_t kcap, cudaStream_t st) {
+    if (int rc = ed_group(e, w, n, d_pub, T, kcap, st)) return rc;
+    const uint32_t nn = (uint32_t)n, *counters = w->zeroed;
+    const uint32_t *perm = nullptr;
+    if (int rc = sbv_launch_length_sort(e, n, d_off, d_perm, st, &perm)) return rc;
+    k_ed_sha512<<<(nn + 127) / 128, 128, 0, st>>>(nn, d_sig, d_pub, d_msgs, d_off, base, d_k, perm, nullptr);
+    e->launches += 1;
+    CU(e, cudaGetLastError());
+    CU(e, cudaEventRecord(w->ev_prep, st));
+    CU(e, cudaStreamWaitEvent(w->s_gen, w->ev_prep, 0));
+    const uint4 *btab = reinterpret_cast<const uint4 *>(d.ed_btab);
+    k_ed_verify<ED_BLOCK><<<(nn + ED_BLOCK - 1) / ED_BLOCK, ED_BLOCK, ED_SMEM, w->s_gen>>>(nn, d_sig, d_pub, d_k, btab, d_ok, w->glist, counters + 2);
+    e->launches += 1;
+    CU(e, cudaGetLastError());
+    CU(e, cudaEventRecord(w->ev_gen, w->s_gen));
+    CU(e, cudaStreamWaitEvent(st, w->ev_tab, 0));
+    k_ed_verify_comb<EDC_BLOCK><<<(nn + EDC_BLOCK - 1) / EDC_BLOCK, EDC_BLOCK, 0, st>>>(
+        nn, d_sig, w->item_kid, w->keyflags, reinterpret_cast<const uint4 *>((uint32_t *)w->ktab), d_k, btab, d_ok, w->klist, counters + 1);
+    e->launches += 1;
+    CU(e, cudaGetLastError());
+    return 0;
+}
+}  // namespace
+
 int sbv_launch_ed25519(sbv_engine *e, Dev &d, size_t n, const uint8_t *d_msgs, const uint64_t *d_off, uint64_t base, const uint8_t *d_sig,
                        const uint8_t *d_pub, uint32_t *d_k, uint32_t *d_perm, uint8_t *d_ok, cudaStream_t st) {
+    const uint32_t T = e->group_threshold > 0 ? (uint32_t)e->group_threshold : 0;
+    const size_t kcap = ed_group_cap(e, n, T);
+    if (kcap) {
+        Dev::Scratch *w = nullptr;
+        if (int rc = sbv_take_scratch(e, d, 0, &ED_COMB_GEOM, n, kcap, st, &w)) return rc;
+        return ed_close(e, w, st, ed_grouped(e, d, w, n, d_msgs, d_off, base, d_sig, d_pub, d_k, d_perm, d_ok, T, kcap, st));
+    }
     const uint32_t *perm = nullptr;
     int rc = sbv_launch_length_sort(e, n, d_off, d_perm, st, &perm);
     if (rc) return rc;
     k_ed_sha512<<<(uint32_t)((n + 127) / 128), 128, 0, st>>>((uint32_t)n, d_sig, d_pub, d_msgs, d_off, base, d_k, perm, nullptr);
     k_ed_verify<ED_BLOCK><<<(uint32_t)((n + ED_BLOCK - 1) / ED_BLOCK), ED_BLOCK, ED_SMEM, st>>>(
-        (uint32_t)n, d_sig, d_pub, d_k, reinterpret_cast<const uint4 *>(d.ed_btab), d_ok);
+        (uint32_t)n, d_sig, d_pub, d_k, reinterpret_cast<const uint4 *>(d.ed_btab), d_ok, nullptr, nullptr);
     e->launches += 2;
     CU(e, cudaGetLastError());
     return 0;
+}
+
+// test hook (debug.cu): the first half of a grouped launch, synchronised
+int sbv_launch_ed_comb_tables(sbv_engine *e, Dev &d, size_t n, const uint8_t *d_pub, cudaStream_t st, Dev::Scratch **out) {
+    *out = nullptr;
+    const uint32_t T = e->group_threshold > 0 ? (uint32_t)e->group_threshold : 0;
+    const size_t kcap = ed_group_cap(e, n, T);
+    if (!kcap) return 0;
+    Dev::Scratch *w = nullptr;
+    if (int rc = sbv_take_scratch(e, d, 0, &ED_COMB_GEOM, n, kcap, st, &w)) return rc;
+    int rc = ed_group(e, w, n, d_pub, T, kcap, st);
+    if (!rc) {
+        const cudaError_t a = cudaStreamWaitEvent(st, w->ev_tab, 0);
+        rc = a != cudaSuccess ? sbv_fail(e, SBV_ERR_CUDA, "cudaStreamWaitEvent: %s", cudaGetErrorString(a)) : 0;
+    }
+    if (!rc) {
+        const cudaError_t a = cudaStreamSynchronize(st);
+        rc = a != cudaSuccess ? sbv_fail(e, SBV_ERR_CUDA, "k_edc_*: %s", cudaGetErrorString(a)) : 0;
+    }
+    if (rc) return ed_close(e, w, st, rc);
+    *out = w;
+    return 0;
+}
+
+// test hook (debug.cu): k_ed_verify_comb with the caller's k over every item, every distinct key with a table
+int sbv_launch_ed_verify_comb_k(sbv_engine *e, Dev &d, size_t n, const uint8_t *d_sig, const uint8_t *d_pub, const uint32_t *d_k, uint8_t *d_ok,
+                                cudaStream_t st) {
+    Dev::Scratch *w = nullptr;
+    if (int rc = sbv_take_scratch(e, d, 0, &ED_COMB_GEOM, n, n, st, &w)) return rc;
+    int rc = ed_group(e, w, n, d_pub, 1, n, st);
+    if (!rc) {
+        const uint32_t nn = (uint32_t)n;
+        const cudaError_t a = cudaStreamWaitEvent(st, w->ev_tab, 0);
+        if (a == cudaSuccess)
+            k_ed_verify_comb<EDC_BLOCK><<<(nn + EDC_BLOCK - 1) / EDC_BLOCK, EDC_BLOCK, 0, st>>>(
+                nn, d_sig, w->item_kid, w->keyflags, reinterpret_cast<const uint4 *>((uint32_t *)w->ktab), d_k, reinterpret_cast<const uint4 *>(d.ed_btab),
+                d_ok, nullptr, nullptr);
+        e->launches += 1;
+        const cudaError_t b = a != cudaSuccess ? a : cudaGetLastError();
+        rc = b != cudaSuccess ? sbv_fail(e, SBV_ERR_CUDA, "k_ed_verify_comb: %s", cudaGetErrorString(b)) : 0;
+    }
+    return ed_close(e, w, st, rc);
 }
 
 // test hook (debug.cu): the production SHA-512 kernel with its digests written out as well
@@ -61,7 +194,7 @@ int sbv_launch_ed_sha512_digest(sbv_engine *e, size_t n, const uint8_t *d_msgs, 
 int sbv_launch_ed_verify_k(sbv_engine *e, Dev &d, size_t n, const uint8_t *d_sig, const uint8_t *d_pub, const uint32_t *d_k, uint8_t *d_ok,
                            cudaStream_t st) {
     k_ed_verify<ED_BLOCK><<<(uint32_t)((n + ED_BLOCK - 1) / ED_BLOCK), ED_BLOCK, ED_SMEM, st>>>(
-        (uint32_t)n, d_sig, d_pub, d_k, reinterpret_cast<const uint4 *>(d.ed_btab), d_ok);
+        (uint32_t)n, d_sig, d_pub, d_k, reinterpret_cast<const uint4 *>(d.ed_btab), d_ok, nullptr, nullptr);
     e->launches += 1;
     CU(e, cudaGetLastError());
     return 0;

@@ -5,7 +5,8 @@
 // sign many requests each (controller.go:233-246).  The C ABI still takes the key with every item (sbv_verify_batch:
 // qx, qy per item), so the engine finds the repetition itself:
 //
-//   k_kg_insert   every item hashes its 64/96-byte key into an open-addressing table (CAS on the item index,
+//   k_kg_insert   every item hashes its key (64/96 bytes of (qx, qy), or a 32-byte Ed25519 encoding: the key views
+//                 KgXY / KgKey32) into an open-addressing table (CAS on the item index,
 //                 full-key compare on collision): rep[i] = first item with the same key; warp-aggregated count
 //   k_kg_assign   representatives whose key occurs >= T times (and while table slots last) get a dense key id
 //   k_kg_route    items are appended to the fixed-base list (their key has a table) or to the generic list
@@ -57,14 +58,45 @@ SBV_DEV bool kg_same_key(const uint8_t *__restrict__ qx_be, const uint8_t *__res
     return diff == 0;
 }
 
-// htab: hmask + 1 slots, all KG_EMPTY on entry; kcnt: n zeros on entry.
+// Key views of k_kg_insert: which bytes of item i make its key.
+// KgXY<C>: the coordinates (qx, qy) of curve C, C::BYTES each (ECDSA).
 template <class C>
-__global__ void __launch_bounds__(256) k_kg_insert(uint32_t n, const uint8_t *__restrict__ qx_be, const uint8_t *__restrict__ qy_be,
-                                                   uint32_t seed, uint32_t hmask, uint32_t *__restrict__ htab,
+struct KgXY {
+    const uint8_t *qx_be, *qy_be;
+    SBV_DEV uint32_t hash(uint32_t i, uint32_t seed) const { return kg_hash<C>(qx_be, qy_be, i, seed); }
+    SBV_DEV bool same(uint32_t i, uint32_t j) const { return kg_same_key<C>(qx_be, qy_be, i, j); }
+};
+// KgKey32: a 32-byte encoding, 16-byte aligned per item (Ed25519, grouped by bytes rather than by the point they decode to)
+struct KgKey32 {
+    const uint8_t *pub;
+    SBV_DEV uint32_t hash(uint32_t i, uint32_t seed) const {
+        const uint32_t *x = reinterpret_cast<const uint32_t *>(pub + (size_t)i * 32);
+        uint32_t h = seed;
+#pragma unroll
+        for (int k = 0; k < 8; k += 2) {
+            h = (h ^ __ldg(x + k)) * 0x9E3779B1u;
+            h = (h ^ __ldg(x + k + 1)) * 0x85EBCA77u;
+            h ^= h >> 15;
+        }
+        return h;
+    }
+    SBV_DEV bool same(uint32_t i, uint32_t j) const {
+        const uint32_t *xi = reinterpret_cast<const uint32_t *>(pub + (size_t)i * 32);
+        const uint32_t *xj = reinterpret_cast<const uint32_t *>(pub + (size_t)j * 32);
+        uint32_t diff = 0;
+#pragma unroll
+        for (int k = 0; k < 8; k++) diff |= __ldg(xi + k) ^ __ldg(xj + k);
+        return diff == 0;
+    }
+};
+
+// htab: hmask + 1 slots, all KG_EMPTY on entry; kcnt: n zeros on entry.  KV: a key view (KgXY, KgKey32).
+template <class KV>
+__global__ void __launch_bounds__(256) k_kg_insert(uint32_t n, KV key, uint32_t seed, uint32_t hmask, uint32_t *__restrict__ htab,
                                                    uint32_t *__restrict__ rep, uint32_t *__restrict__ kcnt) {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
-    uint32_t h = kg_hash<C>(qx_be, qy_be, i, seed) & hmask;
+    uint32_t h = key.hash(i, seed) & hmask;
     uint32_t r;
     for (;;) {
         uint32_t cur = htab[h];
@@ -72,7 +104,7 @@ __global__ void __launch_bounds__(256) k_kg_insert(uint32_t n, const uint8_t *__
             cur = atomicCAS(htab + h, KG_EMPTY, i);
             if (cur == KG_EMPTY) { r = i; break; }
         }
-        if (kg_same_key<C>(qx_be, qy_be, i, cur)) { r = cur; break; }
+        if (key.same(i, cur)) { r = cur; break; }
         h = (h + 1) & hmask;
     }
     rep[i] = r;

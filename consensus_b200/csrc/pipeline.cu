@@ -55,9 +55,12 @@ void each_buffer(Dev::Scratch &x, const ScratchDims &s, V &&visit) {
     visit(x.ktab, q.ktab_words * k * 4, q.ktab_words * kc * 4);
 }
 
+}  // namespace
+
 // Takes the next scratch set of device d for a launch on stream st: waits (on the stream) for the set's previous user
-// and grows the buffers to n items / kcap keys of curve `ops` (growth drains the previous user on the host first).
-int take_scratch(sbv_engine *e, Dev &d, const CurveOps &ops, const KtOps *kt, size_t n, size_t kcap, cudaStream_t st, Dev::Scratch **out) {
+// and grows the buffers to n items with N words per coordinate / kcap keys of table geometry q (growth drains the
+// previous user on the host first).  A buffer never shrinks, so the sets fit the largest launch of either family.
+int sbv_take_scratch(sbv_engine *e, Dev &d, size_t N, const KtGeom *q, size_t n, size_t kcap, cudaStream_t st, Dev::Scratch **out) {
     // round robin over the sets that are not held open between the two halves of a host-buffer launch (at most
     // SBV_LANES < SBV_SCRATCH of them at any time)
     int idx = (int)(d.ws_next++ % SBV_SCRATCH);
@@ -83,7 +86,7 @@ int take_scratch(sbv_engine *e, Dev &d, const CurveOps &ops, const KtOps *kt, si
             CU(e, cudaStreamCreateWithFlags(&x.s_gen, cudaStreamNonBlocking));
         }
     }
-    const ScratchDims dims{(size_t)ops.N, n, kcap, kt ? kt->geom : KtGeom{}};
+    const ScratchDims dims{N, n, kcap, q ? *q : KtGeom{}};
     bool grows = false;
     each_buffer(w, dims, [&](DevBuf &b, size_t need, size_t) { grows = grows || need > b.bytes; });
     if (grows) {
@@ -110,6 +113,8 @@ int take_scratch(sbv_engine *e, Dev &d, const CurveOps &ops, const KtOps *kt, si
     *out = &w;
     return 0;
 }
+
+namespace {
 
 cudaEvent_t *prof_take(sbv_engine *e, Dev &d) {
     if (!e->profiling) return nullptr;
@@ -170,7 +175,7 @@ int sbv_launch_verify_begin(sbv_engine *e, Dev &d, uint8_t curve, size_t n, cons
         if (kcap == 0) kcap = 1;
     }
     Dev::Scratch *w = nullptr;
-    if (int rc = take_scratch(e, d, ops, grouping ? kt : nullptr, n, kcap, st, &w)) return rc;
+    if (int rc = sbv_take_scratch(e, d, (size_t)ops.N, grouping ? &kt->geom : nullptr, n, kcap, st, &w)) return rc;
     w->open = true;  // until the last chunk records the set's `done` event
     vl->w = w; vl->curve = curve; vl->n = n; vl->grouping = grouping; vl->d_qx = d_qx; vl->d_qy = d_qy; vl->chunks = chunks;
     vl->ev = prof_take(e, d);
@@ -339,7 +344,7 @@ int sbv_launch_keyed(sbv_engine *e, Dev &d, uint8_t curve, size_t n, const uint3
     const RegisteredKtOps *kt = ops.kt8;
     const uint32_t nn = (uint32_t)n;
     Dev::Scratch *w = nullptr;
-    if (int rc = take_scratch(e, d, ops, nullptr, n, 0, st, &w)) return rc;
+    if (int rc = sbv_take_scratch(e, d, (size_t)ops.N, nullptr, n, 0, st, &w)) return rc;
     cudaEvent_t *ev = prof_take(e, d);
     if (ev) CU(e, cudaEventRecord(ev[0], st));
     CU(e, ops.prep(nn, d_r, d_s, d_dig, dlen, w->uw, w->flags, st));

@@ -37,8 +37,11 @@
  *    the caller's buffers is in flight after the call returns, and on a fault the output arrays are untouched
  *    or partially written but never read as verdicts (the caller fail-stops).
  *  - Keys that repeat inside a keys-per-item batch are detected on the device and verified against a per-key
- *    fixed-base table built on the spot (SBV_GROUP_THRESHOLD, default 16 occurrences; 0 disables): the verdicts
- *    are the same bit for bit, only cheaper.
+ *    fixed-base table built on the spot (SBV_GROUP_THRESHOLD, default 16 occurrences; 0 disables; at most
+ *    SBV_GROUP_MAX_KEYS tables per launch, and when more keys repeat, which of them get one is not specified;
+ *    launches below SBV_GROUP_MIN_BATCH items are not grouped): the verdicts
+ *    are the same bit for bit, only cheaper.  ECDSA keys are grouped by (qx, qy), Ed25519 keys by their 32 encoded
+ *    bytes; each device groups its own shard.
  *  - There is no CPU fallback: without a usable CUDA device sbv_create fails.
  */
 #ifndef SBV_H
@@ -110,7 +113,9 @@ int sbv_verify_mixed(sbv_engine *e, size_t n, const uint8_t *curve_tag, const ui
  * Accept set = Go crypto/ed25519.Verify (pure Ed25519, no context): S < L; A decodes as edwards25519 Point.SetBytes does
  * (y >= p reduced, "-0" accepted, no subgroup check); k = SHA-512(R || A || M) mod L over the caller's bytes; accept iff
  * the canonical encoding of [S]B - [k]A equals R byte for byte (cofactorless; each signature on its own).  Messages are
- * hashed on the device.  The first call on an engine builds a 384 KiB table of B on every device. */
+ * hashed on the device.  The first call on an engine builds a 384 KiB table of B on every device.  Keys whose 32 bytes
+ * repeat are grouped (see the top of this file): such a key gets a 48 KiB comb table built in the launch, with the same
+ * settings and the same verdicts; two encodings of one point (y >= p, "-0") are two keys. */
 int sbv_ed25519_verify_batch(sbv_engine *e, size_t n, const uint8_t *msgs, const uint64_t *msg_off, const uint8_t *sig,
                              const uint8_t *pub, uint8_t *ok);
 

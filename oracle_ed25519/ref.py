@@ -137,3 +137,26 @@ def small_order_points():
 
 def point_from_affine(x, y):
     return (x, y, 1, x * y % p)
+
+
+def comb_table(A: bytes):
+    """The comb table of a key grouped inside a launch, or None when A does not decode: entry b * 255 + m - 1 (b = 0, 1;
+    m = 1..255) is the affine sum of 2^(16 (8b + t)) A over the set bits t of m."""
+    P = decode(A)
+    if P is None:
+        return None
+    bases = [P]
+    for _ in range(15):
+        Q = bases[-1]
+        for _ in range(16):
+            Q = add(Q, Q)
+        bases.append(Q)
+    out = []
+    for b in range(2):
+        for m in range(1, 256):
+            S = IDENTITY
+            for t in range(8):
+                if (m >> t) & 1:
+                    S = add(S, bases[8 * b + t])
+            out.append(affine(S))
+    return out

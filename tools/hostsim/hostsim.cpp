@@ -22,6 +22,7 @@ namespace sbv { uint32_t tab[1 << 18]; }
 #include "../../consensus_b200/csrc/sha512.cuh"
 #include "../../consensus_b200/csrc/ed25519_verify.cuh"
 #include "../../consensus_b200/csrc/ed25519_keyed.cuh"
+#include "../../consensus_b200/csrc/ed25519_comb.cuh"
 #include "../../consensus_b200/csrc/shards.h"
 #include "../../consensus_b200/csrc/mixed.cuh"
 
@@ -260,7 +261,7 @@ static void verify_grouped_t(uint32_t n, const uint8_t *r, const uint8_t *s, con
     while (hsize < 2 * n) hsize <<= 1;
     std::vector<uint32_t> htab(hsize, KG_EMPTY), rep(n), kcnt(n, 0), keylist(max_keys ? max_keys : 1), klist(n), glist(n), counters(4, 0);
     std::vector<int32_t> keyid(n), item_kid(n);
-    run_grid((n + 255) / 256, 256, [&] { k_kg_insert<C>(n, qx, qy, 0x1234567u, hsize - 1, htab.data(), rep.data(), kcnt.data()); });
+    run_grid((n + 255) / 256, 256, [&] { k_kg_insert(n, KgXY<C>{qx, qy}, 0x1234567u, hsize - 1, htab.data(), rep.data(), kcnt.data()); });
     run_grid((n + 255) / 256, 256, [&] { k_kg_assign(n, rep.data(), kcnt.data(), threshold, max_keys, keyid.data(), keylist.data(), counters.data()); });
     const size_t cap = max_keys ? max_keys : 1;
     constexpr bool comb = std::is_same<C, P256>::value;
@@ -361,7 +362,7 @@ extern "C" int hs_ed25519_verify(size_t n, const uint8_t *msgs, const uint64_t *
     std::vector<uint32_t> k(8 * n + 8);
     run_grid((unsigned)((n + 127) / 128), 128, [&] { k_ed_sha512((uint32_t)n, sig, pub, msgs, off, 0, k.data(), nullptr, nullptr); });
     const uint4 *bt = reinterpret_cast<const uint4 *>(ed_btab_host().data());
-    run_grid((unsigned)((n + 31) / 32), 32, [&] { k_ed_verify<32>((uint32_t)n, sig, pub, k.data(), bt, ok); });
+    run_grid((unsigned)((n + 31) / 32), 32, [&] { k_ed_verify<32>((uint32_t)n, sig, pub, k.data(), bt, ok, nullptr, nullptr); });
     return 0;
 }
 // k_ed_verify alone with the caller's k (8 little-endian limbs per item, each < L; -1 otherwise), as
@@ -376,7 +377,7 @@ extern "C" int hs_ed25519_verify_k(size_t n, const uint8_t *sig, const uint8_t *
         if (!mp_lt<8>(ki, Lm)) return -1;
     }
     const uint4 *bt = reinterpret_cast<const uint4 *>(ed_btab_host().data());
-    run_grid((unsigned)((n + 31) / 32), 32, [&] { k_ed_verify<32>((uint32_t)n, sig, pub, k.data(), bt, ok); });
+    run_grid((unsigned)((n + 31) / 32), 32, [&] { k_ed_verify<32>((uint32_t)n, sig, pub, k.data(), bt, ok, nullptr, nullptr); });
     return 0;
 }
 
@@ -450,6 +451,97 @@ extern "C" int hs_ed25519_verify_registered_k(size_t n, const uint32_t *key_slot
         if (!mp_lt<8>(ki, Lm)) return -1;
     }
     ed_verify_keyed_host(n, key_slot, sig, k.data(), ok);
+    return 0;
+}
+
+// ---- Ed25519 keys grouped inside a keys-per-item launch (ed25519_comb.cuh) ----
+// The first half of a grouped launch as ed_group (inst_ed25519.cu) enqueues it: k_kg_insert over the 32 key bytes,
+// k_kg_assign (threshold T, kcap table slots), the four comb construction kernels, k_kg_route.
+struct EdGroup {
+    std::vector<uint32_t> rep, keylist, klist, glist, counters, ctab;
+    std::vector<int32_t> keyid, item_kid;
+    std::vector<uint8_t> kflags;
+};
+static void ed_group_host(uint32_t n, const uint8_t *pub, uint32_t T, uint32_t kcap, EdGroup &g) {
+    uint32_t hsize = 1;
+    while (hsize < 2 * n) hsize <<= 1;
+    const uint32_t cap = kcap ? kcap : 1;
+    std::vector<uint32_t> htab(hsize, KG_EMPTY), kcnt(n, 0);
+    std::vector<uint32_t> bases(EDC_BASES_WORDS * cap), hs(EDC_HS_WORDS * cap), ztop(EDC_ZTOP_WORDS * cap), pref(EDC_ZTOP_WORDS * cap);
+    g.rep.assign(n, 0); g.klist.assign(n, 0); g.glist.assign(n, 0); g.counters.assign(4, 0);
+    g.keyid.assign(n, -1); g.item_kid.assign(n, -1);
+    g.keylist.assign(cap, 0); g.kflags.assign(cap, 0); g.ctab.assign((size_t)cap * EDC_TAB_WORDS, 0);
+    uint32_t *cnt = g.counters.data();
+    run_grid((n + 255) / 256, 256, [&] { k_kg_insert(n, KgKey32{pub}, 0x1234567u, hsize - 1, htab.data(), g.rep.data(), kcnt.data()); });
+    run_grid((n + 255) / 256, 256, [&] { k_kg_assign(n, g.rep.data(), kcnt.data(), T, kcap, g.keyid.data(), g.keylist.data(), cnt); });
+    const unsigned kb = (cap + 63) / 64, cb = (cap * EDC_NCHAIN + 63) / 64;
+    run_grid(kb, 64, [&] { k_edc_bases(cnt, cap, g.keylist.data(), pub, bases.data(), g.kflags.data()); });
+    run_grid(cb, 64, [&] { k_edc_fill(cnt, cap, bases.data(), g.kflags.data(), hs.data(), ztop.data(), g.ctab.data()); });
+    run_grid(kb, 64, [&] { k_edc_inv(cnt, cap, g.kflags.data(), ztop.data(), pref.data()); });
+    run_grid(cb, 64, [&] { k_edc_final(cnt, cap, g.kflags.data(), hs.data(), ztop.data(), g.ctab.data()); });
+    run_grid((n + 255) / 256, 256, [&] { k_kg_route(n, g.rep.data(), g.keyid.data(), g.item_kid.data(), g.klist.data(), g.glist.data(), cnt); });
+}
+// table slots of a launch of n items, as ed_group_cap (inst_ed25519.cu) counts them with no minimum batch; 0: no grouping
+static uint32_t ed_group_cap_host(uint32_t n, uint32_t T, uint32_t max_keys) {
+    if (T == 0 || n < T || max_keys == 0) return 0;
+    const uint32_t k = std::min(n / T, max_keys);
+    return k ? k : 1;
+}
+// The comb tables of a launch of the n keys of pub at threshold T with at most max_keys tables, as
+// sbv_debug_ed25519_comb_tab reports them: per query item, status 0 and the table (510 x 24 words) at out + q * 12240;
+// 1: no table; 2: a table slot, but the key does not decode.
+extern "C" int hs_ed25519_comb_tab(size_t n, const uint8_t *pub, uint32_t T, uint32_t max_keys, size_t m, const uint32_t *items, int32_t *status,
+                                   uint32_t *out) {
+    const uint32_t kcap = ed_group_cap_host((uint32_t)n, T, max_keys);
+    EdGroup g;
+    if (kcap) ed_group_host((uint32_t)n, pub, T, kcap, g);
+    for (size_t q = 0; q < m; q++) {
+        if (items[q] >= n) return -1;
+        const int32_t kid = kcap ? g.keyid[g.rep[items[q]]] : -1;
+        status[q] = kid < 0 ? 1 : g.kflags[kid] ? 0 : 2;
+        if (status[q] == 0) memcpy(out + q * EDC_TAB_WORDS, g.ctab.data() + (size_t)kid * EDC_TAB_WORDS, EDC_TAB_WORDS * 4);
+    }
+    return 0;
+}
+// k_ed_verify_comb with the caller's k (8 little-endian limbs per item, each < L; -1 otherwise), every distinct key with a
+// table, as sbv_debug_ed25519_verify_comb_k runs it on the device
+extern "C" int hs_ed25519_verify_comb_k(size_t n, const uint8_t *sig, const uint8_t *pub, const uint32_t *k_in, uint8_t *ok) {
+    uint32_t Lm[8];
+    ed_order(Lm);
+    std::vector<uint32_t> k(8 * n + 8);
+    for (size_t i = 0; i < n; i++) {
+        uint32_t ki[8];
+        for (int w = 0; w < 8; w++) k[(size_t)w * n + i] = ki[w] = k_in[i * 8 + w];
+        if (!mp_lt<8>(ki, Lm)) return -1;
+    }
+    if (n == 0) return 0;
+    EdGroup g;
+    ed_group_host((uint32_t)n, pub, 1, (uint32_t)n, g);
+    const uint4 *bt = reinterpret_cast<const uint4 *>(ed_btab_host().data()), *ct = reinterpret_cast<const uint4 *>(g.ctab.data());
+    run_grid((unsigned)((n + 127) / 128), 128,
+             [&] { k_ed_verify_comb<128>((uint32_t)n, sig, g.item_kid.data(), g.kflags.data(), ct, k.data(), bt, ok, nullptr, nullptr); });
+    return 0;
+}
+// the pipeline of sbv_ed25519_verify_batch on one device with grouping: the first half (ed_group_host), k_ed_sha512,
+// k_ed_verify over the generic list and k_ed_verify_comb over the grouped one; T = 0 or fewer than T items: no grouping.
+// stats = {keys found, items on the comb path, items on the generic path}
+extern "C" int hs_ed25519_verify_grouped(size_t n, const uint8_t *msgs, const uint64_t *off, const uint8_t *sig, const uint8_t *pub, uint32_t T,
+                                         uint32_t max_keys, uint8_t *ok, uint32_t *stats) {
+    const uint32_t nn = (uint32_t)n, kcap = ed_group_cap_host(nn, T, max_keys);
+    if (!kcap) {
+        if (stats) { stats[0] = 0; stats[1] = 0; stats[2] = nn; }
+        return hs_ed25519_verify(n, msgs, off, sig, pub, ok);
+    }
+    EdGroup g;
+    ed_group_host(nn, pub, T, kcap, g);
+    std::vector<uint32_t> k(8 * n + 8);
+    run_grid((nn + 127) / 128, 128, [&] { k_ed_sha512(nn, sig, pub, msgs, off, 0, k.data(), nullptr, nullptr); });
+    const uint4 *bt = reinterpret_cast<const uint4 *>(ed_btab_host().data()), *ct = reinterpret_cast<const uint4 *>(g.ctab.data());
+    const uint32_t *cnt = g.counters.data();
+    run_grid((nn + 31) / 32, 32, [&] { k_ed_verify<32>(nn, sig, pub, k.data(), bt, ok, g.glist.data(), cnt + 2); });
+    run_grid((nn + 127) / 128, 128,
+             [&] { k_ed_verify_comb<128>(nn, sig, g.item_kid.data(), g.kflags.data(), ct, k.data(), bt, ok, g.klist.data(), cnt + 1); });
+    if (stats) { stats[0] = cnt[0]; stats[1] = cnt[1]; stats[2] = cnt[2]; }
     return 0;
 }
 
