@@ -157,10 +157,14 @@ inline int sbv_fail(sbv_engine *e, int code, const char *fmt, ...) {
                             __FILE__, __LINE__);                                                      \
     } while (0)
 
+constexpr size_t SBV_NO_PROFILE = ~(size_t)0;
+
 // one keys-per-item launch between its two halves (pipeline.cu)
 struct VerifyLaunch {
     Dev::Scratch *w = nullptr;
-    cudaEvent_t *ev = nullptr;
+    // first of the launch's five profiling events in d.prof_events (SBV_NO_PROFILE: none).  An index, resolved under
+    // e->mu at each use: another thread's launch may grow the vector while this one is held open between its halves.
+    size_t ev = SBV_NO_PROFILE;
     const uint8_t *d_qx = nullptr, *d_qy = nullptr;
     size_t n = 0;
     uint8_t curve = 0;

@@ -116,18 +116,22 @@ int sbv_take_scratch(sbv_engine *e, Dev &d, size_t N, const KtGeom *q, size_t n,
 
 namespace {
 
-cudaEvent_t *prof_take(sbv_engine *e, Dev &d) {
-    if (!e->profiling) return nullptr;
+// The index of five fresh profiling events of device d (SBV_NO_PROFILE: profiling is off).  Growing the vector moves
+// its elements, so a launch keeps the index and takes a pointer only under e->mu (prof_at).
+size_t prof_take(sbv_engine *e, Dev &d) {
+    if (!e->profiling) return SBV_NO_PROFILE;
     if (d.prof_used + 5 > d.prof_events.size()) {
         size_t old = d.prof_events.size();
         d.prof_events.resize(old + 128);
         for (size_t i = old; i < d.prof_events.size(); i++)
-            if (cudaEventCreate(&d.prof_events[i]) != cudaSuccess) { d.prof_events.resize(i); return nullptr; }
+            if (cudaEventCreate(&d.prof_events[i]) != cudaSuccess) { d.prof_events.resize(i); return SBV_NO_PROFILE; }
     }
-    cudaEvent_t *ev = &d.prof_events[d.prof_used];
+    size_t ev = d.prof_used;
     d.prof_used += 5;  // start, after prep, before / after the fixed-base (or generic) kernel, after k_gpart
     return ev;
 }
+
+cudaEvent_t *prof_at(Dev &d, size_t ev) { return ev == SBV_NO_PROFILE ? nullptr : &d.prof_events[ev]; }
 
 }  // namespace
 
@@ -179,7 +183,7 @@ int sbv_launch_verify_begin(sbv_engine *e, Dev &d, uint8_t curve, size_t n, cons
     w->open = true;  // until the last chunk records the set's `done` event
     vl->w = w; vl->curve = curve; vl->n = n; vl->grouping = grouping; vl->d_qx = d_qx; vl->d_qy = d_qy; vl->chunks = chunks;
     vl->ev = prof_take(e, d);
-    if (vl->ev) CU(e, cudaEventRecord(vl->ev[0], st));
+    if (cudaEvent_t *ev = prof_at(d, vl->ev)) CU(e, cudaEventRecord(ev[0], st));
     if (!grouping) return 0;
     uint32_t *counters = w->zeroed, *kcnt = w->zeroed + 4;
     CU(e, cudaMemsetAsync(w->htab, 0xff, (size_t)w->hsize * 4, st));
@@ -208,7 +212,7 @@ int sbv_launch_verify_chunk(sbv_engine *e, Dev &d, const VerifyLaunch &vl, int c
     const uint32_t *gtab = d.gtab[vl.curve];
     // The profile of a launch is that of its last chunk.  A chunked launch starts it again there (nothing of the first
     // half overlaps the last chunk); a launch of one chunk keeps the start of its first half, so the grouping counts as prep.
-    cudaEvent_t *ev = last ? vl.ev : nullptr;
+    cudaEvent_t *ev = last ? prof_at(d, vl.ev) : nullptr;
     if (ev && vl.chunks > 1) CU(e, cudaEventRecord(ev[0], st));
     uint32_t *uw = w->uw + 2 * N * lo, *tscr = w->tscr + 12 * N * lo;
     uint8_t *flags = w->flags + lo;
@@ -345,7 +349,7 @@ int sbv_launch_keyed(sbv_engine *e, Dev &d, uint8_t curve, size_t n, const uint3
     const uint32_t nn = (uint32_t)n;
     Dev::Scratch *w = nullptr;
     if (int rc = sbv_take_scratch(e, d, (size_t)ops.N, nullptr, n, 0, st, &w)) return rc;
-    cudaEvent_t *ev = prof_take(e, d);
+    cudaEvent_t *ev = prof_at(d, prof_take(e, d));
     if (ev) CU(e, cudaEventRecord(ev[0], st));
     CU(e, ops.prep(nn, d_r, d_s, d_dig, dlen, w->uw, w->flags, st));
     if (ev) { CU(e, cudaEventRecord(ev[1], st)); CU(e, cudaEventRecord(ev[4], st)); CU(e, cudaEventRecord(ev[2], st)); }
