@@ -114,6 +114,84 @@ extern "C" int sbv_debug_gtable(sbv_engine *e, uint8_t curve, size_t first, size
     return SBV_OK;
 }
 
+// Copies entries [first, first + count) of the 8-bit window table of registered ECDSA slot `slot` on device 0
+// (sbv_set_keys: entry win * 128 + e - 1 is e * 2^(8 win) * Q, affine Montgomery x then y, 2N limbs).  SBV_ERR_ARG for a
+// slot that is not a key of `curve`, a key that got no table (off the curve, coordinate >= p) or a range outside the table.
+extern "C" int sbv_debug_key_table(sbv_engine *e, uint8_t curve, uint32_t slot, size_t first, size_t count, uint32_t *out) {
+    if (!e || curve > SBV_P384 || !out) return SBV_ERR_ARG;
+    const CurveOps &ops = sbv_ops(curve);
+    const size_t words = 2 * (size_t)ops.N, entries = ops.kt8->geom.ktab_words / words;
+    if (first > entries || count > entries - first) return SBV_ERR_ARG;
+    std::lock_guard<std::mutex> lk(e->mu);
+    Dev &d = e->devs[0];
+    if (slot >= d.n_slots || !d.slot2local[curve]) return SBV_ERR_ARG;
+    CU(e, cudaSetDevice(d.ordinal));
+    int32_t loc = -1;
+    CU(e, cudaMemcpy(&loc, d.slot2local[curve] + slot, sizeof loc, cudaMemcpyDeviceToHost));
+    if (loc < 0 || (uint32_t)loc >= d.n_local[curve]) return SBV_ERR_ARG;
+    uint8_t flag = 0;
+    CU(e, cudaMemcpy(&flag, d.keyflags[curve] + loc, 1, cudaMemcpyDeviceToHost));
+    if (!flag) return SBV_ERR_ARG;
+    CU(e, cudaMemcpyAsync(out, d.ktab[curve] + (size_t)loc * ops.kt8->geom.ktab_words + first * words, count * words * 4, cudaMemcpyDeviceToHost,
+                          d.stream));
+    CU(e, cudaStreamSynchronize(d.stream));
+    return SBV_OK;
+}
+
+// The per-key tables of a keys-per-item launch of the n keys (qx, qy: BYTES each) on device 0: the first half of the
+// launch (sbv_launch_verify_begin: grouping with the engine's SBV_GROUP_* settings and the table construction), then the
+// scratch set goes back (sbv_launch_verify_abort).  For each of the m query items items[q] < n: status[q] = 0 and the
+// key's table at out + q * (table words), as the verification kernel reads it (P-256: CombTab, 512 entries in slot
+// order; P-384: KeyTab<384, 5>, 77 x 16 entries; affine Montgomery x then y, 2N limbs each); 1 when the key got no table
+// (fewer items than the threshold, table slots used up, or a launch that does not group); 2 when it got a table slot but
+// is not a valid key.
+extern "C" int sbv_debug_grouped_key_table(sbv_engine *e, uint8_t curve, size_t n, const uint8_t *qx, const uint8_t *qy, size_t m,
+                                           const uint32_t *items, int32_t *status, uint32_t *out) {
+    if (!e || curve > SBV_P384 || !qx || !qy || (m && (!items || !status || !out)) || n > UINT32_MAX) return SBV_ERR_ARG;
+    for (size_t q = 0; q < m; q++)
+        if (items[q] >= n) return SBV_ERR_ARG;
+    if (n == 0) return SBV_OK;
+    const CurveOps &ops = sbv_ops(curve);
+    const size_t L = (size_t)ops.bytes, words = ops.grouped->geom.ktab_words, kb = (n * L + 255) & ~(size_t)255;
+    std::lock_guard<std::mutex> lk(e->mu);
+    Dev &d = e->devs[0];
+    CU(e, cudaSetDevice(d.ordinal));
+    int rc = sbv_ensure_scratch(e, d, 2 * kb + 1024);
+    if (rc) return rc;
+    uint8_t *dqx = d.d_scratch, *dqy = d.d_scratch + kb;
+    CU(e, cudaMemcpyAsync(dqx, qx, n * L, cudaMemcpyHostToDevice, d.stream));
+    CU(e, cudaMemcpyAsync(dqy, qy, n * L, cudaMemcpyHostToDevice, d.stream));
+    VerifyLaunch vl;
+    if ((rc = sbv_launch_verify_begin(e, d, curve, n, dqx, dqy, d.stream, &vl))) return rc;
+    Dev::Scratch *w = vl.w;
+    uint32_t nkeys = 0;
+    cudaError_t st = cudaSuccess;
+    if (vl.grouping) {
+        st = cudaStreamWaitEvent(d.stream, w->ev_tab, 0);
+        if (st == cudaSuccess) st = cudaStreamSynchronize(d.stream);
+        if (st == cudaSuccess) st = cudaMemcpy(&nkeys, (uint32_t *)w->zeroed, 4, cudaMemcpyDeviceToHost);  // counters[0]: may exceed the slots
+    }
+    const size_t kcap = vl.grouping ? w->keyflags.bytes : 0;  // bound for the key ids read back (they are < the launch's slots)
+    for (size_t q = 0; q < m && st == cudaSuccess; q++) {
+        status[q] = 1;
+        if (!vl.grouping) continue;
+        uint32_t r = 0;
+        int32_t kid = -1;
+        uint8_t flag = 0;
+        st = cudaMemcpy(&r, (uint32_t *)w->rep + items[q], 4, cudaMemcpyDeviceToHost);
+        if (st == cudaSuccess && r < n) st = cudaMemcpy(&kid, (int32_t *)w->keyid + r, 4, cudaMemcpyDeviceToHost);
+        if (kid < 0 || (size_t)kid >= kcap || (uint32_t)kid >= nkeys) continue;
+        if (st == cudaSuccess) st = cudaMemcpy(&flag, (uint8_t *)w->keyflags + kid, 1, cudaMemcpyDeviceToHost);
+        if (st == cudaSuccess && flag)
+            st = cudaMemcpy(out + q * words, (uint32_t *)w->ktab + (size_t)kid * words, words * 4, cudaMemcpyDeviceToHost);
+        if (st == cudaSuccess) status[q] = flag ? 0 : 2;
+    }
+    sbv_launch_verify_abort(vl, d.stream);
+    if (st != cudaSuccess) return sbv_fail(e, SBV_ERR_CUDA, "sbv_debug_grouped_key_table: %s", cudaGetErrorString(st));
+    CU(e, cudaStreamSynchronize(d.stream));
+    return SBV_OK;
+}
+
 // Copies entries [first, first + count) of device 0's fixed-base table of B (k_ed_btab_init: entry win * 128 + j - 1 is
 // j * 256^win * B as y + x, y - x, 2dxy, 24 limbs) to the host, building the table if no Ed25519 call has yet.
 extern "C" int sbv_debug_ed25519_btab(sbv_engine *e, size_t first, size_t count, uint32_t *out) {

@@ -33,18 +33,27 @@ namespace sbv {
 
 constexpr uint32_t KG_EMPTY = 0xffffffffu;
 
+// One word into the running hash: two multiplications with a shift between them, so that no difference in w comes out
+// of the step independent of h (a single multiplication passes a difference in bit 31 through unchanged, and the next
+// word could cancel it for every seed).
+SBV_DEV uint32_t kg_mix(uint32_t h, uint32_t w) {
+    h = (h ^ w) * 0x9E3779B1u;
+    h ^= h >> 15;
+    return h * 0x85EBCA77u;
+}
+// Every word of x and of y enters the hash: keys that differ anywhere hash apart for most seeds, so an adversary who
+// picks the keys of a batch cannot make them share one probe sequence without knowing the engine's seed.
 template <class C>
 SBV_DEV uint32_t kg_hash(const uint8_t *__restrict__ qx_be, const uint8_t *__restrict__ qy_be, uint32_t i, uint32_t seed) {
     const uint32_t *x = reinterpret_cast<const uint32_t *>(qx_be + (size_t)i * C::BYTES);
     const uint32_t *y = reinterpret_cast<const uint32_t *>(qy_be + (size_t)i * C::BYTES);
     uint32_t h = seed;
 #pragma unroll
-    for (int k = 0; k < C::N; k += 2) {
-        h = (h ^ __ldg(x + k)) * 0x9E3779B1u;
-        h = (h ^ __ldg(y + k + 1)) * 0x85EBCA77u;
-        h ^= h >> 15;
+    for (int k = 0; k < C::N; k++) {
+        h = kg_mix(h, __ldg(x + k));
+        h = kg_mix(h, __ldg(y + k));
     }
-    return h;
+    return h ^ (h >> 16);  // the probe index takes the low bits
 }
 template <class C>
 SBV_DEV bool kg_same_key(const uint8_t *__restrict__ qx_be, const uint8_t *__restrict__ qy_be, uint32_t i, uint32_t j) {

@@ -162,8 +162,9 @@ int sbv_init_gtables(sbv_engine *e, Dev &d) {
 //   begin : scratch set, key grouping on st, table construction on the set's side stream   (needs qx, qy)
 //   chunk : k_prep, routing, generic kernel on the second side stream, k_gpart, fixed-base kernel, join
 //           (needs r, s, digest), once per chunk of the batch
-int sbv_launch_verify_begin(sbv_engine *e, Dev &d, uint8_t curve, size_t n, const uint8_t *d_qx, const uint8_t *d_qy, cudaStream_t st,
-                            VerifyLaunch *vl, int chunks) {
+namespace {
+int verify_begin(sbv_engine *e, Dev &d, uint8_t curve, size_t n, const uint8_t *d_qx, const uint8_t *d_qy, cudaStream_t st, VerifyLaunch *vl,
+                 int chunks) {
     *vl = VerifyLaunch{};
     if (n == 0) return 0;
     if (chunks < 1 || chunks > SBV_MAX_CHUNKS) return sbv_fail(e, SBV_ERR_ARG, "bad chunk count %d", chunks);
@@ -195,6 +196,18 @@ int sbv_launch_verify_begin(sbv_engine *e, Dev &d, uint8_t curve, size_t n, cons
     CU(e, cudaEventRecord(w->ev_tab, w->s_tab));
     e->launches += 2 + (curve == 0 ? 5 : 4);  // grouping + table construction
     return 0;
+}
+}  // namespace
+
+// A fault after the scratch set was taken hands it back here, so that no caller leaves it held open.
+int sbv_launch_verify_begin(sbv_engine *e, Dev &d, uint8_t curve, size_t n, const uint8_t *d_qx, const uint8_t *d_qy, cudaStream_t st,
+                            VerifyLaunch *vl, int chunks) {
+    const int rc = verify_begin(e, d, curve, n, d_qx, d_qy, st, vl, chunks);
+    if (rc) {
+        sbv_launch_verify_abort(*vl, st);
+        *vl = VerifyLaunch{};
+    }
+    return rc;
 }
 
 // One chunk of a launch: the items [lo, lo + cn) are a batch of their own as far as the per-item arrays go (every one

@@ -147,6 +147,12 @@ extern "C" int hs_tables(int curve, int kind, size_t nkeys, const uint8_t *qx, c
     return 0;
 }
 
+// kg_hash (the probe start of k_kg_insert) of items 0..n-1 of (qx, qy) under `seed`
+extern "C" int hs_kg_hash(int curve, size_t n, const uint8_t *qx, const uint8_t *qy, uint32_t seed, uint32_t *out) {
+    for (size_t i = 0; i < n; i++) out[i] = curve == 0 ? kg_hash<P256>(qx, qy, (uint32_t)i, seed) : kg_hash<P384>(qx, qy, (uint32_t)i, seed);
+    return 0;
+}
+
 // k_sha256 over a ragged batch, one message per simulated thread (perm: optional processing order, as the counting sort gives it)
 extern "C" int hs_sha256(size_t n, const uint8_t *msgs, const uint64_t *off, uint64_t base, const uint32_t *perm, uint8_t *digest_out) {
     run_grid((unsigned)((n + 127) / 128), 128, [&] { k_sha256((uint32_t)n, msgs, off, base, digest_out, perm); });
