@@ -62,6 +62,34 @@ extern "C" int sbv_debug_ed25519(sbv_engine *e, int op, size_t n, const uint32_t
     return SBV_OK;
 }
 
+namespace {
+__global__ void k_debug_ed25519_point(int op, uint32_t n, const uint32_t *__restrict__ in, uint32_t *__restrict__ out) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    ed_point_dispatch(op, i, in, out);
+}
+}  // namespace
+
+// Ed25519 point ops on device 0: op (operation | ED_PT_* flags) and the ED_POINT_WORDS-word slots of in / out as in
+// ed25519_debug.cuh.  SBV_ERR_ARG for an op or flag the dispatch does not run.
+extern "C" int sbv_debug_ed25519_point(sbv_engine *e, int op, size_t n, const uint32_t *in, uint32_t *out) {
+    if (!e || !ed_point_op_ok(op) || !in || !out || n > UINT32_MAX) return SBV_ERR_ARG;
+    if (n == 0) return SBV_OK;
+    std::lock_guard<std::mutex> lk(e->mu);
+    Dev &d = e->devs[0];
+    CU(e, cudaSetDevice(d.ordinal));
+    const size_t bytes = n * ED_POINT_WORDS * 4;
+    int rc = sbv_ensure_scratch(e, d, 2 * bytes + 1024);
+    if (rc) return rc;
+    uint32_t *din = (uint32_t *)d.d_scratch, *dout = din + n * ED_POINT_WORDS;
+    CU(e, cudaMemcpyAsync(din, in, bytes, cudaMemcpyHostToDevice, d.stream));
+    k_debug_ed25519_point<<<(uint32_t)((n + 63) / 64), 64, 0, d.stream>>>(op, (uint32_t)n, din, dout);
+    CU(e, cudaGetLastError());
+    CU(e, cudaMemcpyAsync(out, dout, bytes, cudaMemcpyDeviceToHost, d.stream));
+    CU(e, cudaStreamSynchronize(d.stream));
+    return SBV_OK;
+}
+
 // The production SHA-512 kernel of Ed25519 on device 0: dig_out = the 64-byte digests of R || A || M (as SHA-512 outputs
 // them), k_out = the 8 little-endian limbs of k = digest mod L per item.  msg_off are offsets into msgs (off[0] may be > 0).
 extern "C" int sbv_debug_ed25519_sha512(sbv_engine *e, size_t n, const uint8_t *msgs, const uint64_t *msg_off, const uint8_t *sig,

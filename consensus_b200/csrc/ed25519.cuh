@@ -304,7 +304,7 @@ SBV_DEV void ed_encode(uint32_t (&enc)[8], const EdP &P) {
 
 // ---- scalars mod L ----
 // r = x mod L for a 512-bit x (16 little-endian limbs): Barrett reduction with b = 2^32, k = 8 (HAC 14.42),
-// mu = floor(2^512 / L) (9 limbs); at most two final subtractions.
+// mu = floor(2^512 / L) (9 limbs); one final subtraction (HAC allows two; this L and mu never need the second).
 SBV_DEV void sc_reduce512(uint32_t (&r)[8], const uint32_t (&x)[16]) {
     const uint32_t mu[9] = {0x0a2c131b, 0xed9ce5a3, 0x086329a7, 0x2106215d, 0xffffffeb, 0xffffffff, 0xffffffff, 0xffffffff, 0x0000000f};
     uint32_t Lm[8];
@@ -338,23 +338,19 @@ SBV_DEV void sc_reduce512(uint32_t (&r)[8], const uint32_t (&x)[16]) {
             c >>= 32;
         }
     }
-    uint32_t t[9];
+    uint32_t t[9], u[9];
     t[0] = sub_cc(x[0], q3L[0]);
 #pragma unroll
     for (int i = 1; i < 9; i++) t[i] = subc_cc(x[i], q3L[i]);
+    // t < 1.2250 L: q - q3 <= 1 for every x < 2^512 (mu = 2^512 / L - 0.2249..., tests/ed25519_arith.py:barrett_bound),
+    // so one conditional subtraction ends in [0, L)
+    u[0] = sub_cc(t[0], Lm[0]);
 #pragma unroll
-    for (int rep = 0; rep < 2; rep++) {  // t < 3L
-        uint32_t u[9];
-        u[0] = sub_cc(t[0], Lm[0]);
+    for (int i = 1; i < 8; i++) u[i] = subc_cc(t[i], Lm[i]);
+    u[8] = subc_cc(t[8], 0);
+    const bool lt = (subc(0, 0) & 1u) != 0;
 #pragma unroll
-        for (int i = 1; i < 8; i++) u[i] = subc_cc(t[i], Lm[i]);
-        u[8] = subc_cc(t[8], 0);
-        const bool lt = (subc(0, 0) & 1u) != 0;
-#pragma unroll
-        for (int i = 0; i < 9; i++) t[i] = lt ? t[i] : u[i];
-    }
-#pragma unroll
-    for (int i = 0; i < 8; i++) r[i] = t[i];
+    for (int i = 0; i < 8; i++) r[i] = lt ? t[i] : u[i];
 }
 SBV_DEV bool sc_lt_order(const uint32_t (&s)[8]) {
     uint32_t Lm[8];

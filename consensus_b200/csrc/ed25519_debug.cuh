@@ -1,5 +1,6 @@
 // ed25519_debug.cuh — test hooks of the Ed25519 arithmetic (debug.cu on the device, tools/hostsim on the CPU).
-// Slots of ED_DEBUG_WORDS little-endian 32-bit words in and out; the operands are a = in[0..8), b = in[8..16).
+// Field and scalar ops: slots of ED_DEBUG_WORDS little-endian 32-bit words in and out; the operands are a = in[0..8),
+// b = in[8..16).  Point ops: wider slots, see ed_point_dispatch.
 #pragma once
 #include "ed25519.cuh"
 
@@ -50,6 +51,68 @@ SBV_DEV void ed_debug_dispatch(int op, uint32_t i, const uint32_t *in_all, uint3
     default: return;
     }
     for (int k = 0; k < 8; k++) out[k] = r[k];
+}
+
+// Point ops: slots of ED_POINT_WORDS words, P = in[0..32) and Q = in[32..64) as extended points (X, Y, Z, T, 8 raw limbs
+// each, any value < 2^256).  The low byte of op is the operation, ED_PT_* flags above it; out[0..32) is the result as the
+// device holds it (not reduced), the rest zero.
+constexpr int ED_POINT_WORDS = 64;
+enum EdPointOp {
+    ED_PT_DOUBLE = 0,  // ed_double<!NO_T>(P); without T, out's T is P.T (not written)
+    ED_PT_ADD = 1,     // ed_add<!NO_T, AFFINE>(P, ed_to_cached(Q), NEG): P + Q or P - Q (AFFINE: Q.Z must be 1, 2Z not read)
+    ED_PT_CACHED = 2,  // ed_to_cached(P): Y+X, Y-X, 2Z, 2dT
+    ED_PT_ENCODE = 3,  // out[0..8) = ed_encode(P), canonical
+};
+constexpr int ED_PT_NO_T = 0x100, ED_PT_AFFINE = 0x200, ED_PT_NEG = 0x400;
+// the ops the dispatch runs: flags only on the ops that take them
+inline bool ed_point_op_ok(int op) {
+    const int base = op & 0xff, flags = op & ~0xff;
+    if (base == ED_PT_DOUBLE) return (flags & ~ED_PT_NO_T) == 0;
+    if (base == ED_PT_ADD) return (flags & ~(ED_PT_NO_T | ED_PT_AFFINE | ED_PT_NEG)) == 0;
+    return (base == ED_PT_CACHED || base == ED_PT_ENCODE) && flags == 0;
+}
+
+SBV_DEV void ed_point_dispatch(int op, uint32_t i, const uint32_t *in_all, uint32_t *out_all) {
+    const uint32_t *in = in_all + (size_t)i * ED_POINT_WORDS;
+    uint32_t *out = out_all + (size_t)i * ED_POINT_WORDS;
+    EdP P, Q;
+    for (int k = 0; k < 8; k++) {
+        P.X[k] = in[k]; P.Y[k] = in[8 + k]; P.Z[k] = in[16 + k]; P.T[k] = in[24 + k];
+        Q.X[k] = in[32 + k]; Q.Y[k] = in[40 + k]; Q.Z[k] = in[48 + k]; Q.T[k] = in[56 + k];
+    }
+    for (int k = 0; k < ED_POINT_WORDS; k++) out[k] = 0;
+    const bool with_t = !(op & ED_PT_NO_T), affine = (op & ED_PT_AFFINE) != 0, neg = (op & ED_PT_NEG) != 0;
+    switch (op & 0xff) {
+    case ED_PT_DOUBLE:
+        if (with_t) ed_double<true>(P);
+        else ed_double<false>(P);
+        break;
+    case ED_PT_ADD: {
+        EdCached c;
+        ed_to_cached(c, Q);
+        if (with_t && affine) ed_add<true, true>(P, c.ypx, c.ymx, c.t2d, c.z2, neg);
+        else if (with_t) ed_add<true, false>(P, c.ypx, c.ymx, c.t2d, c.z2, neg);
+        else if (affine) ed_add<false, true>(P, c.ypx, c.ymx, c.t2d, c.z2, neg);
+        else ed_add<false, false>(P, c.ypx, c.ymx, c.t2d, c.z2, neg);
+        break;
+    }
+    case ED_PT_CACHED: {
+        EdCached c;
+        ed_to_cached(c, P);
+        mp_copy<8>(P.X, c.ypx); mp_copy<8>(P.Y, c.ymx); mp_copy<8>(P.Z, c.z2); mp_copy<8>(P.T, c.t2d);
+        break;
+    }
+    case ED_PT_ENCODE: {
+        uint32_t enc[8];
+        ed_encode(enc, P);
+        for (int k = 0; k < 8; k++) out[k] = enc[k];
+        return;
+    }
+    default: return;
+    }
+    for (int k = 0; k < 8; k++) {
+        out[k] = P.X[k]; out[8 + k] = P.Y[k]; out[16 + k] = P.Z[k]; out[24 + k] = P.T[k];
+    }
 }
 
 }  // namespace sbv

@@ -344,6 +344,13 @@ extern "C" int hs_ed25519_op(int op, size_t n, const uint32_t *in, uint32_t *out
     for (size_t i = 0; i < n; i++) ed_debug_dispatch(op, (uint32_t)i, in, out);
     return 0;
 }
+// point operations of ed25519_debug.cuh, ED_POINT_WORDS-word slots; -1 for an op the dispatch does not run, as
+// sbv_debug_ed25519_point refuses it
+extern "C" int hs_ed25519_point(int op, size_t n, const uint32_t *in, uint32_t *out) {
+    if (!ed_point_op_ok(op)) return -1;
+    for (size_t i = 0; i < n; i++) ed_point_dispatch(op, (uint32_t)i, in, out);
+    return 0;
+}
 // k_ed_sha512 over a ragged batch (perm: optional processing order): k word-major [8][n], and the 16 digest limbs per item
 extern "C" int hs_ed25519_sha512(size_t n, const uint8_t *msgs, const uint64_t *off, uint64_t base, const uint8_t *sig, const uint8_t *pub,
                                  const uint32_t *perm, uint32_t *k_out, uint32_t *dig_out) {
