@@ -69,6 +69,8 @@ struct P256 {
         hi[2] = addc_cc(T[10], m7);
 #pragma unroll
         for (int i = 3; i < 8; i++) hi[i] = addc_cc(T[8 + i], 0);
+        // chains A and B never carry out (T < p*2^256: tests/test_mutant_proofs.py), so these two captures read 0; they
+        // stay because ptxas allocates registers differently without them (k_verify_kt 168 -> 155, k_comb_affine 120 -> 122)
         t16 = addc(0, 0);
         // chain B: + M*2^192 over limbs 6..13
         (void)add_cc(a6, m0);

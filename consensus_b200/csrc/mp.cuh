@@ -284,47 +284,4 @@ SBV_DEV void mont_sqr_sos(uint32_t (&r)[N], const uint32_t (&a)[N], const uint32
     mont_reduce_sos<N>(r, T, m, minv_full);
 }
 
-// Generic word-serial Montgomery reduction: r = T * 2^(-32N) mod m for T < m * 2^(32N),
-// minv = -m^-1 mod 2^32.  Used for arithmetic mod the group order n and for the P-384 field.
-template <int N>
-SBV_DEV void mont_reduce_generic(uint32_t (&r)[N], uint32_t (&T)[2 * N], const uint32_t (&m)[N], uint32_t minv) {
-    uint32_t top = 0;  // carry limb above T[2N-1]
-#pragma unroll
-    for (int i = 0; i < N; i++) {
-        uint32_t q = T[i] * minv;
-        uint64_t c = 0;
-#pragma unroll
-        for (int j = 0; j < N; j++) {
-            uint64_t v = (uint64_t)q * m[j] + T[i + j] + c;
-            T[i + j] = (uint32_t)v;
-            c = v >> 32;
-        }
-#pragma unroll
-        for (int j = i + N; j < 2 * N; j++) {
-            uint64_t v = (uint64_t)T[j] + c;
-            T[j] = (uint32_t)v;
-            c = v >> 32;
-        }
-        top += (uint32_t)c;
-    }
-    uint32_t hi[N], t[N];
-#pragma unroll
-    for (int i = 0; i < N; i++) hi[i] = T[N + i];
-    uint32_t bw = mp_sub<N>(t, hi, m);
-    bool use_t = (top != 0) || (bw == 0);
-    mp_select<N>(r, use_t, t, hi);
-}
-template <int N>
-SBV_DEV void mont_mul_generic(uint32_t (&r)[N], const uint32_t (&a)[N], const uint32_t (&b)[N], const uint32_t (&m)[N], uint32_t minv) {
-    uint32_t T[2 * N];
-    mp_mul<N>(T, a, b);
-    mont_reduce_generic<N>(r, T, m, minv);
-}
-template <int N>
-SBV_DEV void mont_sqr_generic(uint32_t (&r)[N], const uint32_t (&a)[N], const uint32_t (&m)[N], uint32_t minv) {
-    uint32_t T[2 * N];
-    mp_sqr<N>(T, a);
-    mont_reduce_generic<N>(r, T, m, minv);
-}
-
 }  // namespace sbv

@@ -44,6 +44,83 @@ def _sqrt(a, m):
     return x if x * x % m == a % m else None
 
 
+def mod_inv_model(a, m, N, check=True):
+    """mod_inv of curve.cuh on the plain residue a (binary extended GCD, batched trailing-zero strips), limb for limb:
+    returns (x1 = a^-1 mod m, passes of the main loop).  check: assert at every strip that the cofactor is below m, so
+    the conditional subtraction after the shift never fires."""
+    mask = (1 << (32 * N)) - 1
+    minv = -pow(m, -1, 1 << 32) % (1 << 32)
+
+    def strip(t, x):
+        while t & 1 == 0:
+            low = t & 0xFFFFFFFF
+            tz = (low & -low).bit_length() - 1 if low else 31
+            t >>= tz
+            k = ((x & 0xFFFFFFFF) * minv) & ((1 << tz) - 1)
+            x = ((x + k * m) >> tz) & mask
+            assert not check or x < m
+            if x >= m:
+                x -= m
+        return t, x
+
+    u, v, x1, x2 = a, m, 1, 0
+    if u & 1 == 0:
+        u, x1 = strip(u, x1)
+    passes = 0
+    while u != v:
+        passes += 1
+        lt = u < v
+        d = v - u if lt else u - v
+        xd = (x1 - x2) % m
+        if lt:
+            xd = m - xd
+        d, xd = strip(d, xd)
+        if lt:
+            v, x2 = d, xd
+        else:
+            u, x1 = d, xd
+    return x1, passes
+
+
+def longest_inverse_inputs(m, N):
+    """Residues whose mod_inv takes the most passes, 32N - 1 (the bound, tests/test_mutant_proofs.py): a = -m mod 2^k.
+    Then v = m shrinks one bit per pass, (v - a) / 2 with exactly one trailing zero, while u = a stays, for k - 1 passes;
+    the tail of the run takes the rest.  Random residues need ~0.8 * 32N."""
+    W = 32 * N
+    return [(-m) % (1 << k) for k in range(W - 8, W) if mod_inv_model((-m) % (1 << k), m, N)[1] == W - 1]
+
+
+def mp_mul_row_carries(a, b, N):
+    """mp_mul of mp.cuh, limb for limb: the carry out of each row's E and O chains, {(accumulator, row): carry}"""
+    B = 1 << 32
+    A = [(a >> (32 * i)) % B for i in range(N)]
+    Bv = [(b >> (32 * i)) % B for i in range(N)]
+    E, O, out = [0] * (2 * N), [0] * (2 * N), {}
+
+    def chain(acc, cells, i0, j):
+        c = 0
+        for i in range(i0, N, 2):
+            lo, hi = cells(i)
+            t = acc[lo] + A[i] * Bv[j] + c + (acc[hi] << 32)
+            acc[lo], acc[hi], c = t % B, (t >> 32) % B, t >> 64
+        return c
+
+    for j in range(N):
+        if j % 2 == 0:
+            out[("E", j)] = c = chain(E, lambda i: (i + j, i + j + 1), 0, j)
+            E[j + N] = (E[j + N] + c) % B
+            out[("O", j)] = c = chain(O, lambda i: (i + j - 1, i + j), 1, j)
+            O[j + N] = (O[j + N] + c) % B
+        else:
+            out[("E", j)] = c = chain(E, lambda i: (i + j, i + j + 1), 1, j)
+            if j + N + 1 < 2 * N:
+                E[j + N + 1] = (E[j + N + 1] + c) % B
+            out[("O", j)] = c = chain(O, lambda i: (i + j - 1, i + j), 0, j)
+            O[j + N - 1] = (O[j + N - 1] + c) % B
+    assert sum(E[k] << (32 * k) for k in range(2 * N)) + sum(O[k] << (32 * (k + 1)) for k in range(2 * N)) == a * b
+    return out
+
+
 def reduction_value(x, y, m, R):
     """U = (x*y + M*m) / R with M = -x*y/m mod R: the value a Montgomery reduction holds before its final conditional
     subtraction (whatever the algorithm, M is the unique multiplier in [0, R) that clears the low half)."""
@@ -182,36 +259,101 @@ def big_x_points(curve, count):
     return pts
 
 
+def small_x_points(curve, count):
+    """The first `count` points R = (x, y) with x = 1, 2, ... (x^3 - 3x + b a square mod p): x < 2n - p, so r = x + p - n
+    is a scalar in range."""
+    c = ref.CURVES[curve]
+    pts, x = [], 1
+    while len(pts) < count:
+        y = _sqrt((x * x * x - 3 * x + c.b) % c.p, c.p)
+        if y is not None:
+            pts.append((x, y))
+        x += 1
+    assert all(x + c.p - c.n < c.n for x, _ in pts)
+    return pts
+
+
 def big_x_signatures(curve, count, seed, digests=None):
     """Signatures whose R = u1*G + u2*Q has x in [n, p), so a correct verifier accepts r = R.x - n (Go: R.x mod n == r).
-    Random u1, u2; Q = (R - u1*G)/u2, s = r/u2, e = u1*s.  Three rows per R: r = R.x - n (accept), r = R.x (>= n: reject)
-    and r = R.x - n + 1 (reject).  digests: one per R, taken as given (u1 = e*u2/r instead of random), for the hashing
-    entry points.  Returns the batch dict plus "rx" (R.x of every row) and "want" (the verdicts by construction)."""
+    Random u1, u2; Q = (R - u1*G)/u2, s = r/u2, e = u1*s.  Four rows per R: r = R.x - n (accept), r = R.x (>= n: reject),
+    r = R.x - n + 1 (reject), and, on a second point R' with a small x, r = R'.x + p - n (reject: R'.x mod n != r, but
+    r + n = R'.x + p is R'.x mod p, so a verifier that compares (r + n) * Z^2 without checking r < p - n accepts it).
+    digests: one per R, taken as given (u1 = e*u2/r instead of random), for the hashing entry points; the fourth row uses
+    the same digest.  Returns the batch dict plus "rx" (the x of the row's R) and "want" (the verdicts by construction)."""
     c = ref.CURVES[curve]
     L, n = c.size, c.n
     rng = np.random.default_rng(seed)
     rnd = lambda: int.from_bytes(rng.bytes(L + 8), "big") % (n - 1) + 1
     rows, rx, want = [], [], []
-    for i, (x, y) in enumerate(big_x_points(curve, count)):
-        r = x - n
+
+    def signature(x, y, r, dig):
+        """(s, qx, qy, e) with R = u1*G + u2*Q = (x, y) for the row's r"""
         u2 = rnd()
-        if digests is None:
-            u1 = rnd()
-            dig = None
-        else:
-            dig = bytes(np.asarray(digests[i], np.uint8))
-            u1 = ref.hash_to_int(c, dig) * u2 * pow(r, -1, n) % n
+        u1 = rnd() if dig is None else ref.hash_to_int(c, dig) * u2 * pow(r, -1, n) % n
         iu2 = pow(u2, -1, n)
         Q = oracle.lincomb(curve, ((n - u1) * iu2 % n).to_bytes(L, "big"), iu2.to_bytes(L, "big"), x.to_bytes(L, "big"), y.to_bytes(L, "big"))
         qx, qy = (int.from_bytes(v, "big") for v in Q)
         s = r * iu2 % n
-        e = u1 * s % n if dig is None else dig
+        return s, qx, qy, (u1 * s % n if dig is None else dig)
+
+    for i, ((x, y), (x2, y2)) in enumerate(zip(big_x_points(curve, count), small_x_points(curve, count))):
+        dig = None if digests is None else bytes(np.asarray(digests[i], np.uint8))
+        r = x - n
+        s, qx, qy, e = signature(x, y, r, dig)
         for rr, ok in ((r, 1), (x, 0), (r + 1, 0)):
             rows.append((rr, s, qx, qy, e))
             rx.append(x)
             want.append(ok)
+        r2 = x2 + c.p - n
+        rows.append((r2, *signature(x2, y2, r2, dig)))
+        rx.append(x2)
+        want.append(0)
     b = _rows(rows, L)
     b["rx"], b["want"] = rx, np.array(want, np.uint8)
+    return b
+
+
+def sparse_s_signatures(curve, count, seed):
+    """Valid signatures whose s has only its top 32-bit limb set (s = t * 2^(32(N-1))): a zero test that reads fewer limbs
+    takes s for 0 and rejects.  R = k*G, r = R.x mod n, e = s*k - r*d; per signature the row (accept) and the row with
+    e + 1 (reject).  Returns the batch dict plus "want"."""
+    c = ref.CURVES[curve]
+    L, n, N = c.size, c.n, c.size // 4
+    rng = np.random.default_rng(seed)
+    rnd = lambda m: int.from_bytes(rng.bytes(L + 8), "big") % (m - 1) + 1
+    rows, want = [], []
+    for _ in range(count):
+        d, k = rnd(n), rnd(n)
+        qx, qy = ref.pubkey(curve, d)
+        r = ref.scalar_mult(c, k, (c.gx, c.gy))[0] % n
+        s = rnd(n >> (32 * (N - 1))) << (32 * (N - 1))
+        assert 0 < s < n and s % (1 << (32 * (N - 1))) == 0
+        e = (s * k - r * d) % n
+        rows += [(r, s, qx, qy, e), (r, s, qx, qy, (e + 1) % n)]
+        want += [1, 0]
+    b = _rows(rows, L)
+    b["want"] = np.array(want, np.uint8)
+    return b
+
+
+def s_plus_n_signatures(curve, count, seed):
+    """Signatures (r, 1), valid for e = k - r*d, and the same signature with s = n + 1 (>= n: reject).  k_prep computes
+    with s = 1 for an item whose s is out of range, so a kernel that ignores k_prep's range flag accepts the second row.
+    Returns the batch dict plus "want"."""
+    c = ref.CURVES[curve]
+    L, n = c.size, c.n
+    rng = np.random.default_rng(seed)
+    rnd = lambda: int.from_bytes(rng.bytes(L + 8), "big") % (n - 1) + 1
+    rows, want = [], []
+    for _ in range(count):
+        d, k = rnd(), rnd()
+        qx, qy = ref.pubkey(curve, d)
+        r = ref.scalar_mult(c, k, (c.gx, c.gy))[0] % n
+        e = (k - r * d) % n
+        rows += [(r, 1, qx, qy, e), (r, n + 1, qx, qy, e)]
+        want += [1, 0]
+    b = _rows(rows, L)
+    b["want"] = np.array(want, np.uint8)
     return b
 
 

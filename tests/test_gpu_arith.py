@@ -63,6 +63,7 @@ def test_field_ops(eng, curve):
     got = _run(eng, curve, 4, [(x * R % c.p, 0) for x in xs], [(0, 0)] * len(xs))
     assert [g[0] for g in got] == [pow(x, -1, c.p) * R % c.p for x in xs]
     xs = [v for v in edges.edge_values(c.p, rng, 600) if v] + [pow(2, k, c.p) for k in (1, 31, 32, 33, 64, 96, 128, 224, 255, 256, 300)]
+    xs += [a * pow(R, -1, c.p) % c.p for a in edges.longest_inverse_inputs(c.p, N)]   # 32N - 1 passes, the most
     got = _run(eng, curve, 10, [(x * R % c.p, 0) for x in xs], [(0, 0)] * len(xs))   # binary-GCD field inverse (table construction)
     assert [g[0] for g in got] == [pow(x, -1, c.p) * R % c.p for x in xs]
     # scalar-field inverse (binary extended GCD): many random values plus powers of two and their
@@ -71,6 +72,7 @@ def test_field_ops(eng, curve):
     xs += [pow(2, k, c.n) for k in (1, 31, 32, 33, 63, 64, 65, 96, 128, 255, 256, 300, 383)]
     xs += [(pow(2, k, c.n) * pow(R, -1, c.n)) % c.n for k in (32, 64, 96, 200)]   # residue itself a power of two
     xs += [(c.n - pow(2, k, c.n)) % c.n for k in (1, 32, 64, 128)]
+    xs += [a * pow(R, -1, c.n) % c.n for a in edges.longest_inverse_inputs(c.n, N)]
     xs = [v for v in xs if v]
     got = _run(eng, curve, 8, [(x * R % c.n, 0) for x in xs], [(0, 0)] * len(xs))
     assert [g[0] for g in got] == [pow(x, -1, c.n) * R % c.n for x in xs]

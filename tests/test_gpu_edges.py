@@ -77,12 +77,27 @@ def _ecdsa_ref(curve, b):
 @pytest.mark.parametrize("curve", [P256, P384])
 def test_R_x_at_least_n(engines, curve):
     """R.x in [n, p): r = R.x - n accepts (final_check: X == (r + n) * Z^2, only reached when r < p - n), r = R.x is out of
-    range and r + 1 does not match.  Random signatures get there with probability ~2^-128 (P-256) / 2^-190 (P-384)."""
+    range and r + 1 does not match; r = R'.x + p - n with a small R'.x rejects (r + n is R'.x mod p, but r >= p - n).
+    Random signatures get there with probability ~2^-128 (P-256) / 2^-190 (P-384)."""
     b = edges.big_x_signatures(curve, 24, seed=100 + curve)
     n = ref.CURVES[curve].n
-    assert all(x >= n for x in b["rx"]) and b["want"].sum() == 24
+    assert sum(x >= n for x in b["rx"]) == 3 * 24 and b["want"].sum() == 24
     small = {k: b[k][:9] for k in ("r", "s", "qx", "qy", "digest")}
     assert np.array_equal(_ecdsa_ref(curve, small), b["want"][:9])
+    _every_path(engines, curve, b, want=b["want"])
+
+
+@pytest.mark.parametrize("curve", [P256, P384])
+def test_s_with_only_its_top_limb_set(engines, curve):
+    """s = t * 2^(32(N-1)): k_prep's s != 0 check reads every limb — valid signatures accept, their e + 1 rows reject."""
+    b = edges.sparse_s_signatures(curve, 8, seed=300 + curve)
+    _every_path(engines, curve, b, want=b["want"])
+
+
+@pytest.mark.parametrize("curve", [P256, P384])
+def test_s_plus_n_rejects_where_s_1_accepts(engines, curve):
+    """(r, 1) valid and (r, n + 1): k_prep computes the flagged second row with s = 1, so every kernel must read the flag."""
+    b = edges.s_plus_n_signatures(curve, 8, seed=310 + curve)
     _every_path(engines, curve, b, want=b["want"])
 
 
@@ -97,7 +112,7 @@ def test_R_x_at_least_n_chunked_hash_and_verify(curve, thr):
     msgs = [rng.integers(0, 256, int(k), dtype=np.uint8).tobytes() for k in lens]
     digs = np.stack([np.frombuffer(hashlib.sha256(m).digest(), np.uint8) for m in msgs])
     b = edges.big_x_signatures(curve, count, seed=200 + curve, digests=digs)
-    rows = [msgs[i // 3] for i in range(3 * count)]
+    rows = [msgs[i // 4] for i in range(4 * count)]
     off = np.zeros(len(rows) + 1, np.uint64)
     off[1:] = np.cumsum([len(m) for m in rows])
     blob = np.frombuffer(b"".join(rows) + b"\0", np.uint8)

@@ -64,11 +64,14 @@ def test_field_ops(hs, curve):
     xs = [v for v in edges.edge_values(c.p, rng, 10) if v]
     got = _run(hs, curve, 4, [(x * R % c.p, 0) for x in xs], [(0, 0)] * len(xs))
     assert [g[0] for g in got] == [pow(x, -1, c.p) * R % c.p for x in xs]
+    # binary-GCD inverses, with the residues that need the most passes (32N - 1, edges.longest_inverse_inputs)
     xs = [v for v in edges.edge_values(c.p, rng, 300) if v] + [pow(2, k, c.p) for k in (1, 31, 32, 33, 64, 96, 128, 224, 255, 256, 300)]
-    got = _run(hs, curve, 10, [(x * R % c.p, 0) for x in xs], [(0, 0)] * len(xs))   # binary-GCD field inverse
+    xs += [a * pow(R, -1, c.p) % c.p for a in edges.longest_inverse_inputs(c.p, N)]
+    got = _run(hs, curve, 10, [(x * R % c.p, 0) for x in xs], [(0, 0)] * len(xs))
     assert [g[0] for g in got] == [pow(x, -1, c.p) * R % c.p for x in xs]
     xs = [v for v in edges.edge_values(c.n, rng, 200) if v]
     xs += [pow(2, k, c.n) for k in (1, 31, 32, 33, 63, 64, 65, 96, 128, 255, 256, 300, 383)]
+    xs += [a * pow(R, -1, c.n) % c.n for a in edges.longest_inverse_inputs(c.n, N)]
     got = _run(hs, curve, 8, [(x * R % c.n, 0) for x in xs], [(0, 0)] * len(xs))
     assert [g[0] for g in got] == [pow(x, -1, c.n) * R % c.n for x in xs]
 
@@ -205,10 +208,82 @@ def _every_simulated_path(hs, curve, b):
 @pytest.mark.parametrize("curve", [0, 1])
 def test_r_plus_n_accepts_when_R_x_is_at_least_n(hs, curve):
     """R.x in [n, p): r = R.x - n must be accepted (final_check compares X with (r + n) * Z^2), r = R.x (out of range) and
-    r + 1 rejected — on the generic, grouped and registered thread / warp kernels."""
+    r + 1 rejected, and r = R'.x + p - n for a small R'.x rejected (final_check's r < p - n condition) — on the generic,
+    grouped and registered thread / warp kernels."""
+    c = ref.CURVES[curve]
     b = edges.big_x_signatures(curve, 3, seed=7 + curve)
-    assert all(x >= ref.CURVES[curve].n for x in b["rx"]) and 0 < b["want"].sum() < b["want"].size
+    assert [x >= c.n for x in b["rx"]] == [True, True, True, False] * 3 and b["want"].sum() == 3
+    assert all(int.from_bytes(bytes(r), "big") >= c.p - c.n for r in b["r"][3::4])
     _every_simulated_path(hs, curve, b)
+
+
+@pytest.mark.parametrize("curve", [0, 1])
+def test_s_with_only_its_top_limb_set(hs, curve):
+    """s = t * 2^(32(N-1)): k_prep's s != 0 check must read every limb — valid signatures accept and their e + 1 rows
+    reject on every simulated path."""
+    _every_simulated_path(hs, curve, edges.sparse_s_signatures(curve, 4, seed=30 + curve))
+
+
+@pytest.mark.parametrize("curve", [0, 1])
+def test_s_plus_n_rejects_where_s_1_accepts(hs, curve):
+    """(r, 1) valid and (r, n + 1): k_prep flags the second row and computes it with s = 1, so every kernel must read
+    that flag — on every simulated path."""
+    _every_simulated_path(hs, curve, edges.s_plus_n_signatures(curve, 4, seed=40 + curve))
+
+
+@pytest.mark.parametrize("curve", [0, 1])
+def test_key_encodings_at_the_range_edges(hs, curve):
+    """ecdsa_keys.encoding_cases on every simulated path: (x + p, y), (x, y + p), x = p, y = p, (0, 0), all ones — each
+    signature accepts under its canonical key and rejects under the edge encoding (load_key's range checks)."""
+    import ecdsa_keys
+    b, want, _ = ecdsa_keys.encoding_batch(curve, seed=50 + curve)
+    b["want"] = want
+    _every_simulated_path(hs, curve, b)
+
+
+@pytest.mark.parametrize("curve", [0, 1])
+def test_grouping_keys_that_differ_in_one_word_of_y(hs, curve):
+    """A valid key Q and an off-curve key Q' equal to Q but in the last 32-bit word of y, chosen so that both start at the
+    same hash-table slot (kg_hash under the simulation's seed): Q' must get its own group, so its items — Q's valid
+    signatures — reject, while Q's accept (kg_same_key compares every word of x and y)."""
+    import ecdsa_keys
+    c = ref.CURVES[curve]
+    L, m = c.size, 8
+    rng = np.random.default_rng(60 + curve)
+    d = int.from_bytes(rng.bytes(L + 8), "big") % (c.n - 1) + 1
+    Q = ref.pubkey(curve, d)
+    hsize = 1
+    while hsize < 2 * 2 * m:
+        hsize <<= 1
+    hs.hs_kg_hash.restype = C.c_int
+
+    def probe(qx, qy):
+        out = np.zeros(1, np.uint32)
+        assert hs.hs_kg_hash(C.c_int(curve), C.c_size_t(1), _p8(qx), _p8(qy), C.c_uint32(0x1234567), out.ctypes.data_as(C.POINTER(C.c_uint32))) == 0
+        return int(out[0]) & (hsize - 1)
+
+    qx, qy = edges._be(Q[0], L).copy(), edges._be(Q[1], L).copy()
+    start = probe(qx, qy)
+    y2 = qy.copy()
+    for v in range(1, 100000):
+        y2[L - 4:] = np.frombuffer(((int.from_bytes(qy[L - 4:].tobytes(), "big") ^ v) & 0xFFFFFFFF).to_bytes(4, "big"), np.uint8)
+        if probe(qx, y2) == start:
+            break
+    else:
+        raise AssertionError("no colliding probe start")
+    Qy2 = int.from_bytes(y2.tobytes(), "big")
+    assert not ref.on_curve(c, Q[0], Qy2)
+    rows, want = [], []
+    for i in range(m):
+        r, s, e = ecdsa_keys.signature_for(curve, Q, *(int.from_bytes(rng.bytes(L + 8), "big") % (c.n - 1) + 1 for _ in range(2)))
+        rows += [(r, s, Q[0], Q[1], e), (r, s, Q[0], Qy2, e)] if i % 2 else [(r, s, Q[0], Qy2, e), (r, s, Q[0], Q[1], e)]
+        want += [1, 0] if i % 2 else [0, 1]
+    b = edges._rows(rows, L)
+    want = np.array(want, np.uint8)
+    assert np.array_equal(oracle.verify_batch(curve, b["r"], b["s"], b["qx"], b["qy"], b["digest"]), want)
+    got, stats = _verify(hs, curve, b, grouped=(1, 64))
+    assert int(stats[0]) == 2 and int(stats[2]) == 0
+    assert np.array_equal(got, want), np.nonzero(got != want)[0]
 
 
 @pytest.mark.parametrize("curve,dlen", [(0, 32), (0, 48), (0, 20), (1, 64), (1, 48), (1, 28)])
@@ -283,9 +358,10 @@ def test_registered_keys_thread_and_warp_kernels(hs, curve, n):
     kxy[3, L + 3] ^= 8                                           # registered key 3 is not on the curve
     slot = key_idx.copy()
     slot[7] = 99                                                 # no such slot
+    slot[8] = K                                                  # one past the last slot (item 8 is signed by key 0)
     qx, qy = np.ascontiguousarray(kxy[key_idx, :L]), np.ascontiguousarray(kxy[key_idx, L:])
     want = oracle.verify_batch(cv, r, s, qx, qy, b["digest"])
-    want[7] = 0
+    want[7] = want[8] = 0
     assert want[key_idx == 3].sum() == 0 and 0 < want.sum() < n
     kx, ky = np.ascontiguousarray(kxy[:, :L]), np.ascontiguousarray(kxy[:, L:])
     dig = np.ascontiguousarray(b["digest"])

@@ -211,7 +211,9 @@ static void registered_t(uint32_t n, uint32_t nkeys, const uint8_t *kx, const ui
     std::vector<uint32_t> ktab(KtSizes<C, KT>::ktab_words(nkeys));
     std::vector<uint8_t> kflags(nkeys);
     tables_t<C, KT>(nkeys, kx, ky, 0, ktab.data(), kflags.data());
-    std::vector<int32_t> s2l(nkeys);
+    // one entry past the slots, mapped to key 0: a slot check that admits slot == n_slots reads a valid key there and
+    // accepts, where the device would read past the end of the map
+    std::vector<int32_t> s2l(nkeys + 1, 0);
     for (uint32_t i = 0; i < nkeys; i++) s2l[i] = (int32_t)i;
     std::vector<uint32_t> uw((size_t)2 * N * n);
     std::vector<uint8_t> flags(n);
@@ -416,6 +418,9 @@ extern "C" int hs_ed25519_set_keys(size_t n, const uint8_t *pub, uint32_t chunk)
     std::vector<uint32_t> slot_of;
     for (size_t i = 0; i < n; i++)
         if (flag[i]) { g_edk.slot2local[i] = (int32_t)slot_of.size(); slot_of.push_back((uint32_t)i); }
+    // the entry past the last slot maps to slot 0's table: a slot check that admits slot == n then reads a valid table and
+    // accepts slot 0's rows, where the device would read past the end of the map
+    if (n) g_edk.slot2local[n] = g_edk.slot2local[0];
     const uint32_t cnt = (uint32_t)slot_of.size();
     g_edk.ktab.assign((size_t)cnt * ED_KTAB_WORDS + 4, 0);
     const uint32_t per = std::min(cnt, chunk ? chunk : ED_KBUILD_MAX);
