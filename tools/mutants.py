@@ -43,6 +43,7 @@ ED = ["tests/test_hostsim_ed25519_arith.py", "tests/test_hostsim_ed25519.py", "t
       "tests/test_hostsim_ed25519_registered.py", "tests/test_hostsim_ed25519_grouped.py"]
 MIXED = ["tests/test_hostsim_mixed.py"]
 SHARDS = ["tests/test_hostsim_shards.py"]
+WIDE = ["tests/test_hostsim_wide.py"]  # bit lengths, offsets and byte sums past 32 bits
 
 
 def M(id, file, find, repl, tests, equivalent=None, proof=None):
@@ -205,6 +206,9 @@ CATALOGUE = [
     M("sha256_length_bytes", "sha256.cuh", "const uint64_t bits = len * 8;", "const uint64_t bits = len;", ECDSA),
     M("sha256_aligned_tail_word", "sha256.cuh", "uint32_t next = (sh || j < 15) ? __ldg(words + blk * 16 + j + 1) : 0u;",
       "uint32_t next = (j < 15) ? __ldg(words + blk * 16 + j + 1) : 0u;", ECDSA),
+    M("sha256_length_high_word", "sha256.cuh", "w[14] = (uint32_t)(bits >> 32);", "w[14] = 0u;", WIDE),
+    M("sha256_bits_32", "sha256.cuh", "const uint64_t bits = len * 8;", "const uint64_t bits = (uint32_t)len * 8u;", WIDE),
+    M("sha256_offset_32", "sha256.cuh", "const uint64_t o = off[idx] - base;", "const uint64_t o = (uint32_t)(off[idx] - base);", WIDE),
     # ---------------------------------------------------------------- sha512.cuh
     M("sha512_pad_rem", "sha512.cuh", "if (rem < 4) v = (v & (0xffffffffu << (8 * (4 - rem)))) | (0x80u << (8 * (3 - rem)));",
       "if (rem < 4) v = (v & (0xffffffffu << (8 * (4 - rem))));", ED),
@@ -213,6 +217,8 @@ CATALOGUE = [
     M("sha512_length_bytes", "sha512.cuh", "if (blk == nblocks - 1) w[15] = total * 8;", "if (blk == nblocks - 1) w[15] = total;", ED),
     M("sha512_aligned_tail_word", "sha512.cuh", "const uint32_t next = (sh || j < 15) ? __ldg(p + j + 1) : 0u;", "const uint32_t next = (j < 15) ? __ldg(p + j + 1) : 0u;", ED),
     M("sha512_first_block_msg_offset", "sha512.cuh", "sha512_msg16(w32, blk * 128 - 64, len, words, sel, sh);", "sha512_msg16(w32, blk * 128 - 60, len, words, sel, sh);", ED),
+    M("sha512_offset_32", "sha512.cuh", "const uint64_t o = off[idx] - base;", "const uint64_t o = (uint32_t)(off[idx] - base);", WIDE),
+    M("sha512_total_32", "sha512.cuh", "const uint64_t total = 64 + len;  // bytes hashed", "const uint32_t total = 64 + len;  // bytes hashed", WIDE),
     # ---------------------------------------------------------------- ed25519.cuh
     M("fe_fold_second_fold", "ed25519.cuh", "r[0] = add_cc(r[0], (uint32_t)acc * 38u);", "r[0] = add_cc(r[0], 0u);", ED),
     M("fe_fold_wrap", "ed25519.cuh", "r[0] += 38u * c;  // after a wrap the value is < 38^2: no further carry", "(void)c;", ED),
@@ -286,6 +292,12 @@ CATALOGUE = [
       "const uint32_t f = g < m0 ? 0 : g <= m0 + m1 ? 1 : 2, j = g - (f == 0 ? 0 : f == 1 ? m0 : m0 + m1);\n    const MixFamily F = mix_family(p, f);\n    const uint32_t i = F.idx[j];", MIXED),
     M("mix_ok_family_bounds", "mixed.cuh", "const uint32_t f = g < m0 ? 0 : g < m0 + m1 ? 1 : 2, j = g - (f == 0 ? 0 : f == 1 ? m0 : m0 + m1);\n    const MixFamily F = mix_family(p, f);\n    ok[F.idx[j]]",
       "const uint32_t f = g < m0 ? 0 : g < m0 + m1 ? 1 : 2, j = g - (f == 0 ? 0 : f == 1 ? m0 : m0);\n    const MixFamily F = mix_family(p, f);\n    ok[F.idx[j]]", MIXED),
+    M("mix_count_bytes_32", "mixed.cuh", "uint64_t b[MIX_FAMILIES] = {0, 0, 0};\n    const uint32_t lo = t * MIX_TILE", "uint32_t b[MIX_FAMILIES] = {0, 0, 0};\n    const uint32_t lo = t * MIX_TILE", WIDE),
+    M("mix_scan_bytes_32", "mixed.cuh", "uint64_t b[MIX_FAMILIES] = {0, 0, 0};\n    for (uint32_t t = lo; t < hi; t++)", "uint32_t b[MIX_FAMILIES] = {0, 0, 0};\n    for (uint32_t t = lo; t < hi; t++)", WIDE),
+    M("mix_split_pos_32", "mixed.cuh", "uint64_t pos[MIX_FAMILIES];", "uint32_t pos[MIX_FAMILIES];", WIDE),
+    M("mix_split_at_32", "mixed.cuh", "const uint64_t at = f == 0 ? pos[0]", "const uint32_t at = f == 0 ? pos[0]", WIDE),
+    M("mix_compact_src_32", "mixed.cuh", "const uint64_t s = off[i] - base, len", "const uint64_t s = (uint32_t)(off[i] - base), len", WIDE),
+    M("mix_compact_dst_32", "mixed.cuh", "d = F.off[j];", "d = (uint32_t)F.off[j];", WIDE),
     # ---------------------------------------------------------------- shards.h
     M("shard_range_hi", "shards.h", "const size_t lo = n * g / G, hi = n * (g + 1) / G;", "const size_t lo = n * g / G, hi = (n * (g + 1) + G - 1) / G;", SHARDS),
     M("batch_shards_words", "shards.h", "s.wv = std::max(s.wv, (s.vr[g].n + 31) / 32);\n    }\n    return s;\n}\n\n// Commit",
