@@ -26,7 +26,7 @@ SYMBOLS = [
     "sbv_comm_unique_id", "sbv_comm_init_rank", "sbv_comm_ranks", "sbv_gather_verdicts_device", "sbv_gather_words_device",
     "sbv_verify_batch_ranked", "sbv_host_alloc", "sbv_host_free", "sbv_ed25519_verify_batch",
     "sbv_ed25519_set_keys", "sbv_ed25519_verify_registered", "sbv_ed25519_verify_quorum", "sbv_mixed_verify_registered",
-    "sbv_mixed_verify_quorum",
+    "sbv_mixed_verify_quorum", "sbv_mixed_verify_batch",
 ]
 
 
@@ -336,6 +336,28 @@ class Engine:
         vp = C.c_void_p
         self._check(self._lib.sbv_mixed_verify_registered(self._h, C.c_size_t(n), vp(scheme), vp(msgs), vp(off), vp(key_slot), vp(sig96), vp(ok)),
                     "sbv_mixed_verify_registered")
+
+    def mixed_verify_batch(self, scheme, msgs, off, sig96, key96, out=None) -> np.ndarray:
+        """Items of any scheme with the key of each item in one call: scheme, msgs, off and sig96 as in
+        mixed_verify_registered, key96 = n x 96 bytes (P-256 X || Y in [0, 64), P-384 X || Y, Ed25519 encoding in [0, 32)).
+        Returns the n verdict bytes (into `out` if given)."""
+        scheme = _u8(scheme)
+        msgs = _u8(msgs if len(msgs) else np.zeros(1, np.uint8))
+        off = np.ascontiguousarray(off, dtype=np.uint64)
+        sig96, key96 = _u8(sig96), _u8(key96)
+        n = off.size - 1
+        if scheme.size != n or sig96.size != 96 * n or key96.size != 96 * n:
+            raise ValueError("scheme must hold one entry and sig96 and key96 96 bytes per message")
+        ok = out if out is not None else np.zeros(n, np.uint8)
+        self._check(self._lib.sbv_mixed_verify_batch(self._h, C.c_size_t(n), _p8(scheme), _p8(msgs), off.ctypes.data_as(C.POINTER(C.c_uint64)),
+                                                     _p8(sig96), _p8(key96), _p8(ok)), "sbv_mixed_verify_batch")
+        return ok
+
+    def mixed_verify_batch_ptr(self, n, scheme, msgs, off, sig96, key96, ok):
+        """Raw host pointers (ints) — used with pinned buffers."""
+        vp = C.c_void_p
+        self._check(self._lib.sbv_mixed_verify_batch(self._h, C.c_size_t(n), vp(scheme), vp(msgs), vp(off), vp(sig96), vp(key96), vp(ok)),
+                    "sbv_mixed_verify_batch")
 
     def mixed_verify_quorum(self, scheme, msgs, off, key_slot, sig96, instance, sender, signer, digest_match, n_instances, threshold,
                             self_id=None):

@@ -227,20 +227,23 @@ int sbv_launch_ed_verify_registered_k(sbv_engine *e, Dev &d, size_t n, const uin
                                       cudaStream_t st);
 // ---- inst_mixed.cu: mixed ECDSA / Ed25519 shards (mixed.cuh; family f = scheme tag f) ----
 // The device scratch of a shard of n items, m[f] of family f and `bytes` message bytes, carved from one buffer: the
-// uploaded tags, slots and 96-byte rows, the tile prefixes of the split, the shared message buffer of the three families,
-// and per family the compacted arrays and the scratch of its pipeline.
+// uploaded tags, slots (or, keys per item, 96-byte key rows) and 96-byte signature rows, the tile prefixes of the split,
+// the shared message buffer of the three families, and per family the compacted arrays and the scratch of its pipeline.
+// A registered shard has no key arrays (key96, qx, qy are null); a keys-per-item shard has no slots.
 struct MixBufs {
-    uint8_t *tag, *sig96;
+    uint8_t *tag, *sig96, *key96;
     uint32_t *slot_in, *tile_cnt;
     uint64_t *tile_bytes;
     uint8_t *blob;
     uint32_t *idx[3], *slot[3], *perm[3];
     uint8_t *r[3], *s[3], *ok[3], *dig[3], *pub[3];  // dig: SHA-256 digests (ECDSA) or k (Ed25519); pub: Ed25519 only
+    uint8_t *qx[3], *qy[3];                            // keys per item, ECDSA only
     uint64_t *off[3];
 };
-// base == nullptr only sizes; returns the bytes the carve takes
-size_t sbv_mix_carve(uint8_t *base, size_t n, const uint32_t m[3], uint64_t bytes, MixBufs *out);
-// the split of a staged shard (b.tag, b.slot_in, b.sig96, messages at d_msgs with offsets d_off from base) into the families
+// base == nullptr only sizes; returns the bytes the carve takes.  keys: a keys-per-item shard (sbv_mixed_verify_batch).
+size_t sbv_mix_carve(uint8_t *base, size_t n, const uint32_t m[3], uint64_t bytes, bool keys, MixBufs *out);
+// the split of a staged shard (b.tag, b.slot_in or b.key96, b.sig96, messages at d_msgs with offsets d_off from base) into
+// the families
 int sbv_launch_mix_split(sbv_engine *e, const MixBufs &b, size_t n, const uint32_t m[3], const uint8_t *d_msgs, const uint64_t *d_off, uint64_t base,
                          cudaStream_t st);
 // the family verdicts b.ok[f] back into item order in d_ok

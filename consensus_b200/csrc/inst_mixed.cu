@@ -17,7 +17,7 @@ MixPlan plan_of(const MixBufs &b) {
 }  // namespace
 static_assert(MIX_FAMILIES == SBV_ED25519 + 1, "one family per scheme tag");
 
-size_t sbv_mix_carve(uint8_t *base, size_t n, const uint32_t m[3], uint64_t bytes, MixBufs *out) {
+size_t sbv_mix_carve(uint8_t *base, size_t n, const uint32_t m[3], uint64_t bytes, bool keys, MixBufs *out) {
     MixBufs b{};
     size_t at = 0;
     auto take = [&](size_t sz) {
@@ -27,7 +27,8 @@ size_t sbv_mix_carve(uint8_t *base, size_t n, const uint32_t m[3], uint64_t byte
     };
     const size_t ntiles = (n + MIX_TILE - 1) / MIX_TILE;
     b.tag = take(n);
-    b.slot_in = (uint32_t *)take(n * 4);
+    if (keys) b.key96 = take(n * 96);
+    else b.slot_in = (uint32_t *)take(n * 4);
     b.sig96 = take(n * 96);
     b.tile_cnt = (uint32_t *)take(ntiles * MIX_FAMILIES * 4);
     b.tile_bytes = (uint64_t *)take(ntiles * MIX_FAMILIES * 8);
@@ -35,7 +36,11 @@ size_t sbv_mix_carve(uint8_t *base, size_t n, const uint32_t m[3], uint64_t byte
     for (int f = 0; f < MIX_FAMILIES; f++) {
         const size_t k = m[f], L = f == SBV_P256 ? 32 : f == SBV_P384 ? 48 : 64;
         b.idx[f] = (uint32_t *)take(k * 4);
-        b.slot[f] = (uint32_t *)take(k * 4);
+        if (!keys) b.slot[f] = (uint32_t *)take(k * 4);
+        else if (f != SBV_ED25519) {
+            b.qx[f] = take(k * L);
+            b.qy[f] = take(k * L);
+        }
         b.r[f] = take(k * L);
         b.s[f] = f == SBV_ED25519 ? nullptr : take(k * L);
         b.off[f] = (uint64_t *)take((k + 1) * 8);
@@ -54,7 +59,11 @@ int sbv_launch_mix_split(sbv_engine *e, const MixBufs &b, size_t n, const uint32
     const MixPlan p = plan_of(b);
     k_mix_count<<<(ntiles + 255) / 256, 256, 0, st>>>(nn, b.tag, d_off, ntiles, b.tile_cnt, b.tile_bytes);
     k_mix_scan<<<1, MIX_SCAN_THREADS, 0, st>>>(ntiles, b.tile_cnt, b.tile_bytes, p);
-    k_mix_split<<<(ntiles + 255) / 256, 256, 0, st>>>(nn, b.tag, b.slot_in, b.sig96, d_off, ntiles, b.tile_cnt, b.tile_bytes, p);
+    if (b.key96)
+        k_mix_split<true><<<(ntiles + 255) / 256, 256, 0, st>>>(nn, b.tag, nullptr, b.sig96, d_off, ntiles, b.tile_cnt, b.tile_bytes, p, b.key96,
+                                                                 MixKeys{{b.qx[0], b.qx[1]}, {b.qy[0], b.qy[1]}, b.pub[SBV_ED25519]});
+    else
+        k_mix_split<<<(ntiles + 255) / 256, 256, 0, st>>>(nn, b.tag, b.slot_in, b.sig96, d_off, ntiles, b.tile_cnt, b.tile_bytes, p);
     k_mix_compact<<<(uint32_t)(((uint64_t)n * MIX_LANES + 255) / 256), 256, 0, st>>>(nn, m[0], m[1], d_msgs, d_off, base, p);
     e->launches += 4;
     CU(e, cudaGetLastError());

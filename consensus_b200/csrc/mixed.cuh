@@ -1,13 +1,16 @@
 // mixed.cuh — the split of a mixed ECDSA / Ed25519 shard into its three families (P-256, P-384, Ed25519) and the
-// scatter of the family verdicts back into item order (sbv_mixed_verify_registered, sbv_mixed_verify_quorum).
+// scatter of the family verdicts back into item order (sbv_mixed_verify_registered, sbv_mixed_verify_quorum,
+// sbv_mixed_verify_batch).
 //
-// A shard is uploaded as the caller holds it: a scheme tag, a slot, a 96-byte signature row and a message per item.  The
-// split is a stable partition done in tiles of MIX_TILE consecutive items, one thread per tile:
+// A shard is uploaded as the caller holds it: a scheme tag, a slot or a 96-byte key row, a 96-byte signature row and a
+// message per item.  The split is a stable partition done in tiles of MIX_TILE consecutive items, one thread per tile:
 //   k_mix_count    per tile and family: the item count and the message bytes;
 //   k_mix_scan     one block: the exclusive prefixes of both over the tiles, per family, and where each family's messages
 //                  start in the shared message buffer;
 //   k_mix_split    per tile, in item order: each item's index, slot, signature (r and s arrays of width L for ECDSA,
-//                  64-byte R || S rows for Ed25519) and message offset, at the item's rank inside its family;
+//                  64-byte R || S rows for Ed25519) and message offset, at the item's rank inside its family; with
+//                  KEYS, the key row instead of the slot (qx and qy arrays of width L for ECDSA, 32-byte rows for
+//                  Ed25519);
 //   k_mix_compact  MIX_LANES threads per item copy its message bytes to the family's region of the shared buffer, 16
 //                  aligned bytes per store (byte stores only where a 16-byte word is shared with a neighbour);
 //   k_mix_ok       after the family pipelines: ok[idx_f[j]] = ok_f[j].
@@ -35,6 +38,12 @@ struct MixFamily {
 struct MixPlan {
     MixFamily f[MIX_FAMILIES];
     uint8_t *blob;   // the shared message buffer
+};
+// The compacted keys of a keys-per-item shard, in the order of MixFamily: a separate parameter, so that the plan, and
+// with it every kernel of a registered shard, stays as it is.
+struct MixKeys {
+    uint8_t *qx[2], *qy[2];  // P-256 (32 bytes each), P-384 (48 bytes each)
+    uint8_t *pub;            // Ed25519: 32-byte encodings
 };
 
 __device__ __forceinline__ uint64_t mix_align16(uint64_t x) { return (x + 15) & ~(uint64_t)15; }
@@ -120,9 +129,13 @@ __device__ __forceinline__ void mix_copy16(uint8_t *dst, const uint8_t *src, int
     for (int w = 0; w < words16; w++) reinterpret_cast<uint4 *>(dst)[w] = __ldg(reinterpret_cast<const uint4 *>(src) + w);
 }
 
+// KEYS: the shard carries a 96-byte key row per item (key96, packed as sig96 is) instead of a slot; the registered
+// instantiation never reads key96 or k.
+template <bool KEYS = false>
 __global__ void __launch_bounds__(256) k_mix_split(uint32_t n, const uint8_t *__restrict__ tag, const uint32_t *__restrict__ slot,
                                                    const uint8_t *__restrict__ sig96, const uint64_t *__restrict__ off, uint32_t ntiles,
-                                                   const uint32_t *__restrict__ tile_cnt, const uint64_t *__restrict__ tile_bytes, MixPlan p) {
+                                                   const uint32_t *__restrict__ tile_cnt, const uint64_t *__restrict__ tile_bytes, MixPlan p,
+                                                   const uint8_t *__restrict__ key96 = nullptr, MixKeys k = MixKeys{}) {
     const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
     if (t >= ntiles) return;
     uint32_t rank[MIX_FAMILIES];
@@ -140,17 +153,22 @@ __global__ void __launch_bounds__(256) k_mix_split(uint32_t n, const uint8_t *__
         for (int k = 0; k < MIX_FAMILIES; k++)
             if (f == (uint32_t)k) { rank[k]++; pos[k] += len; }
         F.idx[j] = i;
-        F.slot[j] = slot[i];
+        if constexpr (!KEYS) F.slot[j] = slot[i];
         F.off[j] = at;
         const uint8_t *row = sig96 + (size_t)i * 96;
         if (f == 0) {
             mix_copy16(F.r + (size_t)j * 32, row, 2);
             mix_copy16(F.s + (size_t)j * 32, row + 32, 2);
+            if constexpr (KEYS) mix_copy16(k.qx[0] + (size_t)j * 32, key96 + (size_t)i * 96, 2);
+            if constexpr (KEYS) mix_copy16(k.qy[0] + (size_t)j * 32, key96 + (size_t)i * 96 + 32, 2);
         } else if (f == 1) {
             mix_copy16(F.r + (size_t)j * 48, row, 3);
             mix_copy16(F.s + (size_t)j * 48, row + 48, 3);
+            if constexpr (KEYS) mix_copy16(k.qx[1] + (size_t)j * 48, key96 + (size_t)i * 96, 3);
+            if constexpr (KEYS) mix_copy16(k.qy[1] + (size_t)j * 48, key96 + (size_t)i * 96 + 48, 3);
         } else {
             mix_copy16(F.r + (size_t)j * 64, row, 4);
+            if constexpr (KEYS) mix_copy16(k.pub + (size_t)j * 32, key96 + (size_t)i * 96, 2);
         }
     }
 }

@@ -193,6 +193,22 @@ int sbv_ed25519_verify_quorum(sbv_engine *e, size_t n_votes, const uint8_t *msgs
  * the same Ed25519 registry, as in sbv_ed25519_verify_registered. */
 int sbv_mixed_verify_registered(sbv_engine *e, size_t n, const uint8_t *scheme, const uint8_t *msgs, const uint64_t *msg_off,
                                 const uint32_t *key_slot, const uint8_t *sig96, uint8_t *ok);
+/* sbv_mixed_verify_registered with the key of each item carried in the call (client requests of a population that mixes
+ * ECDSA and Ed25519 keys and comes and goes, so that no registry is rebuilt for it).  scheme, msgs, msg_off and sig96 as
+ * in sbv_mixed_verify_registered; key96 = one 96-byte row per item, packed as sig96 is:
+ *   P-256    X || Y, 32 bytes each, big-endian, in bytes [0, 64)
+ *   P-384    X || Y, 48 bytes each, big-endian, filling the row
+ *   Ed25519  the 32-byte RFC 8032 encoding, in bytes [0, 32)
+ * Bytes past the key are ignored.  ok[i] is byte for byte what the single-scheme keys-per-item call returns for item i:
+ * sbv_hash_verify_batch(scheme[i], ...) for ECDSA items (SHA-256 of the message; e = its leftmost 32 bytes for P-384
+ * too), sbv_ed25519_verify_batch for Ed25519 items.  The shard of each device is uploaded once, whole, and split into the
+ * three families on the device, keys included; the ECDSA families run on the call's stream while the Ed25519 one runs
+ * beside them on its second stream, and the verdicts are put back in item order on the device.  Keys that repeat are
+ * grouped per family and per device shard, with the SBV_GROUP_* settings of the single-scheme calls; an ECDSA key and an
+ * Ed25519 key are never one group.  A tag > 2 returns SBV_ERR_ARG with its index in sbv_last_error, before anything is
+ * written or launched.  No registry is read. */
+int sbv_mixed_verify_batch(sbv_engine *e, size_t n, const uint8_t *scheme, const uint8_t *msgs, const uint64_t *msg_off,
+                           const uint8_t *sig96, const uint8_t *key96, uint8_t *ok);
 /* Commit votes of a mixed consenter set verified and counted in one call (verifyVote + processCommits,
  * view.go:519-551, 827-849): ok = the verdicts of sbv_mixed_verify_registered, valid_count / reached = sbv_quorum over
  * them, with the same vote rules, self_id (NULL = no self filter) and threshold.  The verdicts stay on the device.  Votes

@@ -29,14 +29,33 @@ import (
 )
 
 // item is one unit of engine work: verify (r, s) under registry slot `slot` over SHA-256(msg), or, when ed is set,
-// the Ed25519 signature edSig under slot `slot` of the Ed25519 registry over msg (crypto/ed25519.Verify).
+// the Ed25519 signature edSig under slot `slot` of the Ed25519 registry over msg (crypto/ed25519.Verify). When keyed
+// is set the key travels with the item instead of a slot: key = P-256 X || Y, or the Ed25519 key in key[:32].
 type item struct {
 	r, s  [32]byte
 	slot  uint32
 	msg   []byte
 	ed    bool
 	edSig [64]byte
+	keyed bool
+	key   [64]byte
 }
+
+// clientKey is a client key kept on the host (WithClientKeysPerItem): P-256 X || Y, or an Ed25519 key in key[:32].
+type clientKey struct {
+	ed  bool
+	key [64]byte
+}
+
+// Option configures a Verifier at New.
+type Option func(*Verifier)
+
+// WithClientKeysPerItem keeps client keys on the host instead of registering them: SetClientKey and
+// SetClientEd25519Key only record the key, and each request carries its client's key to the engine
+// (sbv_mixed_verify_batch), which groups the keys that repeat inside a flush on the device. No table is built per
+// client key and no flush rebuilds a registry when a client appears, so this suits client populations that come and go
+// between reconfigurations. Consenter keys stay registered. Off by default.
+func WithClientKeysPerItem() Option { return func(v *Verifier) { v.clientKeysPerItem = true } }
 
 // Verifier implements api.Verifier.
 type Verifier struct {
@@ -55,13 +74,16 @@ type Verifier struct {
 	dirty      bool                // the ECDSA registry differs from the engine's
 	edDirty    bool                // the Ed25519 registry differs from the engine's
 
+	clientKeysPerItem bool                 // WithClientKeysPerItem
+	clientKeys        map[string]clientKey // client keys kept on the host (WithClientKeysPerItem)
+
 	pool sync.Pool // *pinned: one block of page-locked memory per in-flight batch
 
 	agg *aggregator
 }
 
 // New opens the engine on the given CUDA devices (1, 2, 4 or 8 of one box).
-func New(devices []int) (*Verifier, error) {
+func New(devices []int, opts ...Option) (*Verifier, error) {
 	ords := make([]C.int, len(devices))
 	for i, d := range devices {
 		ords[i] = C.int(d)
@@ -71,7 +93,10 @@ func New(devices []int) (*Verifier, error) {
 		return nil, fmt.Errorf("sbv_create failed: %d (there is no CPU fallback)", int(rc))
 	}
 	v := &Verifier{eng: eng, slots: map[[64]byte]uint32{}, consenters: map[uint64]uint32{}, clients: map[string]uint32{},
-		edSlots: map[[32]byte]uint32{}, edKeys: map[uint64]uint32{}, edClients: map[string]uint32{}}
+		edSlots: map[[32]byte]uint32{}, edKeys: map[uint64]uint32{}, edClients: map[string]uint32{}, clientKeys: map[string]clientKey{}}
+	for _, o := range opts {
+		o(v)
+	}
 	v.pool.New = func() interface{} { return &pinned{} }
 	v.agg = newAggregator(v.engineBatch, 200*time.Microsecond, 65536)
 	return v, nil
@@ -118,8 +143,12 @@ func (v *Verifier) SetConsenterKey(id uint64, xy [64]byte) {
 }
 func (v *Verifier) SetClientKey(c string, xy [64]byte) {
 	v.mu.Lock()
-	v.clients[c] = v.slotOf(xy)
-	delete(v.edClients, c)
+	if v.clientKeysPerItem {
+		v.clientKeys[c] = clientKey{key: xy}
+	} else {
+		v.clients[c] = v.slotOf(xy)
+		delete(v.edClients, c)
+	}
 	v.mu.Unlock()
 }
 func (v *Verifier) SetVerificationSequence(s uint64) { v.mu.Lock(); v.verSeq = s; v.mu.Unlock() }
@@ -135,28 +164,35 @@ func (v *Verifier) SetConsenterEd25519Key(id uint64, pub [32]byte) {
 
 // SetClientEd25519Key: client `c` signs its requests with crypto/ed25519; the signature field of its requests is the
 // 64-byte R || S over the signed bytes of the request. The key is registered: a key the registry has not seen yet makes
-// the next flush rebuild the Ed25519 registry (see ResetKeys for the cost).
+// the next flush rebuild the Ed25519 registry (see ResetKeys for the cost). With WithClientKeysPerItem the key is
+// only recorded and travels with the client's requests.
 func (v *Verifier) SetClientEd25519Key(c string, pub [32]byte) {
 	v.mu.Lock()
-	v.edClients[c] = v.edSlotOf(pub)
-	delete(v.clients, c)
+	if v.clientKeysPerItem {
+		k := clientKey{ed: true}
+		copy(k.key[:], pub[:])
+		v.clientKeys[c] = k
+	} else {
+		v.edClients[c] = v.edSlotOf(pub)
+		delete(v.clients, c)
+	}
 	v.mu.Unlock()
 }
 
 // ResetKeys drops every key, ECDSA and Ed25519, of consenters and clients. Keys change only with a reconfiguration, i.e. a new verification
 // sequence (dependencies.go:65-66): the application calls ResetKeys, re-registers the new configuration's keys
 // and bumps the sequence, so rotated keys do not pile up in HBM (264 KiB per P-256 key and 384 KiB per Ed25519 key,
-// per GPU). ECDSA client keys of high cardinality should not be registered at all: sbv_hash_verify_batch takes the
-// key with every item and groups the repeated ones on the device. Ed25519 client keys are always registered
-// (SetClientEd25519Key): each new key costs 384 KiB per GPU and makes the next flush rebuild every Ed25519 table
-// (about 8 ms per thousand keys), so a deployment whose Ed25519 clients come and go between reconfigurations should
-// verify their requests with sbv_ed25519_verify_batch instead.
+// per GPU). Registered Ed25519 client keys (SetClientEd25519Key) cost 384 KiB per GPU each, and each new one makes the
+// next flush rebuild every Ed25519 table (about 8 ms per thousand keys): a deployment whose clients, of either scheme,
+// come and go between reconfigurations should open the Verifier WithClientKeysPerItem, so that client keys travel with
+// the requests and repeated ones are grouped on the device instead.
 func (v *Verifier) ResetKeys() {
 	v.mu.Lock()
 	v.registry, v.slots = nil, map[[64]byte]uint32{}
 	v.consenters, v.clients = map[uint64]uint32{}, map[string]uint32{}
 	v.edRegistry, v.edSlots = nil, map[[32]byte]uint32{}
 	v.edKeys, v.edClients = map[uint64]uint32{}, map[string]uint32{}
+	v.clientKeys = map[string]clientKey{}
 	v.dirty, v.edDirty = true, true
 	v.mu.Unlock()
 }
@@ -222,24 +258,55 @@ func (b *pinned) reserve(n int) []byte {
 	return unsafe.Slice((*byte)(b.p), b.cap)[:n]
 }
 
-// engineBatch verifies an aggregated batch in one sbv_mixed_verify_registered call, whatever keys its items hold: the
-// engine splits the items by scheme on the GPU, hashes each message there (SHA-256 for ECDSA, SHA-512(R || A || M) for
-// Ed25519) and verifies it against the item's registered key; verdicts come back in the items' order. The batch is
-// marshalled once, straight into pinned memory (one block per in-flight batch, pooled):
-// rows (96n: P-256 r || s or Ed25519 R || S in bytes [0, 64)) | slot (4n) | off (8(n+1)) | scheme (n) | msgs.
+// engineBatch verifies an aggregated batch in at most two calls, whatever keys its items hold: the items with registered
+// keys in one sbv_mixed_verify_registered call, the items that carry their key (WithClientKeysPerItem) in one
+// sbv_mixed_verify_batch call. The engine splits each call's items by scheme on the GPU, hashes each message there
+// (SHA-256 for ECDSA, SHA-512(R || A || M) for Ed25519) and verifies it; verdicts are put back in the items' order.
 func (v *Verifier) engineBatch(items []item) []byte {
 	v.syncRegistry()
-	n := len(items)
-	ok := make([]byte, n)
-	if n == 0 {
-		return ok
-	}
-	total := 0
+	ok := make([]byte, len(items))
+	var reg, keyed []int
 	for i := range items {
+		if items[i].keyed {
+			keyed = append(keyed, i)
+		} else {
+			reg = append(reg, i)
+		}
+	}
+	for _, idx := range [][]int{reg, keyed} {
+		if len(idx) == 0 {
+			continue
+		}
+		if len(idx) == len(items) {
+			v.engineCall(items, idx, ok)
+			break
+		}
+		part := make([]byte, len(idx))
+		v.engineCall(items, idx, part)
+		for j, i := range idx {
+			ok[i] = part[j]
+		}
+	}
+	return ok
+}
+
+// engineCall verifies items[idx[0]], items[idx[1]], ... (all registered or all keyed) in one engine call, verdict j into
+// ok[j]. The items are marshalled once, straight into pinned memory (one block per in-flight call, pooled):
+// rows (96n: P-256 r || s or Ed25519 R || S in bytes [0, 64)) | keys (96n: P-256 X || Y or the Ed25519 key in bytes
+// [0, 64)) or slots (4n) | off (8(n+1)) | scheme (n) | msgs.
+func (v *Verifier) engineCall(items []item, idx []int, ok []byte) {
+	n := len(idx)
+	keyed := items[idx[0]].keyed
+	total := 0
+	for _, i := range idx {
 		total += len(items[i].msg)
 	}
-	oSlot := 96 * n
-	oOff := (oSlot + 4*n + 7) &^ 7
+	oKey := 96 * n
+	oOff := oKey + 4*n
+	if keyed {
+		oOff = oKey + 96*n
+	}
+	oOff = (oOff + 7) &^ 7
 	oScheme := oOff + 8*(n+1)
 	oMsgs := oScheme + n
 	pb := v.pool.Get().(*pinned)
@@ -247,29 +314,40 @@ func (v *Verifier) engineBatch(items []item) []byte {
 	buf := pb.reserve(oMsgs + total + 16)
 	pos := 0
 	binary.LittleEndian.PutUint64(buf[oOff:], 0)
-	for i := range items {
-		row := buf[96*i : 96*i+96]
-		if items[i].ed {
-			copy(row, items[i].edSig[:])
-			buf[oScheme+i] = byte(C.SBV_ED25519)
+	for j, i := range idx {
+		it := &items[i]
+		row := buf[96*j : 96*j+96]
+		if it.ed {
+			copy(row, it.edSig[:])
+			buf[oScheme+j] = byte(C.SBV_ED25519)
 		} else {
-			copy(row, items[i].r[:])
-			copy(row[32:], items[i].s[:])
-			buf[oScheme+i] = byte(C.SBV_P256)
+			copy(row, it.r[:])
+			copy(row[32:], it.s[:])
+			buf[oScheme+j] = byte(C.SBV_P256)
 		}
-		binary.LittleEndian.PutUint32(buf[oSlot+4*i:], items[i].slot)
-		copy(buf[oMsgs+pos:], items[i].msg)
-		pos += len(items[i].msg)
-		binary.LittleEndian.PutUint64(buf[oOff+8*(i+1):], uint64(pos))
+		if keyed {
+			copy(buf[oKey+96*j:oKey+96*j+96], it.key[:])
+		} else {
+			binary.LittleEndian.PutUint32(buf[oKey+4*j:], it.slot)
+		}
+		copy(buf[oMsgs+pos:], it.msg)
+		pos += len(it.msg)
+		binary.LittleEndian.PutUint64(buf[oOff+8*(j+1):], uint64(pos))
 	}
 	base := uintptr(pb.p)
-	rc := C.sbv_mixed_verify_registered(v.eng, C.size_t(n), (*C.uint8_t)(unsafe.Pointer(base+uintptr(oScheme))),
-		(*C.uint8_t)(unsafe.Pointer(base+uintptr(oMsgs))), (*C.uint64_t)(unsafe.Pointer(base+uintptr(oOff))),
-		(*C.uint32_t)(unsafe.Pointer(base+uintptr(oSlot))), (*C.uint8_t)(unsafe.Pointer(base)), (*C.uint8_t)(unsafe.Pointer(&ok[0])))
-	if rc != 0 {
+	at := func(o int) *C.uint8_t { return (*C.uint8_t)(unsafe.Pointer(base + uintptr(o))) }
+	off := (*C.uint64_t)(unsafe.Pointer(base + uintptr(oOff)))
+	out := (*C.uint8_t)(unsafe.Pointer(&ok[0]))
+	if keyed {
+		if rc := C.sbv_mixed_verify_batch(v.eng, C.size_t(n), at(oScheme), at(oMsgs), off, at(0), at(oKey), out); rc != 0 {
+			v.fault("sbv_mixed_verify_batch", rc)
+		}
+		return
+	}
+	if rc := C.sbv_mixed_verify_registered(v.eng, C.size_t(n), at(oScheme), at(oMsgs), off, (*C.uint32_t)(unsafe.Pointer(base+uintptr(oKey))), at(0),
+		out); rc != 0 {
 		v.fault("sbv_mixed_verify_registered", rc)
 	}
-	return ok
 }
 
 // parseDER: strict SEQUENCE{INTEGER r, INTEGER s} as crypto/ecdsa.VerifyASN1 (minimal, non-negative,
@@ -434,8 +512,24 @@ func (v *Verifier) requestItem(val []byte) (item, types.RequestInfo, error) {
 	v.mu.RLock()
 	slot, known := v.clients[client]
 	edSlot, isEd := v.edClients[client]
+	ck, keyed := v.clientKeys[client]
 	v.mu.RUnlock()
 	info := types.RequestInfo{ClientID: client, ID: id}
+	if keyed {
+		it := item{keyed: true, ed: ck.ed, key: ck.key, msg: signed}
+		if ck.ed {
+			if len(sig) != 64 {
+				return item{}, types.RequestInfo{}, errors.New("malformed request signature")
+			}
+			copy(it.edSig[:], sig)
+			return it, info, nil
+		}
+		var ok bool
+		if it.r, it.s, ok = parseDER(sig); !ok {
+			return item{}, types.RequestInfo{}, errors.New("malformed request signature")
+		}
+		return it, info, nil
+	}
 	if isEd {
 		if len(sig) != 64 { // crypto/ed25519.Verify rejects any other length
 			return item{}, types.RequestInfo{}, errors.New("malformed request signature")

@@ -653,3 +653,52 @@ extern "C" int hs_mixed_verify_registered(size_t n, const uint8_t *tag, const ui
     hs_mixed_scatter(n, m[0], m[1], idx.data(), okf.data(), ok);
     return 0;
 }
+
+// ---- mixed shards with keys per item (k_mix_split<true>, sbv_mixed_verify_batch) ----
+// hs_mixed_split for a keys-per-item shard: key96 (one 96-byte row per item) instead of slots; besides the arrays of
+// hs_mixed_split, qx0 / qy0 (32 B per item), qx1 / qy1 (48 B) and pub2 (32 B) receive the compacted keys
+extern "C" int hs_mixed_split_keys(size_t n, const uint8_t *tag, const uint8_t *key96, const uint8_t *sig96, const uint64_t *off_in, uint32_t m0,
+                                   uint32_t m1, uint32_t *idx, uint8_t *r0, uint8_t *s0, uint8_t *r1, uint8_t *s1, uint8_t *sig2, uint8_t *qx0,
+                                   uint8_t *qy0, uint8_t *qx1, uint8_t *qy1, uint8_t *pub2, uint64_t *off_out) {
+    const MixPlan p = hs_plan(n, m0, m1, idx, nullptr, r0, s0, r1, s1, sig2, off_out, nullptr, nullptr);
+    const MixKeys k{{qx0, qx1}, {qy0, qy1}, pub2};
+    const uint32_t nn = (uint32_t)n, ntiles = (uint32_t)((n + MIX_TILE - 1) / MIX_TILE);
+    std::vector<uint32_t> tc((size_t)MIX_FAMILIES * ntiles + 1);
+    std::vector<uint64_t> tb((size_t)MIX_FAMILIES * ntiles + 1);
+    run_grid((ntiles + 255) / 256, 256, [&] { k_mix_count(nn, tag, off_in, ntiles, tc.data(), tb.data()); });
+    run_grid(1, 1, [&] { k_mix_scan(ntiles, tc.data(), tb.data(), p); });
+    run_grid((ntiles + 255) / 256, 256, [&] { k_mix_split<true>(nn, tag, nullptr, sig96, off_in, ntiles, tc.data(), tb.data(), p, key96, k); });
+    return 0;
+}
+// The pipeline of sbv_mixed_verify_batch on one device: the split with keys, compaction, then per ECDSA family hs_sha256
+// and hs_verify_grouped over the family's compacted keys, hs_ed25519_verify_grouped for the Ed25519 family (T, max_keys:
+// the grouping settings of both), and the scatter.  Tags must be <= 2.
+extern "C" int hs_mixed_verify_batch(size_t n, const uint8_t *tag, const uint8_t *msgs, const uint64_t *off, const uint8_t *sig96, const uint8_t *key96,
+                                     uint32_t T, uint32_t max_keys, uint8_t *ok) {
+    uint32_t m[3] = {0, 0, 0};
+    for (size_t i = 0; i < n; i++) {
+        if (tag[i] > 2) return -1;
+        m[tag[i]]++;
+    }
+    const uint64_t base = off[0], bytes = off[n] - base;
+    std::vector<uint8_t> src(bytes + 16, 0);
+    if (bytes) memcpy(src.data(), msgs + base, bytes);
+    std::vector<uint32_t> idx(n + 1);
+    std::vector<uint8_t> r0(32 * m[0] + 1), s0(32 * m[0] + 1), r1(48 * m[1] + 1), s1(48 * m[1] + 1), sig2(64 * m[2] + 1), qx0(32 * m[0] + 1),
+        qy0(32 * m[0] + 1), qx1(48 * m[1] + 1), qy1(48 * m[1] + 1), pub2(32 * m[2] + 1), blob(bytes + 128, 0), okf(n + 1, 0);
+    std::vector<uint64_t> fo(n + 3);
+    hs_mixed_split_keys(n, tag, key96, sig96, off, m[0], m[1], idx.data(), r0.data(), s0.data(), r1.data(), s1.data(), sig2.data(), qx0.data(), qy0.data(),
+                        qx1.data(), qy1.data(), pub2.data(), fo.data());
+    hs_mixed_compact(n, m[0], m[1], src.data(), off, base, idx.data(), fo.data(), blob.data());
+    const uint32_t at[3] = {0, m[0], m[0] + m[1]};
+    for (int f = 0; f < 2; f++) {
+        if (!m[f]) continue;
+        std::vector<uint8_t> dig(32 * m[f]);
+        hs_sha256(m[f], blob.data(), fo.data() + at[f] + f, 0, nullptr, dig.data());
+        hs_verify_grouped(f, m[f], f ? r1.data() : r0.data(), f ? s1.data() : s0.data(), f ? qx1.data() : qx0.data(), f ? qy1.data() : qy0.data(),
+                          dig.data(), 32, T, max_keys, okf.data() + at[f], nullptr);
+    }
+    if (m[2]) hs_ed25519_verify_grouped(m[2], blob.data(), fo.data() + at[2] + 2, sig2.data(), pub2.data(), T, max_keys, okf.data() + at[2], nullptr);
+    hs_mixed_scatter(n, m[0], m[1], idx.data(), okf.data(), ok);
+    return 0;
+}

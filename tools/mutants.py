@@ -42,6 +42,7 @@ ECDSA = ["tests/test_hostsim.py", "tests/test_hostsim_key_tables.py", "tests/tes
 ED = ["tests/test_hostsim_ed25519_arith.py", "tests/test_hostsim_ed25519.py", "tests/test_hostsim_ed25519_edges.py",
       "tests/test_hostsim_ed25519_registered.py", "tests/test_hostsim_ed25519_grouped.py"]
 MIXED = ["tests/test_hostsim_mixed.py"]
+MIXED_KEYS = ["tests/test_hostsim_mixed_keys.py"]  # keys per item (k_mix_split<true>)
 SHARDS = ["tests/test_hostsim_shards.py"]
 WIDE = ["tests/test_hostsim_wide.py"]  # bit lengths, offsets and byte sums past 32 bits
 
@@ -286,6 +287,12 @@ CATALOGUE = [
     M("mix_scan_close_offsets", "mixed.cuh", "if (tid == 0) p.f[k].off[sc[k][T - 1]] = start[k] + sb[k][T - 1];", "(void)0;", MIXED),
     M("mix_split_rank_family", "mixed.cuh", "const uint32_t j = f == 0 ? rank[0] : f == 1 ? rank[1] : rank[2];", "const uint32_t j = f == 0 ? rank[0] : rank[1];", MIXED),
     M("mix_split_p384_width", "mixed.cuh", "mix_copy16(F.s + (size_t)j * 48, row + 48, 3);", "mix_copy16(F.s + (size_t)j * 48, row + 32, 3);", MIXED),
+    M("mix_split_p384_qy_offset", "mixed.cuh", "mix_copy16(k.qy[1] + (size_t)j * 48, key96 + (size_t)i * 96 + 48, 3);",
+      "mix_copy16(k.qy[1] + (size_t)j * 48, key96 + (size_t)i * 96 + 32, 3);", MIXED_KEYS),
+    M("mix_split_p384_qy_width", "mixed.cuh", "mix_copy16(k.qy[1] + (size_t)j * 48, key96 + (size_t)i * 96 + 48, 3);",
+      "mix_copy16(k.qy[1] + (size_t)j * 48, key96 + (size_t)i * 96 + 48, 2);", MIXED_KEYS),
+    M("mix_split_ed_pub_width", "mixed.cuh", "mix_copy16(k.pub + (size_t)j * 32, key96 + (size_t)i * 96, 2);",
+      "mix_copy16(k.pub + (size_t)j * 32, key96 + (size_t)i * 96, 1);", MIXED_KEYS),
     M("mix_compact_edge_bytes", "mixed.cuh", "const uint64_t a = lo > d ? lo : d, b = lo + 16 < d + len ? lo + 16 : d + len;",
       "const uint64_t a = lo > d ? lo : d, b = lo + 16 < d + len ? lo + 15 : d + len;", MIXED),
     M("mix_compact_family_bounds", "mixed.cuh", "const uint32_t f = g < m0 ? 0 : g < m0 + m1 ? 1 : 2, j = g - (f == 0 ? 0 : f == 1 ? m0 : m0 + m1);\n    const MixFamily F = mix_family(p, f);\n    const uint32_t i = F.idx[j];",
