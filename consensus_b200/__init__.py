@@ -26,7 +26,7 @@ SYMBOLS = [
     "sbv_comm_unique_id", "sbv_comm_init_rank", "sbv_comm_ranks", "sbv_gather_verdicts_device", "sbv_gather_words_device",
     "sbv_verify_batch_ranked", "sbv_host_alloc", "sbv_host_free", "sbv_ed25519_verify_batch",
     "sbv_ed25519_set_keys", "sbv_ed25519_verify_registered", "sbv_ed25519_verify_quorum", "sbv_mixed_verify_registered",
-    "sbv_mixed_verify_quorum", "sbv_mixed_verify_batch",
+    "sbv_mixed_verify_quorum", "sbv_mixed_verify_batch", "sbv_sha384_batch", "sbv_hash384_verify_batch", "sbv_hash384_verify_registered",
 ]
 
 
@@ -173,17 +173,20 @@ class Engine:
                                                     _p8(r), _p8(s), _p8(digest), C.c_uint8(dlen), _p8(ok)), "sbv_verify_registered")
         return ok
 
-    def hash_verify_registered(self, curve, msgs, off, key_slot, r, s) -> np.ndarray:
+    def hash_verify_registered(self, curve, msgs, off, key_slot, r, s, _fn="sbv_hash_verify_registered") -> np.ndarray:
         msgs = _u8(msgs if len(msgs) else np.zeros(1, np.uint8))
         off = np.ascontiguousarray(off, dtype=np.uint64)
         key_slot = np.ascontiguousarray(key_slot, dtype=np.uint32)
         r, s = _u8(r), _u8(s)
         n = off.size - 1
         ok = np.zeros(n, np.uint8)
-        self._check(self._lib.sbv_hash_verify_registered(self._h, C.c_uint8(curve), C.c_size_t(n), _p8(msgs), off.ctypes.data_as(C.POINTER(C.c_uint64)),
-                                                         key_slot.ctypes.data_as(C.POINTER(C.c_uint32)), _p8(r), _p8(s), _p8(ok)),
-                    "sbv_hash_verify_registered")
+        self._check(getattr(self._lib, _fn)(self._h, C.c_uint8(curve), C.c_size_t(n), _p8(msgs), off.ctypes.data_as(C.POINTER(C.c_uint64)),
+                                            key_slot.ctypes.data_as(C.POINTER(C.c_uint32)), _p8(r), _p8(s), _p8(ok)), _fn)
         return ok
+
+    def hash384_verify_registered(self, curve, msgs, off, key_slot, r, s) -> np.ndarray:
+        """hash_verify_registered with e = the leftmost field bytes of SHA-384(M) (Go's ECDSAWithSHA384, ES384)."""
+        return self.hash_verify_registered(curve, msgs, off, key_slot, r, s, _fn="sbv_hash384_verify_registered")
 
     def verify_registered_device(self, curve, n, d_slot, d_r, d_s, d_digest, dlen, d_ok, stream=0, device_index=0):
         vp = C.c_void_p
@@ -203,26 +206,39 @@ class Engine:
                                                    C.c_uint8(dlen), _p8(ok)), "sbv_verify_batch_der")
         return ok
 
-    def sha256_batch(self, msgs, off) -> np.ndarray:
+    def sha256_batch(self, msgs, off, _fn="sbv_sha256_batch", _width=32) -> np.ndarray:
         msgs = _u8(msgs if len(msgs) else np.zeros(1, np.uint8))
         off = np.ascontiguousarray(off, dtype=np.uint64)
         n = off.size - 1
-        out = np.zeros((n, 32), np.uint8)
-        self._check(self._lib.sbv_sha256_batch(self._h, C.c_size_t(n), _p8(msgs), off.ctypes.data_as(C.POINTER(C.c_uint64)),
-                                               _p8(out)), "sbv_sha256_batch")
+        out = np.zeros((n, _width), np.uint8)
+        self._check(getattr(self._lib, _fn)(self._h, C.c_size_t(n), _p8(msgs), off.ctypes.data_as(C.POINTER(C.c_uint64)), _p8(out)), _fn)
         return out
 
-    def hash_verify_batch(self, curve, msgs, off, r, s, qx, qy, want_digest=False):
+    def sha384_batch(self, msgs, off) -> np.ndarray:
+        """SHA-384 of each message (msgs concatenated with off[n+1] byte offsets): n x 48 bytes."""
+        return self.sha256_batch(msgs, off, _fn="sbv_sha384_batch", _width=48)
+
+    def hash_verify_batch(self, curve, msgs, off, r, s, qx, qy, want_digest=False, _fn="sbv_hash_verify_batch", _width=32):
         msgs = _u8(msgs if len(msgs) else np.zeros(1, np.uint8))
         off = np.ascontiguousarray(off, dtype=np.uint64)
         r, s, qx, qy = map(_u8, (r, s, qx, qy))
         n = off.size - 1
         ok = np.zeros(n, np.uint8)
-        dig = np.zeros((n, 32), np.uint8) if want_digest else None
-        self._check(self._lib.sbv_hash_verify_batch(self._h, C.c_uint8(curve), C.c_size_t(n), _p8(msgs),
-                                                    off.ctypes.data_as(C.POINTER(C.c_uint64)), _p8(r), _p8(s), _p8(qx), _p8(qy),
-                                                    _p8(dig) if want_digest else None, _p8(ok)), "sbv_hash_verify_batch")
+        dig = np.zeros((n, _width), np.uint8) if want_digest else None
+        self._check(getattr(self._lib, _fn)(self._h, C.c_uint8(curve), C.c_size_t(n), _p8(msgs), off.ctypes.data_as(C.POINTER(C.c_uint64)),
+                                            _p8(r), _p8(s), _p8(qx), _p8(qy), _p8(dig) if want_digest else None, _p8(ok)), _fn)
         return (ok, dig) if want_digest else ok
+
+    def hash384_verify_batch(self, curve, msgs, off, r, s, qx, qy, want_digest=False):
+        """hash_verify_batch with e = the leftmost field bytes of SHA-384(M) (Go's ECDSAWithSHA384, ES384); the digests, if
+        asked for, are n x 48 bytes."""
+        return self.hash_verify_batch(curve, msgs, off, r, s, qx, qy, want_digest, _fn="sbv_hash384_verify_batch", _width=48)
+
+    def hash384_verify_batch_ptr(self, curve, n, msgs, off, r, s, qx, qy, digest_out, ok):
+        """Raw host pointers (ints; digest_out may be 0) — used with pinned buffers."""
+        vp = C.c_void_p
+        self._check(self._lib.sbv_hash384_verify_batch(self._h, C.c_uint8(curve), C.c_size_t(n), vp(msgs), vp(off), vp(r), vp(s), vp(qx), vp(qy),
+                                                       vp(digest_out or None), vp(ok)), "sbv_hash384_verify_batch")
 
     def ed25519_verify_batch(self, msgs, off, sig, pub, out=None) -> np.ndarray:
         """Ed25519 (Go crypto/ed25519.Verify): msgs concatenated with off[n+1] byte offsets, sig = n x 64 bytes (R || S),

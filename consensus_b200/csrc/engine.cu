@@ -21,6 +21,7 @@
 
 #include "engine.h"
 #include "sha256.cuh"
+#include "sha384.cuh"
 #include "quorum.cuh"
 #include "shards.h"
 
@@ -198,6 +199,16 @@ int sbv_launch_sha256(sbv_engine *e, size_t n, const uint8_t *d_msgs, const uint
     CU(e, cudaGetLastError());
     return 0;
 }
+int sbv_launch_sha384(sbv_engine *e, size_t n, const uint8_t *d_msgs, const uint64_t *d_off, uint64_t base, uint8_t *d_digest, uint32_t *d_perm,
+                      cudaStream_t st) {
+    const uint32_t *perm = nullptr;
+    int rc = sbv_launch_length_sort(e, n, d_off, d_perm, st, &perm);
+    if (rc) return rc;
+    k_sha384<<<(uint32_t)((n + 127) / 128), 128, 0, st>>>((uint32_t)n, d_msgs, d_off, base, d_digest, perm);
+    e->launches += 1;
+    CU(e, cudaGetLastError());
+    return 0;
+}
 // H2D of a caller buffer on the lane's stream (or on st): direct when pinned, else through the lane's pinned staging area at offset
 // `stage_off` (the caller sized it and does not reuse it until the stream has drained).
 int sbv_lane_h2d(sbv_engine *e, Dev::Lane &ln, void *dst, const void *src, size_t bytes, size_t &stage_off, cudaStream_t st) {
@@ -322,13 +333,23 @@ int gather_unpack(sbv_engine *e, int lane, const Shards &s, const std::vector<ui
     return SBV_OK;
 }
 
+// The hash that turns the messages of an ECDSA call into its digests (e = their leftmost field bytes).
+enum class MsgHash : uint8_t { sha256, sha384 };
+uint32_t hash_bytes(MsgHash h) { return h == MsgHash::sha384 ? 48u : 32u; }
+int launch_hash(sbv_engine *e, MsgHash h, size_t n, const uint8_t *d_msgs, const uint64_t *d_off, uint64_t base, uint8_t *d_digest, uint32_t *d_perm,
+                cudaStream_t st) {
+    return h == MsgHash::sha384 ? sbv_launch_sha384(e, n, d_msgs, d_off, base, d_digest, d_perm, st)
+                                : sbv_launch_sha256(e, n, d_msgs, d_off, base, d_digest, d_perm, st);
+}
+
 // One shard of a keys-per-item host-buffer call on device d's lane: what to verify and where it comes from.
 struct BatchSrc {
     const uint8_t *r, *s, *qx, *qy;
-    const uint8_t *digest;      // fixed-width digests, or nullptr: the digests are SHA-256 of the messages below
+    const uint8_t *digest;      // fixed-width digests, or nullptr: the digests are `hash` of the messages below
     uint8_t digest_len;
     const uint8_t *msgs;
     const uint64_t *msg_off;
+    MsgHash hash = MsgHash::sha256;
 };
 
 // Stages items [lo, lo+cnt) and enqueues hashing (if asked for) and the verify pipeline; verdicts land in ln.d_ok (and the
@@ -341,7 +362,7 @@ int stage_and_verify(sbv_engine *e, Dev &d, int lane, uint8_t curve, size_t lo, 
                      size_t *so_out = nullptr) {
     const size_t L = fbytes(curve);
     const bool hashing = b.digest == nullptr;
-    const uint32_t dlen = hashing ? 32u : b.digest_len;
+    const uint32_t dlen = hashing ? hash_bytes(b.hash) : b.digest_len;
     Dev::Lane &ln = d.lanes[lane];
     CU(e, cudaSetDevice(d.ordinal));
     const uint64_t base = hashing ? b.msg_off[lo] : 0, bytes = hashing ? b.msg_off[lo + cnt] - base : 0;
@@ -391,7 +412,7 @@ int stage_and_verify(sbv_engine *e, Dev &d, int lane, uint8_t curve, size_t lo, 
             if (ce == cudaSuccess) ce = cudaStreamWaitEvent(ln.stream, ln.ev_chunk[c], 0);
             if (ce != cudaSuccess) return abandon(sbv_fail(e, SBV_ERR_CUDA, "chunk event: %s", cudaGetErrorString(ce)));
         }
-        if (hashing && cn && (rc = sbv_launch_sha256(e, cn, ln.d_msgs, ln.d_off + clo, base, ln.d_dig + clo * 32, ln.d_perm + clo, ln.stream)))
+        if (hashing && cn && (rc = launch_hash(e, b.hash, cn, ln.d_msgs, ln.d_off + clo, base, ln.d_dig + clo * dlen, ln.d_perm + clo, ln.stream)))
             return abandon(rc);
         std::lock_guard<std::mutex> lk(e->mu);
         rc = sbv_launch_verify_chunk(e, d, vl, c, clo, cn, c == chunks - 1, ln.d_r, ln.d_s, ln.d_dig, dlen, ln.d_ok, ln.stream);

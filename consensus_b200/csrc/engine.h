@@ -265,6 +265,9 @@ int sbv_lane_stream2(sbv_engine *e, Dev::Lane &ln);  // creates the lane's secon
 // d_perm: n + 3072 words of scratch (may be null: no length sort)
 int sbv_launch_sha256(sbv_engine *e, size_t n, const uint8_t *d_msgs, const uint64_t *d_off, uint64_t base, uint8_t *d_digest, uint32_t *d_perm,
                       cudaStream_t st);
+// the same with SHA-384: 48 bytes per message into d_digest
+int sbv_launch_sha384(sbv_engine *e, size_t n, const uint8_t *d_msgs, const uint64_t *d_off, uint64_t base, uint8_t *d_digest, uint32_t *d_perm,
+                      cudaStream_t st);
 // the block-count sort of the SHA-256 launch on its own: *perm = the permutation in d_perm, or nullptr below 2048 items
 int sbv_launch_length_sort(sbv_engine *e, size_t n, const uint64_t *d_off, uint32_t *d_perm, cudaStream_t st, const uint32_t **perm);
 int sbv_lane_h2d(sbv_engine *e, Dev::Lane &ln, void *dst, const void *src, size_t bytes, size_t &stage_off, cudaStream_t st = nullptr);

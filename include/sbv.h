@@ -102,6 +102,25 @@ int sbv_hash_verify_batch(sbv_engine *e, uint8_t curve, size_t n, const uint8_t 
                           const uint8_t *r, const uint8_t *s, const uint8_t *qx, const uint8_t *qy,
                           uint8_t *digest_out, uint8_t *ok);
 
+/* ---- SHA-384 for ECDSA: the digest Go's crypto/x509 (ECDSAWithSHA384), JOSE ES384 and TLS ecdsa_secp384r1_sha384 pair
+ * with P-384.  The three calls below are the SHA-256 forms with SHA-384 in place of SHA-256; msgs / msg_off as in
+ * sbv_sha256_batch (msgs may be NULL when every message is empty).  The same argument checks run before anything is
+ * written: SBV_ERR_ARG for a curve other than SBV_P256 / SBV_P384, null buffers, n >= 2^31 and decreasing offsets.
+ * Multi-device engines shard them as the SHA-256 forms.  Out of scope, SHA-256 or digests only: the sbv_mixed_* calls,
+ * sbv_verify_quorum, the DER front end and the _ranked and _device forms. */
+/* SHA-384 over a ragged batch (msgs / msg_off as in sbv_sha256_batch); digest_out = 48n bytes. */
+int sbv_sha384_batch(sbv_engine *e, size_t n, const uint8_t *msgs, const uint64_t *msg_off, uint8_t *digest_out);
+/* sbv_hash_verify_batch with SHA-384: e = leftmost min(48, field bytes) of SHA-384(M) (the whole digest for P-384,
+ * its leftmost 32 bytes for P-256, as crypto/ecdsa truncates).  The accept set is exactly that of sbv_verify_batch
+ * with digest = SHA-384(M) and digest_len = 48, keys that repeat grouped as there.  digest_out (48n) may be NULL. */
+int sbv_hash384_verify_batch(sbv_engine *e, uint8_t curve, size_t n, const uint8_t *msgs, const uint64_t *msg_off,
+                             const uint8_t *r, const uint8_t *s, const uint8_t *qx, const uint8_t *qy,
+                             uint8_t *digest_out, uint8_t *ok);
+/* sbv_hash_verify_registered with SHA-384 (same e as above): the accept set is exactly that of sbv_verify_registered with
+ * digest = SHA-384(M) and digest_len = 48. */
+int sbv_hash384_verify_registered(sbv_engine *e, uint8_t curve, size_t n, const uint8_t *msgs, const uint64_t *msg_off,
+                                  const uint32_t *key_slot, const uint8_t *r, const uint8_t *s, uint8_t *ok);
+
 /* Mixed-curve batch: curve_tag[i] in {SBV_P256, SBV_P384}; every field is stored in a 48-byte
  * slot (P-256 values right-aligned, i.e. 16 leading zero bytes); digest is 32 bytes per item. */
 int sbv_verify_mixed(sbv_engine *e, size_t n, const uint8_t *curve_tag, const uint8_t *r48, const uint8_t *s48,

@@ -17,6 +17,7 @@ namespace sbv { uint32_t tab[1 << 18]; }
 #include "../../consensus_b200/csrc/debug_ops.cuh"
 #include "../../consensus_b200/csrc/keygroup.cuh"
 #include "../../consensus_b200/csrc/sha256.cuh"
+#include "../../consensus_b200/csrc/sha384.cuh"
 #include "../../consensus_b200/csrc/quorum.cuh"
 #include "../../consensus_b200/csrc/ed25519_debug.cuh"
 #include "../../consensus_b200/csrc/sha512.cuh"
@@ -156,6 +157,11 @@ extern "C" int hs_kg_hash(int curve, size_t n, const uint8_t *qx, const uint8_t 
 // k_sha256 over a ragged batch, one message per simulated thread (perm: optional processing order, as the counting sort gives it)
 extern "C" int hs_sha256(size_t n, const uint8_t *msgs, const uint64_t *off, uint64_t base, const uint32_t *perm, uint8_t *digest_out) {
     run_grid((unsigned)((n + 127) / 128), 128, [&] { k_sha256((uint32_t)n, msgs, off, base, digest_out, perm); });
+    return 0;
+}
+// k_sha384 over a ragged batch, as hs_sha256 (digest_out: 48 bytes per message)
+extern "C" int hs_sha384(size_t n, const uint8_t *msgs, const uint64_t *off, uint64_t base, const uint32_t *perm, uint8_t *digest_out) {
+    run_grid((unsigned)((n + 127) / 128), 128, [&] { k_sha384((uint32_t)n, msgs, off, base, digest_out, perm); });
     return 0;
 }
 

@@ -45,6 +45,7 @@ MIXED = ["tests/test_hostsim_mixed.py"]
 MIXED_KEYS = ["tests/test_hostsim_mixed_keys.py"]  # keys per item (k_mix_split<true>)
 SHARDS = ["tests/test_hostsim_shards.py"]
 WIDE = ["tests/test_hostsim_wide.py"]  # bit lengths, offsets and byte sums past 32 bits
+SHA384 = ["tests/test_hostsim_sha384.py"]
 
 
 def M(id, file, find, repl, tests, equivalent=None, proof=None):
@@ -210,13 +211,22 @@ CATALOGUE = [
     M("sha256_length_high_word", "sha256.cuh", "w[14] = (uint32_t)(bits >> 32);", "w[14] = 0u;", WIDE),
     M("sha256_bits_32", "sha256.cuh", "const uint64_t bits = len * 8;", "const uint64_t bits = (uint32_t)len * 8u;", WIDE),
     M("sha256_offset_32", "sha256.cuh", "const uint64_t o = off[idx] - base;", "const uint64_t o = (uint32_t)(off[idx] - base);", WIDE),
+    # ---------------------------------------------------------------- sha512_core.cuh (SHA-512 and SHA-384)
+    M("sha512_pad_rem", "sha512_core.cuh", "if (rem < 4) v = (v & (0xffffffffu << (8 * (4 - rem)))) | (0x80u << (8 * (3 - rem)));",
+      "if (rem < 4) v = (v & (0xffffffffu << (8 * (4 - rem))));", SHA384 + ED),
+    M("sha512_pad_word", "sha512_core.cuh", "v = 0x80000000u;", "v = 0u;", SHA384 + ED),
+    M("sha512_aligned_tail_word", "sha512_core.cuh", "const uint32_t next = (sh || j < 15) ? __ldg(p + j + 1) : 0u;",
+      "const uint32_t next = (j < 15) ? __ldg(p + j + 1) : 0u;", SHA384 + ED),
+    # ---------------------------------------------------------------- sha384.cuh
+    M("sha384_nblocks", "sha384.cuh", "const uint64_t nblocks = (len + 17 + 127) / 128;", "const uint64_t nblocks = (len + 16 + 127) / 128;", SHA384),
+    M("sha384_second_half_offset", "sha384.cuh", "sha512_msg16(w32 + 16, blk * 128 + 64, len, words, sel, sh);",
+      "sha512_msg16(w32 + 16, blk * 128 + 60, len, words, sel, sh);", SHA384),
+    M("sha384_length_bytes", "sha384.cuh", "w[15] = len << 3;", "w[15] = len;", SHA384),
+    M("sha384_bits_32", "sha384.cuh", "w[15] = len << 3;", "w[15] = (uint32_t)(len << 3);", SHA384),
+    M("sha384_iv", "sha384.cuh", "0x47b5481dbefa4fa4ull", "0x5be0cd19137e2179ull", SHA384),
     # ---------------------------------------------------------------- sha512.cuh
-    M("sha512_pad_rem", "sha512.cuh", "if (rem < 4) v = (v & (0xffffffffu << (8 * (4 - rem)))) | (0x80u << (8 * (3 - rem)));",
-      "if (rem < 4) v = (v & (0xffffffffu << (8 * (4 - rem))));", ED),
-    M("sha512_pad_word", "sha512.cuh", "v = 0x80000000u;", "v = 0u;", ED),
     M("sha512_nblocks", "sha512.cuh", "const uint64_t nblocks = (total + 17 + 127) / 128;", "const uint64_t nblocks = (total + 16 + 127) / 128;", ED),
     M("sha512_length_bytes", "sha512.cuh", "if (blk == nblocks - 1) w[15] = total * 8;", "if (blk == nblocks - 1) w[15] = total;", ED),
-    M("sha512_aligned_tail_word", "sha512.cuh", "const uint32_t next = (sh || j < 15) ? __ldg(p + j + 1) : 0u;", "const uint32_t next = (j < 15) ? __ldg(p + j + 1) : 0u;", ED),
     M("sha512_first_block_msg_offset", "sha512.cuh", "sha512_msg16(w32, blk * 128 - 64, len, words, sel, sh);", "sha512_msg16(w32, blk * 128 - 60, len, words, sel, sh);", ED),
     M("sha512_offset_32", "sha512.cuh", "const uint64_t o = off[idx] - base;", "const uint64_t o = (uint32_t)(off[idx] - base);", WIDE),
     M("sha512_total_32", "sha512.cuh", "const uint64_t total = 64 + len;  // bytes hashed", "const uint32_t total = 64 + len;  // bytes hashed", WIDE),
