@@ -27,6 +27,7 @@ SYMBOLS = [
     "sbv_verify_batch_ranked", "sbv_host_alloc", "sbv_host_free", "sbv_ed25519_verify_batch",
     "sbv_ed25519_set_keys", "sbv_ed25519_verify_registered", "sbv_ed25519_verify_quorum", "sbv_mixed_verify_registered",
     "sbv_mixed_verify_quorum", "sbv_mixed_verify_batch", "sbv_sha384_batch", "sbv_hash384_verify_batch", "sbv_hash384_verify_registered",
+    "sbv_key_cache_reserve", "sbv_key_cache_stats",
 ]
 
 
@@ -123,6 +124,18 @@ class Engine:
         p, v, k = C.c_double(), C.c_double(), C.c_uint64()
         self._check(self._lib.sbv_profile_read(self._h, C.byref(p), C.byref(v), C.byref(k)), "sbv_profile_read")
         return p.value, v.value, k.value
+
+    def key_cache_reserve(self, p256=0, p384=0, ed25519=0):
+        """Reserves, on every device, room for the tables of up to p256 / p384 / ed25519 keys that keys-per-item launches
+        group, and empties any earlier cache; (0, 0, 0) frees it (sbv_key_cache_reserve)."""
+        self._check(self._lib.sbv_key_cache_reserve(self._h, C.c_size_t(p256), C.c_size_t(p384), C.c_size_t(ed25519)),
+                    "sbv_key_cache_reserve")
+
+    def key_cache_stats(self, scheme) -> dict:
+        """{capacity, resident, hits, misses} of one scheme's cache, summed over devices (sbv_key_cache_stats)."""
+        out = (C.c_uint64 * 4)()
+        self._check(self._lib.sbv_key_cache_stats(self._h, C.c_uint8(scheme), out), "sbv_key_cache_stats")
+        return dict(zip(("capacity", "resident", "hits", "misses"), (int(v) for v in out)))
 
     # ---- host-buffer API (numpy arrays, or anything exposing a host pointer via .ctypes) ----
     def verify_batch(self, curve, r, s, qx, qy, digest, out=None) -> np.ndarray:

@@ -1,3 +1,4 @@
+#include <cstring>
 #include <vector>
 
 #include "engine.h"
@@ -400,4 +401,30 @@ extern "C" int sbv_debug_ed25519_verify_registered_k(sbv_engine *e, size_t n, co
     CU(e, cudaMemcpyAsync(ok, dok, n, cudaMemcpyDeviceToHost, d.stream));
     CU(e, cudaStreamSynchronize(d.stream));
     return SBV_OK;
+}
+
+// The cached table of one key on device `device_index` (sbv_key_cache_reserve): key = the exact key bytes of scheme s
+// (qx || qy: 64 / 96 bytes; the 32-byte Ed25519 encoding).  Returns 1 with the table in out (the words of the scheme's
+// per-launch table, as sbv_debug_grouped_key_table / sbv_debug_ed25519_comb_tab read it) when a READY slot holds the key,
+// 0 when none does or no cache is reserved.  Drains the device first.
+extern "C" int sbv_debug_key_cache_entry(sbv_engine *e, int device_index, uint8_t scheme, const uint8_t *key, uint32_t *out) {
+    if (!e || scheme > SBV_ED25519 || !key || !out || device_index < 0 || device_index >= (int)e->devs.size()) return SBV_ERR_ARG;
+    std::lock_guard<std::mutex> lk(e->mu);
+    Dev &d = e->devs[device_index];
+    const Dev::KeyCache &k = d.kc[scheme];
+    if (!k.mem) return 0;
+    const size_t kw = scheme == SBV_P256 ? 16 : scheme == SBV_P384 ? 24 : 8, slots = (size_t)k.map.smask + 1;
+    CU(e, cudaSetDevice(d.ordinal));
+    CU(e, cudaDeviceSynchronize());
+    std::vector<uint32_t> state(slots), keys(slots * kw);
+    CU(e, cudaMemcpy(state.data(), k.map.state, slots * 4, cudaMemcpyDeviceToHost));
+    CU(e, cudaMemcpy(keys.data(), k.map.keys, slots * kw * 4, cudaMemcpyDeviceToHost));
+    for (size_t s = 0; s < slots; s++) {
+        if ((state[s] & 3) != 2 || memcmp(&keys[s * kw], key, kw * 4) != 0) continue;  // low bits 2: KC_READY (key_cache.cuh)
+        uint32_t at = 0;
+        CU(e, cudaMemcpy(&at, k.map.pidx + s, 4, cudaMemcpyDeviceToHost));
+        CU(e, cudaMemcpy(out, k.map.pool + (size_t)at * k.tw4 * 4, k.tw4 * 16, cudaMemcpyDeviceToHost));
+        return 1;
+    }
+    return 0;
 }

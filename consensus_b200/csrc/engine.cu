@@ -493,6 +493,7 @@ void sbv_destroy(sbv_engine *e) {
         sbv_scratch_free(d);
         sbv_keys_free(d);
         sbv_ed_keys_free(d);
+        sbv_key_cache_free(d);
         for (auto &ln : d.lanes) {
             void *lp[] = {ln.d_r, ln.d_s, ln.d_qx, ln.d_qy, ln.d_dig, ln.d_ok, ln.d_slot, ln.d_msgs, ln.d_off, ln.d_perm, ln.d_aux, ln.d_mix};
             for (void *p : lp) if (p) cudaFree(p);

@@ -94,6 +94,16 @@ struct Dev {
     int32_t *ed_slot2local = nullptr;
     uint32_t *ed_ktab = nullptr;
     uint32_t ed_n_slots = 0, ed_n_local = 0;
+    // the opt-in cache of grouped-key tables across launches (sbv_key_cache_reserve), per scheme tag: one allocation holding
+    // the pool, the counters, the map (key_cache.cuh) and one launch area per scratch set (2 + SBV_GROUP_MAX_KEYS words:
+    // the lookup's miss and hit counts and the renumbered keylist of the launch holding that set)
+    struct KeyCache {
+        void *mem = nullptr;
+        KcMap map{};
+        uint32_t *lk = nullptr;
+        size_t lk_words = 0;
+        size_t tw4 = 0;  // 16-byte words per table
+    } kc[3];
     // profiling: event quadruples per verify launch (start, after prep, before / after the dominant kernel)
     std::vector<cudaEvent_t> prof_events;
     size_t prof_used = 0;
@@ -193,6 +203,11 @@ int sbv_init_gtables(sbv_engine *e, Dev &d);
 int sbv_keys_build(sbv_engine *e, Dev &d);  // (re)builds the per-key tables of the registry
 void sbv_keys_free(Dev &d);
 void sbv_scratch_free(Dev &d);
+// ---- key_cache.cu: the grouped-key cache ----
+void sbv_key_cache_free(Dev &d);  // caller has drained the device
+// the launch area of scratch set w in the cache of scheme s for a launch of kcap table slots, or nullptr when none is
+// reserved (or kcap exceeds SBV_GROUP_MAX_KEYS, as only a test hook's launch can); caller holds e->mu
+uint32_t *sbv_key_cache_area(Dev &d, int s, const Dev::Scratch *w, size_t kcap);
 // ---- inst_ed25519.cu: Ed25519 (enqueue only, no sync) ----
 int sbv_ed_btab_ensure(sbv_engine *e, Dev &d);  // caller holds e->mu and has set the device
 // k = SHA-512(R || A || M) mod L into d_k (word-major, 8n words), then the verdicts into d_ok.  d_sig: 64n bytes (R || S),

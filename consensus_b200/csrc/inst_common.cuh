@@ -1,5 +1,6 @@
 // inst_common.cuh — launcher templates behind ops.h.  Each inst_*.cu instantiates one group for one curve.
 #pragma once
+#include "key_cache.cuh"
 #include "keygroup.cuh"
 #include "ops.h"
 
@@ -126,6 +127,22 @@ cudaError_t op_comb_verify(uint32_t n, const int32_t *kidmap, const uint8_t *key
     constexpr int BLOCK = 64;
     k_verify_comb<C, BLOCK, Cfg<C>::COMB_MINB, Cfg<C>::COMB_INL><<<(n + BLOCK - 1) / BLOCK, BLOCK, 0, st>>>(
         n, kidmap, keyflags, r, uw, flags, reinterpret_cast<const uint4 *>(ktab), ok, list, count, gacc);
+    return cudaGetLastError();
+}
+
+template <class C>
+cudaError_t op_kc_lookup(const uint32_t *nkeys_ptr, uint32_t kcap, const uint32_t *keylist, const uint8_t *qx, const uint8_t *qy, KcMap c, uint32_t tw4,
+                         int32_t *keyid, uint32_t *lk, uint8_t *keyflags, uint32_t *ktab, cudaStream_t st) {
+    k_kc_lookup<<<(unsigned)(((size_t)kcap * 32 + 127) / 128), 128, 0, st>>>(nkeys_ptr, kcap, keylist, KcXY<C>{qx, qy}, c, tw4, keyid, lk, keyflags,
+                                                                            reinterpret_cast<uint4 *>(ktab));
+    return cudaGetLastError();
+}
+
+template <class C>
+cudaError_t op_kc_insert(uint32_t kcap, const uint32_t *lk, const uint8_t *qx, const uint8_t *qy, KcMap c, uint32_t tw4, const uint8_t *keyflags,
+                         const uint32_t *ktab, cudaStream_t st) {
+    k_kc_insert<<<(unsigned)(((size_t)kcap * 32 + 127) / 128), 128, 0, st>>>(kcap, lk, KcXY<C>{qx, qy}, c, tw4, keyflags,
+                                                                            reinterpret_cast<const uint4 *>(ktab));
     return cudaGetLastError();
 }
 

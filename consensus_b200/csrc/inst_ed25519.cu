@@ -6,6 +6,7 @@
 #include "ed25519_comb.cuh"
 #include "ed25519_keyed.cuh"
 #include "ed25519_verify.cuh"
+#include "key_cache.cuh"
 #include "keygroup.cuh"
 #include "sha512.cuh"
 
@@ -45,7 +46,8 @@ int sbv_ed_btab_ensure(sbv_engine *e, Dev &d) {
 //   s_gen                                                                              └─ k_ed_verify (keys without a table) ─────────────────┘
 //
 // Keys whose 32 bytes occur at least group_threshold times get a comb table (ed25519_comb.cuh) and their items take
-// k_ed_verify_comb; the table construction (latency-bound: one doubling chain per key) runs beside SHA-512.
+// k_ed_verify_comb; the table construction (latency-bound: one doubling chain per key) runs beside SHA-512.  With a key
+// cache reserved, k_kc_lookup runs after k_kg_assign and k_kc_insert after k_edc_final, as in pipeline.cu.
 namespace {
 constexpr KtGeom ED_COMB_GEOM{EDC_BASES_WORDS, EDC_HS_WORDS, EDC_ZTOP_WORDS, EDC_TAB_WORDS};
 static_assert(SBV_ED_COMB_ENTRIES * SBV_ED_BTAB_ENTRY_WORDS == EDC_TAB_WORDS, "engine.h: comb table");
@@ -60,7 +62,7 @@ size_t ed_group_cap(const sbv_engine *e, size_t n, uint32_t T) {
 
 // On st: the grouping of the n keys of d_pub (at most kcap of them with >= T items get a table slot) and the routing onto
 // w->klist / w->glist (counts at zeroed[1] / zeroed[2]); on w->s_tab: the comb tables, then w->ev_tab.
-int ed_group(sbv_engine *e, Dev::Scratch *w, size_t n, const uint8_t *d_pub, uint32_t T, size_t kcap, cudaStream_t st) {
+int ed_group(sbv_engine *e, Dev &d, Dev::Scratch *w, size_t n, const uint8_t *d_pub, uint32_t T, size_t kcap, cudaStream_t st) {
     const uint32_t nn = (uint32_t)n, cap = (uint32_t)kcap, blocks = (nn + 255) / 256;
     uint32_t *counters = w->zeroed, *kcnt = w->zeroed + 4;
     CU(e, cudaMemsetAsync(w->htab, 0xff, (size_t)w->hsize * 4, st));
@@ -68,17 +70,31 @@ int ed_group(sbv_engine *e, Dev::Scratch *w, size_t n, const uint8_t *d_pub, uin
     k_kg_insert<<<blocks, 256, 0, st>>>(nn, KgKey32{d_pub}, e->hash_seed, w->hsize - 1, w->htab, w->rep, kcnt);
     k_kg_assign<<<blocks, 256, 0, st>>>(nn, w->rep, kcnt, T, cap, w->keyid, w->keylist, counters);
     CU(e, cudaGetLastError());
+    // with a key cache: the lookup renumbers the keys (misses first), copies the hits' tables, and the build makes the misses
+    const Dev::KeyCache &kc = d.kc[SBV_ED25519];
+    uint32_t *lk = sbv_key_cache_area(d, SBV_ED25519, w, kcap);
+    const unsigned wb = (unsigned)(((size_t)cap * 32 + 127) / 128);
+    if (lk) {
+        CU(e, cudaMemsetAsync(lk, 0, 8, st));
+        k_kc_lookup<<<wb, 128, 0, st>>>(counters, cap, w->keylist, KcKey32{d_pub}, kc.map, (uint32_t)kc.tw4, w->keyid, lk, w->keyflags,
+                                        reinterpret_cast<uint4 *>((uint32_t *)w->ktab));
+        CU(e, cudaGetLastError());
+    }
     CU(e, cudaEventRecord(w->ev_group, st));
     CU(e, cudaStreamWaitEvent(w->s_tab, w->ev_group, 0));
     const unsigned kb = (cap + 63) / 64, cb = (unsigned)(((size_t)cap * EDC_NCHAIN + 63) / 64);
-    k_edc_bases<<<kb, 64, 0, w->s_tab>>>(counters, cap, w->keylist, d_pub, w->bases, w->keyflags);
-    k_edc_fill<<<cb, 64, 0, w->s_tab>>>(counters, cap, w->bases, w->keyflags, w->hs, w->ztop, w->ktab);
-    k_edc_inv<<<kb, 64, 0, w->s_tab>>>(counters, cap, w->keyflags, w->ztop, w->pref);
-    k_edc_final<<<cb, 64, 0, w->s_tab>>>(counters, cap, w->keyflags, w->hs, w->ztop, w->ktab);
+    const uint32_t *nk = lk ? lk : counters, *kl = lk ? lk + 2 : (const uint32_t *)w->keylist;
+    k_edc_bases<<<kb, 64, 0, w->s_tab>>>(nk, cap, kl, d_pub, w->bases, w->keyflags);
+    k_edc_fill<<<cb, 64, 0, w->s_tab>>>(nk, cap, w->bases, w->keyflags, w->hs, w->ztop, w->ktab);
+    k_edc_inv<<<kb, 64, 0, w->s_tab>>>(nk, cap, w->keyflags, w->ztop, w->pref);
+    k_edc_final<<<cb, 64, 0, w->s_tab>>>(nk, cap, w->keyflags, w->hs, w->ztop, w->ktab);
+    if (lk)
+        k_kc_insert<<<wb, 128, 0, w->s_tab>>>(cap, lk, KcKey32{d_pub}, kc.map, (uint32_t)kc.tw4, w->keyflags,
+                                              reinterpret_cast<const uint4 *>((uint32_t *)w->ktab));
     CU(e, cudaGetLastError());
     CU(e, cudaEventRecord(w->ev_tab, w->s_tab));
     k_kg_route<<<blocks, 256, 0, st>>>(nn, w->rep, w->keyid, w->item_kid, w->klist, w->glist, counters);
-    e->launches += 7;
+    e->launches += 7 + (lk ? 2 : 0);
     CU(e, cudaGetLastError());
     return 0;
 }
@@ -95,7 +111,7 @@ int ed_close(sbv_engine *e, Dev::Scratch *w, cudaStream_t st, int rc) {
 
 int ed_grouped(sbv_engine *e, Dev &d, Dev::Scratch *w, size_t n, const uint8_t *d_msgs, const uint64_t *d_off, uint64_t base, const uint8_t *d_sig,
                const uint8_t *d_pub, uint32_t *d_k, uint32_t *d_perm, uint8_t *d_ok, uint32_t T, size_t kcap, cudaStream_t st) {
-    if (int rc = ed_group(e, w, n, d_pub, T, kcap, st)) return rc;
+    if (int rc = ed_group(e, d, w, n, d_pub, T, kcap, st)) return rc;
     const uint32_t nn = (uint32_t)n, *counters = w->zeroed;
     const uint32_t *perm = nullptr;
     if (int rc = sbv_launch_length_sort(e, n, d_off, d_perm, st, &perm)) return rc;
@@ -146,7 +162,7 @@ int sbv_launch_ed_comb_tables(sbv_engine *e, Dev &d, size_t n, const uint8_t *d_
     if (!kcap) return 0;
     Dev::Scratch *w = nullptr;
     if (int rc = sbv_take_scratch(e, d, 0, &ED_COMB_GEOM, n, kcap, st, &w)) return rc;
-    int rc = ed_group(e, w, n, d_pub, T, kcap, st);
+    int rc = ed_group(e, d, w, n, d_pub, T, kcap, st);
     if (!rc) {
         const cudaError_t a = cudaStreamWaitEvent(st, w->ev_tab, 0);
         rc = a != cudaSuccess ? sbv_fail(e, SBV_ERR_CUDA, "cudaStreamWaitEvent: %s", cudaGetErrorString(a)) : 0;
@@ -165,7 +181,7 @@ int sbv_launch_ed_verify_comb_k(sbv_engine *e, Dev &d, size_t n, const uint8_t *
                                 cudaStream_t st) {
     Dev::Scratch *w = nullptr;
     if (int rc = sbv_take_scratch(e, d, 0, &ED_COMB_GEOM, n, n, st, &w)) return rc;
-    int rc = ed_group(e, w, n, d_pub, 1, n, st);
+    int rc = ed_group(e, d, w, n, d_pub, 1, n, st);
     if (!rc) {
         const uint32_t nn = (uint32_t)n;
         const cudaError_t a = cudaStreamWaitEvent(st, w->ev_tab, 0);

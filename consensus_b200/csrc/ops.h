@@ -6,6 +6,8 @@
 #include <stddef.h>
 #include <stdint.h>
 
+#include "key_cache.h"
+
 struct KtGeom {  // words per key of a per-key table and of its construction scratch
     size_t bases_words, hs_words, ztop_words, ktab_words;
 };
@@ -49,6 +51,12 @@ struct CurveOps {
     // keys grouped inside a launch (P-256: comb tables; P-384: 5-bit window tables) / registered keys (8-bit windows)
     const GroupedKtOps *grouped;
     const RegisteredKtOps *kt8;
+    // the key cache (key_cache.cuh): k_kc_lookup after the grouping, k_kc_insert after the table construction; tw4 = 16-byte
+    // words per table of `grouped`
+    cudaError_t (*cache_lookup)(const uint32_t *nkeys_ptr, uint32_t kcap, const uint32_t *keylist, const uint8_t *qx, const uint8_t *qy, KcMap c,
+                                uint32_t tw4, int32_t *keyid, uint32_t *lk, uint8_t *keyflags, uint32_t *ktab, cudaStream_t st);
+    cudaError_t (*cache_insert)(uint32_t kcap, const uint32_t *lk, const uint8_t *qx, const uint8_t *qy, KcMap c, uint32_t tw4, const uint8_t *keyflags,
+                                const uint32_t *ktab, cudaStream_t st);
 };
 
 #define SBV_COZ_DECL(NAME)                                                                                                          \

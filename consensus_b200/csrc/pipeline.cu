@@ -11,6 +11,8 @@
 // (latency-bound: one inversion chain) runs beside the table construction (latency-bound: one doubling chain).
 // A large host-buffer batch runs the part after the table fork chunk by chunk, as its chunks arrive.
 // Registered keys (sbv_set_keys) skip the grouping: their tables were built at registration.
+// With a key cache reserved (sbv_key_cache_reserve), k_kc_lookup runs after k_kg_assign on st and k_kc_insert after
+// k_kt_final on s_tab (key_cache.cuh): the build then makes only the tables the cache does not hold.
 #include "engine.h"
 
 namespace {
@@ -190,11 +192,20 @@ int verify_begin(sbv_engine *e, Dev &d, uint8_t curve, size_t n, const uint8_t *
     CU(e, cudaMemsetAsync(w->htab, 0xff, (size_t)w->hsize * 4, st));
     CU(e, cudaMemsetAsync(w->zeroed, 0, (n + 4 + 4 * (size_t)chunks) * 4, st));
     CU(e, ops.group(nn, d_qx, d_qy, e->hash_seed, w->hsize - 1, w->htab, w->rep, kcnt, T, (uint32_t)kcap, w->keyid, w->keylist, counters, st));
+    // with a key cache: the lookup renumbers the keys (misses first), copies the hits' tables, and the build makes the misses
+    const Dev::KeyCache &kc = d.kc[curve];
+    uint32_t *lk = sbv_key_cache_area(d, curve, w, kcap);
+    if (lk) {
+        CU(e, cudaMemsetAsync(lk, 0, 8, st));
+        CU(e, ops.cache_lookup(counters, (uint32_t)kcap, w->keylist, d_qx, d_qy, kc.map, (uint32_t)kc.tw4, w->keyid, lk, w->keyflags, w->ktab, st));
+    }
     CU(e, cudaEventRecord(w->ev_group, st));
     CU(e, cudaStreamWaitEvent(w->s_tab, w->ev_group, 0));
-    CU(e, kt->build(counters + 0, (uint32_t)kcap, w->keylist, d_qx, d_qy, w->bases, w->hs, w->ztop, w->pref, w->ktab, w->keyflags, w->s_tab));
+    CU(e, kt->build(lk ? lk : counters, (uint32_t)kcap, lk ? lk + 2 : w->keylist, d_qx, d_qy, w->bases, w->hs, w->ztop, w->pref, w->ktab, w->keyflags,
+                    w->s_tab));
+    if (lk) CU(e, ops.cache_insert((uint32_t)kcap, lk, d_qx, d_qy, kc.map, (uint32_t)kc.tw4, w->keyflags, w->ktab, w->s_tab));
     CU(e, cudaEventRecord(w->ev_tab, w->s_tab));
-    e->launches += 2 + (curve == 0 ? 5 : 4);  // grouping + table construction
+    e->launches += 2 + (curve == 0 ? 5 : 4) + (lk ? 2 : 0);  // grouping + table construction (+ cache lookup and insert)
     return 0;
 }
 }  // namespace

@@ -265,6 +265,40 @@ int sbv_verify_registered_device(sbv_engine *e, int device_index, uint8_t curve,
                                  const uint8_t *d_r, const uint8_t *d_s, const uint8_t *d_digest, uint8_t digest_len,
                                  uint8_t *d_ok, void *cuda_stream);
 
+/* ---- tables of repeated keys kept across launches (opt-in) ----
+ * Keys that a keys-per-item launch groups (SBV_GROUP_THRESHOLD items or more of one key in a device's shard, within
+ * SBV_GROUP_MIN_BATCH and SBV_GROUP_MAX_KEYS) get a fixed-base table built in the launch.  Client keys of a SmartBFT
+ * deployment come back in every batch but are not configuration, so they cannot be registered; with a cache reserved, the
+ * launch takes the tables of such keys from the cache instead of rebuilding them.  This covers sbv_verify_batch and its
+ * _device, _der and _ranked forms, sbv_hash_verify_batch, sbv_hash384_verify_batch, sbv_verify_mixed, sbv_verify_quorum,
+ * sbv_ed25519_verify_batch and sbv_mixed_verify_batch.
+ *  - Only where a table comes from changes.  The cache serves only keys the launch groups anyway; keys below the threshold
+ *    take the generic kernel, cached or not.  A hit puts the cached table into the launch's table slot; a miss is built as
+ *    without a cache and then inserted if there is room.  A table is a pure function of the key bytes, so routing, the
+ *    verification kernels and every verdict are bit for bit those of an engine without a cache.
+ *  - Keyed by the exact bytes: qx || qy (64 bytes) for P-256, 96 bytes for P-384, the 32-byte encoding for Ed25519 (so
+ *    y >= p and "-0" encodings are keys of their own, as in the grouping).  Entries are compared byte for byte, never by
+ *    hash alone.
+ *  - Only keys whose build flags them valid are inserted: an off-curve ECDSA key or an undecodable Ed25519 key is rebuilt,
+ *    and rejected, in every launch.
+ *  - Fill once, no eviction: a full cache stops inserting.  Reserving again empties it (for example on a
+ *    reconfiguration).  It is independent of both registries and of verification_seq.
+ *  - One cache per device: each device caches the keys of its own shards.
+ *  - Two launches that miss the same key at once both build it; one of them inserts it.
+ *
+ * Reserve, on every device, room for the tables of up to p256 / p384 / ed25519 keys.  The sizes per key are the
+ * per-launch table sizes: 32 KiB for P-256, 118 KiB for P-384, 47.8 KiB for Ed25519, plus a map of a power of two
+ * >= 2 x capacity slots (72 to 104 bytes each).  Replaces and empties any earlier cache.  (0, 0, 0) frees it, and the
+ * engine behaves as if none had been reserved: the same kernels, launch count and memory.  Excludes concurrent launches
+ * as sbv_ed25519_set_keys does (it waits for the calls already enqueueing and drains every device).  SBV_ERR_NOMEM
+ * leaves no cache on any device. */
+int sbv_key_cache_reserve(sbv_engine *e, size_t p256, size_t p384, size_t ed25519);
+/* Per scheme tag (SBV_P256 / SBV_P384 / SBV_ED25519; anything else is SBV_ERR_ARG), summed over devices, for the calls
+ * that have returned (a _device call: once its stream has been synchronised): out[0] capacity, out[1] resident tables,
+ * out[2] grouped keys served from the cache (hits), out[3] grouped valid keys built in the launch while a cache was
+ * reserved (misses; invalid keys count as neither).  All zero without a cache. */
+int sbv_key_cache_stats(sbv_engine *e, uint8_t scheme, uint64_t out[4]);
+
 /* ---- one process per GPU (a Go host may run one node process per device; bench.py does under torchrun) ----
  * The engine of every process is one RANK; the only exchange is the all-gather of packed verdict / quorum bitmasks
  * over NCCL (NVLink / NVSwitch).  Rank 0 calls sbv_comm_unique_id and ships the 128 bytes to the others (any side

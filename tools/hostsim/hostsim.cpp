@@ -16,6 +16,7 @@ thread_local hostsim_warp *hostsim_ctx = nullptr;
 namespace sbv { uint32_t tab[1 << 18]; }
 #include "../../consensus_b200/csrc/debug_ops.cuh"
 #include "../../consensus_b200/csrc/keygroup.cuh"
+#include "../../consensus_b200/csrc/key_cache.cuh"
 #include "../../consensus_b200/csrc/sha256.cuh"
 #include "../../consensus_b200/csrc/sha384.cuh"
 #include "../../consensus_b200/csrc/quorum.cuh"
@@ -707,4 +708,54 @@ extern "C" int hs_mixed_verify_batch(size_t n, const uint8_t *tag, const uint8_t
     if (m[2]) hs_ed25519_verify_grouped(m[2], blob.data(), fo.data() + at[2] + 2, sig2.data(), pub2.data(), T, max_keys, okf.data() + at[2], nullptr);
     hs_mixed_scatter(n, m[0], m[1], idx.data(), okf.data(), ok);
     return 0;
+}
+
+// ---- the key cache (key_cache.cuh) ----
+// The cache of one family on one device as caller-owned arrays (state / keys / pidx: smask + 1 slots; pool: cap tables of
+// tw4 16-byte words; stats: 4 counters), so that a test can run launches against it and inspect or set any slot.
+// fam: 0 = P-256 and 1 = P-384 (keys qx || qy of items of a, b), 2 = Ed25519 (32-byte keys of items of a; b unused).
+static KcMap hs_kc_map(uint32_t *state, uint32_t *keys, uint32_t *pidx, uint32_t *pool, unsigned long long *stats, uint32_t smask, uint32_t cap,
+                       uint32_t seed) {
+    return KcMap{state, keys, pidx, pool, stats, smask, cap, seed};
+}
+template <class F>
+static int hs_kc_fam(int fam, const uint8_t *a, const uint8_t *b, F &&f) {
+    if (fam == 0) f(KcXY<P256>{a, b});
+    else if (fam == 1) f(KcXY<P384>{a, b});
+    else if (fam == 2) f(KcKey32{a});
+    else return -1;
+    return 0;
+}
+// k_kc_lookup over the launch's grouped keys (count *nkeys, key k = item keylist[k]); lk: 2 + kcap words, zeroed here
+extern "C" int hs_kc_lookup(int fam, const uint8_t *a, const uint8_t *b, const uint32_t *nkeys, uint32_t kcap, const uint32_t *keylist,
+                            uint32_t *state, uint32_t *keys, uint32_t *pidx, uint32_t *pool, unsigned long long *stats, uint32_t smask, uint32_t cap,
+                            uint32_t seed, uint32_t tw4, int32_t *keyid, uint32_t *lk, uint8_t *keyflags, uint32_t *ktab) {
+    const KcMap c = hs_kc_map(state, keys, pidx, pool, stats, smask, cap, seed);
+    lk[0] = lk[1] = 0;
+    return hs_kc_fam(fam, a, b, [&](auto key) {
+        run_grid_lockstep((unsigned)(((size_t)kcap * 32 + 127) / 128), 128, [&] {
+            k_kc_lookup(nkeys, kcap, keylist, key, c, tw4, keyid, lk, keyflags, reinterpret_cast<uint4 *>(ktab));
+        });
+    });
+}
+// k_kc_insert after the build of the launch's misses (ktab[0, lk[0]), keyflags)
+extern "C" int hs_kc_insert(int fam, const uint8_t *a, const uint8_t *b, uint32_t kcap, const uint32_t *lk, uint32_t *state, uint32_t *keys,
+                            uint32_t *pidx, uint32_t *pool, unsigned long long *stats, uint32_t smask, uint32_t cap, uint32_t seed, uint32_t tw4,
+                            const uint8_t *keyflags, const uint32_t *ktab) {
+    const KcMap c = hs_kc_map(state, keys, pidx, pool, stats, smask, cap, seed);
+    return hs_kc_fam(fam, a, b, [&](auto key) {
+        run_grid_lockstep((unsigned)(((size_t)kcap * 32 + 127) / 128), 128, [&] {
+            k_kc_insert(kcap, lk, key, c, tw4, keyflags, reinterpret_cast<const uint4 *>(ktab));
+        });
+    });
+}
+// the first probe slot of item i's key (kc_hash(key) & smask), or with fp != 0 its fingerprint (kc_fp)
+extern "C" uint32_t hs_kc_slot(int fam, const uint8_t *a, const uint8_t *b, uint32_t i, uint32_t seed, uint32_t smask, int fp) {
+    uint32_t h = 0;
+    hs_kc_fam(fam, a, b, [&](auto key) {
+        uint32_t w[decltype(key)::W];
+        key.load(i, w);
+        h = fp ? kc_fp(w, seed) : kc_hash(w, seed) & smask;
+    });
+    return h;
 }

@@ -46,6 +46,7 @@ MIXED_KEYS = ["tests/test_hostsim_mixed_keys.py"]  # keys per item (k_mix_split<
 SHARDS = ["tests/test_hostsim_shards.py"]
 WIDE = ["tests/test_hostsim_wide.py"]  # bit lengths, offsets and byte sums past 32 bits
 SHA384 = ["tests/test_hostsim_sha384.py"]
+KEY_CACHE = ["tests/test_hostsim_key_cache.py"]
 
 
 def M(id, file, find, repl, tests, equivalent=None, proof=None):
@@ -322,6 +323,33 @@ CATALOGUE = [
     M("quorum_shards_trailing_votes", "shards.h", "const uint32_t *b = g == G - 1 ? instance + n_votes :", "const uint32_t *b = false ? instance + n_votes :", SHARDS),
     M("quorum_shards_instance_words", "shards.h", "s.wi = std::max(s.wi, (ir.n + 31) / 32);", "s.wi = std::max(s.wi, ir.n / 32);", SHARDS),
     M("unpack_reached_offset", "shards.h", "reached[s.ir[g].lo + i] = bit(w + s.wv, i);", "reached[s.ir[g].lo + i] = bit(w + s.wi, i);", SHARDS),
+    # ---------------------------------------------------------------- key_cache.cuh
+    M("kc_find_busy_hits", "key_cache.cuh", "if (s == ready && kc_same<W>(c, h, w)) return (int32_t)h;",
+      "if ((s & ~3u) == (ready & ~3u) && kc_same<W>(c, h, w)) return (int32_t)h;", KEY_CACHE),
+    M("kc_same_half_key", "key_cache.cuh", "for (int k = 0; k < W; k++) diff |= kc_ld(s + k) ^ w[k];", "for (int k = 0; k < W / 2; k++) diff |= kc_ld(s + k) ^ w[k];",
+      KEY_CACHE),
+    M("kc_lookup_no_clamp", "key_cache.cuh", "if (nk > kcap) nk = kcap;", "(void)0;", KEY_CACHE),
+    M("kc_lookup_miss_id", "key_cache.cuh", "id = (int32_t)atomicAdd(lk + 0, 1u);", "id = (int32_t)atomicAdd(lk + 1, 1u);", KEY_CACHE),
+    M("kc_lookup_hit_id", "key_cache.cuh", "id = (int32_t)(nk - 1 - atomicAdd(lk + 1, 1u));", "id = (int32_t)(nk - atomicAdd(lk + 1, 1u));", KEY_CACHE),
+    M("kc_lookup_hit_flag", "key_cache.cuh", "keyflags[id] = 1;", "(void)0;", KEY_CACHE),
+    M("kc_lookup_hit_count", "key_cache.cuh", "atomicAdd(c.stats + 2, 1ull);", "(void)0;", KEY_CACHE),
+    M("kc_lookup_keylist", "key_cache.cuh", "lk[2 + id] = item;", "lk[2 + k] = item;", KEY_CACHE),
+    M("kc_lookup_keyid", "key_cache.cuh", "keyid[item] = id;", "(void)0;", KEY_CACHE),
+    M("kc_lookup_copy_stride", "key_cache.cuh", "for (uint32_t i = lane; i < tw4; i += 32) dst[i] = kc_ld(src + i);",
+      "for (uint32_t i = lane; i < tw4; i += 64) dst[i] = kc_ld(src + i);", KEY_CACHE),
+    M("kc_insert_invalid", "key_cache.cuh", "if (k >= m || !keyflags[k]) return;", "if (k >= m) return;", KEY_CACHE),
+    M("kc_insert_miss_count", "key_cache.cuh", "atomicAdd(c.stats + 3, 1ull);", "(void)0;", KEY_CACHE),
+    M("kc_claim_past_busy", "key_cache.cuh", "if ((s & 3u) == KC_BUSY) return -1;", "if ((s & 3u) == KC_BUSY) continue;", KEY_CACHE),
+    M("kc_claim_other_fingerprint", "key_cache.cuh", "if ((s & ~3u) != fp) continue;", "(void)0;", KEY_CACHE),
+    M("kc_claim_same_key", "key_cache.cuh", "if (kc_same<W>(c, h, w)) return -1;", "(void)0;", KEY_CACHE),
+    M("kc_claim_full_pool", "key_cache.cuh", "if (*(const volatile unsigned long long *)c.stats >= c.cap) return -1;", "(void)0;", KEY_CACHE),
+    M("kc_insert_pidx", "key_cache.cuh", "c.pidx[slot] = (uint32_t)at;", "c.pidx[slot] = 0;", KEY_CACHE),
+    M("kc_insert_key_words", "key_cache.cuh", "for (int i = 0; i < KV::W; i++) kw[i] = w[i];", "for (int i = 1; i < KV::W; i++) kw[i] = w[i];", KEY_CACHE),
+    M("kc_insert_pool_entry", "key_cache.cuh", "uint4 *dst = reinterpret_cast<uint4 *>(c.pool) + (size_t)at * tw4;",
+      "uint4 *dst = reinterpret_cast<uint4 *>(c.pool) + (size_t)at;", KEY_CACHE),
+    M("kc_insert_publish", "key_cache.cuh", "kc_store_release(c.state + slot, kc_fp<KV::W>(w, c.seed) | KC_READY);",
+      "kc_store_release(c.state + slot, kc_fp<KV::W>(w, c.seed) | KC_BUSY);", KEY_CACHE),
+    M("kc_insert_resident_count", "key_cache.cuh", "atomicAdd(c.stats + 1, 1ull);", "(void)0;", KEY_CACHE),
 ]
 
 
