@@ -167,31 +167,29 @@ extern "C" int sbv_debug_key_table(sbv_engine *e, uint8_t curve, uint32_t slot, 
     return SBV_OK;
 }
 
-// The per-key tables of a keys-per-item launch of the n keys (qx, qy: BYTES each) on device 0: the first half of the
-// launch (sbv_launch_verify_begin: grouping with the engine's SBV_GROUP_* settings and the table construction), then the
-// scratch set goes back (sbv_launch_verify_abort).  For each of the m query items items[q] < n: status[q] = 0 and the
-// key's table at out + q * (table words), as the verification kernel reads it (P-256: CombTab, 512 entries in slot
-// order; P-384: KeyTab<384, 5>, 77 x 16 entries; affine Montgomery x then y, 2N limbs each); 1 when the key got no table
-// (fewer items than the threshold, table slots used up, or a launch that does not group); 2 when it got a table slot but
-// is not a valid key.
-extern "C" int sbv_debug_grouped_key_table(sbv_engine *e, uint8_t curve, size_t n, const uint8_t *qx, const uint8_t *qy, size_t m,
-                                           const uint32_t *items, int32_t *status, uint32_t *out) {
-    if (!e || curve > SBV_P384 || !qx || !qy || (m && (!items || !status || !out)) || n > UINT32_MAX) return SBV_ERR_ARG;
+namespace {
+// The tables of a keys-per-item launch of scheme s over the n keys of a (and b: ECDSA qy, else nullptr), key_bytes per key
+// in each, on device 0: the first half of the launch (sbv_launch_verify_begin: grouping with the engine's SBV_GROUP_*
+// settings and the table construction), then the scratch set goes back.  For each of the m query items items[q] < n:
+// status[q] = 0 and the key's table at out + q * (table words), as the verification kernel reads it; 1 when the key got
+// no table (fewer items than the threshold, table slots used up, or a launch that does not group); 2 when it got a
+// table slot but is not a valid key.
+int grouped_tables(sbv_engine *e, const char *what, uint8_t scheme, size_t n, size_t key_bytes, const uint8_t *a, const uint8_t *b, size_t m,
+                   const uint32_t *items, int32_t *status, uint32_t *out) {
     for (size_t q = 0; q < m; q++)
         if (items[q] >= n) return SBV_ERR_ARG;
     if (n == 0) return SBV_OK;
-    const CurveOps &ops = sbv_ops(curve);
-    const size_t L = (size_t)ops.bytes, words = ops.grouped->geom.ktab_words, kb = (n * L + 255) & ~(size_t)255;
+    const size_t words = sbv_group_ops(scheme).kt->geom.ktab_words, kb = (n * key_bytes + 255) & ~(size_t)255;
     std::lock_guard<std::mutex> lk(e->mu);
     Dev &d = e->devs[0];
     CU(e, cudaSetDevice(d.ordinal));
     int rc = sbv_ensure_scratch(e, d, 2 * kb + 1024);
     if (rc) return rc;
-    uint8_t *dqx = d.d_scratch, *dqy = d.d_scratch + kb;
-    CU(e, cudaMemcpyAsync(dqx, qx, n * L, cudaMemcpyHostToDevice, d.stream));
-    CU(e, cudaMemcpyAsync(dqy, qy, n * L, cudaMemcpyHostToDevice, d.stream));
+    uint8_t *da = d.d_scratch, *db = b ? d.d_scratch + kb : nullptr;
+    CU(e, cudaMemcpyAsync(da, a, n * key_bytes, cudaMemcpyHostToDevice, d.stream));
+    if (b) CU(e, cudaMemcpyAsync(db, b, n * key_bytes, cudaMemcpyHostToDevice, d.stream));
     VerifyLaunch vl;
-    if ((rc = sbv_launch_verify_begin(e, d, curve, n, dqx, dqy, d.stream, &vl))) return rc;
+    if ((rc = sbv_launch_verify_begin(e, d, scheme, n, da, db, d.stream, &vl))) return rc;
     Dev::Scratch *w = vl.w;
     uint32_t nkeys = 0;
     cudaError_t st = cudaSuccess;
@@ -215,10 +213,32 @@ extern "C" int sbv_debug_grouped_key_table(sbv_engine *e, uint8_t curve, size_t 
             st = cudaMemcpy(out + q * words, (uint32_t *)w->ktab + (size_t)kid * words, words * 4, cudaMemcpyDeviceToHost);
         if (st == cudaSuccess) status[q] = flag ? 0 : 2;
     }
-    sbv_launch_verify_abort(vl, d.stream);
-    if (st != cudaSuccess) return sbv_fail(e, SBV_ERR_CUDA, "sbv_debug_grouped_key_table: %s", cudaGetErrorString(st));
+    if (st != cudaSuccess) return sbv_launch_verify_close(e, vl, d.stream, sbv_fail(e, SBV_ERR_CUDA, "%s: %s", what, cudaGetErrorString(st)));
+    if ((rc = sbv_launch_verify_close(e, vl, d.stream, 0))) return rc;
     CU(e, cudaStreamSynchronize(d.stream));
     return SBV_OK;
+}
+
+// Every k (8 little-endian limbs per item) is < L: the kernels only ever see reduced k, and their recoding of the top
+// window assumes bit 255 clear.
+bool k_below_l(size_t n, const uint32_t *k) {
+    static const uint32_t L[8] = {0x5cf5d3ed, 0x5812631a, 0xa2f79cd6, 0x14def9de, 0, 0, 0, 0x10000000};
+    for (size_t i = 0; i < n; i++) {
+        int w = 7;
+        while (w > 0 && k[i * 8 + w] == L[w]) w--;
+        if (k[i * 8 + w] >= L[w]) return false;
+    }
+    return true;
+}
+}  // namespace
+
+// The per-key tables of a keys-per-item launch of the n keys (qx, qy: BYTES each) on device 0, as grouped_tables reads
+// them (P-256: CombTab, 512 entries in slot order; P-384: KeyTab<384, 5>, 77 x 16 entries; affine Montgomery x then y,
+// 2N limbs each).
+extern "C" int sbv_debug_grouped_key_table(sbv_engine *e, uint8_t curve, size_t n, const uint8_t *qx, const uint8_t *qy, size_t m,
+                                           const uint32_t *items, int32_t *status, uint32_t *out) {
+    if (!e || curve > SBV_P384 || !qx || !qy || (m && (!items || !status || !out)) || n > UINT32_MAX) return SBV_ERR_ARG;
+    return grouped_tables(e, "sbv_debug_grouped_key_table", curve, n, (size_t)sbv_ops(curve).bytes, qx, qy, m, items, status, out);
 }
 
 // Copies entries [first, first + count) of device 0's fixed-base table of B (k_ed_btab_init: entry win * 128 + j - 1 is
@@ -241,12 +261,7 @@ extern "C" int sbv_debug_ed25519_btab(sbv_engine *e, size_t first, size_t count,
 // reduced k, and its recoding of the top window assumes bit 255 clear).  sig: 64 bytes per item (R || S), pub: 32.
 extern "C" int sbv_debug_ed25519_verify_k(sbv_engine *e, size_t n, const uint8_t *sig, const uint8_t *pub, const uint32_t *k, uint8_t *ok) {
     if (!e || !sig || !pub || !k || !ok || n > UINT32_MAX) return SBV_ERR_ARG;
-    static const uint32_t L[8] = {0x5cf5d3ed, 0x5812631a, 0xa2f79cd6, 0x14def9de, 0, 0, 0, 0x10000000};
-    for (size_t i = 0; i < n; i++) {
-        int w = 7;
-        while (w > 0 && k[i * 8 + w] == L[w]) w--;
-        if (k[i * 8 + w] >= L[w]) return SBV_ERR_ARG;
-    }
+    if (!k_below_l(n, k)) return SBV_ERR_ARG;
     if (n == 0) return SBV_OK;
     std::lock_guard<std::mutex> lk(e->mu);
     Dev &d = e->devs[0];
@@ -290,45 +305,13 @@ extern "C" int sbv_debug_ed25519_ktab(sbv_engine *e, uint32_t slot, size_t first
     return SBV_OK;
 }
 
-// The comb tables of a keys-per-item launch of the n keys of pub (32 bytes each) on device 0, grouped with the engine's
-// settings (SBV_GROUP_THRESHOLD, SBV_GROUP_MAX_KEYS, SBV_GROUP_MIN_BATCH).  For each of the m query items items[q] < n:
-// status[q] = 0 and the key's table at out + q * 510 * 24 (entry b * 255 + mask - 1 = the sum of 2^(16 (8b + t)) * A over
-// the set bits t of mask, as y + x, y - x, 2dxy, 24 limbs); 1 when the key got no table (fewer items than the threshold,
-// table slots used up, or a launch that does not group); 2 when it got a table slot but does not decode.
+// The comb tables of a keys-per-item launch of the n keys of pub (32 bytes each) on device 0, as grouped_tables reads them
+// (entry b * 255 + mask - 1 = the sum of 2^(16 (8b + t)) * A over the set bits t of mask, as y + x, y - x, 2dxy, 24
+// limbs; 510 entries); status 2: the key does not decode.
 extern "C" int sbv_debug_ed25519_comb_tab(sbv_engine *e, size_t n, const uint8_t *pub, size_t m, const uint32_t *items, int32_t *status,
                                           uint32_t *out) {
     if (!e || !pub || (m && (!items || !status || !out)) || n > UINT32_MAX) return SBV_ERR_ARG;
-    for (size_t q = 0; q < m; q++)
-        if (items[q] >= n) return SBV_ERR_ARG;
-    if (n == 0) return SBV_OK;
-    std::lock_guard<std::mutex> lk(e->mu);
-    Dev &d = e->devs[0];
-    CU(e, cudaSetDevice(d.ordinal));
-    int rc = sbv_ensure_scratch(e, d, n * 32 + 1024);
-    if (rc) return rc;
-    CU(e, cudaMemcpyAsync(d.d_scratch, pub, n * 32, cudaMemcpyHostToDevice, d.stream));
-    Dev::Scratch *w = nullptr;
-    if ((rc = sbv_launch_ed_comb_tables(e, d, n, d.d_scratch, d.stream, &w))) return rc;
-    const size_t words = SBV_ED_COMB_ENTRIES * SBV_ED_BTAB_ENTRY_WORDS;
-    for (size_t q = 0; q < m && !rc; q++) {
-        status[q] = 1;
-        if (!w) continue;
-        uint32_t r = 0;
-        int32_t kid = -1;
-        uint8_t flag = 0;
-        cudaError_t st = cudaMemcpy(&r, (uint32_t *)w->rep + items[q], 4, cudaMemcpyDeviceToHost);
-        if (st == cudaSuccess) st = cudaMemcpy(&kid, (int32_t *)w->keyid + r, 4, cudaMemcpyDeviceToHost);
-        if (st == cudaSuccess && kid >= 0) st = cudaMemcpy(&flag, (uint8_t *)w->keyflags + kid, 1, cudaMemcpyDeviceToHost);
-        if (st == cudaSuccess && kid >= 0 && flag)
-            st = cudaMemcpy(out + q * words, (uint32_t *)w->ktab + (size_t)kid * words, words * 4, cudaMemcpyDeviceToHost);
-        if (st != cudaSuccess) rc = sbv_fail(e, SBV_ERR_CUDA, "sbv_debug_ed25519_comb_tab: %s", cudaGetErrorString(st));
-        else if (kid >= 0) status[q] = flag ? 0 : 2;
-    }
-    if (w) {
-        const cudaError_t st = cudaEventRecord(w->done, d.stream);
-        if (!rc && st != cudaSuccess) rc = sbv_fail(e, SBV_ERR_CUDA, "cudaEventRecord: %s", cudaGetErrorString(st));
-    }
-    return rc;
+    return grouped_tables(e, "sbv_debug_ed25519_comb_tab", SBV_ED25519, n, 32, pub, nullptr, m, items, status, out);
 }
 
 // The comb kernel of grouped keys (k_ed_verify_comb) on device 0 with the caller's k in place of SHA-512(R || A || M) mod
@@ -336,12 +319,7 @@ extern "C" int sbv_debug_ed25519_comb_tab(sbv_engine *e, size_t n, const uint8_t
 // each < L (SBV_ERR_ARG otherwise); sig = R || S (64 bytes), pub = 32 bytes per item.
 extern "C" int sbv_debug_ed25519_verify_comb_k(sbv_engine *e, size_t n, const uint8_t *sig, const uint8_t *pub, const uint32_t *k, uint8_t *ok) {
     if (!e || !sig || !pub || !k || !ok || n > UINT32_MAX) return SBV_ERR_ARG;
-    static const uint32_t L[8] = {0x5cf5d3ed, 0x5812631a, 0xa2f79cd6, 0x14def9de, 0, 0, 0, 0x10000000};
-    for (size_t i = 0; i < n; i++) {
-        int w = 7;
-        while (w > 0 && k[i * 8 + w] == L[w]) w--;
-        if (k[i * 8 + w] >= L[w]) return SBV_ERR_ARG;
-    }
+    if (!k_below_l(n, k)) return SBV_ERR_ARG;
     if (n == 0) return SBV_OK;
     std::lock_guard<std::mutex> lk(e->mu);
     Dev &d = e->devs[0];
@@ -372,12 +350,7 @@ extern "C" int sbv_debug_ed25519_verify_comb_k(sbv_engine *e, size_t n, const ui
 extern "C" int sbv_debug_ed25519_verify_registered_k(sbv_engine *e, size_t n, const uint32_t *key_slot, const uint8_t *sig, const uint32_t *k,
                                                      uint8_t *ok) {
     if (!e || !key_slot || !sig || !k || !ok || n > UINT32_MAX) return SBV_ERR_ARG;
-    static const uint32_t L[8] = {0x5cf5d3ed, 0x5812631a, 0xa2f79cd6, 0x14def9de, 0, 0, 0, 0x10000000};
-    for (size_t i = 0; i < n; i++) {
-        int w = 7;
-        while (w > 0 && k[i * 8 + w] == L[w]) w--;
-        if (k[i * 8 + w] >= L[w]) return SBV_ERR_ARG;
-    }
+    if (!k_below_l(n, k)) return SBV_ERR_ARG;
     if (n == 0) return SBV_OK;
     std::lock_guard<std::mutex> lk(e->mu);
     Dev &d = e->devs[0];
@@ -413,7 +386,7 @@ extern "C" int sbv_debug_key_cache_entry(sbv_engine *e, int device_index, uint8_
     Dev &d = e->devs[device_index];
     const Dev::KeyCache &k = d.kc[scheme];
     if (!k.mem) return 0;
-    const size_t kw = scheme == SBV_P256 ? 16 : scheme == SBV_P384 ? 24 : 8, slots = (size_t)k.map.smask + 1;
+    const size_t kw = sbv_group_ops(scheme).key_words, slots = (size_t)k.map.smask + 1;
     CU(e, cudaSetDevice(d.ordinal));
     CU(e, cudaDeviceSynchronize());
     std::vector<uint32_t> state(slots), keys(slots * kw);

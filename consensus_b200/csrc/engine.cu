@@ -391,8 +391,7 @@ int stage_and_verify(sbv_engine *e, Dev &d, int lane, uint8_t curve, size_t lo, 
     }
     auto abandon = [&](int code) {  // a fault between the halves: hand the scratch set back (the caller fail-stops anyway)
         std::lock_guard<std::mutex> lk(e->mu);
-        sbv_launch_verify_abort(vl, ln.stream);
-        return code;
+        return sbv_launch_verify_close(e, vl, ln.stream, code);
     };
     for (int c = 0; c < chunks; c++) {
         const size_t clo = (size_t)c * per < cnt ? (size_t)c * per : cnt, cn = cnt - clo < per ? cnt - clo : per;
@@ -416,7 +415,7 @@ int stage_and_verify(sbv_engine *e, Dev &d, int lane, uint8_t curve, size_t lo, 
             return abandon(rc);
         std::lock_guard<std::mutex> lk(e->mu);
         rc = sbv_launch_verify_chunk(e, d, vl, c, clo, cn, c == chunks - 1, ln.d_r, ln.d_s, ln.d_dig, dlen, ln.d_ok, ln.stream);
-        if (rc) { sbv_launch_verify_abort(vl, ln.stream); return rc; }
+        if (rc) return sbv_launch_verify_close(e, vl, ln.stream, rc);
     }
     if (so_out) *so_out = so;
     return 0;

@@ -171,13 +171,13 @@ constexpr size_t SBV_NO_PROFILE = ~(size_t)0;
 
 // one keys-per-item launch between its two halves (pipeline.cu)
 struct VerifyLaunch {
-    Dev::Scratch *w = nullptr;
+    Dev::Scratch *w = nullptr;  // nullptr: no scratch set held (n = 0, or an Ed25519 launch that does not group)
     // first of the launch's five profiling events in d.prof_events (SBV_NO_PROFILE: none).  An index, resolved under
     // e->mu at each use: another thread's launch may grow the vector while this one is held open between its halves.
     size_t ev = SBV_NO_PROFILE;
     const uint8_t *d_qx = nullptr, *d_qy = nullptr;
     size_t n = 0;
-    uint8_t curve = 0;
+    uint8_t scheme = 0;
     bool grouping = false;
     int chunks = 1;   // the second half comes in this many chunks (sbv_launch_verify_chunk)
 };
@@ -186,9 +186,15 @@ struct VerifyLaunch {
 // keys-per-item: k_prep, key grouping, per-key tables for repeated keys, fixed-base kernel + generic kernel for the rest
 int sbv_launch_verify(sbv_engine *e, Dev &d, uint8_t curve, size_t n, const uint8_t *d_r, const uint8_t *d_s, const uint8_t *d_qx,
                       const uint8_t *d_qy, const uint8_t *d_dig, uint32_t dlen, uint8_t *d_ok, cudaStream_t st);
-int sbv_launch_verify_begin(sbv_engine *e, Dev &d, uint8_t curve, size_t n, const uint8_t *d_qx, const uint8_t *d_qy, cudaStream_t st, VerifyLaunch *vl,
-                            int chunks = 1);
-void sbv_launch_verify_abort(const VerifyLaunch &vl, cudaStream_t st);  // hand the scratch set back after a fault between the halves
+// The first half of a keys-per-item launch of n items of scheme s (keys as GroupOps takes them): a scratch set, the
+// grouping of the keys with the engine's SBV_GROUP_* settings on st and the tables of the grouped keys on the set's side
+// stream, ending in ev_tab.  every_key: every distinct key gets a table slot whatever the settings (a test hook's launch).
+// An ECDSA launch always holds a scratch set (its per-item buffers) and takes its profiling events here.
+int sbv_launch_verify_begin(sbv_engine *e, Dev &d, uint8_t scheme, size_t n, const uint8_t *d_qx, const uint8_t *d_qy, cudaStream_t st, VerifyLaunch *vl,
+                            int chunks = 1, bool every_key = false);
+// Hands the scratch set back: waits for the generic kernel on the second side stream, and with rc != 0 (a fault before the
+// join) for the tables too, then records the set's `done` event.  Returns rc, or a fault of its own.
+int sbv_launch_verify_close(sbv_engine *e, const VerifyLaunch &vl, cudaStream_t st, int rc);
 // second half for items [lo, lo + cn) of chunk c (the pointers are those of the WHOLE batch; a launch of one chunk has
 // c = 0, lo = 0, cn = n); `last` closes the launch
 int sbv_launch_verify_chunk(sbv_engine *e, Dev &d, const VerifyLaunch &vl, int c, size_t lo, size_t cn, bool last, const uint8_t *d_r, const uint8_t *d_s,
@@ -217,10 +223,6 @@ int sbv_ed_btab_ensure(sbv_engine *e, Dev &d);  // caller holds e->mu and has se
 int sbv_launch_ed25519(sbv_engine *e, Dev &d, size_t n, const uint8_t *d_msgs, const uint64_t *d_off, uint64_t base, const uint8_t *d_sig,
                        const uint8_t *d_pub, uint32_t *d_k, uint32_t *d_perm, uint8_t *d_ok, cudaStream_t st);
 // test hooks (caller holds e->mu; the table of B must exist):
-// the grouping and comb tables of a keys-per-item launch of the n keys of d_pub with the engine's settings, finished
-// (synchronised) on return; *w = the scratch set holding them (rep, keyid, keyflags, ktab), or nullptr when the launch
-// would not group.  The caller records (*w)->done when it has read them.
-int sbv_launch_ed_comb_tables(sbv_engine *e, Dev &d, size_t n, const uint8_t *d_pub, cudaStream_t st, Dev::Scratch **w);
 // k_ed_verify_comb over every item with the caller's k (word-major [8][n], every k < L); every distinct key gets a table
 int sbv_launch_ed_verify_comb_k(sbv_engine *e, Dev &d, size_t n, const uint8_t *d_sig, const uint8_t *d_pub, const uint32_t *d_k, uint8_t *d_ok,
                                 cudaStream_t st);
@@ -266,8 +268,6 @@ int sbv_launch_mix_ok(sbv_engine *e, const MixBufs &b, size_t n, const uint32_t 
 
 // shape of the table of B (ed25519_verify.cuh: ED_BWINS x ED_BENT entries of ED_BWORDS words; checked in inst_ed25519.cu)
 constexpr size_t SBV_ED_BTAB_ENTRIES = 32 * 128, SBV_ED_BTAB_ENTRY_WORDS = 24;
-// entries of a per-launch comb table (ed25519_comb.cuh: 2 blocks x 255 entries of 24 words; checked in inst_ed25519.cu)
-constexpr size_t SBV_ED_COMB_ENTRIES = 2 * 255;
 
 // ---- engine.cu helpers shared with the other translation units ----
 int sbv_lane_acquire(sbv_engine *e);            // blocks until a lane index is free; returns it

@@ -1,5 +1,6 @@
 // inst_ed25519.cu — launchers of the Ed25519 kernels (sha512.cuh, ed25519_verify.cuh, ed25519_keyed.cuh,
-// ed25519_comb.cuh) behind engine.h, and the registry of registered Ed25519 keys.
+// ed25519_comb.cuh) behind engine.h, the Ed25519 entry of the grouping table (ops.h: GroupOps), and the registry of
+// registered Ed25519 keys.
 #include <vector>
 
 #include "engine.h"
@@ -39,7 +40,7 @@ int sbv_ed_btab_ensure(sbv_engine *e, Dev &d) {
 }
 
 // ---- keys per item ----
-// A keys-per-item launch (pipeline.cu draws the same for ECDSA):
+// A keys-per-item launch: the first half is sbv_launch_verify_begin (pipeline.cu) over the grouping table below, then
 //
 //   st     memsets  k_kg_insert  k_kg_assign ─┬─ k_kg_route  length sort  k_ed_sha512 ─┬──────────── (wait tables) k_ed_verify_comb ─ (wait generic) ─ done
 //   s_tab                                     └─ k_edc_bases  k_edc_fill  k_edc_inv  k_edc_final ──┘
@@ -47,74 +48,63 @@ int sbv_ed_btab_ensure(sbv_engine *e, Dev &d) {
 //
 // Keys whose 32 bytes occur at least group_threshold times get a comb table (ed25519_comb.cuh) and their items take
 // k_ed_verify_comb; the table construction (latency-bound: one doubling chain per key) runs beside SHA-512.  With a key
-// cache reserved, k_kc_lookup runs after k_kg_assign and k_kc_insert after k_edc_final, as in pipeline.cu.
+// cache reserved, k_kc_lookup runs after k_kg_assign and k_kc_insert after k_edc_final, as for ECDSA.
 namespace {
 constexpr KtGeom ED_COMB_GEOM{EDC_BASES_WORDS, EDC_HS_WORDS, EDC_ZTOP_WORDS, EDC_TAB_WORDS};
-static_assert(SBV_ED_COMB_ENTRIES * SBV_ED_BTAB_ENTRY_WORDS == EDC_TAB_WORDS, "engine.h: comb table");
+static_assert(EDC_TAB_WORDS == 2 * 255 * SBV_ED_BTAB_ENTRY_WORDS, "debug.cu: sbv_debug_ed25519_comb_tab's table of 510 entries");
 
-// table slots of a launch of n items at threshold T, as the ECDSA launches count them; 0: the launch does not group
-size_t ed_group_cap(const sbv_engine *e, size_t n, uint32_t T) {
-    if (T == 0 || n < T || n < (size_t)e->group_min_batch || e->group_max_keys <= 0) return 0;
-    size_t kcap = n / T;
-    if (kcap > (size_t)e->group_max_keys) kcap = (size_t)e->group_max_keys;
-    return kcap ? kcap : 1;
+// The GroupOps of Ed25519: the key is (pub, nullptr).
+cudaError_t edg_group(uint32_t n, const uint8_t *pub, const uint8_t *, uint32_t seed, uint32_t hmask, uint32_t *htab, uint32_t *rep, uint32_t *kcnt,
+                      uint32_t threshold, uint32_t max_keys, int32_t *keyid, uint32_t *keylist, uint32_t *counters, cudaStream_t st) {
+    const unsigned blocks = (n + 255) / 256;
+    k_kg_insert<<<blocks, 256, 0, st>>>(n, KgKey32{pub}, seed, hmask, htab, rep, kcnt);
+    k_kg_assign<<<blocks, 256, 0, st>>>(n, rep, kcnt, threshold, max_keys, keyid, keylist, counters);
+    return cudaGetLastError();
 }
 
-// On st: the grouping of the n keys of d_pub (at most kcap of them with >= T items get a table slot) and the routing onto
-// w->klist / w->glist (counts at zeroed[1] / zeroed[2]); on w->s_tab: the comb tables, then w->ev_tab.
-int ed_group(sbv_engine *e, Dev &d, Dev::Scratch *w, size_t n, const uint8_t *d_pub, uint32_t T, size_t kcap, cudaStream_t st) {
-    const uint32_t nn = (uint32_t)n, cap = (uint32_t)kcap, blocks = (nn + 255) / 256;
-    uint32_t *counters = w->zeroed, *kcnt = w->zeroed + 4;
-    CU(e, cudaMemsetAsync(w->htab, 0xff, (size_t)w->hsize * 4, st));
-    CU(e, cudaMemsetAsync(w->zeroed, 0, (n + 4) * 4, st));
-    k_kg_insert<<<blocks, 256, 0, st>>>(nn, KgKey32{d_pub}, e->hash_seed, w->hsize - 1, w->htab, w->rep, kcnt);
-    k_kg_assign<<<blocks, 256, 0, st>>>(nn, w->rep, kcnt, T, cap, w->keyid, w->keylist, counters);
-    CU(e, cudaGetLastError());
-    // with a key cache: the lookup renumbers the keys (misses first), copies the hits' tables, and the build makes the misses
-    const Dev::KeyCache &kc = d.kc[SBV_ED25519];
-    uint32_t *lk = sbv_key_cache_area(d, SBV_ED25519, w, kcap);
-    const unsigned wb = (unsigned)(((size_t)cap * 32 + 127) / 128);
-    if (lk) {
-        CU(e, cudaMemsetAsync(lk, 0, 8, st));
-        k_kc_lookup<<<wb, 128, 0, st>>>(counters, cap, w->keylist, KcKey32{d_pub}, kc.map, (uint32_t)kc.tw4, w->keyid, lk, w->keyflags,
-                                        reinterpret_cast<uint4 *>((uint32_t *)w->ktab));
-        CU(e, cudaGetLastError());
-    }
-    CU(e, cudaEventRecord(w->ev_group, st));
-    CU(e, cudaStreamWaitEvent(w->s_tab, w->ev_group, 0));
+cudaError_t edg_build(const uint32_t *nk, uint32_t cap, const uint32_t *kl, const uint8_t *pub, const uint8_t *, uint32_t *bases, uint32_t *hs,
+                      uint32_t *ztop, uint32_t *pref, uint32_t *ktab, uint8_t *keyflags, cudaStream_t st) {
     const unsigned kb = (cap + 63) / 64, cb = (unsigned)(((size_t)cap * EDC_NCHAIN + 63) / 64);
-    const uint32_t *nk = lk ? lk : counters, *kl = lk ? lk + 2 : (const uint32_t *)w->keylist;
-    k_edc_bases<<<kb, 64, 0, w->s_tab>>>(nk, cap, kl, d_pub, w->bases, w->keyflags);
-    k_edc_fill<<<cb, 64, 0, w->s_tab>>>(nk, cap, w->bases, w->keyflags, w->hs, w->ztop, w->ktab);
-    k_edc_inv<<<kb, 64, 0, w->s_tab>>>(nk, cap, w->keyflags, w->ztop, w->pref);
-    k_edc_final<<<cb, 64, 0, w->s_tab>>>(nk, cap, w->keyflags, w->hs, w->ztop, w->ktab);
-    if (lk)
-        k_kc_insert<<<wb, 128, 0, w->s_tab>>>(cap, lk, KcKey32{d_pub}, kc.map, (uint32_t)kc.tw4, w->keyflags,
-                                              reinterpret_cast<const uint4 *>((uint32_t *)w->ktab));
-    CU(e, cudaGetLastError());
-    CU(e, cudaEventRecord(w->ev_tab, w->s_tab));
-    k_kg_route<<<blocks, 256, 0, st>>>(nn, w->rep, w->keyid, w->item_kid, w->klist, w->glist, counters);
-    e->launches += 7 + (lk ? 2 : 0);
+    k_edc_bases<<<kb, 64, 0, st>>>(nk, cap, kl, pub, bases, keyflags);
+    k_edc_fill<<<cb, 64, 0, st>>>(nk, cap, bases, keyflags, hs, ztop, ktab);
+    k_edc_inv<<<kb, 64, 0, st>>>(nk, cap, keyflags, ztop, pref);
+    k_edc_final<<<cb, 64, 0, st>>>(nk, cap, keyflags, hs, ztop, ktab);
+    return cudaGetLastError();
+}
+
+cudaError_t edg_cache_lookup(const uint32_t *nkeys_ptr, uint32_t kcap, const uint32_t *keylist, const uint8_t *pub, const uint8_t *, KcMap c, uint32_t tw4,
+                             int32_t *keyid, uint32_t *lk, uint8_t *keyflags, uint32_t *ktab, cudaStream_t st) {
+    k_kc_lookup<<<(unsigned)(((size_t)kcap * 32 + 127) / 128), 128, 0, st>>>(nkeys_ptr, kcap, keylist, KcKey32{pub}, c, tw4, keyid, lk, keyflags,
+                                                                            reinterpret_cast<uint4 *>(ktab));
+    return cudaGetLastError();
+}
+
+cudaError_t edg_cache_insert(uint32_t kcap, const uint32_t *lk, const uint8_t *pub, const uint8_t *, KcMap c, uint32_t tw4, const uint8_t *keyflags,
+                             const uint32_t *ktab, cudaStream_t st) {
+    k_kc_insert<<<(unsigned)(((size_t)kcap * 32 + 127) / 128), 128, 0, st>>>(kcap, lk, KcKey32{pub}, c, tw4, keyflags,
+                                                                            reinterpret_cast<const uint4 *>(ktab));
+    return cudaGetLastError();
+}
+
+const KtOps ED_COMB = {ED_COMB_GEOM, edg_build};
+
+// k_kg_route after the first half: the items of keys with a table onto w->klist, the rest onto w->glist (counts at
+// zeroed[1] / zeroed[2])
+int ed_route(sbv_engine *e, const VerifyLaunch &vl, cudaStream_t st) {
+    Dev::Scratch *w = vl.w;
+    k_kg_route<<<(uint32_t)((vl.n + 255) / 256), 256, 0, st>>>((uint32_t)vl.n, w->rep, w->keyid, w->item_kid, w->klist, w->glist, w->zeroed);
+    e->launches += 1;
     CU(e, cudaGetLastError());
     return 0;
 }
 
-// Hands the set back behind everything the launch enqueued on its side streams: on success and after a fault alike.
-int ed_close(sbv_engine *e, Dev::Scratch *w, cudaStream_t st, int rc) {
-    if (rc) cudaStreamWaitEvent(st, w->ev_tab, 0);  // a fault before the join: the tables may still be in flight
-    const cudaError_t a = cudaStreamWaitEvent(st, w->ev_gen, 0), b = cudaEventRecord(w->done, st);
-    if (rc) return rc;
-    CU(e, a);
-    CU(e, b);
-    return 0;
-}
-
-int ed_grouped(sbv_engine *e, Dev &d, Dev::Scratch *w, size_t n, const uint8_t *d_msgs, const uint64_t *d_off, uint64_t base, const uint8_t *d_sig,
-               const uint8_t *d_pub, uint32_t *d_k, uint32_t *d_perm, uint8_t *d_ok, uint32_t T, size_t kcap, cudaStream_t st) {
-    if (int rc = ed_group(e, d, w, n, d_pub, T, kcap, st)) return rc;
-    const uint32_t nn = (uint32_t)n, *counters = w->zeroed;
+int ed_grouped(sbv_engine *e, Dev &d, const VerifyLaunch &vl, const uint8_t *d_msgs, const uint64_t *d_off, uint64_t base, const uint8_t *d_sig,
+               const uint8_t *d_pub, uint32_t *d_k, uint32_t *d_perm, uint8_t *d_ok, cudaStream_t st) {
+    if (int rc = ed_route(e, vl, st)) return rc;
+    Dev::Scratch *w = vl.w;
+    const uint32_t nn = (uint32_t)vl.n, *counters = w->zeroed;
     const uint32_t *perm = nullptr;
-    if (int rc = sbv_launch_length_sort(e, n, d_off, d_perm, st, &perm)) return rc;
+    if (int rc = sbv_launch_length_sort(e, vl.n, d_off, d_perm, st, &perm)) return rc;
     k_ed_sha512<<<(nn + 127) / 128, 128, 0, st>>>(nn, d_sig, d_pub, d_msgs, d_off, base, d_k, perm, nullptr);
     e->launches += 1;
     CU(e, cudaGetLastError());
@@ -132,17 +122,30 @@ int ed_grouped(sbv_engine *e, Dev &d, Dev::Scratch *w, size_t n, const uint8_t *
     CU(e, cudaGetLastError());
     return 0;
 }
+
+// the comb kernel over every item (no list) with the caller's k
+int ed_comb_k(sbv_engine *e, Dev &d, const VerifyLaunch &vl, const uint8_t *d_sig, const uint32_t *d_k, uint8_t *d_ok, cudaStream_t st) {
+    if (int rc = ed_route(e, vl, st)) return rc;
+    Dev::Scratch *w = vl.w;
+    const uint32_t nn = (uint32_t)vl.n;
+    CU(e, cudaStreamWaitEvent(st, w->ev_tab, 0));
+    k_ed_verify_comb<EDC_BLOCK><<<(nn + EDC_BLOCK - 1) / EDC_BLOCK, EDC_BLOCK, 0, st>>>(
+        nn, d_sig, w->item_kid, w->keyflags, reinterpret_cast<const uint4 *>((uint32_t *)w->ktab), d_k, reinterpret_cast<const uint4 *>(d.ed_btab), d_ok,
+        nullptr, nullptr);
+    e->launches += 1;
+    CU(e, cudaGetLastError());
+    return 0;
+}
 }  // namespace
+
+const GroupOps sbv_group_ed25519 = {&ED_COMB, KcKey32::W, 4, edg_group, edg_cache_lookup, edg_cache_insert};
 
 int sbv_launch_ed25519(sbv_engine *e, Dev &d, size_t n, const uint8_t *d_msgs, const uint64_t *d_off, uint64_t base, const uint8_t *d_sig,
                        const uint8_t *d_pub, uint32_t *d_k, uint32_t *d_perm, uint8_t *d_ok, cudaStream_t st) {
-    const uint32_t T = e->group_threshold > 0 ? (uint32_t)e->group_threshold : 0;
-    const size_t kcap = ed_group_cap(e, n, T);
-    if (kcap) {
-        Dev::Scratch *w = nullptr;
-        if (int rc = sbv_take_scratch(e, d, 0, &ED_COMB_GEOM, n, kcap, st, &w)) return rc;
-        return ed_close(e, w, st, ed_grouped(e, d, w, n, d_msgs, d_off, base, d_sig, d_pub, d_k, d_perm, d_ok, T, kcap, st));
-    }
+    VerifyLaunch vl;
+    if (int rc = sbv_launch_verify_begin(e, d, SBV_ED25519, n, d_pub, nullptr, st, &vl)) return rc;
+    if (vl.grouping)
+        return sbv_launch_verify_close(e, vl, st, ed_grouped(e, d, vl, d_msgs, d_off, base, d_sig, d_pub, d_k, d_perm, d_ok, st));
     const uint32_t *perm = nullptr;
     int rc = sbv_launch_length_sort(e, n, d_off, d_perm, st, &perm);
     if (rc) return rc;
@@ -154,46 +157,12 @@ int sbv_launch_ed25519(sbv_engine *e, Dev &d, size_t n, const uint8_t *d_msgs, c
     return 0;
 }
 
-// test hook (debug.cu): the first half of a grouped launch, synchronised
-int sbv_launch_ed_comb_tables(sbv_engine *e, Dev &d, size_t n, const uint8_t *d_pub, cudaStream_t st, Dev::Scratch **out) {
-    *out = nullptr;
-    const uint32_t T = e->group_threshold > 0 ? (uint32_t)e->group_threshold : 0;
-    const size_t kcap = ed_group_cap(e, n, T);
-    if (!kcap) return 0;
-    Dev::Scratch *w = nullptr;
-    if (int rc = sbv_take_scratch(e, d, 0, &ED_COMB_GEOM, n, kcap, st, &w)) return rc;
-    int rc = ed_group(e, d, w, n, d_pub, T, kcap, st);
-    if (!rc) {
-        const cudaError_t a = cudaStreamWaitEvent(st, w->ev_tab, 0);
-        rc = a != cudaSuccess ? sbv_fail(e, SBV_ERR_CUDA, "cudaStreamWaitEvent: %s", cudaGetErrorString(a)) : 0;
-    }
-    if (!rc) {
-        const cudaError_t a = cudaStreamSynchronize(st);
-        rc = a != cudaSuccess ? sbv_fail(e, SBV_ERR_CUDA, "k_edc_*: %s", cudaGetErrorString(a)) : 0;
-    }
-    if (rc) return ed_close(e, w, st, rc);
-    *out = w;
-    return 0;
-}
-
 // test hook (debug.cu): k_ed_verify_comb with the caller's k over every item, every distinct key with a table
 int sbv_launch_ed_verify_comb_k(sbv_engine *e, Dev &d, size_t n, const uint8_t *d_sig, const uint8_t *d_pub, const uint32_t *d_k, uint8_t *d_ok,
                                 cudaStream_t st) {
-    Dev::Scratch *w = nullptr;
-    if (int rc = sbv_take_scratch(e, d, 0, &ED_COMB_GEOM, n, n, st, &w)) return rc;
-    int rc = ed_group(e, d, w, n, d_pub, 1, n, st);
-    if (!rc) {
-        const uint32_t nn = (uint32_t)n;
-        const cudaError_t a = cudaStreamWaitEvent(st, w->ev_tab, 0);
-        if (a == cudaSuccess)
-            k_ed_verify_comb<EDC_BLOCK><<<(nn + EDC_BLOCK - 1) / EDC_BLOCK, EDC_BLOCK, 0, st>>>(
-                nn, d_sig, w->item_kid, w->keyflags, reinterpret_cast<const uint4 *>((uint32_t *)w->ktab), d_k, reinterpret_cast<const uint4 *>(d.ed_btab),
-                d_ok, nullptr, nullptr);
-        e->launches += 1;
-        const cudaError_t b = a != cudaSuccess ? a : cudaGetLastError();
-        rc = b != cudaSuccess ? sbv_fail(e, SBV_ERR_CUDA, "k_ed_verify_comb: %s", cudaGetErrorString(b)) : 0;
-    }
-    return ed_close(e, w, st, rc);
+    VerifyLaunch vl;
+    if (int rc = sbv_launch_verify_begin(e, d, SBV_ED25519, n, d_pub, nullptr, st, &vl, 1, true)) return rc;
+    return sbv_launch_verify_close(e, vl, st, ed_comb_k(e, d, vl, d_sig, d_k, d_ok, st));
 }
 
 // test hook (debug.cu): the production SHA-512 kernel with its digests written out as well

@@ -1,14 +1,10 @@
 // key_cache.cu — the grouped-key cache of each device: reserve, free and statistics (sbv_key_cache_reserve /
-// sbv_key_cache_stats).  The kernels are in key_cache.cuh; pipeline.cu and inst_ed25519.cu enqueue them.
+// sbv_key_cache_stats).  The kernels are in key_cache.cuh; pipeline.cu enqueues them through the grouping table (ops.h).
 #include <cstring>
 
 #include "engine.h"
 
 namespace {
-constexpr size_t KC_KEY_WORDS[3] = {16, 24, 8};  // qx || qy of P-256, of P-384, the Ed25519 encoding
-
-size_t table_words(int s) { return s < 2 ? sbv_ops(s).grouped->geom.ktab_words : SBV_ED_COMB_ENTRIES * SBV_ED_BTAB_ENTRY_WORDS; }
-
 // One allocation: pool [cap][table words], stats [4] (u64), state [slots], pidx [slots], keys [slots][key words], then the
 // SBV_SCRATCH launch areas.  The part after the pool is zeroed: an empty map and zero counters.
 int kc_alloc(sbv_engine *e, Dev &d, int s, size_t cap) {
@@ -16,7 +12,8 @@ int kc_alloc(sbv_engine *e, Dev &d, int s, size_t cap) {
     if (cap > ((size_t)1 << 30)) return sbv_fail(e, SBV_ERR_NOMEM, "sbv_key_cache_reserve: %zu tables for scheme %d", cap, s);
     uint32_t slots = 1;
     while (slots < 2 * cap) slots <<= 1;
-    const size_t tw = table_words(s), kw = KC_KEY_WORDS[s];
+    const GroupOps &g = sbv_group_ops(s);
+    const size_t tw = g.kt->geom.ktab_words, kw = g.key_words;
     const size_t lkw = 2 + (size_t)(e->group_max_keys > 0 ? e->group_max_keys : 0);
     if (cap > SIZE_MAX / (tw * 4)) return sbv_fail(e, SBV_ERR_NOMEM, "sbv_key_cache_reserve: %zu tables for scheme %d", cap, s);
     const size_t pool = cap * tw * 4, rest = 32 + (size_t)slots * (2 + kw) * 4 + SBV_SCRATCH * lkw * 4;

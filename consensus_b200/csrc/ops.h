@@ -37,9 +37,6 @@ struct CurveOps {
     cudaError_t (*gtable_init)(uint32_t *gtab, cudaStream_t st);
     cudaError_t (*prep)(uint32_t n, const uint8_t *r, const uint8_t *s, const uint8_t *dig, uint32_t dlen, uint32_t *uw, uint8_t *flags,
                         cudaStream_t st);
-    // key grouping: insert + assign (two launches); buffers zeroed / 0xff-filled by the caller
-    cudaError_t (*group)(uint32_t n, const uint8_t *qx, const uint8_t *qy, uint32_t seed, uint32_t hmask, uint32_t *htab, uint32_t *rep,
-                         uint32_t *kcnt, uint32_t threshold, uint32_t max_keys, int32_t *keyid, uint32_t *keylist, uint32_t *counters, cudaStream_t st);
     // routing of a range of items onto the fixed-base and the generic list (launches route chunk by chunk: rep / item_kid /
     // klist / glist point at the chunk, the indices written to the lists are chunk-local, counters are the chunk's own)
     cudaError_t (*route)(uint32_t n, const uint32_t *rep, const int32_t *keyid, int32_t *item_kid, uint32_t *klist, uint32_t *glist,
@@ -51,8 +48,20 @@ struct CurveOps {
     // keys grouped inside a launch (P-256: comb tables; P-384: 5-bit window tables) / registered keys (8-bit windows)
     const GroupedKtOps *grouped;
     const RegisteredKtOps *kt8;
+};
+
+// The first half of a keys-per-item launch of one scheme (pipeline.cu: sbv_launch_verify_begin): the grouping of the
+// repeated keys, the key cache and the tables of the grouped keys.  A key comes in as (qx, qy) for ECDSA and as (the
+// 32-byte encoding, nullptr) for Ed25519.
+struct GroupOps {
+    const KtOps *kt;      // the geometry and the construction of the tables (P-256: comb; P-384: 5-bit windows; Ed25519: comb)
+    size_t key_words;     // 32-bit words of a key as the cache stores and compares it
+    int build_launches;   // kernels kt->build enqueues
+    // insert + assign (two launches); buffers zeroed / 0xff-filled by the caller
+    cudaError_t (*group)(uint32_t n, const uint8_t *qx, const uint8_t *qy, uint32_t seed, uint32_t hmask, uint32_t *htab, uint32_t *rep,
+                         uint32_t *kcnt, uint32_t threshold, uint32_t max_keys, int32_t *keyid, uint32_t *keylist, uint32_t *counters, cudaStream_t st);
     // the key cache (key_cache.cuh): k_kc_lookup after the grouping, k_kc_insert after the table construction; tw4 = 16-byte
-    // words per table of `grouped`
+    // words per table
     cudaError_t (*cache_lookup)(const uint32_t *nkeys_ptr, uint32_t kcap, const uint32_t *keylist, const uint8_t *qx, const uint8_t *qy, KcMap c,
                                 uint32_t tw4, int32_t *keyid, uint32_t *lk, uint8_t *keyflags, uint32_t *ktab, cudaStream_t st);
     cudaError_t (*cache_insert)(uint32_t kcap, const uint32_t *lk, const uint8_t *qx, const uint8_t *qy, KcMap c, uint32_t tw4, const uint8_t *keyflags,
@@ -68,3 +77,6 @@ extern const CurveOps sbv_ops_p256, sbv_ops_p384;
 extern const GroupedKtOps sbv_comb_p256, sbv_kt5_p384;
 extern const RegisteredKtOps sbv_kt8_p256, sbv_kt8_p384;
 inline const CurveOps &sbv_ops(int curve) { return curve == 0 ? sbv_ops_p256 : sbv_ops_p384; }
+extern const GroupOps sbv_group_p256, sbv_group_p384, sbv_group_ed25519;
+// by scheme tag: SBV_P256, SBV_P384, SBV_ED25519
+inline const GroupOps &sbv_group_ops(int scheme) { return scheme == 0 ? sbv_group_p256 : scheme == 1 ? sbv_group_p384 : sbv_group_ed25519; }

@@ -2,6 +2,7 @@
 //
 // Keys-per-item batch (sbv_verify_batch*, sbv_hash_verify_batch, sbv_verify_mixed):
 //
+//          ├──────────────── begin (every scheme) ─────┤
 //   st     memsets  k_kg_insert  k_kg_assign ─┬─ k_prep  k_kg_route ─┬─ k_gpart ──────────────────────────────────┬─ (wait tables) k_verify_comb ─ (wait generic) ─ done
 //   s_tab                                     └─ k_kt_bases4  k_comb_affine  k_comb_fill  k_kt_inv  k_kt_final ─┘
 //   s_gen                                                             └─ k_verify_coz (keys without a table) ──────────────────────────────────┘
@@ -13,6 +14,8 @@
 // Registered keys (sbv_set_keys) skip the grouping: their tables were built at registration.
 // With a key cache reserved (sbv_key_cache_reserve), k_kc_lookup runs after k_kg_assign on st and k_kc_insert after
 // k_kt_final on s_tab (key_cache.cuh): the build then makes only the tables the cache does not hold.
+// The first half up to the fork and the table construction is one function for P-256, P-384 and Ed25519 (verify_begin),
+// driven by the scheme's entry of the grouping table (ops.h: GroupOps); Ed25519's second half is in inst_ed25519.cu.
 #include "engine.h"
 
 namespace {
@@ -161,61 +164,66 @@ int sbv_init_gtables(sbv_engine *e, Dev &d) {
 
 // The keys-per-item pipeline in two halves, so that a host-buffer call can upload the keys first and let the grouping
 // and the table construction (the latency-bound part) run while the rest of the batch is still on its way:
-//   begin : scratch set, key grouping on st, table construction on the set's side stream   (needs qx, qy)
-//   chunk : k_prep, routing, generic kernel on the second side stream, k_gpart, fixed-base kernel, join
-//           (needs r, s, digest), once per chunk of the batch
+//   begin : scratch set, key grouping on st, table construction on the set's side stream   (needs the keys)
+//   ECDSA chunk : k_prep, routing, generic kernel on the second side stream, k_gpart, fixed-base kernel, join
+//                 (needs r, s, digest), once per chunk of the batch
+//   Ed25519 (inst_ed25519.cu) : routing, SHA-512, generic kernel on the second side stream, comb kernel, join
 namespace {
-int verify_begin(sbv_engine *e, Dev &d, uint8_t curve, size_t n, const uint8_t *d_qx, const uint8_t *d_qy, cudaStream_t st, VerifyLaunch *vl,
-                 int chunks) {
+// Table slots of a keys-per-item launch of n items; 0: the launch does not group (SBV_GROUP_THRESHOLD = 0, fewer items
+// than the threshold or than SBV_GROUP_MIN_BATCH, or SBV_GROUP_MAX_KEYS <= 0).
+size_t group_slots(const sbv_engine *e, size_t n) {
+    const size_t T = e->group_threshold > 0 ? (size_t)e->group_threshold : 0;
+    if (T == 0 || n < T || n < (size_t)e->group_min_batch || e->group_max_keys <= 0) return 0;
+    return std::min(n / T, (size_t)e->group_max_keys);
+}
+
+int verify_begin(sbv_engine *e, Dev &d, uint8_t scheme, size_t n, const uint8_t *d_qx, const uint8_t *d_qy, cudaStream_t st, VerifyLaunch *vl,
+                 int chunks, bool every_key) {
     *vl = VerifyLaunch{};
     if (n == 0) return 0;
     if (chunks < 1 || chunks > SBV_MAX_CHUNKS) return sbv_fail(e, SBV_ERR_ARG, "bad chunk count %d", chunks);
-    const CurveOps &ops = sbv_ops(curve);
-    const KtOps *kt = ops.grouped;
-    const uint32_t nn = (uint32_t)n;
-    const uint32_t T = e->group_threshold > 0 ? (uint32_t)e->group_threshold : 0;
-    const bool grouping = T > 0 && n >= T && n >= (size_t)e->group_min_batch && e->group_max_keys > 0;
-    size_t kcap = 0;
-    if (grouping) {
-        kcap = n / T;
-        if (kcap > (size_t)e->group_max_keys) kcap = (size_t)e->group_max_keys;
-        if (kcap == 0) kcap = 1;
-    }
+    const GroupOps &g = sbv_group_ops(scheme);
+    const bool ecdsa = scheme != SBV_ED25519;
+    const size_t N = ecdsa ? (size_t)sbv_ops(scheme).N : 0, kcap = every_key ? n : group_slots(e, n);
+    if (kcap == 0 && !ecdsa) return 0;  // an Ed25519 launch that does not group holds no scratch set
     Dev::Scratch *w = nullptr;
-    if (int rc = sbv_take_scratch(e, d, (size_t)ops.N, grouping ? &kt->geom : nullptr, n, kcap, st, &w)) return rc;
-    w->open = true;  // until the last chunk records the set's `done` event
-    vl->w = w; vl->curve = curve; vl->n = n; vl->grouping = grouping; vl->d_qx = d_qx; vl->d_qy = d_qy; vl->chunks = chunks;
-    vl->ev = prof_take(e, d);
-    if (cudaEvent_t *ev = prof_at(d, vl->ev)) CU(e, cudaEventRecord(ev[0], st));
-    if (!grouping) return 0;
+    if (int rc = sbv_take_scratch(e, d, N, kcap ? &g.kt->geom : nullptr, n, kcap, st, &w)) return rc;
+    w->open = true;  // until the launch records the set's `done` event
+    vl->w = w; vl->scheme = scheme; vl->n = n; vl->grouping = kcap > 0; vl->d_qx = d_qx; vl->d_qy = d_qy; vl->chunks = chunks;
+    if (ecdsa) {  // sbv_profile_read reports the ECDSA launches
+        vl->ev = prof_take(e, d);
+        if (cudaEvent_t *ev = prof_at(d, vl->ev)) CU(e, cudaEventRecord(ev[0], st));
+    }
+    if (!kcap) return 0;
+    const uint32_t T = every_key ? 1 : (uint32_t)e->group_threshold;
     uint32_t *counters = w->zeroed, *kcnt = w->zeroed + 4;
     CU(e, cudaMemsetAsync(w->htab, 0xff, (size_t)w->hsize * 4, st));
     CU(e, cudaMemsetAsync(w->zeroed, 0, (n + 4 + 4 * (size_t)chunks) * 4, st));
-    CU(e, ops.group(nn, d_qx, d_qy, e->hash_seed, w->hsize - 1, w->htab, w->rep, kcnt, T, (uint32_t)kcap, w->keyid, w->keylist, counters, st));
+    CU(e, g.group((uint32_t)n, d_qx, d_qy, e->hash_seed, w->hsize - 1, w->htab, w->rep, kcnt, T, (uint32_t)kcap, w->keyid, w->keylist, counters, st));
     // with a key cache: the lookup renumbers the keys (misses first), copies the hits' tables, and the build makes the misses
-    const Dev::KeyCache &kc = d.kc[curve];
-    uint32_t *lk = sbv_key_cache_area(d, curve, w, kcap);
+    const Dev::KeyCache &kc = d.kc[scheme];
+    uint32_t *lk = sbv_key_cache_area(d, scheme, w, kcap);
     if (lk) {
         CU(e, cudaMemsetAsync(lk, 0, 8, st));
-        CU(e, ops.cache_lookup(counters, (uint32_t)kcap, w->keylist, d_qx, d_qy, kc.map, (uint32_t)kc.tw4, w->keyid, lk, w->keyflags, w->ktab, st));
+        CU(e, g.cache_lookup(counters, (uint32_t)kcap, w->keylist, d_qx, d_qy, kc.map, (uint32_t)kc.tw4, w->keyid, lk, w->keyflags, w->ktab, st));
     }
     CU(e, cudaEventRecord(w->ev_group, st));
     CU(e, cudaStreamWaitEvent(w->s_tab, w->ev_group, 0));
-    CU(e, kt->build(lk ? lk : counters, (uint32_t)kcap, lk ? lk + 2 : w->keylist, d_qx, d_qy, w->bases, w->hs, w->ztop, w->pref, w->ktab, w->keyflags,
-                    w->s_tab));
-    if (lk) CU(e, ops.cache_insert((uint32_t)kcap, lk, d_qx, d_qy, kc.map, (uint32_t)kc.tw4, w->keyflags, w->ktab, w->s_tab));
+    CU(e, g.kt->build(lk ? lk : counters, (uint32_t)kcap, lk ? lk + 2 : w->keylist, d_qx, d_qy, w->bases, w->hs, w->ztop, w->pref, w->ktab, w->keyflags,
+                      w->s_tab));
+    if (lk) CU(e, g.cache_insert((uint32_t)kcap, lk, d_qx, d_qy, kc.map, (uint32_t)kc.tw4, w->keyflags, w->ktab, w->s_tab));
     CU(e, cudaEventRecord(w->ev_tab, w->s_tab));
-    e->launches += 2 + (curve == 0 ? 5 : 4) + (lk ? 2 : 0);  // grouping + table construction (+ cache lookup and insert)
+    e->launches += 2 + g.build_launches + (lk ? 2 : 0);  // grouping + table construction (+ cache lookup and insert)
     return 0;
 }
 }  // namespace
 
 // A fault after the scratch set was taken hands it back here, so that no caller leaves it held open.
-int sbv_launch_verify_begin(sbv_engine *e, Dev &d, uint8_t curve, size_t n, const uint8_t *d_qx, const uint8_t *d_qy, cudaStream_t st,
-                            VerifyLaunch *vl, int chunks) {
-    const int rc = verify_begin(e, d, curve, n, d_qx, d_qy, st, vl, chunks);
+int sbv_launch_verify_begin(sbv_engine *e, Dev &d, uint8_t scheme, size_t n, const uint8_t *d_qx, const uint8_t *d_qy, cudaStream_t st,
+                            VerifyLaunch *vl, int chunks, bool every_key) {
+    const int rc = verify_begin(e, d, scheme, n, d_qx, d_qy, st, vl, chunks, every_key);
     if (rc) {
-        sbv_launch_verify_abort(*vl, st);
+        sbv_launch_verify_close(e, *vl, st, rc);
         *vl = VerifyLaunch{};
     }
     return rc;
@@ -229,11 +237,11 @@ int sbv_launch_verify_chunk(sbv_engine *e, Dev &d, const VerifyLaunch &vl, int c
     if (vl.n == 0) return 0;
     Dev::Scratch *w = vl.w;
     if (c < 0 || c >= vl.chunks || lo + cn > vl.n) return sbv_fail(e, SBV_ERR_ARG, "bad chunk");
-    const CurveOps &ops = sbv_ops(vl.curve);
+    const CurveOps &ops = sbv_ops(vl.scheme);
     const GroupedKtOps *kt = ops.grouped;
     const size_t N = (size_t)ops.N, L = (size_t)ops.bytes;
     const uint32_t nn = (uint32_t)cn;
-    const uint32_t *gtab = d.gtab[vl.curve];
+    const uint32_t *gtab = d.gtab[vl.scheme];
     // The profile of a launch is that of its last chunk.  A chunked launch starts it again there (nothing of the first
     // half overlaps the last chunk); a launch of one chunk keeps the start of its first half, so the grouping counts as prep.
     cudaEvent_t *ev = last ? prof_at(d, vl.ev) : nullptr;
@@ -280,14 +288,18 @@ int sbv_launch_verify_chunk(sbv_engine *e, Dev &d, const VerifyLaunch &vl, int c
     return 0;
 }
 
-// A fault between the halves: the set goes back, but only behind whatever the first half left running on its side stream.
-void sbv_launch_verify_abort(const VerifyLaunch &vl, cudaStream_t st) {
+// On success and after a fault alike, the set goes back only behind everything the launch enqueued on its side streams.
+int sbv_launch_verify_close(sbv_engine *e, const VerifyLaunch &vl, cudaStream_t st, int rc) {
     Dev::Scratch *w = vl.w;
-    if (!w || !w->open) return;
-    if (vl.grouping) cudaStreamWaitEvent(st, w->ev_tab, 0);
-    cudaStreamWaitEvent(st, w->ev_gen, 0);   // a chunk's generic kernel (a never-recorded event is a no-op)
-    cudaEventRecord(w->done, st);
+    if (!w || !w->open) return rc;
+    if (rc && vl.grouping) cudaStreamWaitEvent(st, w->ev_tab, 0);
+    // the generic kernel (a never-recorded event is a no-op)
+    const cudaError_t a = cudaStreamWaitEvent(st, w->ev_gen, 0), b = cudaEventRecord(w->done, st);
     w->open = false;
+    if (rc) return rc;
+    CU(e, a);
+    CU(e, b);
+    return 0;
 }
 
 int sbv_launch_verify(sbv_engine *e, Dev &d, uint8_t curve, size_t n, const uint8_t *d_r, const uint8_t *d_s, const uint8_t *d_qx,

@@ -1,8 +1,8 @@
 """Ed25519 keys grouped inside a keys-per-item launch (sbv_ed25519_verify_batch) on the device: engines at
 SBV_GROUP_THRESHOLD = 0, 1, 2 and 16 give verdicts byte-identical to OpenSSL and to each other on every corpus shape;
 the comb tables (sbv_debug_ed25519_comb_tab) and the comb kernel with crafted k (sbv_debug_ed25519_verify_comb_k) equal
-the CPU simulation's; which keys get a table; pinned and pageable input, concurrent callers, the fault convention and a
-two-device engine.  tests/test_hostsim_ed25519_grouped.py runs the same sets on the CPU simulation."""
+the CPU simulation's; which keys get a table; the kernel launches of each call; pinned and pageable input, concurrent
+callers, the fault convention and a two-device engine.  tests/test_hostsim_ed25519_grouped.py runs the same sets on the CPU simulation."""
 import ctypes as C
 import os
 import subprocess
@@ -13,6 +13,7 @@ import pytest
 
 import ed25519_edges as edges
 import ed25519_grouped as grp
+import launch_counts as lc
 import oracle_ed25519 as oe
 from oracle_ed25519 import corpus, ref
 from test_gpu_round2 import _engine
@@ -30,6 +31,9 @@ def _p(a):
 @pytest.fixture(scope="module")
 def engines():
     es = {T: _engine(SBV_GROUP_THRESHOLD=T) for T in THRESHOLDS}
+    c = corpus.make_corpus(64, seed=499, n_keys=2, crafted_max=0)
+    for T, e in es.items():  # the first Ed25519 call of a device also builds the table of B (k_ed_btab_init)
+        assert _launches(e, c)[1] == lc.ed25519(64, {"SBV_GROUP_THRESHOLD": T}) + 1, T
     yield es
     for e in es.values():
         e.close()
@@ -44,12 +48,20 @@ def hs(tmp_path_factory):
     return C.CDLL(out)
 
 
+def _launches(e, c):
+    """The verdicts of c, and the kernels the call launched."""
+    before = e.kernel_launches
+    got = e.ed25519_verify_batch(c["msgs"], c["off"], c["sig"], c["pub"])
+    return got, e.kernel_launches - before
+
+
 def _all_equal(engines, c, want=None):
     if want is None:
         want = oe.verify_batch(c["msgs"], c["off"], c["sig"], c["pub"])
     for T, e in engines.items():
-        got = e.ed25519_verify_batch(c["msgs"], c["off"], c["sig"], c["pub"])
+        got, k = _launches(e, c)
         assert np.array_equal(got, want), (T, np.nonzero(got != want)[0][:10])
+        assert k == lc.ed25519(len(c["sig"]), {"SBV_GROUP_THRESHOLD": T}), (T, k)
     return want
 
 
@@ -179,7 +191,9 @@ def test_max_keys_overflow_goes_generic():
     want = oe.verify_batch(c["msgs"], c["off"], c["sig"], c["pub"])
     e = _engine(SBV_GROUP_THRESHOLD=16, SBV_GROUP_MAX_KEYS=4)
     try:
-        assert np.array_equal(e.ed25519_verify_batch(c["msgs"], c["off"], c["sig"], c["pub"]), want)
+        got, k = _launches(e, c)
+        assert np.array_equal(got, want)
+        assert k == lc.ed25519(8192, {"SBV_GROUP_MAX_KEYS": 4}) + 1  # + k_ed_btab_init
         uniq, first, cnt = np.unique(c["pub"], axis=0, return_index=True, return_counts=True)
         items = first[cnt >= 16]
         assert items.size > 4

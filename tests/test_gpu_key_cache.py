@@ -3,7 +3,8 @@ sbv_mixed_verify_batch, a cold call (inserts) and a warm call (hits) give verdic
 and to OpenSSL, on corpora with flipped messages, r or s = 0 and = n, S >= L, an off-curve key and an undecodable Ed25519
 key repeated past the threshold, and the y >= p and "-0" encodings of one point.  The statistics count the grouped valid
 keys; a cached table equals the table a fresh launch builds; a full cache, a chunked engine, _device calls on a caller
-stream, six concurrent callers, re-reserving, freeing, argument faults and a two-device engine."""
+stream, six concurrent callers, re-reserving, freeing, argument faults and a two-device engine; the kernel launches of
+each call, with and without a cache, grouped or not, chunked or not (tests/launch_counts.py)."""
 import ctypes as C
 import os
 import threading
@@ -13,6 +14,7 @@ import pytest
 
 import ecdsa_keys as ek
 import ed25519_edges as edges
+import launch_counts as lc
 import mixed_keys_cases as mk
 import oracle
 from oracle.ecdsa_ref import CURVES
@@ -105,6 +107,26 @@ def _run(eng, cp, call):
     return _family(eng, cp, {"p256": P256, "p384": P384, "ed": ED}[call])
 
 
+def _counted(eng, cp, call):
+    """_run, and the kernels it launched."""
+    before = eng.kernel_launches
+    idx, ok = _run(eng, cp, call)
+    return idx, ok, eng.kernel_launches - before
+
+
+def _want_launches(cp, call, cached=(), env=None):
+    n = [int((cp["scheme"] == c).sum()) for c in (P256, P384, ED)]
+    if call == "mixed":
+        return lc.mixed(n, env, cached)
+    if call == "ed":
+        return lc.ed25519(n[ED], env, cached)
+    c = P384 if call == "p384" else P256
+    return lc.ecdsa(c, n[c], call != "p256_digest", env, cached)
+
+
+ALL = (P256, P384, ED)
+
+
 def _schemes(call):
     return {"mixed": (P256, P384, ED), "p256": (P256,), "p256_digest": (P256,), "p384": (P384,), "ed": (ED,)}[call]
 
@@ -153,18 +175,21 @@ def test_cold_and_warm_calls(plain, cp, grouped, call):
     idx, base = _run(plain, cp, call)
     _check(base, cp, idx, "uncached")
     assert 0 < base.sum() < base.size
+    assert _counted(plain, cp, call)[2] == _want_launches(cp, call)
     eng = _engine()
     try:
         eng.key_cache_reserve(64, 64, 64)
-        _, cold = _run(eng, cp, call)
+        _, cold, k = _counted(eng, cp, call)
         _check(cold, cp, idx, "cold")
+        assert k == _want_launches(cp, call, ALL) + (ED in _schemes(call))  # + k_ed_btab_init: the engine's first Ed25519 call
         G = {c: len(grouped[c]) for c in _schemes(call)}
         for c in (P256, P384, ED):
             st = eng.key_cache_stats(c)
             g = G.get(c, 0)
             assert st == {"capacity": 64, "resident": g, "hits": 0, "misses": g}, (c, st)
-        _, warm = _run(eng, cp, call)
+        _, warm, k = _counted(eng, cp, call)
         _check(warm, cp, idx, "warm")
+        assert k == _want_launches(cp, call, ALL)
         for c, g in G.items():
             assert eng.key_cache_stats(c) == {"capacity": 64, "resident": g, "hits": g, "misses": g}, c
             for key, table in grouped[c].items():
@@ -205,13 +230,19 @@ def test_full_cache(cp, grouped):
 
 
 def test_chunked_engine(cp, grouped):
-    eng = _engine({"SBV_CHUNK_ITEMS": 256})
+    env = {"SBV_CHUNK_ITEMS": 256}
+    eng = _engine(env)
     try:
+        for call in ("p256", "p256_digest", "p384", "mixed"):
+            idx, got, k = _counted(eng, cp, call)
+            _check(got, cp, idx, call)
+            assert k == _want_launches(cp, call, (), env) + (call == "mixed"), call  # + k_ed_btab_init
         eng.key_cache_reserve(64, 64, 64)
         for call in ("p256", "p384", "mixed"):
             for _ in range(2):
-                idx, got = _run(eng, cp, call)
+                idx, got, k = _counted(eng, cp, call)
                 _check(got, cp, idx, call)
+                assert k == _want_launches(cp, call, ALL, env), call
         assert eng.key_cache_stats(P256)["resident"] == len(grouped[P256])
         assert eng.key_cache_stats(P384)["hits"] == 3 * len(grouped[P384])
     finally:
@@ -281,8 +312,9 @@ def test_reserve_again_empties_and_zero_frees(plain, cp, grouped):
             return e.kernel_launches - before
 
         uncached = launches(plain)
+        assert uncached == _want_launches(cp, "p256")
         eng.key_cache_reserve(64, 64, 64)
-        assert launches(eng) == uncached + 2  # k_kc_lookup and k_kc_insert
+        assert launches(eng) == uncached + 2 == _want_launches(cp, "p256", ALL)  # k_kc_lookup and k_kc_insert
         g = len(grouped[P256])
         assert eng.key_cache_stats(P256)["resident"] == g
         eng.key_cache_reserve(64, 64, 64)
@@ -295,6 +327,23 @@ def test_reserve_again_empties_and_zero_frees(plain, cp, grouped):
             assert eng.key_cache_stats(c) == {"capacity": 0, "resident": 0, "hits": 0, "misses": 0}
         idx, got = _run(eng, cp, "mixed")
         _check(got, cp, idx, "freed")
+    finally:
+        eng.close()
+
+
+@pytest.mark.parametrize("env", [{"SBV_GROUP_THRESHOLD": 0}, {"SBV_GROUP_THRESHOLD": 0, "SBV_CHUNK_ITEMS": 256}], ids=["one-chunk", "chunked"])
+def test_a_launch_that_does_not_group_never_reads_the_cache(cp, env):
+    eng = _engine(env)
+    try:
+        for reserve in ((0, 0, 0), (64, 64, 64)):
+            eng.key_cache_reserve(*reserve)
+            for call in ("p256", "p256_digest", "p384", "ed", "mixed"):
+                idx, got, k = _counted(eng, cp, call)
+                _check(got, cp, idx, call)
+                first_ed = call == "ed" and reserve == (0, 0, 0)  # + k_ed_btab_init
+                assert k == _want_launches(cp, call, ALL if reserve[0] else (), env) + first_ed, (reserve, call)
+            for c in ALL:
+                assert eng.key_cache_stats(c) == {"capacity": reserve[c], "resident": 0, "hits": 0, "misses": 0}
     finally:
         eng.close()
 

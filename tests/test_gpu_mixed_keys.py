@@ -8,6 +8,7 @@ import threading
 import numpy as np
 import pytest
 
+import launch_counts as lc
 import mixed_keys_cases as mk
 
 pytestmark = pytest.mark.gpu
@@ -106,18 +107,31 @@ def test_keys_repeating_around_the_threshold(eng):
     _check(eng, cp)
 
 
-@pytest.mark.parametrize("env", [{"SBV_GROUP_THRESHOLD": 0}, {"SBV_GROUP_MAX_KEYS": 3}, {"SBV_GROUP_THRESHOLD": 2, "SBV_GROUP_MAX_KEYS": 5}],
-                         ids=["no-grouping", "max-keys-3", "threshold-2-max-keys-5"])
+def _launches(e, fn, cp):
+    """fn(e, cp), and the kernels it launched."""
+    before = e.kernel_launches
+    got = fn(e, cp)
+    return got, e.kernel_launches - before
+
+
+@pytest.mark.parametrize("env", [{"SBV_GROUP_THRESHOLD": 0}, {"SBV_GROUP_MAX_KEYS": 3}, {"SBV_GROUP_THRESHOLD": 2, "SBV_GROUP_MAX_KEYS": 5},
+                                 {"SBV_CHUNK_ITEMS": 256}, {"SBV_GROUP_THRESHOLD": 0, "SBV_CHUNK_ITEMS": 256}],
+                         ids=["no-grouping", "max-keys-3", "threshold-2-max-keys-5", "chunked", "no-grouping-chunked"])
 def test_other_grouping_settings_give_identical_verdicts(eng, pools, env):
     rng = np.random.default_rng(7)
     tag = mk.tag_pattern("runs", 2400, rng)
     key_idx = _repeats(tag, [40] * 10, rng) % 24  # ten keys repeated in every family: more than the tables of max-keys-3 / -5
     cp = mk.make_corpus(tag, pools, seed=8, hi=80, corrupt=0.3, key_idx=key_idx)
     want = _check(eng, cp)
+    n = [int((tag == c).sum()) for c in (mk.P256, mk.P384, mk.ED)]
     e2 = _engine(env)
     try:
-        assert np.array_equal(_mixed(e2, cp), want)
-        assert np.array_equal(_single(e2, cp), want)
+        got, k = _launches(e2, _mixed, cp)
+        assert np.array_equal(got, want)
+        assert k == lc.mixed(n, env) + 1  # + k_ed_btab_init: the engine's first Ed25519 call
+        got, k = _launches(e2, _single, cp)
+        assert np.array_equal(got, want)
+        assert k == lc.ecdsa(mk.P256, n[0], env=env) + lc.ecdsa(mk.P384, n[1], env=env) + lc.ed25519(n[2], env)
     finally:
         e2.close()
 

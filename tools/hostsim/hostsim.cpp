@@ -480,8 +480,8 @@ extern "C" int hs_ed25519_verify_registered_k(size_t n, const uint32_t *key_slot
 }
 
 // ---- Ed25519 keys grouped inside a keys-per-item launch (ed25519_comb.cuh) ----
-// The first half of a grouped launch as ed_group (inst_ed25519.cu) enqueues it: k_kg_insert over the 32 key bytes,
-// k_kg_assign (threshold T, kcap table slots), the four comb construction kernels, k_kg_route.
+// The first half of a grouped launch as sbv_launch_verify_begin (pipeline.cu) enqueues it for Ed25519: k_kg_insert over
+// the 32 key bytes, k_kg_assign (threshold T, kcap table slots), the four comb construction kernels; then k_kg_route.
 struct EdGroup {
     std::vector<uint32_t> rep, keylist, klist, glist, counters, ctab;
     std::vector<int32_t> keyid, item_kid;
@@ -506,7 +506,7 @@ static void ed_group_host(uint32_t n, const uint8_t *pub, uint32_t T, uint32_t k
     run_grid(cb, 64, [&] { k_edc_final(cnt, cap, g.kflags.data(), hs.data(), ztop.data(), g.ctab.data()); });
     run_grid((n + 255) / 256, 256, [&] { k_kg_route(n, g.rep.data(), g.keyid.data(), g.item_kid.data(), g.klist.data(), g.glist.data(), cnt); });
 }
-// table slots of a launch of n items, as ed_group_cap (inst_ed25519.cu) counts them with no minimum batch; 0: no grouping
+// table slots of a launch of n items, as group_slots (pipeline.cu) counts them with no minimum batch; 0: no grouping
 static uint32_t ed_group_cap_host(uint32_t n, uint32_t T, uint32_t max_keys) {
     if (T == 0 || n < T || max_keys == 0) return 0;
     const uint32_t k = std::min(n / T, max_keys);
