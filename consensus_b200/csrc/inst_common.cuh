@@ -11,6 +11,8 @@ template <class C> struct Cfg;
 // P-256: the fixed-base kernels run with their multiplications inlined at 6 blocks per SM (window kernel 168 registers,
 // comb kernel 150, no spills; the window kernel is equal or slightly ahead of the out-of-line build at 7 blocks, which
 // spills); the generic kernel likewise at 6 blocks (no spills) now that it only sees the keys that do not repeat.
+// COMB_INL also inlines the loops of the comb tables' build (k_kt_bases2, k_comb_fill, k_kt_final: 71, 105 and 96
+// registers, no spills; one site per multiplication of each loop).
 template <> struct Cfg<P256> {
     static constexpr int COZ_MINB = 6, GPART_MINB = 6, KT_MINB = 6, COMB_MINB = 6;
     static constexpr bool KT_INL = true, COMB_INL = true;
@@ -112,11 +114,12 @@ cudaError_t op_comb_build(const uint32_t *nkeys_ptr, uint32_t cap, const uint32_
     using CT = CombTab<C>;
     const unsigned kb = (cap + 63) / 64;
     const unsigned cb = (unsigned)(((size_t)cap * CT::NCHAIN + 63) / 64);
-    k_kt_bases4<C, CT><<<(unsigned)(((size_t)cap * 4 + 127) / 128), 128, 0, st>>>(nkeys_ptr, cap, keylist, qx, qy, bases, keyflags);
+    constexpr bool INL = Cfg<C>::COMB_INL;
+    k_kt_bases2<C, CT, INL><<<(unsigned)(((size_t)cap * 2 + 127) / 128), 128, 0, st>>>(nkeys_ptr, cap, keylist, qx, qy, bases, keyflags);
     k_comb_affine<C><<<kb, 64, 0, st>>>(nkeys_ptr, cap, keyflags, bases, pref);
-    k_comb_fill<C><<<cb, 64, 0, st>>>(nkeys_ptr, cap, bases, keyflags, hs, ztop, ktab);
+    k_comb_fill<C, INL><<<cb, 64, 0, st>>>(nkeys_ptr, cap, bases, keyflags, hs, ztop, ktab);
     k_kt_inv<C, CT><<<kb, 64, 0, st>>>(nkeys_ptr, cap, keyflags, ztop, pref);
-    k_kt_final<C, CT><<<cb, 64, 0, st>>>(nkeys_ptr, cap, bases, keyflags, hs, ztop, ktab);
+    k_kt_final<C, CT, INL><<<cb, 64, 0, st>>>(nkeys_ptr, cap, bases, keyflags, hs, ztop, ktab);
     return cudaGetLastError();
 }
 

@@ -10,9 +10,9 @@
 //                 full-key compare on collision): rep[i] = first item with the same key; warp-aggregated count
 //   k_kg_assign   representatives whose key occurs >= T times (and while table slots last) get a dense key id
 //   k_kg_route    items are appended to the fixed-base list (their key has a table) or to the generic list
-//   k_kt_bases4   four lanes per key: validate the key, the bases B_i = 2^(STEP*i) * Q of its table — a chain of
-//                 doublings whose independent multiplications run on different lanes (k_kt_bases, one thread per key,
-//                 is its reference in the CPU simulation)
+//   k_kt_bases4   four lanes per key (window tables) / k_kt_bases2 two lanes per key (comb): validate the key, the
+//                 bases B_i = 2^(STEP*i) * Q of its table — a chain of doublings whose independent multiplications run
+//                 on different lanes (k_kt_bases, one thread per key, is their reference in the CPU simulation)
 //   k_comb_affine one thread per key (comb): the 16 bases to affine with one inversion
 //   k_comb_fill   one thread per (key, chain) (comb): the 16 entries of a chain, one mixed addition per Gray-code step
 //   k_kt_fill     one thread per (key, window) (window table): e*B_w for e = 1..2^(W-1) with co-Z additions (5M+2S
@@ -24,6 +24,9 @@
 // Keys grouped inside a launch get a comb table (CombTab, kernels.cuh), read by k_verify_comb: P-256: 240 doublings +
 // 512 mixed additions (~11 multiplications) + 512 conversions (~6) + two inversions per key ~ 3.5 generic verifications;
 // a comb verification (15 doublings + 32 additions + the u1*G half) is ~5x cheaper than a generic one, so T = 16 pays.
+// In issued warp instructions (sm_90a SASS) a P-256 comb table costs ~16 K in the doubling chain (1,037 per doubling
+// for 16 keys), ~35 K in k_comb_fill (2,167 per mixed addition, inlined) and ~15 K in k_kt_final (911 per entry,
+// inlined), against ~275 K for the 64 verifications of a key in k_verify_comb and k_gpart.
 // Registered keys (sbv_set_keys) get a window table (KeyTab, W = 8), read by k_verify_kt: built once per key set, so
 // its verifications are the ones to make cheapest — no doublings at all.
 #pragma once
@@ -286,6 +289,120 @@ __global__ void __launch_bounds__(128) k_kt_bases4(const uint32_t *__restrict__ 
     }
 }
 
+// k_kt_bases2 — the same chain with TWO LANES PER KEY (the comb tables' builder): the eight multiplications of a doubling
+// are two per level, so both lanes work at every level and the dependent length stays four:
+//   level 1   lane 0: delta = Z^2                 lane 1: bb = (2Y)^2
+//   level 2   lane 0: (X-delta)*(X+delta)         lane 1: beta4 = X*bb
+//   level 3   lane 0: alpha^2                     lane 1: bb^2 (8Y^4 = half of it)
+//   level 4   lane 0: alpha*(beta4 - X3)          lane 1: Z3 = (2Y)*Z
+// with three 8-word pair exchanges per doubling (beta4 to lane 0; 8Y^4 and X3 crossing; Z3 and Y3 crossing).  Against
+// k_kt_bases4 a warp carries 16 keys instead of 8 and both levels 1 and 3 are squarings, so a key costs about half the
+// issued instructions for the same dependent chain.  Lane 0 holds (X, Y, Z) after every doubling and stores the bases.
+template <class C, class KT, bool INL>
+__global__ void __launch_bounds__(128) k_kt_bases2(const uint32_t *__restrict__ nkeys_ptr, uint32_t cap, const uint32_t *__restrict__ keylist,
+                                                   const uint8_t *__restrict__ qx_be, const uint8_t *__restrict__ qy_be,
+                                                   uint32_t *__restrict__ bases, uint8_t *__restrict__ keyflags) {
+    using A = typename PickArith<C, INL>::type;  // arithmetic policy of the doubling loop
+    constexpr int N = C::N;
+    const uint32_t gt = blockIdx.x * blockDim.x + threadIdx.x;
+    const uint32_t k = gt >> 1, role = gt & 1;
+    uint32_t nkeys = __ldg(nkeys_ptr);
+    if (nkeys > cap) nkeys = cap;
+    if (k >= nkeys) return;  // a pair leaves together
+    const unsigned pbase = (threadIdx.x & 31) & ~1u, pmask = 3u << pbase, other = pbase + (role ^ 1);
+    const uint32_t item = keylist ? keylist[k] : k;
+    uint32_t X[N], Y[N], Z[N];
+    const bool good = load_key<C>(X, Y, qx_be, qy_be, item);  // the two lanes agree
+    if (role == 0) keyflags[k] = good ? 1 : 0;
+    if (!good) return;
+    C::get_one(Z);
+    // v <- the other lane's v
+    auto xchg = [&](uint32_t (&v)[N]) {
+#pragma unroll
+        for (int i = 0; i < N; i++) v[i] = __shfl_sync(pmask, v[i], other);
+    };
+#pragma unroll 1
+    for (int win = 0; win < KT::NBASE; win++) {
+        if (win) {
+#pragma unroll 1
+            for (int d = 0; d < KT::STEP; d++) {
+                uint32_t s[N], a[N], b[N], r1[N], r2[N], r3[N], r4[N], t1[N], t2[N];
+                C::fadd(s, Y, Y);
+                // level 1: delta | bb
+                mp_select<N>(a, role == 1, s, Z);
+                A::fsqr(r1, a);
+                // level 2: (X-delta)(X+delta) | beta4 = X*bb
+                C::fsub(t1, X, r1);
+                C::fadd(t2, X, r1);
+                mp_select<N>(a, role == 1, X, t1);
+                mp_select<N>(b, role == 1, r1, t2);
+                A::fmul(r2, a, b);
+                uint32_t beta4[N], alpha[N];
+                mp_copy<N>(beta4, r2);
+                xchg(beta4);  // lane 0 receives beta4 (lane 1 keeps its own in r2)
+                // level 3: alpha^2 | bb^2
+                C::fadd(t1, r2, r2);
+                C::fadd(alpha, t1, r2);  // 3 (X - delta)(X + delta) on lane 0
+                mp_select<N>(a, role == 1, r1, alpha);
+                A::fsqr(r3, a);
+                // lane 0: X3 = alpha^2 - 2*beta4 ; lane 1: 8Y^4 = bb^2 / 2 ; then each takes the other's
+                uint32_t x3[N], c8[N];
+                C::fadd(t1, beta4, beta4);
+                C::fsub(t2, r3, t1);
+                C::fhalf(t1, r3);
+                mp_select<N>(x3, role == 1, t1, t2);
+                xchg(x3);  // lane 0: 8Y^4 ; lane 1: X3
+                mp_select<N>(c8, role == 1, t1, x3);
+                mp_select<N>(x3, role == 1, x3, t2);
+                // level 4: alpha*(beta4 - X3) | Z3 = 2Y*Z
+                C::fsub(t1, beta4, x3);
+                mp_select<N>(a, role == 1, s, alpha);
+                mp_select<N>(b, role == 1, Z, t1);
+                A::fmul(r4, a, b);
+                // lane 0: Y3 = r4 - 8Y^4 ; lane 1: Z3 = r4 ; then each takes the other's
+                C::fsub(t2, r4, c8);
+                mp_select<N>(t1, role == 1, r4, t2);
+                xchg(t1);  // lane 0: Z3 ; lane 1: Y3
+                mp_copy<N>(X, x3);
+                mp_select<N>(Y, role == 1, t1, t2);
+                mp_select<N>(Z, role == 1, r4, t1);
+            }
+        }
+        if (role == 0) {
+            uint32_t *o = bases + (size_t)win * 3 * N * cap + k;
+#pragma unroll
+            for (int i = 0; i < N; i++) { o[(size_t)i * cap] = X[i]; o[(size_t)(N + i) * cap] = Y[i]; o[(size_t)(2 * N + i) * cap] = Z[i]; }
+        }
+    }
+}
+
+// One table entry (x, y: 2N words, 16-byte aligned) in 16-byte accesses.  The threads of a warp work on different chains,
+// a chain's entries apart, so every access instruction touches 32 lines: 2N/4 vector accesses per entry instead of 2N
+// scalar ones cut the memory requests of the table kernels fourfold.
+template <int N>
+SBV_DEV void st_entry(uint32_t *o, const uint32_t (&x)[N], const uint32_t (&y)[N]) {
+    uint4 *v = reinterpret_cast<uint4 *>(o);
+#pragma unroll
+    for (int i = 0; i < N / 4; i++) {
+        uint4 a, b;
+        a.x = x[4 * i]; a.y = x[4 * i + 1]; a.z = x[4 * i + 2]; a.w = x[4 * i + 3];
+        b.x = y[4 * i]; b.y = y[4 * i + 1]; b.z = y[4 * i + 2]; b.w = y[4 * i + 3];
+        v[i] = a;
+        v[N / 4 + i] = b;
+    }
+}
+// plain loads (not __ldg: k_kt_final rewrites the entries it reads)
+template <int N>
+SBV_DEV void ld_entry(const uint32_t *o, uint32_t (&x)[N], uint32_t (&y)[N]) {
+    const uint4 *v = reinterpret_cast<const uint4 *>(o);
+#pragma unroll
+    for (int i = 0; i < N / 4; i++) {
+        const uint4 a = v[i], b = v[N / 4 + i];
+        x[4 * i] = a.x; x[4 * i + 1] = a.y; x[4 * i + 2] = a.z; x[4 * i + 3] = a.w;
+        y[4 * i] = b.x; y[4 * i + 1] = b.y; y[4 * i + 2] = b.z; y[4 * i + 3] = b.w;
+    }
+}
+
 // co-Z addition (Meloni): P = (X1, Y1, Z) and Q = (X2, Y2, Z) share Z.  R = P + Q -> (X3, Y3, Z3) and P is
 // re-expressed with the same Z3 = Z * (X1 - X2); h receives X1 - X2 (the ratio Z3 / Z).  5M + 2S.
 // P != +-Q is the caller's business (multiples e*B, e >= 2, of a point of prime order never meet B).
@@ -406,10 +523,12 @@ __global__ void __launch_bounds__(64) k_kt_inv(const uint32_t *__restrict__ nkey
     }
 }
 
-template <class C, class KT>
+// INL: the multiplications inlined (Inl<C>); the comb tables' build takes it, its loop has a single conversion site.
+template <class C, class KT, bool INL = false>
 __global__ void __launch_bounds__(64) k_kt_final(const uint32_t *__restrict__ nkeys_ptr, uint32_t cap, const uint32_t *__restrict__ bases,
                                                  const uint8_t *__restrict__ keyflags, const uint32_t *__restrict__ hs,
                                                  const uint32_t *__restrict__ ztop, uint32_t *__restrict__ ktab) {
+    using A = typename PickArith<C, INL>::type;  // arithmetic policy
     constexpr int N = C::N;
     const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
     uint32_t nkeys = __ldg(nkeys_ptr);
@@ -428,30 +547,26 @@ __global__ void __launch_bounds__(64) k_kt_final(const uint32_t *__restrict__ nk
     // overlap the six multiplications)
     uint32_t x[N], y[N], h[N];
     {
-        const uint32_t *oe = out + (size_t)(KT::ENT - 1) * 2 * N;
-#pragma unroll
-        for (int i = 0; i < N; i++) { x[i] = oe[i]; y[i] = oe[N + i]; }
+        ld_entry<N>(out + (size_t)(KT::ENT - 1) * 2 * N, x, y);
     }
 #pragma unroll 1
     for (int e = KT::ENT; e >= 1; e--) {
         uint32_t nx[N], ny[N], nh[N];
         if (e >= 2) {
-            const uint32_t *on = out + (size_t)(e - 2) * 2 * N;
             const uint32_t *hp = hs + ((size_t)win * (KT::ENT - 1) + (e - 2)) * N * cap + k;
+            ld_entry<N>(out + (size_t)(e - 2) * 2 * N, nx, ny);
 #pragma unroll
-            for (int i = 0; i < N; i++) { nx[i] = on[i]; ny[i] = on[N + i]; nh[i] = hp[(size_t)i * cap]; }
+            for (int i = 0; i < N; i++) nh[i] = hp[(size_t)i * cap];
         }
-        uint32_t *oe = out + (size_t)(e - 1) * 2 * N;
         uint32_t z2[N], z3[N];
-        C::fsqr(z2, zi);
-        C::fmul(z3, z2, zi);
-        C::fmul(x, x, z2);
-        C::fmul(y, y, z3);
-#pragma unroll
-        for (int i = 0; i < N; i++) { oe[i] = x[i]; oe[N + i] = y[i]; }
+        A::fsqr(z2, zi);
+        A::fmul(z3, z2, zi);
+        A::fmul(x, x, z2);
+        A::fmul(y, y, z3);
+        st_entry<N>(out + (size_t)(e - 1) * 2 * N, x, y);
         if (e >= 2) {  // 1/Z_{e-1} = (1/Z_e) * H_e
             mp_copy<N>(h, nh);
-            C::fmul(zi, zi, h);
+            A::fmul(zi, zi, h);
             mp_copy<N>(x, nx); mp_copy<N>(y, ny);
         }
     }
@@ -509,15 +624,18 @@ __global__ void __launch_bounds__(64) k_comb_affine(const uint32_t *__restrict__
 // k_kt_final needs: Jacobian X, Y of every slot in ktab, the Z ratio H of every step in hs, the last Z in ztop.
 // The chain of hi = 0 starts at infinity: its first step is a copy of P_(8b) (Z = 1, H = 1), and its slot 0 (m = 0,
 // never read) is left as (0, 0).
+// The high teeth are steps of the same loop ahead of the Gray walk, so the loop has ONE addition site and its
+// multiplications can be inlined (INL: Inl<C>) within the instruction cache.
 // No exceptional case arises: every point on a chain is s*Q with s a sum of distinct powers 2^(SPACING*c), so
 // 0 < s < 2^(15*SPACING + 1) <= 2^361 < n, and Q has prime order n.  An addition of +P_t (t not in the sum) meets the
 // accumulator only if s = 2^(SPACING*t) (impossible: distinct binary expansions) or s + 2^(SPACING*t) = n (too small);
 // an addition of -P_t (t in the sum) only if s = -2^(SPACING*t) mod n (too small) or the sum becomes empty — and a Gray
 // walk never returns to 0, while the chains with hi != 0 keep their high teeth.
-template <class C>
+template <class C, bool INL>
 __global__ void __launch_bounds__(64) k_comb_fill(const uint32_t *__restrict__ nkeys_ptr, uint32_t cap, const uint32_t *__restrict__ bases,
                                                   const uint8_t *__restrict__ keyflags, uint32_t *__restrict__ hs,
                                                   uint32_t *__restrict__ ztop, uint32_t *__restrict__ ktab) {
+    using A = typename PickArith<C, INL>::type;  // arithmetic policy of the loop
     constexpr int N = C::N;
     using CT = CombTab<C>;
     const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
@@ -534,52 +652,39 @@ __global__ void __launch_bounds__(64) k_comb_fill(const uint32_t *__restrict__ n
     };
     uint32_t *out = ktab + ((size_t)k * CT::NCHAIN + ch) * CT::ENT * 2 * N;
     auto store = [&](int slot, const uint32_t (&x)[N], const uint32_t (&y)[N], const uint32_t (&h)[N]) {
-        uint32_t *o = out + (size_t)slot * 2 * N;
-#pragma unroll
-        for (int i = 0; i < N; i++) { o[i] = x[i]; o[N + i] = y[i]; }
+        st_entry<N>(out + (size_t)slot * 2 * N, x, y);
         if (slot) {
             uint32_t *hp = hs + ((size_t)ch * (CT::ENT - 1) + (slot - 1)) * N * cap + k;
 #pragma unroll
             for (int i = 0; i < N; i++) hp[(size_t)i * cap] = h[i];
         }
     };
-    Jac<C> P;
-    uint32_t x[N], y[N], h[N];
+    Jac<A> P;
+    uint32_t x[N], y[N], h[N], zero[N];
+#pragma unroll
+    for (int i = 0; i < N; i++) zero[i] = 0;
     C::get_one(P.Z);
     C::get_one(h);
-    int first;  // first slot the Gray walk produces
-    if (hi == 0) {
-        uint32_t zero[N];
-#pragma unroll
-        for (int i = 0; i < N; i++) zero[i] = 0;
-        store(0, zero, zero, h);
-        base(CT::TEETH * b, P.X, P.Y);
-        store(1, P.X, P.Y, h);
-        first = 2;
-    } else {
-        bool empty = true;
+    if (hi == 0) store(0, zero, zero, h);
+    const int nhigh = __popc(hi);  // steps before the Gray walk
+    int rest = hi;                 // high teeth still to add
 #pragma unroll 1
-        for (int i = 0; i < 4; i++) {
-            if (!((hi >> i) & 1)) continue;
-            base(CT::TEETH * b + 4 + i, x, y);
-            if (empty) { mp_copy<N>(P.X, x); mp_copy<N>(P.Y, y); empty = false; }
-            else pt_madd_table<C>(P, x, y, h);
+    for (int st = 0; st < nhigh + CT::ENT - 1; st++) {
+        const int kk = st - nhigh + 1;  // the slot the step produces; <= 0 while the high teeth go in (0: the last of them)
+        int tooth;
+        bool sub = false;
+        if (kk <= 0) {
+            tooth = 4 + __ffs(rest) - 1;
+            rest &= rest - 1;
+        } else {
+            tooth = __ffs(kk) - 1;                        // gray(kk - 1) -> gray(kk) flips this bit
+            sub = !(((kk ^ (kk >> 1)) >> tooth) & 1);     // the bit goes off: subtract
         }
-        store(0, P.X, P.Y, h);
-        first = 1;
-    }
-#pragma unroll 1
-    for (int kk = first; kk < CT::ENT; kk++) {
-        const int tooth = __ffs(kk) - 1;                           // gray(kk - 1) -> gray(kk) flips this bit
         base(CT::TEETH * b + tooth, x, y);
-        if (!(((kk ^ (kk >> 1)) >> tooth) & 1)) {                  // the bit goes off: subtract
-            uint32_t zero[N];
-#pragma unroll
-            for (int i = 0; i < N; i++) zero[i] = 0;
-            C::fsub(y, zero, y);
-        }
-        pt_madd_table<C>(P, x, y, h);
-        store(kk, P.X, P.Y, h);
+        if (sub) C::fsub(y, zero, y);
+        if (st == 0) { mp_copy<N>(P.X, x); mp_copy<N>(P.Y, y); }  // from infinity: Z = 1, H = 1
+        else pt_madd_table<A>(P, x, y, h);
+        if (kk >= 0) store(kk, P.X, P.Y, h);
     }
     uint32_t *zp = ztop + (size_t)ch * N * cap + k;
 #pragma unroll

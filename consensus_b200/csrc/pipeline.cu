@@ -4,7 +4,7 @@
 //
 //          ├──────────────── begin (every scheme) ─────┤
 //   st     memsets  k_kg_insert  k_kg_assign ─┬─ k_prep  k_kg_route ─┬─ k_gpart ──────────────────────────────────┬─ (wait tables) k_verify_comb ─ (wait generic) ─ done
-//   s_tab                                     └─ k_kt_bases4  k_comb_affine  k_comb_fill  k_kt_inv  k_kt_final ─┘
+//   s_tab                                     └─ k_kt_bases2  k_comb_affine  k_comb_fill  k_kt_inv  k_kt_final ─┘
 //   s_gen                                                             └─ k_verify_coz (keys without a table) ──────────────────────────────────┘
 //
 // Keys that occur at least `group_threshold` times in the batch get a fixed-base table built on the spot (keygroup.cuh: a

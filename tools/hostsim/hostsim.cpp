@@ -102,25 +102,35 @@ static void run_grid_lockstep(unsigned blocks, unsigned threads, F &&body) {
 }
 
 // the product's construction kernels for a window table (KT = KeyTab) or a comb table (KT = CombTab) of up to `cap` keys,
-// *cnt of them, key k = item keylist[k] of qx / qy (keylist NULL: item k).  four != 0: the doubling chain by k_kt_bases4
-// (four lanes per key, in lockstep), else by the one-thread-per-key k_kt_bases.  ktab: KtSizes::ktab_words(cap) words of
+// *cnt of them, key k = item keylist[k] of qx / qy (keylist NULL: item k).  four == 1: the doubling chain by k_kt_bases4
+// (four lanes per key, in lockstep), four == 2: by k_kt_bases2 (two lanes per key, in lockstep; what libsbv.so runs for a
+// comb), else by the one-thread-per-key k_kt_bases.  ktab: KtSizes::ktab_words(cap) words of
 // final affine tables, kflags: cap validity flags.
+template <class C, class KT>
+static void bases_t(const uint32_t *cnt, uint32_t cap, const uint32_t *keylist, const uint8_t *qx, const uint8_t *qy, int four, uint32_t *bases,
+                    uint8_t *kflags) {
+    constexpr bool COMB = std::is_same<KT, CombTab<C>>::value;  // the comb build runs inlined multiplications, as in libsbv.so
+    if (four == 2) run_grid_lockstep((unsigned)(((size_t)cap * 2 + 127) / 128), 128, [&] { k_kt_bases2<C, KT, COMB>(cnt, cap, keylist, qx, qy, bases, kflags); });
+    else if (four) run_grid_lockstep((unsigned)(((size_t)cap * 4 + 127) / 128), 128, [&] { k_kt_bases4<C, KT>(cnt, cap, keylist, qx, qy, bases, kflags); });
+    else run_grid((cap + 63) / 64, 64, [&] { k_kt_bases<C, KT>(cnt, cap, keylist, qx, qy, bases, kflags); });
+}
+
 template <class C, class KT>
 static void build_t(const uint32_t *cnt, uint32_t cap, const uint32_t *keylist, const uint8_t *qx, const uint8_t *qy, int four, uint32_t *ktab,
                     uint8_t *kflags) {
     using KS = KtSizes<C, KT>;
     std::vector<uint32_t> bases(KS::bases_words(cap)), hs(KS::hs_words(cap)), ztop(KS::ztop_words(cap)), pref(KS::ztop_words(cap));
     const unsigned kb = (cap + 63) / 64, cb = (unsigned)(((size_t)cap * KT::NCHAIN + 63) / 64);
-    if (four) run_grid_lockstep((unsigned)(((size_t)cap * 4 + 127) / 128), 128, [&] { k_kt_bases4<C, KT>(cnt, cap, keylist, qx, qy, bases.data(), kflags); });
-    else run_grid(kb, 64, [&] { k_kt_bases<C, KT>(cnt, cap, keylist, qx, qy, bases.data(), kflags); });
-    if constexpr (std::is_same<KT, CombTab<C>>::value) {
+    constexpr bool COMB = std::is_same<KT, CombTab<C>>::value;
+    bases_t<C, KT>(cnt, cap, keylist, qx, qy, four, bases.data(), kflags);
+    if constexpr (COMB) {
         run_grid(kb, 64, [&] { k_comb_affine<C>(cnt, cap, kflags, bases.data(), pref.data()); });
-        run_grid(cb, 64, [&] { k_comb_fill<C>(cnt, cap, bases.data(), kflags, hs.data(), ztop.data(), ktab); });
+        run_grid(cb, 64, [&] { k_comb_fill<C, true>(cnt, cap, bases.data(), kflags, hs.data(), ztop.data(), ktab); });
     } else {
         run_grid(cb, 64, [&] { k_kt_fill<C, KT::STEP>(cnt, cap, bases.data(), kflags, hs.data(), ztop.data(), ktab); });
     }
     run_grid(kb, 64, [&] { k_kt_inv<C, KT>(cnt, cap, kflags, ztop.data(), pref.data()); });
-    run_grid(cb, 64, [&] { k_kt_final<C, KT>(cnt, cap, bases.data(), kflags, hs.data(), ztop.data(), ktab); });
+    run_grid(cb, 64, [&] { k_kt_final<C, KT, COMB>(cnt, cap, bases.data(), kflags, hs.data(), ztop.data(), ktab); });
 }
 
 template <class C, class KT>
@@ -146,6 +156,15 @@ extern "C" int hs_tables(int curve, int kind, size_t nkeys, const uint8_t *qx, c
     else if (kind == 2) return -1;
     else if (kind == 1) tables_t<P384, KeyTab<384, 8>>(k, qx, qy, four, ktab_out, flags_out);
     else tables_t<P384, KeyTab<384, 5>>(k, qx, qy, four, ktab_out, flags_out);
+    return 0;
+}
+
+// the Jacobian bases of P-256 comb tables for keys 0..nkeys-1, by the chain `four` selects (as in build_t), before
+// k_comb_affine: KtSizes::bases_words(nkeys) words, layout [c][3N words][nkeys]
+extern "C" int hs_comb_bases(size_t nkeys, const uint8_t *qx, const uint8_t *qy, int four, uint32_t *bases_out, uint8_t *flags_out) {
+    const uint32_t k = (uint32_t)nkeys;
+    memset(bases_out, 0, KtSizes<P256, CombTab<P256>>::bases_words(nkeys) * 4);
+    bases_t<P256, CombTab<P256>>(&k, k, nullptr, qx, qy, four, bases_out, flags_out);
     return 0;
 }
 

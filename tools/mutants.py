@@ -198,9 +198,9 @@ CATALOGUE = [
     M("k_kt_fill_last_entry", "keygroup.cuh", "for (int e = 3; e <= KT::ENT; e++) {", "for (int e = 3; e < KT::ENT; e++) {", ECDSA),
     M("k_kt_inv_prefix", "keygroup.cuh", "C::fmul(zi, inv, pv);\n        C::fmul(inv, inv, z);\n#pragma unroll\n        for (int i = 0; i < N; i++) zp[(size_t)i * cap] = zi[i];",
       "mp_copy<N>(zi, inv);\n        C::fmul(inv, inv, z);\n#pragma unroll\n        for (int i = 0; i < N; i++) zp[(size_t)i * cap] = zi[i];", ECDSA),
-    M("k_kt_final_ratio", "keygroup.cuh", "C::fmul(zi, zi, h);\n            mp_copy<N>(x, nx);", "mp_copy<N>(x, nx);", ECDSA),
-    M("k_comb_fill_no_subtract", "keygroup.cuh", "if (!(((kk ^ (kk >> 1)) >> tooth) & 1)) {", "if (false) {", ECDSA),
-    M("k_comb_fill_high_teeth", "keygroup.cuh", "base(CT::TEETH * b + 4 + i, x, y);", "base(CT::TEETH * b + 3 + i, x, y);", ECDSA),
+    M("k_kt_final_ratio", "keygroup.cuh", "A::fmul(zi, zi, h);\n            mp_copy<N>(x, nx);", "mp_copy<N>(x, nx);", ECDSA),
+    M("k_comb_fill_no_subtract", "keygroup.cuh", "sub = !(((kk ^ (kk >> 1)) >> tooth) & 1);", "sub = false;", ECDSA),
+    M("k_comb_fill_high_teeth", "keygroup.cuh", "tooth = 4 + __ffs(rest) - 1;", "tooth = 3 + __ffs(rest) - 1;", ECDSA),
     # ---------------------------------------------------------------- sha256.cuh
     M("sha256_pad_rem", "sha256.cuh", "if (rem < 4) v = (v & (0xffffffffu << (8 * (4 - rem)))) | (0x80u << (8 * (3 - rem)));\n                } else if (p == len) {",
       "if (rem < 4) v = (v & (0xffffffffu << (8 * (4 - rem))));\n                } else if (p == len) {", ECDSA),
