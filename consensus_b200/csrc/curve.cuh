@@ -470,6 +470,28 @@ SBV_DEV bool pt_add_m(Jac<C> &P, const uint32_t (&x2)[C::N], const uint32_t (&y2
     }
     return false;
 }
+// P = the affine point (x, y_in), negated if `neg`, or the point at infinity (1, 1, 0) if `skip`: bit for bit what
+// pt_add_m<C, 1> makes of the accumulators' starting value (1, 1, 0) and that point.  A pass whose accumulator starts at
+// infinity loads its first entry with this instead of spending a complete addition on it.
+template <class C>
+SBV_DEV void pt_seed(Jac<C> &P, const uint32_t (&x)[C::N], const uint32_t (&y_in)[C::N], bool neg, bool skip) {
+    constexpr int N = C::N;
+    uint32_t y[N], zero[N], one[N];
+#pragma unroll
+    for (int i = 0; i < N; i++) zero[i] = 0;
+    {
+        uint32_t ny[N];
+        C::fsub(ny, zero, y_in);
+        mp_select<N>(y, neg, ny, y_in);
+    }
+    C::get_one(one);
+#pragma unroll
+    for (int i = 0; i < N; i++) {
+        P.X[i] = skip ? one[i] : x[i];
+        P.Y[i] = skip ? one[i] : y[i];
+        P.Z[i] = skip ? 0u : one[i];
+    }
+}
 template <class C, bool AFFINE>
 SBV_DEV void pt_add(Jac<C> &P, const uint32_t (&x2)[C::N], const uint32_t (&y2)[C::N], const uint32_t (&z2)[C::N], bool neg, bool skip) {
     if (AFFINE) pt_add_m<C, 1>(P, x2, y2, z2, z2, z2, neg, skip);

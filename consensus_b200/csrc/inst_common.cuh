@@ -9,10 +9,12 @@ namespace sbv {
 // Blocks of 64 threads per SM (MINB) and inlined multiplications (INL) of each kernel, per curve.
 template <class C> struct Cfg;
 // P-256: the fixed-base kernels run with their multiplications inlined at 6 blocks per SM (window kernel 168 registers,
-// comb kernel 150, no spills; the window kernel is equal or slightly ahead of the out-of-line build at 7 blocks, which
+// comb kernel 152, no spills; the window kernel is equal or slightly ahead of the out-of-line build at 7 blocks, which
 // spills); the generic kernel likewise at 6 blocks (no spills) now that it only sees the keys that do not repeat.
 // COMB_INL also inlines the loops of the comb tables' build (k_kt_bases2, k_comb_fill, k_kt_final: 71, 105 and 96
-// registers, no spills; one site per multiplication of each loop).
+// registers, no spills; one site per multiplication of each loop).  k_gpart keeps its multiplications out of line (138
+// registers): inlined (146 registers, no spills) it ran 14 % faster alone but did not raise the pipelined throughput
+// (DESIGN.md §10).
 template <> struct Cfg<P256> {
     static constexpr int COZ_MINB = 6, GPART_MINB = 6, KT_MINB = 6, COMB_MINB = 6;
     static constexpr bool KT_INL = true, COMB_INL = true;

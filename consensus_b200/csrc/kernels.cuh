@@ -10,9 +10,10 @@
 //                        thread: on-curve check, 4-bit signed window over a common-Z table of Q (shared memory,
 //                        bank = lane, + coalesced global scratch), 256 doublings interleaved with 65 additions, 16
 //                        comb additions for u1*G with the next gather in flight, final X == r*Z^2 comparison
-//   k_gpart              u1*G alone, for the items of keys that repeat inside a batch
+//   k_gpart              u1*G alone, for the items of keys that repeat inside a batch (window 0 loaded, 15 additions)
 //   k_verify_comb        FIXED-BASE path for P-256 keys that repeat inside a batch (comb table of the key, keygroup.cuh
-//                        builds it on the fly): 32 comb additions and 15 doublings for u2*Q, then k_gpart's u1*G
+//                        builds it on the fly): 31 comb additions (the first entry is loaded) and 15 doublings for
+//                        u2*Q, then k_gpart's u1*G
 //   k_verify_kt          FIXED-BASE path over a window table: registered keys (sbv_set_keys, 8-bit windows, built once
 //                        per key set) and P-384 keys that repeat inside a batch (5-bit windows): no doublings,
 //                        NWIN(W) signed-window additions for u2*Q + the comb additions for u1*G
@@ -256,17 +257,26 @@ SBV_DEV bool load_key(uint32_t (&qxm)[C::N], uint32_t (&qym)[C::N], const uint8_
 
 // acc += u1*G from the fixed-base comb: GWINS complete points.  The next entry (a random gather from the
 // table, an L2 hit for most entries) is in flight while the current one is added.
-template <class C>
+// FROM_INF: acc is the point at infinity on entry (k_gpart): window 0's entry is loaded into it (pt_seed) instead of
+// added, and the loop adds windows 1..GWINS-1.
+template <class C, bool FROM_INF = false>
 SBV_DEV void add_u1G(Jac<C> &acc, const uint32_t *__restrict__ uw, uint32_t n, uint32_t idx, const uint4 *__restrict__ gtab) {
     constexpr int N = C::N;
     constexpr int EU4 = 2 * N / 4;
+    constexpr int W0 = FROM_INF ? 1 : 0;  // first window added
     uint32_t one[N];
     C::get_one(one);
     uint32_t gx[N], gy[N];
-    uint32_t gb = comb_digit_u1<C>(uw, n, idx, 0);
-    load_affine<C>(gx, gy, gtab + (size_t)gb * EU4);
+    uint32_t gb = comb_digit_u1<C>(uw, n, idx, W0);
+    load_affine<C>(gx, gy, gtab + (((size_t)W0 << C::GW) + gb) * EU4);
+    if constexpr (FROM_INF) {
+        uint32_t sx[N], sy[N];
+        const uint32_t sb = comb_digit_u1<C>(uw, n, idx, 0);
+        load_affine<C>(sx, sy, gtab + (size_t)sb * EU4);
+        pt_seed<C>(acc, sx, sy, false, sb == 0);
+    }
 #pragma unroll 1
-    for (int win = 0; win < C::GWINS; win++) {
+    for (int win = W0; win < C::GWINS; win++) {
         uint32_t ngx[N], ngy[N];
         uint32_t ngb = 0;
         if (win + 1 < C::GWINS) {
@@ -453,7 +463,7 @@ template <class C> struct PickArith<C, true> { using type = Inl<C>; };
 // k_gpart — the u1*G half of a fixed-base verification on its own: needs only the scalars, so the grouped pipeline runs
 // it while the per-key tables are still being built; k_verify_comb (k_verify_kt<…, REG = false>) then closes with (starts
 // from) the stored point.
-// gacc: [3N][n] words (X, Y, Z of item idx at column idx).
+// gacc: [3N][n] words (X, Y, Z of item idx at column idx).  The accumulator starts at infinity: window 0 is loaded, not added.
 template <class C, int BLOCK, int MINB>
 __global__ void __launch_bounds__(BLOCK, MINB) k_gpart(uint32_t n, const uint32_t *__restrict__ uw, const uint4 *__restrict__ gtab,
                                                         uint32_t *__restrict__ gacc) {
@@ -461,11 +471,7 @@ __global__ void __launch_bounds__(BLOCK, MINB) k_gpart(uint32_t n, const uint32_
     const uint32_t idx = blockIdx.x * BLOCK + threadIdx.x;
     if (idx >= n) return;
     Jac<C> acc;
-    C::get_one(acc.X);
-    C::get_one(acc.Y);
-#pragma unroll
-    for (int i = 0; i < N; i++) acc.Z[i] = 0;
-    add_u1G<C>(acc, uw, n, idx, gtab);
+    add_u1G<C, true>(acc, uw, n, idx, gtab);
 #pragma unroll
     for (int i = 0; i < N; i++) {
         gacc[(size_t)i * n + idx] = acc.X[i];
@@ -516,11 +522,6 @@ __global__ void __launch_bounds__(BLOCK, MINB) k_verify_kt(uint32_t n, const uin
             acc.Y[i] = __ldg(gacc + (size_t)(N + i) * n + idx);
             acc.Z[i] = __ldg(gacc + (size_t)(2 * N + i) * n + idx);
         }
-    } else {
-        mp_copy<N>(acc.X, one);
-        mp_copy<N>(acc.Y, one);
-#pragma unroll
-        for (int i = 0; i < N; i++) acc.Z[i] = 0;
     }
     // window w < NWIN: signed digit of u2 into the key's table; w >= NWIN: comb digit of u1 into the table of G
     auto fetch = [&](int w, uint32_t (&x)[N], uint32_t (&y)[N], bool &neg, bool &skip) {
@@ -539,8 +540,14 @@ __global__ void __launch_bounds__(BLOCK, MINB) k_verify_kt(uint32_t n, const uin
     uint32_t cx[N], cy[N];
     bool cneg, cskip;
     fetch(0, cx, cy, cneg, cskip);
+    int w0 = 0;  // first window added
+    if (!gacc) {  // the accumulator starts at infinity: window 0's entry is loaded, not added
+        pt_seed<A>(acc, cx, cy, cneg, cskip);
+        fetch(1, cx, cy, cneg, cskip);
+        w0 = 1;
+    }
 #pragma unroll 1
-    for (int w = 0; w < TOTAL; w++) {
+    for (int w = w0; w < TOTAL; w++) {
         uint32_t nx[N], ny[N];
         bool nneg = false, nskip = true;
         if (w + 1 < TOTAL) fetch(w + 1, nx, ny, nneg, nskip);
@@ -557,7 +564,8 @@ __global__ void __launch_bounds__(BLOCK, MINB) k_verify_kt(uint32_t n, const uin
 // addition per block; then u1*G, after the last doubling: one general addition of k_gpart's point (gacc).
 // One inlined addition site and one doubling site in one loop: the addition hands its exceptional case (accumulator ==
 // entry) to the doubling site (pt_add_m<…, DEFER>) instead of carrying its own copy of the doubling, and the next table
-// entry (a random 64-byte gather) is in flight while the current one is added.  The additions stay complete.
+// entry (a random 64-byte gather) is in flight while the current one is added.  The additions stay complete.  The first
+// step's entry is loaded into the accumulator (pt_seed), so the loop adds steps 1..KADD-1.
 template <class C, int BLOCK, int MINB, bool INL>
 __global__ void __launch_bounds__(BLOCK, MINB) k_verify_comb(uint32_t n, const int32_t *__restrict__ kidmap, const uint8_t *__restrict__ keyflags,
                                                               const uint8_t *__restrict__ r_be, const uint32_t *__restrict__ uw,
@@ -579,11 +587,6 @@ __global__ void __launch_bounds__(BLOCK, MINB) k_verify_comb(uint32_t n, const i
     const uint4 *kt = ktab + (size_t)kid * CT::POINTS * EU4;
     uint32_t one[N];
     C::get_one(one);
-    Jac<A> acc;
-    mp_copy<N>(acc.X, one);
-    mp_copy<N>(acc.Y, one);
-#pragma unroll
-    for (int i = 0; i < N; i++) acc.Z[i] = 0;
     // step s: column SPACING-1 - s/2, block s%2 of u2's comb
     auto fetch = [&](int s, uint32_t (&x)[N], uint32_t (&y)[N], bool &skip) {
         const int b = s & 1;
@@ -593,8 +596,15 @@ __global__ void __launch_bounds__(BLOCK, MINB) k_verify_comb(uint32_t n, const i
     };
     uint32_t cx[N], cy[N];
     bool cskip;
-    fetch(0, cx, cy, cskip);
-    int s = 0, dbl = 0;  // dbl: doublings due before the addition of step s
+    fetch(1, cx, cy, cskip);
+    Jac<A> acc;
+    {  // step 0 meets the accumulator at infinity: its entry is loaded, not added
+        uint32_t sx[N], sy[N];
+        bool sskip;
+        fetch(0, sx, sy, sskip);
+        pt_seed<A>(acc, sx, sy, false, sskip);
+    }
+    int s = 1, dbl = 0;  // dbl: doublings due before the addition of step s
 #pragma unroll 1
     while (s < KADD || dbl) {
         if (dbl) {

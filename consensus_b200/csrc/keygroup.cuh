@@ -26,7 +26,7 @@
 // a comb verification (15 doublings + 32 additions + the u1*G half) is ~5x cheaper than a generic one, so T = 16 pays.
 // In issued warp instructions (sm_90a SASS) a P-256 comb table costs ~16 K in the doubling chain (1,037 per doubling
 // for 16 keys), ~35 K in k_comb_fill (2,167 per mixed addition, inlined) and ~15 K in k_kt_final (911 per entry,
-// inlined), against ~275 K for the 64 verifications of a key in k_verify_comb and k_gpart.
+// inlined), against ~266 K for the 64 verifications of a key in k_verify_comb and k_gpart.
 // Registered keys (sbv_set_keys) get a window table (KeyTab, W = 8), read by k_verify_kt: built once per key set, so
 // its verifications are the ones to make cheapest — no doublings at all.
 #pragma once

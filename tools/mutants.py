@@ -47,6 +47,7 @@ SHARDS = ["tests/test_hostsim_shards.py"]
 WIDE = ["tests/test_hostsim_wide.py"]  # bit lengths, offsets and byte sums past 32 bits
 SHA384 = ["tests/test_hostsim_sha384.py"]
 KEY_CACHE = ["tests/test_hostsim_key_cache.py"]
+SEEDED = ["tests/test_hostsim_seeded_passes.py"]  # the first entry of a pass loaded, not added (pt_seed)
 
 
 def M(id, file, find, repl, tests, equivalent=None, proof=None):
@@ -167,6 +168,11 @@ CATALOGUE = [
     M("load_key_no_y_range", "kernels.cuh", "bool good = mp_lt<N>(x, pmod) && mp_lt<N>(y, pmod);", "bool good = mp_lt<N>(x, pmod);", ECDSA),
     M("load_key_b_dropped", "kernels.cuh", "C::fadd(rhs, rhs, b);", "(void)b;", ECDSA),
     M("add_u1G_skip_ignored", "kernels.cuh", "pt_add<C, true>(acc, gx, gy, one, false, gb == 0);", "pt_add<C, true>(acc, gx, gy, one, false, false);", ECDSA),
+    M("add_u1G_seed_zero_digit", "kernels.cuh", "pt_seed<C>(acc, sx, sy, false, sb == 0);", "pt_seed<C>(acc, sx, sy, false, false);", SEEDED + ECDSA),
+    M("add_u1G_seed_window_added_again", "kernels.cuh", "constexpr int W0 = FROM_INF ? 1 : 0;", "constexpr int W0 = 0;", SEEDED + ECDSA),
+    M("pt_seed_infinity_z", "curve.cuh", "P.Z[i] = skip ? 0u : one[i];", "P.Z[i] = one[i];", SEEDED + ECDSA),
+    M("pt_seed_negation_ignored", "curve.cuh", "mp_select<N>(y, neg, ny, y_in);\n    }\n    C::get_one(one);", "mp_copy<N>(y, y_in);\n    }\n    C::get_one(one);",
+      SEEDED + ECDSA),
     M("k_verify_kt_slot_range", "kernels.cuh", "kid = sl < n_slots ? kidmap[sl] : -1;", "kid = sl <= n_slots ? kidmap[sl] : -1;", ECDSA),
     M("k_verify_kt_entry_index", "kernels.cuh", "load_affine<C>(x, y, kt + ((size_t)w * KT::ENT + (e ? e - 1 : 0)) * EU4);",
       "load_affine<C>(x, y, kt + ((size_t)w * KT::ENT + (e > 1 ? e - 2 : 0)) * EU4);", ECDSA),
@@ -176,6 +182,11 @@ CATALOGUE = [
       "dbl = 0; pt_add_m<A, 1, true>(acc, cx, cy, one, one, one, false, cskip);", ECDSA,
       equivalent="the comb accumulator and the entry it meets are distinct binary numbers below n: they never coincide",
       proof="tests/test_mutant_proofs.py::test_comb_accumulator_never_equals_its_next_entry"),
+    M("k_verify_comb_seed_zero_mask", "kernels.cuh", "pt_seed<A>(acc, sx, sy, false, sskip);", "pt_seed<A>(acc, sx, sy, false, false);", SEEDED + ECDSA),
+    M("k_verify_comb_loop_from_step_0", "kernels.cuh", "int s = 1, dbl = 0;", "int s = 0, dbl = 0;", SEEDED + ECDSA),
+    M("k_verify_kt_seed_zero_digit", "kernels.cuh", "pt_seed<A>(acc, cx, cy, cneg, cskip);", "pt_seed<A>(acc, cx, cy, cneg, false);", SEEDED + ECDSA),
+    M("k_verify_kt_seed_sign_ignored", "kernels.cuh", "pt_seed<A>(acc, cx, cy, cneg, cskip);", "pt_seed<A>(acc, cx, cy, false, cskip);", SEEDED + ECDSA),
+    M("k_verify_kt_loop_from_window_0", "kernels.cuh", "        w0 = 1;\n", "        w0 = 0;\n", SEEDED + ECDSA),
     M("k_verify_comb_closing_skip", "kernels.cuh", "pt_add<C, false>(fin, g.X, g.Y, g.Z, false, mp_is_zero<N>(g.Z));",
       "pt_add<C, false>(fin, g.X, g.Y, g.Z, false, false);", ECDSA),
     M("k_verify_kt_warp_tree_flag", "kernels.cuh", "pt_add<C, false>(acc, x2, y2, z2, false, mp_is_zero<N>(z2));",
