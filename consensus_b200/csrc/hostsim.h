@@ -52,7 +52,6 @@ static inline int __clz(int x) { return x ? __builtin_clz((unsigned)x) : 32; }
 static inline int __popc(unsigned x) { return __builtin_popcount(x); }
 static inline uint32_t __umulhi(uint32_t a, uint32_t b) { return (uint32_t)(((uint64_t)a * b) >> 32); }
 static inline void __syncthreads() {}
-static inline void __syncwarp(unsigned = 0xffffffffu) {}
 static inline void __threadfence() {}
 // Warp primitives.  Default: one simulated thread at a time — a "ballot" sees only the caller, a shuffle returns the caller's
 // own value (thread-per-item kernels never depend on them).  LOCKSTEP mode (hostsim_ctx set by the driver, one OS thread
@@ -81,6 +80,13 @@ static inline void hostsim_exchange(unsigned mask, uint32_t v, uint32_t (&all)[3
         w->cv.wait(lk, [&] { return s.gen != g; });
     }
     memcpy(all, s.out, sizeof s.out);  // still under the lock: the next meeting cannot complete before every lane has left this one
+}
+// LOCKSTEP mode: a barrier of the lanes of `mask` (the warp's shared memory is the extern `tab`, one array that the lanes
+// of the running warp share)
+static inline void __syncwarp(unsigned mask = 0xffffffffu) {
+    if (!hostsim_ctx) return;
+    uint32_t all[32];
+    hostsim_exchange(mask, 0, all);
 }
 static inline unsigned __ballot_sync(unsigned mask, int p) {
     if (!hostsim_ctx) return p ? 1u : 0u;

@@ -11,7 +11,7 @@ template <class C> struct Cfg;
 // P-256: the fixed-base kernels run with their multiplications inlined at 6 blocks per SM (window kernel 168 registers,
 // comb kernel 152, no spills; the window kernel is equal or slightly ahead of the out-of-line build at 7 blocks, which
 // spills); the generic kernel likewise at 6 blocks (no spills) now that it only sees the keys that do not repeat.
-// COMB_INL also inlines the loops of the comb tables' build (k_kt_bases2, k_comb_fill, k_kt_final: 71, 105 and 96
+// COMB_INL also inlines the loops of the comb tables' build (k_kt_bases2, k_comb_fill_warp, k_comb_final: 71, 102 and 96
 // registers, no spills; one site per multiplication of each loop).  k_gpart keeps its multiplications out of line (138
 // registers): inlined (146 registers, no spills) it ran 14 % faster alone but did not raise the pipelined throughput
 // (DESIGN.md §10).
@@ -115,13 +115,15 @@ cudaError_t op_comb_build(const uint32_t *nkeys_ptr, uint32_t cap, const uint32_
                           uint32_t *bases, uint32_t *hs, uint32_t *ztop, uint32_t *pref, uint32_t *ktab, uint8_t *keyflags, cudaStream_t st) {
     using CT = CombTab<C>;
     const unsigned kb = (cap + 63) / 64;
-    const unsigned cb = (unsigned)(((size_t)cap * CT::NCHAIN + 63) / 64);
+    const unsigned wb = (unsigned)(((size_t)cap * 32 + 63) / 64);  // a warp per key
     constexpr bool INL = Cfg<C>::COMB_INL;
+    constexpr size_t fill_smem = (size_t)2 * CT::NBASE * 2 * C::N * 4;                 // two warps x 16 affine bases
+    constexpr size_t final_smem = (size_t)2 * 32 * (CT::ENT / 2 * 2 * C::N / 4 + 1) * 16;  // two warps x 32 half chains
     k_kt_bases2<C, CT, INL><<<(unsigned)(((size_t)cap * 2 + 127) / 128), 128, 0, st>>>(nkeys_ptr, cap, keylist, qx, qy, bases, keyflags);
     k_comb_affine<C><<<kb, 64, 0, st>>>(nkeys_ptr, cap, keyflags, bases, pref);
-    k_comb_fill<C, INL><<<cb, 64, 0, st>>>(nkeys_ptr, cap, bases, keyflags, hs, ztop, ktab);
-    k_kt_inv<C, CT><<<kb, 64, 0, st>>>(nkeys_ptr, cap, keyflags, ztop, pref);
-    k_kt_final<C, CT, INL><<<cb, 64, 0, st>>>(nkeys_ptr, cap, bases, keyflags, hs, ztop, ktab);
+    k_comb_fill_warp<C, INL><<<wb, 64, fill_smem, st>>>(nkeys_ptr, cap, bases, keyflags, hs, ztop);
+    k_kt_inv<C, CT, CombScr<C>><<<kb, 64, 0, st>>>(nkeys_ptr, cap, keyflags, ztop, pref);
+    k_comb_final<C, INL><<<wb, 64, final_smem, st>>>(nkeys_ptr, cap, keyflags, hs, ztop, ktab);
     return cudaGetLastError();
 }
 

@@ -14,19 +14,20 @@
 //                 bases B_i = 2^(STEP*i) * Q of its table — a chain of doublings whose independent multiplications run
 //                 on different lanes (k_kt_bases, one thread per key, is their reference in the CPU simulation)
 //   k_comb_affine one thread per key (comb): the 16 bases to affine with one inversion
-//   k_comb_fill   one thread per (key, chain) (comb): the 16 entries of a chain, one mixed addition per Gray-code step
+//   k_comb_fill_warp  a warp per key, lane = chain (comb): the 16 entries of a chain, one mixed addition per Gray-code step
 //   k_kt_fill     one thread per (key, window) (window table): e*B_w for e = 1..2^(W-1) with co-Z additions (5M+2S
 //                 each — the chain of Z ratios that comes with them is exactly what the inversion needs)
 //   k_kt_inv      one thread per key: ONE field inversion for all chains of the key (Montgomery's trick across
 //                 the chains' top Z's)
 //   k_kt_final    one thread per (key, chain): back-substitute the Z ratios, convert to affine, in place
+//   k_comb_final  a warp per key, lane = chain (comb): the same conversion, the table written once in whole lines
 //
 // Keys grouped inside a launch get a comb table (CombTab, kernels.cuh), read by k_verify_comb: P-256: 240 doublings +
 // 512 mixed additions (~11 multiplications) + 512 conversions (~6) + two inversions per key ~ 3.5 generic verifications;
 // a comb verification (15 doublings + 32 additions + the u1*G half) is ~5x cheaper than a generic one, so T = 16 pays.
 // In issued warp instructions (sm_90a SASS) a P-256 comb table costs ~16 K in the doubling chain (1,037 per doubling
-// for 16 keys), ~35 K in k_comb_fill (2,167 per mixed addition, inlined) and ~15 K in k_kt_final (911 per entry,
-// inlined), against ~266 K for the 64 verifications of a key in k_verify_comb and k_gpart.
+// for 16 keys), ~39 K in k_comb_fill_warp (2,167 per mixed addition, inlined; 18 steps of a warp carry one) and ~15 K
+// in k_comb_final (911 per entry, inlined), against ~266 K for the 64 verifications of a key in k_verify_comb and k_gpart.
 // Registered keys (sbv_set_keys) get a window table (KeyTab, W = 8), read by k_verify_kt: built once per key set, so
 // its verifications are the ones to make cheapest — no doublings at all.
 #pragma once
@@ -172,8 +173,8 @@ static __global__ void __launch_bounds__(256) k_kg_route(uint32_t n, const uint3
 }
 
 // ---- table construction -------------------------------------------------------------------------------------
-// Scratch layout (cap = key capacity of the buffers; lanes of a warp are consecutive keys, so every access below
-// is coalesced):
+// Scratch layout of the window tables and of the comb's bases (cap = key capacity of the buffers; lanes of a warp are
+// consecutive keys, so every access below is coalesced; the rest of the comb's scratch is CombScr):
 //   bases [i][3N words][cap]                Jacobian B_i = 2^(STEP*i) * Q (the comb's are made affine in place)
 //   hs    [win][e = 2..ENT][N words][cap]   Z ratios along chain win: Z_e = Z_{e-1} * H_e  (window: H_2 = 2*Y_B, Z_1 = Z_B)
 //   ztop  [win][N words][cap]               Z_ENT of the chain; k_kt_inv overwrites it with its inverse
@@ -487,8 +488,14 @@ __global__ void __launch_bounds__(64) k_kt_fill(const uint32_t *__restrict__ nke
     for (int i = 0; i < N; i++) zp[(size_t)i * cap] = zacc[i];
 }
 
-// ztop[win] <- 1 / ztop[win] for all chains of a key with one inversion
-template <class C, class KT>
+// Word i of chain ch's Z in ztop / pref: [chain][N words][cap] (window tables; the comb's layout is CombScr)
+template <int N>
+struct ZByChain {
+    SBV_DEV static size_t at(uint32_t k, int ch, int i, uint32_t cap) { return ((size_t)ch * N + i) * cap + k; }
+};
+
+// ztop[win] <- 1 / ztop[win] for all chains of a key with one inversion (ZL: the layout of ztop and pref)
+template <class C, class KT, class ZL = ZByChain<C::N>>
 __global__ void __launch_bounds__(64) k_kt_inv(const uint32_t *__restrict__ nkeys_ptr, uint32_t cap, const uint8_t *__restrict__ keyflags,
                                                uint32_t *__restrict__ ztop, uint32_t *__restrict__ pref) {
     constexpr int N = C::N;
@@ -501,10 +508,12 @@ __global__ void __launch_bounds__(64) k_kt_inv(const uint32_t *__restrict__ nkey
 #pragma unroll 1
     for (int win = 0; win < KT::NCHAIN; win++) {
         uint32_t z[N];
-        const uint32_t *zp = ztop + (size_t)win * N * cap + k;
-        uint32_t *pp = pref + (size_t)win * N * cap + k;
 #pragma unroll
-        for (int i = 0; i < N; i++) { z[i] = zp[(size_t)i * cap]; pp[(size_t)i * cap] = run[i]; }  // product of the windows before
+        for (int i = 0; i < N; i++) {
+            const size_t a = ZL::at(k, win, i, cap);
+            z[i] = ztop[a];
+            pref[a] = run[i];  // product of the windows before
+        }
         C::fmul(run, run, z);
     }
     uint32_t inv[N];
@@ -512,14 +521,12 @@ __global__ void __launch_bounds__(64) k_kt_inv(const uint32_t *__restrict__ nkey
 #pragma unroll 1
     for (int win = KT::NCHAIN - 1; win >= 0; win--) {
         uint32_t z[N], pv[N], zi[N];
-        uint32_t *zp = ztop + (size_t)win * N * cap + k;
-        const uint32_t *pp = pref + (size_t)win * N * cap + k;
 #pragma unroll
-        for (int i = 0; i < N; i++) { z[i] = zp[(size_t)i * cap]; pv[i] = pp[(size_t)i * cap]; }
+        for (int i = 0; i < N; i++) { const size_t a = ZL::at(k, win, i, cap); z[i] = ztop[a]; pv[i] = pref[a]; }
         C::fmul(zi, inv, pv);
         C::fmul(inv, inv, z);
 #pragma unroll
-        for (int i = 0; i < N; i++) zp[(size_t)i * cap] = zi[i];
+        for (int i = 0; i < N; i++) ztop[ZL::at(k, win, i, cap)] = zi[i];
     }
 }
 
@@ -575,7 +582,8 @@ __global__ void __launch_bounds__(64) k_kt_final(const uint32_t *__restrict__ nk
 
 // ---- comb tables (CombTab, kernels.cuh) -------------------------------------------------------------------------
 // k_kt_bases4<C, CombTab<C>> leaves the 16 bases P_c = 2^(SPACING*c) * Q in Jacobian form; k_comb_affine makes them
-// affine, k_comb_fill walks the 32 chains, and k_kt_inv / k_kt_final finish the table as they do a window table.
+// affine, k_comb_fill_warp walks the 32 chains a warp per key, k_kt_inv inverts the chains' top Z's as for a window
+// table, and k_comb_final converts the entries and writes the table.
 
 // bases -> affine (x, y in place of X, Y) with ONE inversion per key (Montgomery's trick over the 16 Z's; pref: prefix
 // products, [c][N words][cap])
@@ -622,6 +630,8 @@ __global__ void __launch_bounds__(64) k_comb_affine(const uint32_t *__restrict__
 // One thread per (key, chain), chain = (block b, high nibble hi): slot 0 = the sum of the high teeth of hi, then the 15
 // Gray codes of the low nibble, one mixed addition of +-P_(8b+t) per step (t = the bit the step flips).  Records what
 // k_kt_final needs: Jacobian X, Y of every slot in ktab, the Z ratio H of every step in hs, the last Z in ztop.
+// The reference for k_comb_fill_warp in the CPU simulation (tools/hostsim), with k_kt_inv and k_kt_final over the
+// window tables' scratch layout; libsbv.so launches k_comb_fill_warp and k_comb_final.
 // The chain of hi = 0 starts at infinity: its first step is a copy of P_(8b) (Z = 1, H = 1), and its slot 0 (m = 0,
 // never read) is left as (0, 0).
 // The high teeth are steps of the same loop ahead of the Gray walk, so the loop has ONE addition site and its
@@ -691,12 +701,179 @@ __global__ void __launch_bounds__(64) k_comb_fill(const uint32_t *__restrict__ n
     for (int i = 0; i < N; i++) zp[(size_t)i * cap] = P.Z[i];
 }
 
+// Scratch of the comb build as libsbv.so runs it (k_comb_fill_warp, k_kt_inv, k_comb_final): a warp per key, lane =
+// chain, so every buffer is key-major with the chain innermost, in 16-byte words — one access of a warp covers 512
+// contiguous bytes.  Indices in uint4:
+//   hs   [key][ Z ratios [slot-1][N/4][chain] | Jacobian X, Y [slot][2N/4: X then Y][chain] ]
+//   ztop [key][N/4][chain], pref alike   Z of slot 15 of the chain; k_kt_inv overwrites it with its inverse
+// The affine table (ktab) keeps its layout (CombTab::slot) and is written once, by k_comb_final.
+template <class C>
+struct CombScr {
+    using CT = CombTab<C>;
+    static constexpr int Q = C::N / 4;  // 16-byte words per coordinate
+    static constexpr size_t KEY = (size_t)((CT::ENT - 1) * Q + CT::ENT * 2 * Q) * CT::NCHAIN;  // uint4 of hs per key
+    SBV_DEV static size_t hs(uint32_t k, int slot, int w) { return k * KEY + ((size_t)(slot - 1) * Q + w) * CT::NCHAIN; }
+    SBV_DEV static size_t jac(uint32_t k, int slot, int w) { return k * KEY + ((size_t)(CT::ENT - 1) * Q + (size_t)slot * 2 * Q + w) * CT::NCHAIN; }
+    SBV_DEV static size_t z(uint32_t k, int w) { return ((size_t)k * Q + w) * CT::NCHAIN; }
+    // word i of chain ch's Z (k_kt_inv, one thread per key: ZL)
+    SBV_DEV static size_t at(uint32_t k, int ch, int i, uint32_t) { return (z(k, i / 4) + ch) * 4 + (i & 3); }
+};
+
+template <int N>
+SBV_DEV uint4 quad(const uint32_t (&v)[N], int w) { return make_uint4(v[4 * w], v[4 * w + 1], v[4 * w + 2], v[4 * w + 3]); }
+template <int N>
+SBV_DEV void unquad(uint32_t (&v)[N], int w, const uint4 q) { v[4 * w] = q.x; v[4 * w + 1] = q.y; v[4 * w + 2] = q.z; v[4 * w + 3] = q.w; }
+
+// A warp per key, lane = chain (b, hi) = (lane >> 4, lane & 15): the chains of k_comb_fill, each lane doing exactly the
+// steps, in the same order and with the same operands, that k_comb_fill's thread of that chain does — so the Jacobian
+// entries, the Z ratios and the last Z are those of k_comb_fill, bit for bit.  What changes is when: a chain with popc(hi)
+// high teeth takes popc(hi) + 15 steps, and it starts 4 - popc(hi) steps late, so that at step s every working lane makes
+// slot s - 3 and the warp's stores of that slot are contiguous.  The 16 affine bases of the key (1 KiB) are read once per
+// warp into shared memory (dynamic: 2N words per base and warp).
+// No exceptional case arises, for the reason given above k_comb_fill: the additions of a chain are k_comb_fill's, and
+// every point on it is s*Q with 0 < s < 2^(15*SPACING + 1) < n a sum of distinct powers 2^(SPACING*c); +P_t meets the
+// accumulator only if s = 2^(SPACING*t) or s + 2^(SPACING*t) = n, -P_t only if s = -2^(SPACING*t) mod n or the sum empties,
+// and neither the high teeth (always added, never removed) nor the Gray walk (never back to 0) empties it.
+template <class C, bool INL>
+__global__ void __launch_bounds__(64) k_comb_fill_warp(const uint32_t *__restrict__ nkeys_ptr, uint32_t cap, const uint32_t *__restrict__ bases,
+                                                       const uint8_t *__restrict__ keyflags, uint32_t *__restrict__ hs, uint32_t *__restrict__ ztop) {
+    using A = typename PickArith<C, INL>::type;  // arithmetic policy of the loop
+    constexpr int N = C::N, Q = N / 4, HT = CombTab<C>::TEETH / 2;  // HT: high teeth of a block
+    using CT = CombTab<C>;
+    using S = CombScr<C>;
+    static_assert(CT::NCHAIN == 32 && CT::NBASE * 2 == 32, "a lane per chain; a lane per coordinate of a base");
+    const uint32_t k = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, ch = threadIdx.x & 31;
+    uint32_t nkeys = __ldg(nkeys_ptr);
+    if (nkeys > cap) nkeys = cap;
+    if (k >= nkeys || !keyflags[k]) return;  // a warp leaves together
+    extern __shared__ uint32_t tab[];
+    uint32_t *pb = tab + (threadIdx.x >> 5) * CT::NBASE * 2 * N;  // [c][x, y][N words]
+    {
+        const uint32_t *o = bases + ((size_t)(ch >> 1) * 3 + (ch & 1)) * N * cap + k;  // lane 2c + j: coordinate j of P_c
+#pragma unroll
+        for (int i = 0; i < N; i++) pb[ch * N + i] = o[(size_t)i * cap];
+    }
+    __syncwarp();
+    uint4 *h4 = reinterpret_cast<uint4 *>(hs), *z4 = reinterpret_cast<uint4 *>(ztop);
+    auto store = [&](int slot, const uint32_t (&x)[N], const uint32_t (&y)[N], const uint32_t (&h)[N]) {
+#pragma unroll
+        for (int w = 0; w < Q; w++) { h4[S::jac(k, slot, w) + ch] = quad<N>(x, w); h4[S::jac(k, slot, Q + w) + ch] = quad<N>(y, w); }
+        if (slot) {
+#pragma unroll
+            for (int w = 0; w < Q; w++) h4[S::hs(k, slot, w) + ch] = quad<N>(h, w);
+        }
+    };
+    const int b = (int)(ch >> 4), hi = (int)(ch & 15), nhigh = __popc(hi);
+    Jac<A> P;
+    uint32_t x[N], y[N], h[N], zero[N];
+#pragma unroll
+    for (int i = 0; i < N; i++) zero[i] = 0;
+    C::get_one(P.Z);
+    C::get_one(h);
+    if (hi == 0) store(0, zero, zero, h);
+    int rest = hi;  // high teeth still to add
+#pragma unroll 1
+    for (int s = 0; s < HT + CT::ENT - 1; s++) {
+        const int st = s - (HT - nhigh);  // the chain's own step (k_comb_fill's st)
+        if (st < 0) continue;
+        const int kk = s - (HT - 1);      // the slot the step produces; <= 0 while the high teeth go in (0: the last of them)
+        int tooth;
+        bool neg = false;
+        if (kk <= 0) {
+            tooth = HT + __ffs(rest) - 1;
+            rest &= rest - 1;
+        } else {
+            tooth = __ffs(kk) - 1;                       // gray(kk - 1) -> gray(kk) flips this bit
+            neg = !(((kk ^ (kk >> 1)) >> tooth) & 1);    // the bit goes off: subtract
+        }
+        const uint32_t *pt = pb + (CT::TEETH * b + tooth) * 2 * N;
+#pragma unroll
+        for (int i = 0; i < N; i++) { x[i] = pt[i]; y[i] = pt[N + i]; }
+        if (neg) C::fsub(y, zero, y);
+        if (st == 0) { mp_copy<N>(P.X, x); mp_copy<N>(P.Y, y); }  // from infinity: Z = 1, H = 1
+        else pt_madd_table<A>(P, x, y, h);
+        if (kk >= 0) store(kk, P.X, P.Y, h);
+    }
+#pragma unroll
+    for (int w = 0; w < Q; w++) z4[S::z(k, w) + ch] = quad<N>(P.Z, w);
+}
+
+// A warp per key, lane = chain: k_kt_final's conversion of the comb (1/Z_e walked from e = 16 down to 1, five
+// multiplications per entry), reading k_comb_fill_warp's scratch, then the affine entries into ktab in its layout.  A
+// chain's entries are contiguous there (CombTab::slot), so each lane stages half a chain (8 entries) in shared memory
+// and the warp writes the 32 half chains one at a time: 512 contiguous bytes per store instruction.  Shared memory:
+// 32 lanes x (8 entries x 2N/4 + 1 padding) 16-byte words per warp (P-256: 16.5 KiB); the padding word spreads the lanes'
+// rows over the banks.
+template <class C, bool INL>
+__global__ void __launch_bounds__(64) k_comb_final(const uint32_t *__restrict__ nkeys_ptr, uint32_t cap, const uint8_t *__restrict__ keyflags,
+                                                   const uint32_t *__restrict__ hs, const uint32_t *__restrict__ ztop, uint32_t *__restrict__ ktab) {
+    using A = typename PickArith<C, INL>::type;  // arithmetic policy
+    constexpr int N = C::N, Q = N / 4;
+    using CT = CombTab<C>;
+    using S = CombScr<C>;
+    constexpr int HALF = CT::ENT / 2, ROW = HALF * 2 * Q + 1;  // entries per flush; stage row of a lane in uint4
+    static_assert(CT::NCHAIN == 32 && HALF * 2 * Q == 32, "a lane per chain; a half chain is one 16-byte word per lane");
+    const uint32_t k = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, ch = threadIdx.x & 31;
+    uint32_t nkeys = __ldg(nkeys_ptr);
+    if (nkeys > cap) nkeys = cap;
+    if (k >= nkeys || !keyflags[k]) return;  // a warp leaves together
+    extern __shared__ uint32_t tab[];
+    uint4 *stage = reinterpret_cast<uint4 *>(tab) + (threadIdx.x >> 5) * 32 * ROW;
+    const uint4 *h4 = reinterpret_cast<const uint4 *>(hs), *z4 = reinterpret_cast<const uint4 *>(ztop);
+    uint4 *out = reinterpret_cast<uint4 *>(ktab) + (size_t)k * CT::POINTS * 2 * Q;
+    uint32_t zi[N];  // 1 / Z_e, walking e = ENT .. 1
+#pragma unroll
+    for (int w = 0; w < Q; w++) unquad<N>(zi, w, z4[S::z(k, w) + ch]);
+    auto load = [&](int slot, uint32_t (&x)[N], uint32_t (&y)[N]) {
+#pragma unroll
+        for (int w = 0; w < Q; w++) { unquad<N>(x, w, h4[S::jac(k, slot, w) + ch]); unquad<N>(y, w, h4[S::jac(k, slot, Q + w) + ch]); }
+    };
+    // entry e-1 and its Z ratio are loaded before entry e is converted (independent addresses: the loads overlap the
+    // multiplications)
+    uint32_t x[N], y[N];
+    load(CT::ENT - 1, x, y);
+#pragma unroll 1
+    for (int e = CT::ENT; e >= 1; e--) {
+        uint32_t nx[N], ny[N], nh[N];
+        if (e >= 2) {
+            load(e - 2, nx, ny);
+#pragma unroll
+            for (int w = 0; w < Q; w++) unquad<N>(nh, w, h4[S::hs(k, e - 1, w) + ch]);
+        }
+        uint32_t z2[N], z3[N];
+        A::fsqr(z2, zi);
+        A::fmul(z3, z2, zi);
+        A::fmul(x, x, z2);
+        A::fmul(y, y, z3);
+        uint4 *row = stage + ch * ROW + ((e - 1) % HALF) * 2 * Q;
+#pragma unroll
+        for (int w = 0; w < Q; w++) { row[w] = quad<N>(x, w); row[Q + w] = quad<N>(y, w); }
+        if ((e - 1) % HALF == 0) {  // slots e-1 .. e-1+HALF-1 of every chain are staged: chain j's are word ch of its half
+            __syncwarp();
+            uint4 *o = out + (size_t)(e - 1) * 2 * Q + ch;
+#pragma unroll 4
+            for (int j = 0; j < CT::NCHAIN; j++) o[(size_t)j * CT::ENT * 2 * Q] = stage[j * ROW + ch];
+            __syncwarp();
+        }
+        if (e >= 2) {  // 1/Z_{e-1} = (1/Z_e) * H_e
+            A::fmul(zi, zi, nh);
+            mp_copy<N>(x, nx); mp_copy<N>(y, ny);
+        }
+    }
+}
+
+template <class KT> struct IsComb { static constexpr bool value = false; };
+template <class C> struct IsComb<CombTab<C>> { static constexpr bool value = true; };
+
 // words of scratch the builder needs for `cap` keys (KT: KeyTab or CombTab)
 template <class C, class KT_>
 struct KtSizes {
     using KT = KT_;
     static constexpr size_t bases_words(size_t cap) { return (size_t)KT::NBASE * 3 * C::N * cap; }
-    static constexpr size_t hs_words(size_t cap) { return (size_t)KT::NCHAIN * (KT::ENT - 1) * C::N * cap; }
+    // the Z ratios; for a comb also the Jacobian entries (CombScr)
+    static constexpr size_t hs_words(size_t cap) {
+        return IsComb<KT>::value ? CombScr<C>::KEY * 4 * cap : (size_t)KT::NCHAIN * (KT::ENT - 1) * C::N * cap;
+    }
     static constexpr size_t ztop_words(size_t cap) { return (size_t)KT::NCHAIN * C::N * cap; }
     static constexpr size_t ktab_words(size_t cap) { return KT::POINTS * 2 * C::N * cap; }
 };

@@ -4,7 +4,7 @@
 //
 //          ├──────────────── begin (every scheme) ─────┤
 //   st     memsets  k_kg_insert  k_kg_assign ─┬─ k_prep  k_kg_route ─┬─ k_gpart ──────────────────────────────────┬─ (wait tables) k_verify_comb ─ (wait generic) ─ done
-//   s_tab                                     └─ k_kt_bases2  k_comb_affine  k_comb_fill  k_kt_inv  k_kt_final ─┘
+//   s_tab                                     └─ k_kt_bases2  k_comb_affine  k_comb_fill_warp  k_kt_inv  k_comb_final ─┘
 //   s_gen                                                             └─ k_verify_coz (keys without a table) ──────────────────────────────────┘
 //
 // Keys that occur at least `group_threshold` times in the batch get a fixed-base table built on the spot (keygroup.cuh: a
@@ -13,7 +13,7 @@
 // A large host-buffer batch runs the part after the table fork chunk by chunk, as its chunks arrive.
 // Registered keys (sbv_set_keys) skip the grouping: their tables were built at registration.
 // With a key cache reserved (sbv_key_cache_reserve), k_kc_lookup runs after k_kg_assign on st and k_kc_insert after
-// k_kt_final on s_tab (key_cache.cuh): the build then makes only the tables the cache does not hold.
+// the table construction on s_tab (key_cache.cuh): the build then makes only the tables the cache does not hold.
 // The first half up to the fork and the table construction is one function for P-256, P-384 and Ed25519 (verify_begin),
 // driven by the scheme's entry of the grouping table (ops.h: GroupOps); Ed25519's second half is in inst_ed25519.cu.
 #include "engine.h"

@@ -115,22 +115,81 @@ static void bases_t(const uint32_t *cnt, uint32_t cap, const uint32_t *keylist, 
     else run_grid((cap + 63) / 64, 64, [&] { k_kt_bases<C, KT>(cnt, cap, keylist, qx, qy, bases, kflags); });
 }
 
+// What the comb build leaves between its kernels, in one order whatever the scratch layout (key k = 0..cap-1, chain ch):
+// jac [k][ch][slot][2N] the fill's Jacobian X, Y; hs [k][ch][slot-1][N] its Z ratios; ztop [k][ch][N] 1 / Z of slot 15
+// after k_kt_inv.  NULL: not wanted.
+struct CombInner {
+    uint32_t *jac = nullptr, *hs = nullptr, *ztop = nullptr;
+};
+
+// The comb part of the build after the doubling chain: warp = 1 as libsbv.so runs it (k_comb_fill_warp and k_comb_final,
+// a warp per key, in lockstep; CombScr scratch), warp = 0 by the one-thread-per-chain reference (k_comb_fill and
+// k_kt_final over the window tables' scratch layout).
+template <class C>
+static void comb_t(const uint32_t *cnt, uint32_t cap, bool warp, uint32_t *bases, uint32_t *ktab, uint8_t *kflags, const CombInner &in) {
+    using CT = CombTab<C>;
+    using KS = KtSizes<C, CT>;
+    using S = CombScr<C>;
+    constexpr int N = C::N;
+    std::vector<uint32_t> hs(KS::hs_words(cap)), ztop(KS::ztop_words(cap)), pref(KS::ztop_words(cap));
+    const unsigned kb = (cap + 63) / 64, cb = (unsigned)(((size_t)cap * CT::NCHAIN + 63) / 64), wb = (unsigned)(((size_t)cap * 32 + 63) / 64);
+    run_grid(kb, 64, [&] { k_comb_affine<C>(cnt, cap, kflags, bases, pref.data()); });
+    // word i of slot `slot` of chain ch of key k in each layout; jac: w = 0 .. 2N-1 over X then Y
+    auto jac_at = [&](uint32_t k, int ch, int slot, int i) -> uint32_t {
+        return warp ? hs[(S::jac(k, slot, i / 4) + ch) * 4 + (i & 3)] : ktab[((size_t)(k * CT::NCHAIN + ch) * CT::ENT + slot) * 2 * N + i];
+    };
+    auto hs_at = [&](uint32_t k, int ch, int slot, int i) -> uint32_t {
+        return warp ? hs[(S::hs(k, slot, i / 4) + ch) * 4 + (i & 3)] : hs[(((size_t)ch * (CT::ENT - 1) + slot - 1) * N + i) * cap + k];
+    };
+    if (warp) run_grid_lockstep(wb, 64, [&] { k_comb_fill_warp<C, true>(cnt, cap, bases, kflags, hs.data(), ztop.data()); });
+    else run_grid(cb, 64, [&] { k_comb_fill<C, true>(cnt, cap, bases, kflags, hs.data(), ztop.data(), ktab); });
+    for (uint32_t k = 0; k < cap; k++)
+        for (int ch = 0; ch < CT::NCHAIN; ch++)
+            for (int slot = 0; slot < CT::ENT; slot++) {
+                for (int i = 0; in.jac && i < 2 * N; i++) in.jac[((size_t)(k * CT::NCHAIN + ch) * CT::ENT + slot) * 2 * N + i] = jac_at(k, ch, slot, i);
+                for (int i = 0; in.hs && slot && i < N; i++) in.hs[((size_t)(k * CT::NCHAIN + ch) * (CT::ENT - 1) + slot - 1) * N + i] = hs_at(k, ch, slot, i);
+            }
+    if (warp) run_grid(kb, 64, [&] { k_kt_inv<C, CT, S>(cnt, cap, kflags, ztop.data(), pref.data()); });
+    else run_grid(kb, 64, [&] { k_kt_inv<C, CT>(cnt, cap, kflags, ztop.data(), pref.data()); });
+    for (uint32_t k = 0; in.ztop && k < cap; k++)
+        for (int ch = 0; ch < CT::NCHAIN; ch++)
+            for (int i = 0; i < N; i++)
+                in.ztop[((size_t)k * CT::NCHAIN + ch) * N + i] = ztop[warp ? S::at(k, ch, i, cap) : ZByChain<N>::at(k, ch, i, cap)];
+    if (warp) run_grid_lockstep(wb, 64, [&] { k_comb_final<C, true>(cnt, cap, kflags, hs.data(), ztop.data(), ktab); });
+    else run_grid(cb, 64, [&] { k_kt_final<C, CT, true>(cnt, cap, bases, kflags, hs.data(), ztop.data(), ktab); });
+}
+
 template <class C, class KT>
 static void build_t(const uint32_t *cnt, uint32_t cap, const uint32_t *keylist, const uint8_t *qx, const uint8_t *qy, int four, uint32_t *ktab,
                     uint8_t *kflags) {
     using KS = KtSizes<C, KT>;
-    std::vector<uint32_t> bases(KS::bases_words(cap)), hs(KS::hs_words(cap)), ztop(KS::ztop_words(cap)), pref(KS::ztop_words(cap));
-    const unsigned kb = (cap + 63) / 64, cb = (unsigned)(((size_t)cap * KT::NCHAIN + 63) / 64);
-    constexpr bool COMB = std::is_same<KT, CombTab<C>>::value;
+    std::vector<uint32_t> bases(KS::bases_words(cap));
     bases_t<C, KT>(cnt, cap, keylist, qx, qy, four, bases.data(), kflags);
-    if constexpr (COMB) {
-        run_grid(kb, 64, [&] { k_comb_affine<C>(cnt, cap, kflags, bases.data(), pref.data()); });
-        run_grid(cb, 64, [&] { k_comb_fill<C, true>(cnt, cap, bases.data(), kflags, hs.data(), ztop.data(), ktab); });
+    if constexpr (std::is_same<KT, CombTab<C>>::value) {
+        comb_t<C>(cnt, cap, true, bases.data(), ktab, kflags, CombInner{});
     } else {
+        std::vector<uint32_t> hs(KS::hs_words(cap)), ztop(KS::ztop_words(cap)), pref(KS::ztop_words(cap));
+        const unsigned kb = (cap + 63) / 64, cb = (unsigned)(((size_t)cap * KT::NCHAIN + 63) / 64);
         run_grid(cb, 64, [&] { k_kt_fill<C, KT::STEP>(cnt, cap, bases.data(), kflags, hs.data(), ztop.data(), ktab); });
+        run_grid(kb, 64, [&] { k_kt_inv<C, KT>(cnt, cap, kflags, ztop.data(), pref.data()); });
+        run_grid(cb, 64, [&] { k_kt_final<C, KT>(cnt, cap, bases.data(), kflags, hs.data(), ztop.data(), ktab); });
     }
-    run_grid(kb, 64, [&] { k_kt_inv<C, KT>(cnt, cap, kflags, ztop.data(), pref.data()); });
-    run_grid(cb, 64, [&] { k_kt_final<C, KT, COMB>(cnt, cap, bases.data(), kflags, hs.data(), ztop.data(), ktab); });
+}
+
+// P-256 comb tables of nkeys keys in a build of capacity cap >= nkeys (the surplus slots stay untouched: zeros), by the
+// path `warp` selects (comb_t), with what the build leaves between its kernels (CombInner; each output may be NULL)
+extern "C" int hs_comb_build(int warp, size_t nkeys, size_t cap, const uint8_t *qx, const uint8_t *qy, uint32_t *ktab_out, uint32_t *jac_out,
+                             uint32_t *hs_out, uint32_t *ztop_out, uint8_t *flags_out) {
+    using KS = KtSizes<P256, CombTab<P256>>;
+    if (nkeys > cap) return -1;
+    const uint32_t cnt = (uint32_t)nkeys, c = (uint32_t)cap;
+    std::vector<uint32_t> bases(KS::bases_words(cap)), ktab(KS::ktab_words(cap), 0);
+    std::vector<uint8_t> kflags(cap, 0);
+    bases_t<P256, CombTab<P256>>(&cnt, c, nullptr, qx, qy, 2, bases.data(), kflags.data());
+    comb_t<P256>(&cnt, c, warp != 0, bases.data(), ktab.data(), kflags.data(), CombInner{jac_out, hs_out, ztop_out});
+    memcpy(ktab_out, ktab.data(), ktab.size() * 4);
+    memcpy(flags_out, kflags.data(), cap);
+    return 0;
 }
 
 template <class C, class KT>

@@ -47,7 +47,8 @@ SHARDS = ["tests/test_hostsim_shards.py"]
 WIDE = ["tests/test_hostsim_wide.py"]  # bit lengths, offsets and byte sums past 32 bits
 SHA384 = ["tests/test_hostsim_sha384.py"]
 KEY_CACHE = ["tests/test_hostsim_key_cache.py"]
-SEEDED = ["tests/test_hostsim_seeded_passes.py"]  # the first entry of a pass loaded, not added (pt_seed)
+SEEDED = ["tests/test_hostsim_seeded_passes.py"]
+COMB_WARP = ["tests/test_hostsim_comb_warp.py"]  # the comb build a warp per key against the one-thread-per-chain reference  # the first entry of a pass loaded, not added (pt_seed)
 
 
 def M(id, file, find, repl, tests, equivalent=None, proof=None):
@@ -207,11 +208,20 @@ CATALOGUE = [
     M("k_kt_bases4_level2_select", "keygroup.cuh", "mp_select<N>(a, role == 2, bb, a);", "mp_select<N>(a, role == 1, bb, a);", ECDSA),
     M("k_kt_fill_h2", "keygroup.cuh", "C::fadd(h, by, by);\n    pt_double<C>(P);", "mp_copy<N>(h, by);\n    pt_double<C>(P);", ECDSA),
     M("k_kt_fill_last_entry", "keygroup.cuh", "for (int e = 3; e <= KT::ENT; e++) {", "for (int e = 3; e < KT::ENT; e++) {", ECDSA),
-    M("k_kt_inv_prefix", "keygroup.cuh", "C::fmul(zi, inv, pv);\n        C::fmul(inv, inv, z);\n#pragma unroll\n        for (int i = 0; i < N; i++) zp[(size_t)i * cap] = zi[i];",
-      "mp_copy<N>(zi, inv);\n        C::fmul(inv, inv, z);\n#pragma unroll\n        for (int i = 0; i < N; i++) zp[(size_t)i * cap] = zi[i];", ECDSA),
+    M("k_kt_inv_prefix", "keygroup.cuh", "C::fmul(zi, inv, pv);\n        C::fmul(inv, inv, z);\n#pragma unroll\n        for (int i = 0; i < N; i++) ztop[ZL::at(k, win, i, cap)] = zi[i];",
+      "mp_copy<N>(zi, inv);\n        C::fmul(inv, inv, z);\n#pragma unroll\n        for (int i = 0; i < N; i++) ztop[ZL::at(k, win, i, cap)] = zi[i];", ECDSA),
     M("k_kt_final_ratio", "keygroup.cuh", "A::fmul(zi, zi, h);\n            mp_copy<N>(x, nx);", "mp_copy<N>(x, nx);", ECDSA),
-    M("k_comb_fill_no_subtract", "keygroup.cuh", "sub = !(((kk ^ (kk >> 1)) >> tooth) & 1);", "sub = false;", ECDSA),
-    M("k_comb_fill_high_teeth", "keygroup.cuh", "tooth = 4 + __ffs(rest) - 1;", "tooth = 3 + __ffs(rest) - 1;", ECDSA),
+    # k_comb_fill is the CPU simulation's reference for k_comb_fill_warp: the comparison of the two kills its mutants
+    M("k_comb_fill_no_subtract", "keygroup.cuh", "sub = !(((kk ^ (kk >> 1)) >> tooth) & 1);", "sub = false;", COMB_WARP),
+    M("k_comb_fill_high_teeth", "keygroup.cuh", "tooth = 4 + __ffs(rest) - 1;", "tooth = 3 + __ffs(rest) - 1;", COMB_WARP),
+    M("k_comb_fill_warp_no_negate", "keygroup.cuh", "neg = !(((kk ^ (kk >> 1)) >> tooth) & 1);", "neg = false;", ECDSA + COMB_WARP),
+    M("k_comb_fill_warp_high_teeth", "keygroup.cuh", "tooth = HT + __ffs(rest) - 1;", "tooth = HT - 1 + __ffs(rest) - 1;", ECDSA + COMB_WARP),
+    M("k_comb_fill_warp_base_lane", "keygroup.cuh", "for (int i = 0; i < N; i++) pb[ch * N + i] = o[(size_t)i * cap];",
+      "for (int i = 0; i < N; i++) pb[(ch ^ 1) * N + i] = o[(size_t)i * cap];", ECDSA + COMB_WARP),
+    M("k_comb_fill_warp_ratio_slot", "keygroup.cuh", "for (int w = 0; w < Q; w++) h4[S::hs(k, slot, w) + ch] = quad<N>(h, w);",
+      "for (int w = 0; w < Q; w++) h4[S::hs(k, slot, w) + ch] = quad<N>(x, w);", ECDSA + COMB_WARP),
+    M("k_comb_final_ratio", "keygroup.cuh", "A::fmul(zi, zi, nh);", "(void)nh;", ECDSA + COMB_WARP),
+    M("k_comb_final_transpose", "keygroup.cuh", "= stage[j * ROW + ch];", "= stage[ch * ROW + j];", ECDSA + COMB_WARP),
     # ---------------------------------------------------------------- sha256.cuh
     M("sha256_pad_rem", "sha256.cuh", "if (rem < 4) v = (v & (0xffffffffu << (8 * (4 - rem)))) | (0x80u << (8 * (3 - rem)));\n                } else if (p == len) {",
       "if (rem < 4) v = (v & (0xffffffffu << (8 * (4 - rem))));\n                } else if (p == len) {", ECDSA),
