@@ -27,7 +27,7 @@ SYMBOLS = [
     "sbv_verify_batch_ranked", "sbv_host_alloc", "sbv_host_free", "sbv_ed25519_verify_batch",
     "sbv_ed25519_set_keys", "sbv_ed25519_verify_registered", "sbv_ed25519_verify_quorum", "sbv_mixed_verify_registered",
     "sbv_mixed_verify_quorum", "sbv_mixed_verify_batch", "sbv_sha384_batch", "sbv_hash384_verify_batch", "sbv_hash384_verify_registered",
-    "sbv_key_cache_reserve", "sbv_key_cache_stats",
+    "sbv_key_cache_reserve", "sbv_key_cache_stats", "sbv_key_cache_reserve_evicting", "sbv_key_cache_stats_ex",
 ]
 
 
@@ -136,6 +136,19 @@ class Engine:
         out = (C.c_uint64 * 4)()
         self._check(self._lib.sbv_key_cache_stats(self._h, C.c_uint8(scheme), out), "sbv_key_cache_stats")
         return dict(zip(("capacity", "resident", "hits", "misses"), (int(v) for v in out)))
+
+    def key_cache_reserve_evicting(self, p256=0, p384=0, ed25519=0):
+        """As key_cache_reserve, but the caches replace their least recently used tables when full (16 ways per set;
+        each capacity is rounded up to a multiple of 16); (0, 0, 0) frees them (sbv_key_cache_reserve_evicting)."""
+        self._check(self._lib.sbv_key_cache_reserve_evicting(self._h, C.c_size_t(p256), C.c_size_t(p384), C.c_size_t(ed25519)),
+                    "sbv_key_cache_reserve_evicting")
+
+    def key_cache_stats_ex(self, scheme) -> dict:
+        """{capacity, resident, hits, misses, evictions, given_up} of one scheme's cache, summed over devices
+        (sbv_key_cache_stats_ex); the fill-once cache reports 0 for the last two."""
+        out = (C.c_uint64 * 6)()
+        self._check(self._lib.sbv_key_cache_stats_ex(self._h, C.c_uint8(scheme), out), "sbv_key_cache_stats_ex")
+        return dict(zip(("capacity", "resident", "hits", "misses", "evictions", "given_up"), (int(v) for v in out)))
 
     # ---- host-buffer API (numpy arrays, or anything exposing a host pointer via .ctypes) ----
     def verify_batch(self, curve, r, s, qx, qy, digest, out=None) -> np.ndarray:

@@ -376,7 +376,7 @@ extern "C" int sbv_debug_ed25519_verify_registered_k(sbv_engine *e, size_t n, co
     return SBV_OK;
 }
 
-// The cached table of one key on device `device_index` (sbv_key_cache_reserve): key = the exact key bytes of scheme s
+// The cached table of one key on device `device_index` (sbv_key_cache_reserve or _evicting): key = the exact key bytes of scheme s
 // (qx || qy: 64 / 96 bytes; the 32-byte Ed25519 encoding).  Returns 1 with the table in out (the words of the scheme's
 // per-launch table, as sbv_debug_grouped_key_table / sbv_debug_ed25519_comb_tab read it) when a READY slot holds the key,
 // 0 when none does or no cache is reserved.  Drains the device first.
@@ -389,6 +389,18 @@ extern "C" int sbv_debug_key_cache_entry(sbv_engine *e, int device_index, uint8_
     const size_t kw = sbv_group_ops(scheme).key_words, slots = (size_t)k.map.smask + 1;
     CU(e, cudaSetDevice(d.ordinal));
     CU(e, cudaDeviceSynchronize());
+    if (k.evicting) {  // key_cache_assoc.cuh: way i is pool entry i
+        std::vector<unsigned long long> st(k.capacity);
+        std::vector<uint32_t> kv(k.capacity * kw);
+        CU(e, cudaMemcpy(st.data(), k.amap.state, k.capacity * 8, cudaMemcpyDeviceToHost));
+        CU(e, cudaMemcpy(kv.data(), k.amap.keys, k.capacity * kw * 4, cudaMemcpyDeviceToHost));
+        for (size_t i = 0; i < k.capacity; i++) {
+            if ((st[i] & 3) != 2 || memcmp(&kv[i * kw], key, kw * 4) != 0) continue;
+            CU(e, cudaMemcpy(out, k.amap.pool + i * k.tw4 * 4, k.tw4 * 16, cudaMemcpyDeviceToHost));
+            return 1;
+        }
+        return 0;
+    }
     std::vector<uint32_t> state(slots), keys(slots * kw);
     CU(e, cudaMemcpy(state.data(), k.map.state, slots * 4, cudaMemcpyDeviceToHost));
     CU(e, cudaMemcpy(keys.data(), k.map.keys, slots * kw * 4, cudaMemcpyDeviceToHost));
@@ -400,4 +412,17 @@ extern "C" int sbv_debug_key_cache_entry(sbv_engine *e, int device_index, uint8_
         return 1;
     }
     return 0;
+}
+
+// The hash seed and set count of the evicting cache of scheme s on device `device_index` (key_cache_assoc.cuh: key w is in
+// set umulhi(kc_hash(w, seed), sets)), so that a test can predict which keys compete for one set.  Returns 1 with out[0] =
+// seed, out[1] = sets; 0 when no evicting cache is reserved.
+extern "C" int sbv_debug_key_cache_sets(sbv_engine *e, int device_index, uint8_t scheme, uint32_t *out) {
+    if (!e || scheme > SBV_ED25519 || !out || device_index < 0 || device_index >= (int)e->devs.size()) return SBV_ERR_ARG;
+    std::lock_guard<std::mutex> lk(e->mu);
+    const Dev::KeyCache &k = e->devs[device_index].kc[scheme];
+    if (!k.mem || !k.evicting) return 0;
+    out[0] = k.amap.seed;
+    out[1] = k.amap.sets;
+    return 1;
 }

@@ -96,10 +96,16 @@ struct Dev {
     uint32_t ed_n_slots = 0, ed_n_local = 0;
     // the opt-in cache of grouped-key tables across launches (sbv_key_cache_reserve), per scheme tag: one allocation holding
     // the pool, the counters, the map (key_cache.cuh) and one launch area per scratch set (2 + SBV_GROUP_MAX_KEYS words:
-    // the lookup's miss and hit counts and the renumbered keylist of the launch holding that set)
+    // the lookup's miss and hit counts and the renumbered keylist of the launch holding that set).  An evicting cache
+    // (sbv_key_cache_reserve_evicting) holds the set-associative map of key_cache_assoc.cuh instead, and stamps every
+    // grouped launch with the next value of `stamp` (taken under e->mu).
     struct KeyCache {
         void *mem = nullptr;
+        bool evicting = false;
         KcMap map{};
+        KcaMap amap{};
+        unsigned long long stamp = 0;
+        size_t capacity = 0;  // tables (evicting: rounded up to a multiple of KCA_WAYS)
         uint32_t *lk = nullptr;
         size_t lk_words = 0;
         size_t tw4 = 0;  // 16-byte words per table

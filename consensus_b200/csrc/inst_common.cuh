@@ -1,6 +1,7 @@
 // inst_common.cuh — launcher templates behind ops.h.  Each inst_*.cu instantiates one group for one curve.
 #pragma once
 #include "key_cache.cuh"
+#include "key_cache_assoc.cuh"
 #include "keygroup.cuh"
 #include "ops.h"
 
@@ -150,6 +151,22 @@ cudaError_t op_kc_insert(uint32_t kcap, const uint32_t *lk, const uint8_t *qx, c
                          const uint32_t *ktab, cudaStream_t st) {
     k_kc_insert<<<(unsigned)(((size_t)kcap * 32 + 127) / 128), 128, 0, st>>>(kcap, lk, KcXY<C>{qx, qy}, c, tw4, keyflags,
                                                                             reinterpret_cast<const uint4 *>(ktab));
+    return cudaGetLastError();
+}
+
+template <class C>
+cudaError_t op_kca_lookup(const uint32_t *nkeys_ptr, uint32_t kcap, const uint32_t *keylist, const uint8_t *qx, const uint8_t *qy, KcaMap c,
+                          unsigned long long now, uint32_t tw4, int32_t *keyid, uint32_t *lk, uint8_t *keyflags, uint32_t *ktab, cudaStream_t st) {
+    k_kca_lookup<<<(unsigned)(((size_t)kcap * 32 + 127) / 128), 128, 0, st>>>(nkeys_ptr, kcap, keylist, KcXY<C>{qx, qy}, c, now, tw4, keyid, lk,
+                                                                             keyflags, reinterpret_cast<uint4 *>(ktab));
+    return cudaGetLastError();
+}
+
+template <class C>
+cudaError_t op_kca_insert(uint32_t kcap, const uint32_t *lk, const uint8_t *qx, const uint8_t *qy, KcaMap c, unsigned long long now, uint32_t tw4,
+                          const uint8_t *keyflags, const uint32_t *ktab, cudaStream_t st) {
+    k_kca_insert<<<(unsigned)(((size_t)kcap * 32 + 127) / 128), 128, 0, st>>>(kcap, lk, KcXY<C>{qx, qy}, c, now, tw4, keyflags,
+                                                                             reinterpret_cast<const uint4 *>(ktab));
     return cudaGetLastError();
 }
 

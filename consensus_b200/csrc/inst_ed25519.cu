@@ -8,6 +8,7 @@
 #include "ed25519_keyed.cuh"
 #include "ed25519_verify.cuh"
 #include "key_cache.cuh"
+#include "key_cache_assoc.cuh"
 #include "keygroup.cuh"
 #include "sha512.cuh"
 
@@ -48,7 +49,8 @@ int sbv_ed_btab_ensure(sbv_engine *e, Dev &d) {
 //
 // Keys whose 32 bytes occur at least group_threshold times get a comb table (ed25519_comb.cuh) and their items take
 // k_ed_verify_comb; the table construction (latency-bound: one doubling chain per key) runs beside SHA-512.  With a key
-// cache reserved, k_kc_lookup runs after k_kg_assign and k_kc_insert after k_edc_final, as for ECDSA.
+// cache reserved, k_kc_lookup runs after k_kg_assign and k_kc_insert after k_edc_final, as for ECDSA (k_kca_lookup and
+// k_kca_insert for an evicting cache).
 namespace {
 constexpr KtGeom ED_COMB_GEOM{EDC_BASES_WORDS, EDC_HS_WORDS, EDC_ZTOP_WORDS, EDC_TAB_WORDS};
 static_assert(EDC_TAB_WORDS == 2 * 255 * SBV_ED_BTAB_ENTRY_WORDS, "debug.cu: sbv_debug_ed25519_comb_tab's table of 510 entries");
@@ -83,6 +85,20 @@ cudaError_t edg_cache_insert(uint32_t kcap, const uint32_t *lk, const uint8_t *p
                              const uint32_t *ktab, cudaStream_t st) {
     k_kc_insert<<<(unsigned)(((size_t)kcap * 32 + 127) / 128), 128, 0, st>>>(kcap, lk, KcKey32{pub}, c, tw4, keyflags,
                                                                             reinterpret_cast<const uint4 *>(ktab));
+    return cudaGetLastError();
+}
+
+cudaError_t edg_evict_lookup(const uint32_t *nkeys_ptr, uint32_t kcap, const uint32_t *keylist, const uint8_t *pub, const uint8_t *, KcaMap c,
+                             unsigned long long now, uint32_t tw4, int32_t *keyid, uint32_t *lk, uint8_t *keyflags, uint32_t *ktab, cudaStream_t st) {
+    k_kca_lookup<<<(unsigned)(((size_t)kcap * 32 + 127) / 128), 128, 0, st>>>(nkeys_ptr, kcap, keylist, KcKey32{pub}, c, now, tw4, keyid, lk, keyflags,
+                                                                             reinterpret_cast<uint4 *>(ktab));
+    return cudaGetLastError();
+}
+
+cudaError_t edg_evict_insert(uint32_t kcap, const uint32_t *lk, const uint8_t *pub, const uint8_t *, KcaMap c, unsigned long long now, uint32_t tw4,
+                             const uint8_t *keyflags, const uint32_t *ktab, cudaStream_t st) {
+    k_kca_insert<<<(unsigned)(((size_t)kcap * 32 + 127) / 128), 128, 0, st>>>(kcap, lk, KcKey32{pub}, c, now, tw4, keyflags,
+                                                                             reinterpret_cast<const uint4 *>(ktab));
     return cudaGetLastError();
 }
 
@@ -138,7 +154,7 @@ int ed_comb_k(sbv_engine *e, Dev &d, const VerifyLaunch &vl, const uint8_t *d_si
 }
 }  // namespace
 
-const GroupOps sbv_group_ed25519 = {&ED_COMB, KcKey32::W, 4, edg_group, edg_cache_lookup, edg_cache_insert};
+const GroupOps sbv_group_ed25519 = {&ED_COMB, KcKey32::W, 4, edg_group, edg_cache_lookup, edg_cache_insert, edg_evict_lookup, edg_evict_insert};
 
 int sbv_launch_ed25519(sbv_engine *e, Dev &d, size_t n, const uint8_t *d_msgs, const uint64_t *d_off, uint64_t base, const uint8_t *d_sig,
                        const uint8_t *d_pub, uint32_t *d_k, uint32_t *d_perm, uint8_t *d_ok, cudaStream_t st) {

@@ -66,6 +66,11 @@ struct GroupOps {
                                 uint32_t tw4, int32_t *keyid, uint32_t *lk, uint8_t *keyflags, uint32_t *ktab, cudaStream_t st);
     cudaError_t (*cache_insert)(uint32_t kcap, const uint32_t *lk, const uint8_t *qx, const uint8_t *qy, KcMap c, uint32_t tw4, const uint8_t *keyflags,
                                 const uint32_t *ktab, cudaStream_t st);
+    // the evicting cache (key_cache_assoc.cuh): k_kca_lookup / k_kca_insert in the same places; now = the launch's stamp
+    cudaError_t (*evict_lookup)(const uint32_t *nkeys_ptr, uint32_t kcap, const uint32_t *keylist, const uint8_t *qx, const uint8_t *qy, KcaMap c,
+                                unsigned long long now, uint32_t tw4, int32_t *keyid, uint32_t *lk, uint8_t *keyflags, uint32_t *ktab, cudaStream_t st);
+    cudaError_t (*evict_insert)(uint32_t kcap, const uint32_t *lk, const uint8_t *qx, const uint8_t *qy, KcaMap c, unsigned long long now, uint32_t tw4,
+                                const uint8_t *keyflags, const uint32_t *ktab, cudaStream_t st);
 };
 
 #define SBV_COZ_DECL(NAME)                                                                                                          \

@@ -13,7 +13,9 @@
 // A large host-buffer batch runs the part after the table fork chunk by chunk, as its chunks arrive.
 // Registered keys (sbv_set_keys) skip the grouping: their tables were built at registration.
 // With a key cache reserved (sbv_key_cache_reserve), k_kc_lookup runs after k_kg_assign on st and k_kc_insert after
-// the table construction on s_tab (key_cache.cuh): the build then makes only the tables the cache does not hold.
+// the table construction on s_tab (key_cache.cuh): the build then makes only the tables the cache does not hold.  An
+// evicting cache (sbv_key_cache_reserve_evicting) runs k_kca_lookup and k_kca_insert in the same places
+// (key_cache_assoc.cuh).
 // The first half up to the fork and the table construction is one function for P-256, P-384 and Ed25519 (verify_begin),
 // driven by the scheme's entry of the grouping table (ops.h: GroupOps); Ed25519's second half is in inst_ed25519.cu.
 #include "engine.h"
@@ -201,17 +203,23 @@ int verify_begin(sbv_engine *e, Dev &d, uint8_t scheme, size_t n, const uint8_t 
     CU(e, cudaMemsetAsync(w->zeroed, 0, (n + 4 + 4 * (size_t)chunks) * 4, st));
     CU(e, g.group((uint32_t)n, d_qx, d_qy, e->hash_seed, w->hsize - 1, w->htab, w->rep, kcnt, T, (uint32_t)kcap, w->keyid, w->keylist, counters, st));
     // with a key cache: the lookup renumbers the keys (misses first), copies the hits' tables, and the build makes the misses
-    const Dev::KeyCache &kc = d.kc[scheme];
+    // (an evicting cache: the same with the launch's stamp, key_cache_assoc.cuh)
+    Dev::KeyCache &kc = d.kc[scheme];
     uint32_t *lk = sbv_key_cache_area(d, scheme, w, kcap);
+    const unsigned long long now = lk && kc.evicting ? ++kc.stamp : 0;
     if (lk) {
         CU(e, cudaMemsetAsync(lk, 0, 8, st));
-        CU(e, g.cache_lookup(counters, (uint32_t)kcap, w->keylist, d_qx, d_qy, kc.map, (uint32_t)kc.tw4, w->keyid, lk, w->keyflags, w->ktab, st));
+        if (kc.evicting)
+            CU(e, g.evict_lookup(counters, (uint32_t)kcap, w->keylist, d_qx, d_qy, kc.amap, now, (uint32_t)kc.tw4, w->keyid, lk, w->keyflags, w->ktab, st));
+        else
+            CU(e, g.cache_lookup(counters, (uint32_t)kcap, w->keylist, d_qx, d_qy, kc.map, (uint32_t)kc.tw4, w->keyid, lk, w->keyflags, w->ktab, st));
     }
     CU(e, cudaEventRecord(w->ev_group, st));
     CU(e, cudaStreamWaitEvent(w->s_tab, w->ev_group, 0));
     CU(e, g.kt->build(lk ? lk : counters, (uint32_t)kcap, lk ? lk + 2 : w->keylist, d_qx, d_qy, w->bases, w->hs, w->ztop, w->pref, w->ktab, w->keyflags,
                       w->s_tab));
-    if (lk) CU(e, g.cache_insert((uint32_t)kcap, lk, d_qx, d_qy, kc.map, (uint32_t)kc.tw4, w->keyflags, w->ktab, w->s_tab));
+    if (lk && kc.evicting) CU(e, g.evict_insert((uint32_t)kcap, lk, d_qx, d_qy, kc.amap, now, (uint32_t)kc.tw4, w->keyflags, w->ktab, w->s_tab));
+    else if (lk) CU(e, g.cache_insert((uint32_t)kcap, lk, d_qx, d_qy, kc.map, (uint32_t)kc.tw4, w->keyflags, w->ktab, w->s_tab));
     CU(e, cudaEventRecord(w->ev_tab, w->s_tab));
     e->launches += 2 + g.build_launches + (lk ? 2 : 0);  // grouping + table construction (+ cache lookup and insert)
     return 0;

@@ -281,8 +281,9 @@ int sbv_verify_registered_device(sbv_engine *e, int device_index, uint8_t curve,
  *    hash alone.
  *  - Only keys whose build flags them valid are inserted: an off-curve ECDSA key or an undecodable Ed25519 key is rebuilt,
  *    and rejected, in every launch.
- *  - Fill once, no eviction: a full cache stops inserting.  Reserving again empties it (for example on a
- *    reconfiguration).  It is independent of both registries and of verification_seq.
+ *  - Fill once, no eviction: a full cache stops inserting (sbv_key_cache_reserve_evicting below reserves a cache that
+ *    replaces its least recently used entries instead).  Reserving again empties it (for example on a reconfiguration).
+ *    It is independent of both registries and of verification_seq.
  *  - One cache per device: each device caches the keys of its own shards.
  *  - Two launches that miss the same key at once both build it; one of them inserts it.
  *
@@ -298,6 +299,29 @@ int sbv_key_cache_reserve(sbv_engine *e, size_t p256, size_t p384, size_t ed2551
  * out[2] grouped keys served from the cache (hits), out[3] grouped valid keys built in the launch while a cache was
  * reserved (misses; invalid keys count as neither).  All zero without a cache. */
 int sbv_key_cache_stats(sbv_engine *e, uint8_t scheme, uint64_t out[4]);
+/* The evicting mode: reserves, on every device, caches that replace entries when full, so that the keys in use now stay
+ * resident when the client population outgrows the cache or changes over time.  Which keys are served is as above: only
+ * grouped keys, compared byte for byte, only valid keys inserted, one cache per device, and a table is a pure function of
+ * the key bytes, so verdicts, routing and launch count are bit for bit those of an engine without a cache (the same two
+ * extra launches per grouped launch as the fill-once mode).
+ *  - Set-associative, 16 ways per set.  A requested capacity is rounded up to a multiple of 16 (out[0] of both stats calls
+ *    reports the rounded capacity); the key bytes' hash picks the set.
+ *  - Replacement: least recently used within the set, where "used" means looked up as a hit or inserted, ordered by a
+ *    launch sequence number (one per grouped launch, per device and scheme).  A missed valid key takes an empty way, else
+ *    the set's least recently used way that no launch is copying out of and that no launch at or after its own has used:
+ *    a launch never evicts a table it has used itself.  With none, the insert is given up and counted.
+ *  - Two launches that miss the same key at once may both insert it; both entries hold the same table.
+ * The sizes per key are those of sbv_key_cache_reserve, plus 16 bytes of map per way beside the key bytes.  Works like
+ * sbv_key_cache_reserve otherwise: per device and per scheme it replaces and empties any earlier cache of either mode,
+ * (0, 0, 0) frees it, it excludes concurrent launches and drains every device, and SBV_ERR_NOMEM leaves no cache on any
+ * device. */
+int sbv_key_cache_reserve_evicting(sbv_engine *e, size_t p256, size_t p384, size_t ed25519);
+/* out[0..3] as sbv_key_cache_stats; out[4] evictions (valid tables replaced by another key's table); out[5] inserts given
+ * up (a missed valid key that found no way it could take: every way of its set busy with another key, being read, or
+ * used by its own or a later launch).  The fill-once mode counts neither: out[4] is 0 as it never evicts, and out[5] is 0
+ * because its kernels are left as they were (a full fill-once cache gives up every insert: out[3] - out[1] of them, less
+ * the keys two launches inserted at once).  SBV_ERR_ARG for a scheme tag above SBV_ED25519 or a null out. */
+int sbv_key_cache_stats_ex(sbv_engine *e, uint8_t scheme, uint64_t out[6]);
 
 /* ---- one process per GPU (a Go host may run one node process per device; bench.py does under torchrun) ----
  * The engine of every process is one RANK; the only exchange is the all-gather of packed verdict / quorum bitmasks

@@ -63,7 +63,30 @@ func WithClientKeysPerItem() Option { return func(v *Verifier) { v.clientKeysPer
 // fills once and is never evicted; each key costs 32 KiB (P-256), 118 KiB (P-384) or 47.8 KiB (Ed25519) of device memory
 // per GPU. Verdicts are the same with or without it. Off by default.
 func WithKeyCache(p256, p384, ed25519 int) Option {
-	return func(v *Verifier) { v.keyCache = [3]int{p256, p384, ed25519} }
+	return func(v *Verifier) { v.keyCache, v.keyCacheEvicting = [3]int{p256, p384, ed25519}, false }
+}
+
+// WithEvictingKeyCache is WithKeyCache with a cache that replaces its least recently used tables when full
+// (sbv_key_cache_reserve_evicting): for client populations larger than the cache, or that change over time. Each capacity
+// is rounded up to a multiple of 16. Give it more ways than the clients that should stay resident, because keys hash into
+// sets of 16 unevenly: 4,096 ways held all of 1,024 hot keys, and 1,024 ways held 921. Verdicts are the same with or
+// without it. Off by default.
+func WithEvictingKeyCache(p256, p384, ed25519 int) Option {
+	return func(v *Verifier) { v.keyCache, v.keyCacheEvicting = [3]int{p256, p384, ed25519}, true }
+}
+
+// KeyCacheStats returns, for scheme 0 (P-256), 1 (P-384) or 2 (Ed25519), the capacity, resident tables, hits, misses,
+// evictions and inserts given up of the grouped-key cache, summed over devices (sbv_key_cache_stats_ex).
+func (v *Verifier) KeyCacheStats(scheme uint8) ([6]uint64, error) {
+	var out [6]C.uint64_t
+	if rc := C.sbv_key_cache_stats_ex(v.eng, C.uint8_t(scheme), &out[0]); rc != 0 {
+		return [6]uint64{}, fmt.Errorf("sbv_key_cache_stats_ex failed: %d: %s", int(rc), C.GoString(C.sbv_last_error(v.eng)))
+	}
+	var r [6]uint64
+	for i := range out {
+		r[i] = uint64(out[i])
+	}
+	return r, nil
 }
 
 // Verifier implements api.Verifier.
@@ -85,7 +108,8 @@ type Verifier struct {
 
 	clientKeysPerItem bool                 // WithClientKeysPerItem
 	clientKeys        map[string]clientKey // client keys kept on the host (WithClientKeysPerItem)
-	keyCache          [3]int               // WithKeyCache: tables per scheme
+	keyCache          [3]int               // WithKeyCache / WithEvictingKeyCache: tables per scheme
+	keyCacheEvicting  bool                 // WithEvictingKeyCache
 
 	pool sync.Pool // *pinned: one block of page-locked memory per in-flight batch
 
@@ -108,8 +132,16 @@ func New(devices []int, opts ...Option) (*Verifier, error) {
 		o(v)
 	}
 	if c := v.keyCache; c != [3]int{} {
-		if rc := C.sbv_key_cache_reserve(eng, C.size_t(c[0]), C.size_t(c[1]), C.size_t(c[2])); rc != 0 {
-			err := fmt.Errorf("sbv_key_cache_reserve failed: %d: %s", int(rc), C.GoString(C.sbv_last_error(eng)))
+		name := "sbv_key_cache_reserve"
+		var rc C.int
+		if v.keyCacheEvicting {
+			name = "sbv_key_cache_reserve_evicting"
+			rc = C.sbv_key_cache_reserve_evicting(eng, C.size_t(c[0]), C.size_t(c[1]), C.size_t(c[2]))
+		} else {
+			rc = C.sbv_key_cache_reserve(eng, C.size_t(c[0]), C.size_t(c[1]), C.size_t(c[2]))
+		}
+		if rc != 0 {
+			err := fmt.Errorf("%s failed: %d: %s", name, int(rc), C.GoString(C.sbv_last_error(eng)))
 			C.sbv_destroy(eng)
 			return nil, err
 		}

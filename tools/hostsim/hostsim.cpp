@@ -17,6 +17,7 @@ namespace sbv { uint32_t tab[1 << 18]; }
 #include "../../consensus_b200/csrc/debug_ops.cuh"
 #include "../../consensus_b200/csrc/keygroup.cuh"
 #include "../../consensus_b200/csrc/key_cache.cuh"
+#include "../../consensus_b200/csrc/key_cache_assoc.cuh"
 #include "../../consensus_b200/csrc/sha256.cuh"
 #include "../../consensus_b200/csrc/sha384.cuh"
 #include "../../consensus_b200/csrc/quorum.cuh"
@@ -836,4 +837,47 @@ extern "C" uint32_t hs_kc_slot(int fam, const uint8_t *a, const uint8_t *b, uint
         h = fp ? kc_fp(w, seed) : kc_hash(w, seed) & smask;
     });
     return h;
+}
+
+// ---- the evicting key cache (key_cache_assoc.cuh) ----
+// The cache of one family as caller-owned arrays: state and stamp (u64) and keys of sets * KCA_WAYS ways, pool: one table
+// of tw4 16-byte words per way, stats: 6 counters.  fam as for hs_kc_lookup; now: the launch's stamp.
+static KcaMap hs_kca_map(unsigned long long *state, unsigned long long *stamp, uint32_t *keys, uint32_t *pool, unsigned long long *stats, uint32_t sets,
+                         uint32_t seed) {
+    return KcaMap{state, stamp, keys, pool, stats, sets, seed};
+}
+// k_kca_lookup over the launch's grouped keys (count *nkeys, key k = item keylist[k]); lk: 2 + kcap words, zeroed here
+extern "C" int hs_kca_lookup(int fam, const uint8_t *a, const uint8_t *b, const uint32_t *nkeys, uint32_t kcap, const uint32_t *keylist,
+                             unsigned long long *state, unsigned long long *stamp, uint32_t *keys, uint32_t *pool, unsigned long long *stats, uint32_t sets,
+                             uint32_t seed, unsigned long long now, uint32_t tw4, int32_t *keyid, uint32_t *lk, uint8_t *keyflags, uint32_t *ktab) {
+    const KcaMap c = hs_kca_map(state, stamp, keys, pool, stats, sets, seed);
+    lk[0] = lk[1] = 0;
+    return hs_kc_fam(fam, a, b, [&](auto key) {
+        run_grid_lockstep((unsigned)(((size_t)kcap * 32 + 127) / 128), 128, [&] {
+            k_kca_lookup(nkeys, kcap, keylist, key, c, now, tw4, keyid, lk, keyflags, reinterpret_cast<uint4 *>(ktab));
+        });
+    });
+}
+// k_kca_insert after the build of the launch's misses (ktab[0, lk[0]), keyflags)
+extern "C" int hs_kca_insert(int fam, const uint8_t *a, const uint8_t *b, uint32_t kcap, const uint32_t *lk, unsigned long long *state,
+                             unsigned long long *stamp, uint32_t *keys, uint32_t *pool, unsigned long long *stats, uint32_t sets, uint32_t seed,
+                             unsigned long long now, uint32_t tw4, const uint8_t *keyflags, const uint32_t *ktab) {
+    const KcaMap c = hs_kca_map(state, stamp, keys, pool, stats, sets, seed);
+    return hs_kc_fam(fam, a, b, [&](auto key) {
+        run_grid_lockstep((unsigned)(((size_t)kcap * 32 + 127) / 128), 128, [&] {
+            k_kca_insert(kcap, lk, key, c, now, tw4, keyflags, reinterpret_cast<const uint4 *>(ktab));
+        });
+    });
+}
+// the set of item i's key (its first way is set * KCA_WAYS), and in *fp its fingerprint as the state word holds it
+extern "C" uint32_t hs_kca_set(int fam, const uint8_t *a, const uint8_t *b, uint32_t i, uint32_t seed, uint32_t sets, unsigned long long *fp) {
+    uint32_t set = 0;
+    hs_kc_fam(fam, a, b, [&](auto key) {
+        uint32_t w[decltype(key)::W];
+        key.load(i, w);
+        const KcaMap c{nullptr, nullptr, nullptr, nullptr, nullptr, sets, seed};
+        set = kca_base(c, w) / KCA_WAYS;
+        *fp = kca_fp(w, seed);
+    });
+    return set;
 }

@@ -18,7 +18,8 @@ terminate, so mutants only ever run in the CPU simulation.
 
 Not covered, because the CPU simulation does not compile it: the PTX branch of the carry primitives in mp.cuh (the
 simulation emulates the carry flag in C++) and every `#if defined(__CUDA_ARCH__)` block (warp-aggregated atomics of
-k_kg_insert and k_kg_route).
+k_kg_insert and k_kg_route), nor the re-check of key_cache_assoc.cuh's pin after a lost CAS, which only a concurrent
+launch can reach (the simulation runs one warp at a time).
 
     python tools/mutants.py -j 8                 # the whole catalogue
     python tools/mutants.py --only final_check_pmn mod_inv_cap_32n
@@ -47,6 +48,7 @@ SHARDS = ["tests/test_hostsim_shards.py"]
 WIDE = ["tests/test_hostsim_wide.py"]  # bit lengths, offsets and byte sums past 32 bits
 SHA384 = ["tests/test_hostsim_sha384.py"]
 KEY_CACHE = ["tests/test_hostsim_key_cache.py"]
+KEY_CACHE_EVICT = ["tests/test_hostsim_key_cache_evict.py"]
 SEEDED = ["tests/test_hostsim_seeded_passes.py"]
 COMB_WARP = ["tests/test_hostsim_comb_warp.py"]  # the comb build a warp per key against the one-thread-per-chain reference  # the first entry of a pass loaded, not added (pt_seed)
 
@@ -371,6 +373,47 @@ CATALOGUE = [
     M("kc_insert_publish", "key_cache.cuh", "kc_store_release(c.state + slot, kc_fp<KV::W>(w, c.seed) | KC_READY);",
       "kc_store_release(c.state + slot, kc_fp<KV::W>(w, c.seed) | KC_BUSY);", KEY_CACHE),
     M("kc_insert_resident_count", "key_cache.cuh", "atomicAdd(c.stats + 1, 1ull);", "(void)0;", KEY_CACHE),
+    # ---------------------------------------------------------------- key_cache_assoc.cuh
+    M("kca_lookup_busy_candidate", "key_cache_assoc.cuh", "lane < KCA_WAYS && (s & ~KCA_PINS) == (fp | KC_READY));",
+      "lane < KCA_WAYS && (s >> 32) == (fp >> 32));", KEY_CACHE_EVICT,
+      equivalent="kca_pin re-reads the state word and pins only a READY word with the fingerprint: a BUSY candidate is a miss either way",
+      proof="tests/test_hostsim_key_cache_evict.py::test_busy_way_is_a_miss_and_blocks_an_insert_of_its_fingerprint"),
+    M("kca_pin_no_compare", "key_cache_assoc.cuh", "if (kca_same<W>(c, way, w)) return (int32_t)way;", "return (int32_t)way;", KEY_CACHE_EVICT),
+    M("kca_pin_mismatch_kept", "key_cache_assoc.cuh", "atomicAdd(c.state + way, 0ull - KCA_PIN);  // refilled", "(void)0;  // refilled", KEY_CACHE_EVICT),
+    M("kca_same_half_key", "key_cache_assoc.cuh", "for (int k = 0; k < W; k++) diff |= kc_ld(s + k) ^ w[k];",
+      "for (int k = 0; k < W / 2; k++) diff |= kc_ld(s + k) ^ w[k];", KEY_CACHE_EVICT),
+    M("kca_lookup_no_clamp", "key_cache_assoc.cuh", "if (nk > kcap) nk = kcap;", "(void)0;", KEY_CACHE_EVICT),
+    M("kca_lookup_hit_id", "key_cache_assoc.cuh", "id = (int32_t)(nk - 1 - atomicAdd(lk + 1, 1u));", "id = (int32_t)(nk - atomicAdd(lk + 1, 1u));",
+      KEY_CACHE_EVICT),
+    M("kca_lookup_hit_flag", "key_cache_assoc.cuh", "keyflags[id] = 1;", "(void)0;", KEY_CACHE_EVICT),
+    M("kca_lookup_no_stamp", "key_cache_assoc.cuh", "atomicMax(c.stamp + way, now);", "(void)0;", KEY_CACHE_EVICT),
+    M("kca_lookup_hit_count", "key_cache_assoc.cuh", "atomicAdd(c.stats + 2, 1ull);", "(void)0;", KEY_CACHE_EVICT),
+    M("kca_lookup_no_unpin", "key_cache_assoc.cuh", "        __threadfence();\n        atomicAdd(c.state + way, 0ull - KCA_PIN);\n    }",
+      "        __threadfence();\n    }", KEY_CACHE_EVICT),
+    M("kca_lookup_copy_stride", "key_cache_assoc.cuh", "for (uint32_t i = lane; i < tw4; i += 32) dst[i] = kc_ld(src + i);",
+      "for (uint32_t i = lane; i < tw4; i += 64) dst[i] = kc_ld(src + i);", KEY_CACHE_EVICT),
+    M("kca_insert_invalid", "key_cache_assoc.cuh", "if (k >= m || !keyflags[k]) return;", "if (k >= m) return;", KEY_CACHE_EVICT),
+    M("kca_insert_miss_count", "key_cache_assoc.cuh", "if (lane == 0) atomicAdd(c.stats + 3, 1ull);", "(void)0;", KEY_CACHE_EVICT),
+    M("kca_insert_past_busy", "key_cache_assoc.cuh", "(st == KC_BUSY || (st == KC_READY && kca_same<KV::W>(c, base + lane, w)));",
+      "(st == KC_READY && kca_same<KV::W>(c, base + lane, w));", KEY_CACHE_EVICT),
+    M("kca_insert_duplicate", "key_cache_assoc.cuh", "(st == KC_BUSY || (st == KC_READY && kca_same<KV::W>(c, base + lane, w)));",
+      "(st == KC_BUSY);", KEY_CACHE_EVICT),
+    M("kca_insert_evict_pinned", "key_cache_assoc.cuh", "if (lane < KCA_WAYS && st == KC_READY && (s & KCA_PINS) == 0) {",
+      "if (lane < KCA_WAYS && st == KC_READY) {", KEY_CACHE_EVICT),
+    M("kca_insert_evict_current", "key_cache_assoc.cuh", "if (a < now) age = a;", "age = a;", KEY_CACHE_EVICT),
+    M("kca_insert_not_lru", "key_cache_assoc.cuh", "lo = o < lo ? o : lo;", "lo = o > lo && o != ~0ull ? o : lo;", KEY_CACHE_EVICT),
+    M("kca_insert_evict_before_empty", "key_cache_assoc.cuh", "const unsigned pick = empty ? empty : __ballot_sync(",
+      "const unsigned pick = !empty ? empty : __ballot_sync(", KEY_CACHE_EVICT),
+    M("kca_insert_no_stamp", "key_cache_assoc.cuh", "c.stamp[way] = now;", "(void)0;", KEY_CACHE_EVICT),
+    M("kca_insert_key_words", "key_cache_assoc.cuh", "for (int i = 0; i < KV::W; i++) kw[i] = w[i];", "for (int i = 1; i < KV::W; i++) kw[i] = w[i];",
+      KEY_CACHE_EVICT),
+    M("kca_insert_pool_entry", "key_cache_assoc.cuh", "uint4 *dst = reinterpret_cast<uint4 *>(c.pool) + (size_t)way * tw4;",
+      "uint4 *dst = reinterpret_cast<uint4 *>(c.pool) + (size_t)way;", KEY_CACHE_EVICT),
+    M("kca_insert_publish", "key_cache_assoc.cuh", "kca_store_release(c.state + way, fp | KC_READY);", "kca_store_release(c.state + way, fp | KC_BUSY);",
+      KEY_CACHE_EVICT),
+    M("kca_insert_counter", "key_cache_assoc.cuh", "atomicAdd(c.stats + (evict ? 4 : 1), 1ull);", "atomicAdd(c.stats + 1, 1ull);", KEY_CACHE_EVICT),
+    M("kca_insert_give_up_count", "key_cache_assoc.cuh", "if (lane == 0 && !there) atomicAdd(c.stats + 5, 1ull);", "(void)0;", KEY_CACHE_EVICT),
+    M("kca_set_index", "key_cache_assoc.cuh", "return __umulhi(kc_hash<W>(w, c.seed), c.sets) * KCA_WAYS;", "return 0;", KEY_CACHE_EVICT),
 ]
 
 
