@@ -51,6 +51,7 @@ KEY_CACHE = ["tests/test_hostsim_key_cache.py"]
 KEY_CACHE_EVICT = ["tests/test_hostsim_key_cache_evict.py"]
 SEEDED = ["tests/test_hostsim_seeded_passes.py"]
 COMB_WARP = ["tests/test_hostsim_comb_warp.py"]  # the comb build a warp per key against the one-thread-per-chain reference  # the first entry of a pass loaded, not added (pt_seed)
+TABLE_SHAPES = ["tests/test_hostsim_table_shapes.py"]  # every entry of the per-key tables at the key counts where the builds turn over
 
 
 def M(id, file, find, repl, tests, equivalent=None, proof=None):
@@ -304,6 +305,39 @@ CATALOGUE = [
     M("edc_mask_high_row", "ed25519_comb.cuh", "m |= ((v >> (16 + j)) & 1u) << (2 * w + 1);", "(void)0;", ED),
     M("edc_verify_s_range", "ed25519_comb.cuh", "if (!sc_lt_order(s)) { ok_out[idx] = 0; return; }", "(void)s;", ED),
     M("edc_verify_doubling_step", "ed25519_comb.cuh", "if (key && step && (step & 1) == 0) ed_double<true>(acc);", "if (key && step && (step & 3) == 0) ed_double<true>(acc);", ED),
+    # the grids and the [...][cap] scratch of the per-key builds: faults that damage only the keys past a block or a
+    # chunk, or only a launch whose capacity is not its key count (test_hostsim_table_shapes.py runs those shapes).
+    # The Ed25519 files alone kill each of these as well, through verdicts and the tables of a few keys
+    # (test_hostsim_ed25519_grouped.py: the threshold test's launch of 4 slots for 3 keys, the crafted-k and pipeline
+    # runs; test_hostsim_ed25519_registered.py: the tables of 4 keys and the chunked build)
+    M("edc_bases_block_index", "ed25519_comb.cuh",
+      "const uint32_t q = blockIdx.x * blockDim.x + threadIdx.x;\n    uint32_t nkeys = __ldg(nkeys_ptr);\n    if (nkeys > cap) nkeys = cap;\n    if (q >= nkeys) return;",
+      "const uint32_t q = threadIdx.x;\n    uint32_t nkeys = __ldg(nkeys_ptr);\n    if (nkeys > cap) nkeys = cap;\n    if (q >= nkeys) return;", TABLE_SHAPES + ED),
+    M("edc_inv_block_index", "ed25519_comb.cuh",
+      "const uint32_t q = blockIdx.x * blockDim.x + threadIdx.x;\n    uint32_t nkeys = __ldg(nkeys_ptr);\n    if (nkeys > cap) nkeys = cap;\n    if (q >= nkeys || !keyflags[q]) return;",
+      "const uint32_t q = threadIdx.x;\n    uint32_t nkeys = __ldg(nkeys_ptr);\n    if (nkeys > cap) nkeys = cap;\n    if (q >= nkeys || !keyflags[q]) return;", TABLE_SHAPES + ED),
+    M("edc_fill_split_by_cap", "ed25519_comb.cuh", "const uint32_t q = t % nkeys, ch = t / nkeys;\n    if (!keyflags[q]) return;\n    const int b = (int)(ch >> 4), hi = (int)(ch & 15);\n    uint32_t *tab = ctab + (size_t)q * EDC_TAB_WORDS + (size_t)b * EDC_ENT * ED_BWORDS;\n    EdP P;",
+      "const uint32_t q = t % cap, ch = t / cap;\n    if (!keyflags[q]) return;\n    const int b = (int)(ch >> 4), hi = (int)(ch & 15);\n    uint32_t *tab = ctab + (size_t)q * EDC_TAB_WORDS + (size_t)b * EDC_ENT * ED_BWORDS;\n    EdP P;", TABLE_SHAPES + ED),
+    M("edc_final_split_by_cap", "ed25519_comb.cuh", "const uint32_t q = t % nkeys, ch = t / nkeys;\n    if (!keyflags[q]) return;\n    const int b = (int)(ch >> 4), hi = (int)(ch & 15);\n    uint32_t *tab = ctab + (size_t)q * EDC_TAB_WORDS + (size_t)b * EDC_ENT * ED_BWORDS;\n    uint32_t inv[8], d2[8];",
+      "const uint32_t q = t % cap, ch = t / cap;\n    if (!keyflags[q]) return;\n    const int b = (int)(ch >> 4), hi = (int)(ch & 15);\n    uint32_t *tab = ctab + (size_t)q * EDC_TAB_WORDS + (size_t)b * EDC_ENT * ED_BWORDS;\n    uint32_t inv[8], d2[8];", TABLE_SHAPES + ED),
+    M("edc_fill_table_mod_32", "ed25519_comb.cuh", "uint32_t *tab = ctab + (size_t)q * EDC_TAB_WORDS + (size_t)b * EDC_ENT * ED_BWORDS;\n    EdP P;",
+      "uint32_t *tab = ctab + (size_t)(q % 32) * EDC_TAB_WORDS + (size_t)b * EDC_ENT * ED_BWORDS;\n    EdP P;", TABLE_SHAPES + ED),
+    M("edc_final_table_mod_32", "ed25519_comb.cuh", "uint32_t *tab = ctab + (size_t)q * EDC_TAB_WORDS + (size_t)b * EDC_ENT * ED_BWORDS;\n    uint32_t inv[8], d2[8];",
+      "uint32_t *tab = ctab + (size_t)(q % 32) * EDC_TAB_WORDS + (size_t)b * EDC_ENT * ED_BWORDS;\n    uint32_t inv[8], d2[8];", TABLE_SHAPES + ED),
+    M("edc_bases_stride_nkeys", "ed25519_comb.cuh", "        }\n        uint32_t *o = bases + (size_t)c * 32 * cap + q;",
+      "        }\n        uint32_t *o = bases + (size_t)c * 32 * nkeys + q;", TABLE_SHAPES + ED),
+    M("edc_hs_stride_nkeys", "ed25519_comb.cuh", "uint32_t *hp = hs + ((size_t)ch * EDC_CHAIN + s) * 8 * cap + q;\n#pragma unroll\n        for (int i = 0; i < 8; i++) { o[i] = P.X[i];",
+      "uint32_t *hp = hs + ((size_t)ch * EDC_CHAIN + s) * 8 * nkeys + q;\n#pragma unroll\n        for (int i = 0; i < 8; i++) { o[i] = P.X[i];", TABLE_SHAPES + ED),
+    M("edc_ztop_stride_nkeys", "ed25519_comb.cuh", "uint32_t *zp = ztop + (size_t)ch * 8 * cap + q;\n#pragma unroll\n    for (int i = 0; i < 8; i++) zp[(size_t)i * cap] = run[i];",
+      "uint32_t *zp = ztop + (size_t)ch * 8 * nkeys + q;\n#pragma unroll\n    for (int i = 0; i < 8; i++) zp[(size_t)i * cap] = run[i];", TABLE_SHAPES + ED),
+    M("edc_pref_stride_nkeys", "ed25519_comb.cuh", "uint32_t *pp = pref + (size_t)ch * 8 * cap + q;\n#pragma unroll\n        for (int i = 0; i < 8; i++) { z[i] = zp[(size_t)i * cap]; pp[(size_t)i * cap] = run[i]; }",
+      "uint32_t *pp = pref + (size_t)ch * 8 * nkeys + q;\n#pragma unroll\n        for (int i = 0; i < 8; i++) { z[i] = zp[(size_t)i * cap]; pp[(size_t)i * cap] = run[i]; }", TABLE_SHAPES + ED),
+    M("ed_ktab_key_split", "ed25519_keyed.cuh", "const uint32_t q = t % nkeys;", "const uint32_t q = t / ED_BWINS;", TABLE_SHAPES + ED),
+    M("ed_ktab_window_major_tables", "ed25519_keyed.cuh", "uint32_t *out = tab + ((size_t)q * ED_BWINS + win) * ED_BENT * ED_BWORDS;",
+      "uint32_t *out = tab + ((size_t)win * nkeys + q) * ED_BENT * ED_BWORDS;", TABLE_SHAPES + ED),
+    M("ed_ktab_slots_contiguous", "ed25519_keyed.cuh", "const uint32_t *src = xy + (size_t)__ldg(slot_of + q) * 16;",
+      "const uint32_t *src = xy + (size_t)(__ldg(slot_of) + q) * 16;", TABLE_SHAPES + ED),
+    M("ed_ktab_grid_guard", "ed25519_keyed.cuh", "if (t >= T) return;\n    const uint32_t q = t % nkeys;", "if (t > T) return;\n    const uint32_t q = t % nkeys;", TABLE_SHAPES + ED),
     # ---------------------------------------------------------------- quorum.cuh
     M("quorum_ignores_signer", "quorum.cuh", "if (signer[v] != snd) return;", "(void)signer;", ECDSA),
     M("quorum_counts_self", "quorum.cuh", "if (self_id && self_id[inst] == snd) return;", "(void)self_id;", ECDSA),
