@@ -15,6 +15,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libsbv.so")
 
 P256, P384, ED25519 = 0, 1, 2  # scheme tags of the mixed calls (the other calls take P256 / P384 only)
+P256_SHA384, P384_SHA384 = 3, 4  # ECDSA over SHA-384: scheme tags of the mixed384 calls only
 FIELD_BYTES = {P256: 32, P384: 48}
 
 SYMBOLS = [
@@ -28,6 +29,7 @@ SYMBOLS = [
     "sbv_ed25519_set_keys", "sbv_ed25519_verify_registered", "sbv_ed25519_verify_quorum", "sbv_mixed_verify_registered",
     "sbv_mixed_verify_quorum", "sbv_mixed_verify_batch", "sbv_sha384_batch", "sbv_hash384_verify_batch", "sbv_hash384_verify_registered",
     "sbv_key_cache_reserve", "sbv_key_cache_stats", "sbv_key_cache_reserve_evicting", "sbv_key_cache_stats_ex",
+    "sbv_mixed384_verify_registered", "sbv_mixed384_verify_batch", "sbv_mixed384_verify_quorum",
 ]
 
 
@@ -355,7 +357,7 @@ class Engine:
                                                         vp(signer), vp(digest_match), C.c_size_t(n_instances), vp(self_id), C.c_uint32(threshold),
                                                         vp(ok), vp(valid_count), vp(reached)), "sbv_ed25519_verify_quorum")
 
-    def mixed_verify_registered(self, scheme, msgs, off, key_slot, sig96, out=None) -> np.ndarray:
+    def mixed_verify_registered(self, scheme, msgs, off, key_slot, sig96, out=None, _fn="sbv_mixed_verify_registered") -> np.ndarray:
         """Registered-key items of any scheme in one call: scheme[i] in {P256, P384, ED25519}, msgs concatenated with off[n+1]
         byte offsets, key_slot[i] a slot of the item's own registry (set_keys / ed25519_set_keys), sig96 = n x 96 bytes
         (P-256 r || s in [0, 64), P-384 r || s, Ed25519 R || S in [0, 64)).  Returns the n verdict bytes (into `out` if given)."""
@@ -368,18 +370,24 @@ class Engine:
         if scheme.size != n or sig96.size != 96 * n or key_slot.size != n:
             raise ValueError("scheme and key_slot must hold one entry and sig96 96 bytes per message")
         ok = out if out is not None else np.zeros(n, np.uint8)
-        self._check(self._lib.sbv_mixed_verify_registered(self._h, C.c_size_t(n), _p8(scheme), _p8(msgs), off.ctypes.data_as(C.POINTER(C.c_uint64)),
-                                                          key_slot.ctypes.data_as(C.POINTER(C.c_uint32)), _p8(sig96), _p8(ok)),
-                    "sbv_mixed_verify_registered")
+        self._check(getattr(self._lib, _fn)(self._h, C.c_size_t(n), _p8(scheme), _p8(msgs), off.ctypes.data_as(C.POINTER(C.c_uint64)),
+                                            key_slot.ctypes.data_as(C.POINTER(C.c_uint32)), _p8(sig96), _p8(ok)), _fn)
         return ok
 
-    def mixed_verify_registered_ptr(self, n, scheme, msgs, off, key_slot, sig96, ok):
+    def mixed_verify_registered_ptr(self, n, scheme, msgs, off, key_slot, sig96, ok, _fn="sbv_mixed_verify_registered"):
         """Raw host pointers (ints) — used with pinned buffers."""
         vp = C.c_void_p
-        self._check(self._lib.sbv_mixed_verify_registered(self._h, C.c_size_t(n), vp(scheme), vp(msgs), vp(off), vp(key_slot), vp(sig96), vp(ok)),
-                    "sbv_mixed_verify_registered")
+        self._check(getattr(self._lib, _fn)(self._h, C.c_size_t(n), vp(scheme), vp(msgs), vp(off), vp(key_slot), vp(sig96), vp(ok)), _fn)
 
-    def mixed_verify_batch(self, scheme, msgs, off, sig96, key96, out=None) -> np.ndarray:
+    def mixed384_verify_registered(self, scheme, msgs, off, key_slot, sig96, out=None) -> np.ndarray:
+        """mixed_verify_registered with ECDSA over SHA-384 too: scheme[i] in {P256, P384, ED25519, P256_SHA384, P384_SHA384};
+        P256_SHA384 / P384_SHA384 items are packed as P256 / P384 items and hashed with SHA-384."""
+        return self.mixed_verify_registered(scheme, msgs, off, key_slot, sig96, out, _fn="sbv_mixed384_verify_registered")
+
+    def mixed384_verify_registered_ptr(self, n, scheme, msgs, off, key_slot, sig96, ok):
+        self.mixed_verify_registered_ptr(n, scheme, msgs, off, key_slot, sig96, ok, _fn="sbv_mixed384_verify_registered")
+
+    def mixed_verify_batch(self, scheme, msgs, off, sig96, key96, out=None, _fn="sbv_mixed_verify_batch") -> np.ndarray:
         """Items of any scheme with the key of each item in one call: scheme, msgs, off and sig96 as in
         mixed_verify_registered, key96 = n x 96 bytes (P-256 X || Y in [0, 64), P-384 X || Y, Ed25519 encoding in [0, 32)).
         Returns the n verdict bytes (into `out` if given)."""
@@ -391,18 +399,24 @@ class Engine:
         if scheme.size != n or sig96.size != 96 * n or key96.size != 96 * n:
             raise ValueError("scheme must hold one entry and sig96 and key96 96 bytes per message")
         ok = out if out is not None else np.zeros(n, np.uint8)
-        self._check(self._lib.sbv_mixed_verify_batch(self._h, C.c_size_t(n), _p8(scheme), _p8(msgs), off.ctypes.data_as(C.POINTER(C.c_uint64)),
-                                                     _p8(sig96), _p8(key96), _p8(ok)), "sbv_mixed_verify_batch")
+        self._check(getattr(self._lib, _fn)(self._h, C.c_size_t(n), _p8(scheme), _p8(msgs), off.ctypes.data_as(C.POINTER(C.c_uint64)),
+                                            _p8(sig96), _p8(key96), _p8(ok)), _fn)
         return ok
 
-    def mixed_verify_batch_ptr(self, n, scheme, msgs, off, sig96, key96, ok):
+    def mixed_verify_batch_ptr(self, n, scheme, msgs, off, sig96, key96, ok, _fn="sbv_mixed_verify_batch"):
         """Raw host pointers (ints) — used with pinned buffers."""
         vp = C.c_void_p
-        self._check(self._lib.sbv_mixed_verify_batch(self._h, C.c_size_t(n), vp(scheme), vp(msgs), vp(off), vp(sig96), vp(key96), vp(ok)),
-                    "sbv_mixed_verify_batch")
+        self._check(getattr(self._lib, _fn)(self._h, C.c_size_t(n), vp(scheme), vp(msgs), vp(off), vp(sig96), vp(key96), vp(ok)), _fn)
+
+    def mixed384_verify_batch(self, scheme, msgs, off, sig96, key96, out=None) -> np.ndarray:
+        """mixed_verify_batch with ECDSA over SHA-384 too (scheme tags as in mixed384_verify_registered)."""
+        return self.mixed_verify_batch(scheme, msgs, off, sig96, key96, out, _fn="sbv_mixed384_verify_batch")
+
+    def mixed384_verify_batch_ptr(self, n, scheme, msgs, off, sig96, key96, ok):
+        self.mixed_verify_batch_ptr(n, scheme, msgs, off, sig96, key96, ok, _fn="sbv_mixed384_verify_batch")
 
     def mixed_verify_quorum(self, scheme, msgs, off, key_slot, sig96, instance, sender, signer, digest_match, n_instances, threshold,
-                            self_id=None):
+                            self_id=None, _fn="sbv_mixed_verify_quorum"):
         """Commit votes of a mixed consenter set: the items of mixed_verify_registered, verified and counted on the device
         (votes grouped by non-decreasing instance).  Returns (ok, valid_count, reached)."""
         scheme = _u8(scheme)
@@ -426,19 +440,29 @@ class Engine:
             sid = self_id.ctypes.data_as(C.POINTER(C.c_uint16))
         u16 = lambda a: a.ctypes.data_as(C.POINTER(C.c_uint16))
         u32 = lambda a: a.ctypes.data_as(C.POINTER(C.c_uint32))
-        self._check(self._lib.sbv_mixed_verify_quorum(self._h, C.c_size_t(n), _p8(scheme), _p8(msgs), off.ctypes.data_as(C.POINTER(C.c_uint64)),
-                                                      u32(key_slot), _p8(sig96), u32(instance), u16(sender), u16(signer), _p8(digest_match),
-                                                      C.c_size_t(n_instances), sid, C.c_uint32(threshold), _p8(ok), u32(cnt), _p8(reached)),
-                    "sbv_mixed_verify_quorum")
+        self._check(getattr(self._lib, _fn)(self._h, C.c_size_t(n), _p8(scheme), _p8(msgs), off.ctypes.data_as(C.POINTER(C.c_uint64)),
+                                            u32(key_slot), _p8(sig96), u32(instance), u16(sender), u16(signer), _p8(digest_match),
+                                            C.c_size_t(n_instances), sid, C.c_uint32(threshold), _p8(ok), u32(cnt), _p8(reached)), _fn)
         return ok, cnt, reached
 
     def mixed_verify_quorum_ptr(self, n, scheme, msgs, off, key_slot, sig96, instance, sender, signer, digest_match, n_instances, self_id,
-                                threshold, ok, valid_count, reached):
+                                threshold, ok, valid_count, reached, _fn="sbv_mixed_verify_quorum"):
         """Raw host pointers (ints; self_id may be None) — used with pinned buffers."""
         vp = C.c_void_p
-        self._check(self._lib.sbv_mixed_verify_quorum(self._h, C.c_size_t(n), vp(scheme), vp(msgs), vp(off), vp(key_slot), vp(sig96), vp(instance),
-                                                      vp(sender), vp(signer), vp(digest_match), C.c_size_t(n_instances), vp(self_id),
-                                                      C.c_uint32(threshold), vp(ok), vp(valid_count), vp(reached)), "sbv_mixed_verify_quorum")
+        self._check(getattr(self._lib, _fn)(self._h, C.c_size_t(n), vp(scheme), vp(msgs), vp(off), vp(key_slot), vp(sig96), vp(instance),
+                                            vp(sender), vp(signer), vp(digest_match), C.c_size_t(n_instances), vp(self_id),
+                                            C.c_uint32(threshold), vp(ok), vp(valid_count), vp(reached)), _fn)
+
+    def mixed384_verify_quorum(self, scheme, msgs, off, key_slot, sig96, instance, sender, signer, digest_match, n_instances, threshold,
+                               self_id=None):
+        """mixed_verify_quorum with ECDSA over SHA-384 too (scheme tags as in mixed384_verify_registered)."""
+        return self.mixed_verify_quorum(scheme, msgs, off, key_slot, sig96, instance, sender, signer, digest_match, n_instances, threshold,
+                                        self_id, _fn="sbv_mixed384_verify_quorum")
+
+    def mixed384_verify_quorum_ptr(self, n, scheme, msgs, off, key_slot, sig96, instance, sender, signer, digest_match, n_instances, self_id,
+                                   threshold, ok, valid_count, reached):
+        self.mixed_verify_quorum_ptr(n, scheme, msgs, off, key_slot, sig96, instance, sender, signer, digest_match, n_instances, self_id,
+                                     threshold, ok, valid_count, reached, _fn="sbv_mixed384_verify_quorum")
 
     def verify_mixed(self, curve_tag, r48, s48, qx48, qy48, digest32) -> np.ndarray:
         curve_tag, r48, s48, qx48, qy48, digest32 = map(_u8, (curve_tag, r48, s48, qx48, qy48, digest32))

@@ -22,6 +22,7 @@
 #include "engine.h"
 #include "sha256.cuh"
 #include "sha384.cuh"
+#include "mixed_hash.cuh"
 #include "quorum.cuh"
 #include "shards.h"
 
@@ -205,6 +206,22 @@ int sbv_launch_sha384(sbv_engine *e, size_t n, const uint8_t *d_msgs, const uint
     int rc = sbv_launch_length_sort(e, n, d_off, d_perm, st, &perm);
     if (rc) return rc;
     k_sha384<<<(uint32_t)((n + 127) / 128), 128, 0, st>>>((uint32_t)n, d_msgs, d_off, base, d_digest, perm);
+    e->launches += 1;
+    CU(e, cudaGetLastError());
+    return 0;
+}
+int sbv_launch_mix_alg(sbv_engine *e, size_t n, uint8_t *d_tag, uint8_t *d_alg, cudaStream_t st) {
+    k_mix_alg<<<(uint32_t)((n + 255) / 256), 256, 0, st>>>((uint32_t)n, d_tag, d_alg);
+    e->launches += 1;
+    CU(e, cudaGetLastError());
+    return 0;
+}
+int sbv_launch_sha2_sel(sbv_engine *e, size_t n, const uint8_t *d_msgs, const uint64_t *d_off, uint64_t base, const uint32_t *d_idx,
+                        const uint8_t *d_alg, uint32_t dlen, uint8_t *d_digest, uint32_t *d_perm, cudaStream_t st) {
+    const uint32_t *perm = nullptr;
+    int rc = sbv_launch_length_sort(e, n, d_off, d_perm, st, &perm);
+    if (rc) return rc;
+    k_sha2_sel<<<(uint32_t)((n + 127) / 128), 128, 0, st>>>((uint32_t)n, d_msgs, d_off, base, d_idx, d_alg, dlen, d_digest, perm);
     e->launches += 1;
     CU(e, cudaGetLastError());
     return 0;

@@ -252,19 +252,22 @@ int sbv_launch_ed_verify_registered_k(sbv_engine *e, Dev &d, size_t n, const uin
 // The device scratch of a shard of n items, m[f] of family f and `bytes` message bytes, carved from one buffer: the
 // uploaded tags, slots (or, keys per item, 96-byte key rows) and 96-byte signature rows, the tile prefixes of the split,
 // the shared message buffer of the three families, and per family the compacted arrays and the scratch of its pipeline.
-// A registered shard has no key arrays (key96, qx, qy are null); a keys-per-item shard has no slots.
+// A registered shard has no key arrays (key96, qx, qy are null); a keys-per-item shard has no slots.  alg: the SHA-384 flag
+// of each item (mixed_hash.cuh: k_mix_alg), carved only for a shard that holds SHA-384 items.
 struct MixBufs {
-    uint8_t *tag, *sig96, *key96;
+    uint8_t *tag, *sig96, *key96, *alg;
     uint32_t *slot_in, *tile_cnt;
     uint64_t *tile_bytes;
     uint8_t *blob;
     uint32_t *idx[3], *slot[3], *perm[3];
-    uint8_t *r[3], *s[3], *ok[3], *dig[3], *pub[3];  // dig: SHA-256 digests (ECDSA) or k (Ed25519); pub: Ed25519 only
+    uint8_t *r[3], *s[3], *ok[3], *dig[3], *pub[3];  // dig: the ECDSA e (32 bytes per item, 48 for a P-384 family with
+                                                       // SHA-384 items) or k (Ed25519); pub: Ed25519 only
     uint8_t *qx[3], *qy[3];                            // keys per item, ECDSA only
     uint64_t *off[3];
 };
 // base == nullptr only sizes; returns the bytes the carve takes.  keys: a keys-per-item shard (sbv_mixed_verify_batch).
-size_t sbv_mix_carve(uint8_t *base, size_t n, const uint32_t m[3], uint64_t bytes, bool keys, MixBufs *out);
+// m384 (may be null): the SHA-384 items of the P-256 and P-384 families; when either is nonzero the carve adds alg.
+size_t sbv_mix_carve(uint8_t *base, size_t n, const uint32_t m[3], uint64_t bytes, bool keys, MixBufs *out, const uint32_t *m384 = nullptr);
 // the split of a staged shard (b.tag, b.slot_in or b.key96, b.sig96, messages at d_msgs with offsets d_off from base) into
 // the families
 int sbv_launch_mix_split(sbv_engine *e, const MixBufs &b, size_t n, const uint32_t m[3], const uint8_t *d_msgs, const uint64_t *d_off, uint64_t base,
@@ -289,6 +292,12 @@ int sbv_launch_sha256(sbv_engine *e, size_t n, const uint8_t *d_msgs, const uint
 // the same with SHA-384: 48 bytes per message into d_digest
 int sbv_launch_sha384(sbv_engine *e, size_t n, const uint8_t *d_msgs, const uint64_t *d_off, uint64_t base, uint8_t *d_digest, uint32_t *d_perm,
                       cudaStream_t st);
+// mixed_hash.cuh: k_mix_alg over the n uploaded tags of a mixed shard (tags 3 and 4 to their family, flags into d_alg)
+int sbv_launch_mix_alg(sbv_engine *e, size_t n, uint8_t *d_tag, uint8_t *d_alg, cudaStream_t st);
+// mixed_hash.cuh: k_sha2_sel over the n items of one family (d_idx: their shard indices, d_alg: the shard's flags), dlen
+// bytes of e per item into d_digest, behind the block-count sort of sbv_launch_sha256
+int sbv_launch_sha2_sel(sbv_engine *e, size_t n, const uint8_t *d_msgs, const uint64_t *d_off, uint64_t base, const uint32_t *d_idx,
+                        const uint8_t *d_alg, uint32_t dlen, uint8_t *d_digest, uint32_t *d_perm, cudaStream_t st);
 // the block-count sort of the SHA-256 launch on its own: *perm = the permutation in d_perm, or nullptr below 2048 items
 int sbv_launch_length_sort(sbv_engine *e, size_t n, const uint64_t *d_off, uint32_t *d_perm, cudaStream_t st, const uint32_t **perm);
 int sbv_lane_h2d(sbv_engine *e, Dev::Lane &ln, void *dst, const void *src, size_t bytes, size_t &stage_off, cudaStream_t st = nullptr);

@@ -17,7 +17,7 @@ MixPlan plan_of(const MixBufs &b) {
 }  // namespace
 static_assert(MIX_FAMILIES == SBV_ED25519 + 1, "one family per scheme tag");
 
-size_t sbv_mix_carve(uint8_t *base, size_t n, const uint32_t m[3], uint64_t bytes, bool keys, MixBufs *out) {
+size_t sbv_mix_carve(uint8_t *base, size_t n, const uint32_t m[3], uint64_t bytes, bool keys, MixBufs *out, const uint32_t *m384) {
     MixBufs b{};
     size_t at = 0;
     auto take = [&](size_t sz) {
@@ -46,9 +46,11 @@ size_t sbv_mix_carve(uint8_t *base, size_t n, const uint32_t m[3], uint64_t byte
         b.off[f] = (uint64_t *)take((k + 1) * 8);
         b.ok[f] = take(k);
         b.perm[f] = (uint32_t *)take((k + 3 * 1024) * 4);
-        b.dig[f] = take(k * 32);  // ECDSA: the SHA-256 digests; Ed25519: k, word-major
+        // ECDSA: e, 32 bytes per item, or 48 for a P-384 family with SHA-384 items; Ed25519: k, word-major
+        b.dig[f] = take(k * (f == SBV_P384 && m384 && m384[SBV_P384] ? 48 : 32));
         b.pub[f] = f == SBV_ED25519 ? take(k * 32) : nullptr;
     }
+    if (m384 && (m384[SBV_P256] || m384[SBV_P384])) b.alg = take(n);
     if (out) *out = b;
     return at;
 }

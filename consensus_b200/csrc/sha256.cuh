@@ -42,22 +42,17 @@ __device__ __forceinline__ void sha256_compress(uint32_t (&h)[8], uint32_t (&w)[
     h[0] += a; h[1] += b; h[2] += c; h[3] += d; h[4] += e; h[5] += f; h[6] += g; h[7] += hh;
 }
 
-// digest_out: 32 bytes per message, big-endian words (the byte string SHA-256 defines)
-// perm (optional): message processed by thread t is perm[t] — the launcher sorts messages by block
-// count (longest first) so the 32 lanes of a warp hash messages of equal length instead of all
-// waiting for the longest one.
-__global__ void __launch_bounds__(128) k_sha256(uint32_t n, const uint8_t *__restrict__ msgs,
-                                                const uint64_t *__restrict__ off, uint64_t base, uint8_t *__restrict__ digest_out,
-                                                const uint32_t *__restrict__ perm) {
-    const uint32_t tix = blockIdx.x * blockDim.x + threadIdx.x;
-    if (tix >= n) return;
-    const uint32_t idx = perm ? perm[tix] : tix;
+// The SHA-256 state h after message idx of the batch (offsets off relative to base): the per-message body of k_sha256,
+// shared with k_sha2_sel (mixed_hash.cuh).
+__device__ __forceinline__ void sha256_msg(uint32_t (&h)[8], const uint8_t *__restrict__ msgs, const uint64_t *__restrict__ off, uint64_t base,
+                                           uint32_t idx) {
     const uint64_t o = off[idx] - base;
     const uint64_t len = off[idx + 1] - off[idx];
     const uint32_t *words = reinterpret_cast<const uint32_t *>(msgs + (o & ~(uint64_t)3));
     const uint32_t sh = (uint32_t)(o & 3);
     const uint32_t sel = (sh + 3) | ((sh + 2) << 4) | ((sh + 1) << 8) | (sh << 12);
-    uint32_t h[8] = {0x6a09e667, 0xbb67ae85, 0x3c6ef372, 0xa54ff53a, 0x510e527f, 0x9b05688c, 0x1f83d9ab, 0x5be0cd19};
+    h[0] = 0x6a09e667; h[1] = 0xbb67ae85; h[2] = 0x3c6ef372; h[3] = 0xa54ff53a;
+    h[4] = 0x510e527f; h[5] = 0x9b05688c; h[6] = 0x1f83d9ab; h[7] = 0x5be0cd19;
     const uint64_t nblocks = (len + 9 + 63) / 64;
     for (uint64_t blk = 0; blk < nblocks; blk++) {
         uint32_t w[16];
@@ -93,6 +88,20 @@ __global__ void __launch_bounds__(128) k_sha256(uint32_t n, const uint8_t *__res
         }
         sha256_compress(h, w);
     }
+}
+
+// digest_out: 32 bytes per message, big-endian words (the byte string SHA-256 defines)
+// perm (optional): message processed by thread t is perm[t] — the launcher sorts messages by block
+// count (longest first) so the 32 lanes of a warp hash messages of equal length instead of all
+// waiting for the longest one.
+__global__ void __launch_bounds__(128) k_sha256(uint32_t n, const uint8_t *__restrict__ msgs,
+                                                const uint64_t *__restrict__ off, uint64_t base, uint8_t *__restrict__ digest_out,
+                                                const uint32_t *__restrict__ perm) {
+    const uint32_t tix = blockIdx.x * blockDim.x + threadIdx.x;
+    if (tix >= n) return;
+    const uint32_t idx = perm ? perm[tix] : tix;
+    uint32_t h[8];
+    sha256_msg(h, msgs, off, base, idx);
     uint4 *out = reinterpret_cast<uint4 *>(digest_out + (size_t)idx * 32);
     out[0] = make_uint4(__byte_perm(h[0], 0, 0x0123), __byte_perm(h[1], 0, 0x0123), __byte_perm(h[2], 0, 0x0123), __byte_perm(h[3], 0, 0x0123));
     out[1] = make_uint4(__byte_perm(h[4], 0, 0x0123), __byte_perm(h[5], 0, 0x0123), __byte_perm(h[6], 0, 0x0123), __byte_perm(h[7], 0, 0x0123));

@@ -56,8 +56,9 @@ extern "C" {
 typedef struct sbv_engine sbv_engine;
 
 /* Scheme tags.  The calls that take a curve (or a curve tag per item) accept SBV_P256 and SBV_P384 only and return
- * SBV_ERR_ARG for SBV_ED25519; only the sbv_mixed_* calls take all three. */
-enum { SBV_P256 = 0, SBV_P384 = 1, SBV_ED25519 = 2 };
+ * SBV_ERR_ARG for anything above; the sbv_mixed_* calls take the first three, where SBV_P256 and SBV_P384 are ECDSA over
+ * SHA-256; only the sbv_mixed384_* calls also take SBV_P256_SHA384 and SBV_P384_SHA384, ECDSA over SHA-384. */
+enum { SBV_P256 = 0, SBV_P384 = 1, SBV_ED25519 = 2, SBV_P256_SHA384 = 3, SBV_P384_SHA384 = 4 };
 enum {
     SBV_OK = 0,
     SBV_ERR_ARG = -1,   /* bad argument */
@@ -106,8 +107,8 @@ int sbv_hash_verify_batch(sbv_engine *e, uint8_t curve, size_t n, const uint8_t 
  * with P-384.  The three calls below are the SHA-256 forms with SHA-384 in place of SHA-256; msgs / msg_off as in
  * sbv_sha256_batch (msgs may be NULL when every message is empty).  The same argument checks run before anything is
  * written: SBV_ERR_ARG for a curve other than SBV_P256 / SBV_P384, null buffers, n >= 2^31 and decreasing offsets.
- * Multi-device engines shard them as the SHA-256 forms.  Out of scope, SHA-256 or digests only: the sbv_mixed_* calls,
- * sbv_verify_quorum, the DER front end and the _ranked and _device forms. */
+ * Multi-device engines shard them as the SHA-256 forms.  Mixed batches with SHA-384 items go through the sbv_mixed384_*
+ * calls.  Out of scope, SHA-256 or digests only: sbv_verify_quorum, the DER front end and the _ranked and _device forms. */
 /* SHA-384 over a ragged batch (msgs / msg_off as in sbv_sha256_batch); digest_out = 48n bytes. */
 int sbv_sha384_batch(sbv_engine *e, size_t n, const uint8_t *msgs, const uint64_t *msg_off, uint8_t *digest_out);
 /* sbv_hash_verify_batch with SHA-384: e = leftmost min(48, field bytes) of SHA-384(M) (the whole digest for P-384,
@@ -238,6 +239,26 @@ int sbv_mixed_verify_quorum(sbv_engine *e, size_t n_votes, const uint8_t *scheme
                             const uint32_t *key_slot, const uint8_t *sig96, const uint32_t *instance, const uint16_t *sender,
                             const uint16_t *signer, const uint8_t *digest_match, size_t n_instances, const uint16_t *self_id,
                             uint32_t threshold, uint8_t *ok, uint32_t *valid_count, uint8_t *reached);
+
+/* The three mixed calls with ECDSA over SHA-384 among the items: each has the arguments of its sbv_mixed_* counterpart and
+ * accepts scheme tags 0 to 4.  Tags 0 to 2 mean what they mean there; a batch of those tags only returns byte for byte
+ * what the counterpart returns.  SBV_P256_SHA384 and SBV_P384_SHA384 items are packed as P-256 and P-384 items (sig96,
+ * key96 and registry slots of sbv_set_keys alike) and are verified with e = the leftmost min(48, field bytes) of
+ * SHA-384(M): ok[i] is byte for byte what sbv_hash384_verify_registered (or, keys per item, sbv_hash384_verify_batch)
+ * returns for the item on its curve.  A tag > 4 returns SBV_ERR_ARG with its index in sbv_last_error, before anything is
+ * written or launched; the other argument checks are those of the counterpart.  The split into the three curve families
+ * is that of the counterpart, so keys that repeat are grouped per curve whichever hash their items use; each family is
+ * hashed by one launch that picks SHA-256 or SHA-384 per item. */
+int sbv_mixed384_verify_registered(sbv_engine *e, size_t n, const uint8_t *scheme, const uint8_t *msgs, const uint64_t *msg_off,
+                                   const uint32_t *key_slot, const uint8_t *sig96, uint8_t *ok);
+int sbv_mixed384_verify_batch(sbv_engine *e, size_t n, const uint8_t *scheme, const uint8_t *msgs, const uint64_t *msg_off,
+                              const uint8_t *sig96, const uint8_t *key96, uint8_t *ok);
+/* ok = the verdicts of sbv_mixed384_verify_registered; valid_count / reached as in sbv_mixed_verify_quorum (the same vote
+ * rules, sharded by instance on a multi-device engine). */
+int sbv_mixed384_verify_quorum(sbv_engine *e, size_t n_votes, const uint8_t *scheme, const uint8_t *msgs, const uint64_t *msg_off,
+                               const uint32_t *key_slot, const uint8_t *sig96, const uint32_t *instance, const uint16_t *sender,
+                               const uint16_t *signer, const uint8_t *digest_match, size_t n_instances, const uint16_t *self_id,
+                               uint32_t threshold, uint8_t *ok, uint32_t *valid_count, uint8_t *reached);
 
 /* computeQuorum(n) -> (q, f), internal/bft/util.go:183-187. */
 void sbv_compute_quorum(uint64_t n, uint32_t *q, uint32_t *f);

@@ -28,6 +28,7 @@ namespace sbv { uint32_t tab[1 << 18]; }
 #include "../../consensus_b200/csrc/ed25519_comb.cuh"
 #include "../../consensus_b200/csrc/shards.h"
 #include "../../consensus_b200/csrc/mixed.cuh"
+#include "../../consensus_b200/csrc/mixed_hash.cuh"
 
 using namespace sbv;
 
@@ -737,6 +738,21 @@ extern "C" int hs_mixed_verify_registered(size_t n, const uint8_t *tag, const ui
     }
     if (m[2]) hs_ed25519_verify_registered(m[2], blob.data(), fo.data() + at[2] + 2, slot.data() + at[2], sig2.data(), okf.data() + at[2]);
     hs_mixed_scatter(n, m[0], m[1], idx.data(), okf.data(), ok);
+    return 0;
+}
+
+// ---- SHA-384 items in mixed shards (mixed_hash.cuh, sbv_mixed384_*) ----
+// k_mix_alg over n tags in place: tags 3 and 4 become 0 and 1, sha384[i] = whether item i is over SHA-384
+extern "C" int hs_mix_alg(size_t n, uint8_t *tag, uint8_t *sha384) {
+    run_grid((unsigned)((n + 255) / 256), 256, [&] { k_mix_alg((uint32_t)n, tag, sha384); });
+    return 0;
+}
+// k_sha2_sel over the n items of one family: messages at off[j] - base in msgs (readable 8 bytes past the last one), idx[j]
+// their shard index, sha384 the shard's flags, dlen (32 or 48) bytes of e per item into digest_out; perm: optional
+// processing order, as the counting sort gives it
+extern "C" int hs_sha2_sel(size_t n, const uint8_t *msgs, const uint64_t *off, uint64_t base, const uint32_t *idx, const uint8_t *sha384, uint32_t dlen,
+                           const uint32_t *perm, uint8_t *digest_out) {
+    run_grid((unsigned)((n + 127) / 128), 128, [&] { k_sha2_sel((uint32_t)n, msgs, off, base, idx, sha384, dlen, digest_out, perm); });
     return 0;
 }
 

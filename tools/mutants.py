@@ -51,7 +51,8 @@ KEY_CACHE = ["tests/test_hostsim_key_cache.py"]
 KEY_CACHE_EVICT = ["tests/test_hostsim_key_cache_evict.py"]
 SEEDED = ["tests/test_hostsim_seeded_passes.py"]
 COMB_WARP = ["tests/test_hostsim_comb_warp.py"]  # the comb build a warp per key against the one-thread-per-chain reference  # the first entry of a pass loaded, not added (pt_seed)
-TABLE_SHAPES = ["tests/test_hostsim_table_shapes.py"]  # every entry of the per-key tables at the key counts where the builds turn over
+TABLE_SHAPES = ["tests/test_hostsim_table_shapes.py"]
+MIXED384 = ["tests/test_hostsim_mixed384.py"]  # k_mix_alg and k_sha2_sel (mixed_hash.cuh)  # every entry of the per-key tables at the key counts where the builds turn over
 
 
 def M(id, file, find, repl, tests, equivalent=None, proof=None):
@@ -347,6 +348,16 @@ CATALOGUE = [
     M("quorum_scan_other_instance", "quorum.cuh", "if (instance[j] - inst_base != inst) break;", "(void)0;", ECDSA),
     M("quorum_reached_gt", "quorum.cuh", "reached[i] = valid_count[i] >= threshold ? 1 : 0;", "reached[i] = valid_count[i] > threshold ? 1 : 0;", ECDSA),
     M("pack_bits_tail", "quorum.cuh", "const uint32_t bit = (i < n && ok[i]) ? 1u : 0u;", "const uint32_t bit = ok[i] ? 1u : 0u;", ECDSA),
+    # ---------------------------------------------------------------- mixed_hash.cuh
+    M("mix_alg_tag_map", "mixed_hash.cuh", "tag[i] = (uint8_t)(wide ? t - MIX_TAG_SHA384 : t);", "tag[i] = (uint8_t)t;", MIXED384),
+    M("mix_alg_flag", "mixed_hash.cuh", "sha384[i] = wide ? 1 : 0;", "sha384[i] = 0;", MIXED384),
+    M("mix_alg_threshold", "mixed_hash.cuh", "const bool wide = t >= MIX_TAG_SHA384;", "const bool wide = t > MIX_TAG_SHA384;", MIXED384),
+    M("sha2_sel_flag_by_shard_index", "mixed_hash.cuh", "if (sha384[idx[j]]) {", "if (sha384[j]) {", MIXED384),
+    M("sha2_sel_p384_sha256_offset", "mixed_hash.cuh", "if (dlen == 48) *out++ = make_uint4(0u, 0u, 0u, 0u);", "if (dlen == 48) *out = make_uint4(0u, 0u, 0u, 0u);",
+      MIXED384),
+    M("sha2_sel_p384_sha256_zeros", "mixed_hash.cuh", "if (dlen == 48) *out++ = make_uint4(0u, 0u, 0u, 0u);", "if (dlen == 48) out++;", MIXED384),
+    M("sha2_sel_p256_truncation", "mixed_hash.cuh", "if (dlen == 48)\n            out[2] =", "if (dlen >= 32)\n            out[2] =", MIXED384),
+    M("sha2_sel_slot_width", "mixed_hash.cuh", "digest_out + (size_t)j * dlen);", "digest_out + (size_t)j * 48);", MIXED384),
     # ---------------------------------------------------------------- mixed.cuh
     M("mix_count_tile_end", "mixed.cuh", "const uint32_t lo = t * MIX_TILE, hi = n - lo < MIX_TILE ? n : lo + MIX_TILE;\n    for (uint32_t i = lo; i < hi; i++) {\n        const uint32_t f = tag[i];\n        const uint64_t len",
       "const uint32_t lo = t * MIX_TILE, hi = n - lo <= MIX_TILE ? n - 1 : lo + MIX_TILE;\n    for (uint32_t i = lo; i < hi; i++) {\n        const uint32_t f = tag[i];\n        const uint64_t len", MIXED),
