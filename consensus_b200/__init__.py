@@ -17,6 +17,8 @@ LIB_PATH = os.path.join(_HERE, "libsbv.so")
 P256, P384, ED25519 = 0, 1, 2  # scheme tags of the mixed calls (the other calls take P256 / P384 only)
 P256_SHA384, P384_SHA384 = 3, 4  # ECDSA over SHA-384: scheme tags of the mixed384 calls only
 FIELD_BYTES = {P256: 32, P384: 48}
+SHA256, SHA384, SHA512 = 0, 1, 2  # hash tags of the RSA calls (SBV_HASH_*)
+HASH_BYTES = {SHA256: 32, SHA384: 48, SHA512: 64}
 
 SYMBOLS = [
     "sbv_create", "sbv_destroy", "sbv_last_error", "sbv_device_count", "sbv_verify_batch",
@@ -30,6 +32,7 @@ SYMBOLS = [
     "sbv_mixed_verify_quorum", "sbv_mixed_verify_batch", "sbv_sha384_batch", "sbv_hash384_verify_batch", "sbv_hash384_verify_registered",
     "sbv_key_cache_reserve", "sbv_key_cache_stats", "sbv_key_cache_reserve_evicting", "sbv_key_cache_stats_ex",
     "sbv_mixed384_verify_registered", "sbv_mixed384_verify_batch", "sbv_mixed384_verify_quorum",
+    "sbv_sha512_batch", "sbv_rsa_verify_batch", "sbv_rsa_hash_verify_batch",
 ]
 
 
@@ -261,6 +264,53 @@ class Engine:
         """hash_verify_batch with e = the leftmost field bytes of SHA-384(M) (Go's ECDSAWithSHA384, ES384); the digests, if
         asked for, are n x 48 bytes."""
         return self.hash_verify_batch(curve, msgs, off, r, s, qx, qy, want_digest, _fn="sbv_hash384_verify_batch", _width=48)
+
+    def sha512_batch(self, msgs, off) -> np.ndarray:
+        """SHA-512 of each message (msgs concatenated with off[n+1] byte offsets): n x 64 bytes."""
+        return self.sha256_batch(msgs, off, _fn="sbv_sha512_batch", _width=64)
+
+    def sha512_batch_ptr(self, n, msgs, off, digest_out):
+        """Raw host pointers (ints) — used with pinned buffers."""
+        vp = C.c_void_p
+        self._check(self._lib.sbv_sha512_batch(self._h, C.c_size_t(n), vp(msgs), vp(off), vp(digest_out)), "sbv_sha512_batch")
+
+    def rsa_verify_batch(self, hash, digest, sig, modulus, pub_exp, out=None) -> np.ndarray:
+        """RSA PKCS #1 v1.5 (Go crypto/rsa.VerifyPKCS1v15) over supplied digests: hash in {SHA256, SHA384, SHA512};
+        digest = n x hLen bytes, sig and modulus = n x k bytes big-endian (k = 256, 384 or 512), pub_exp = n uint32."""
+        pub_exp = np.ascontiguousarray(pub_exp, dtype=np.uint32)
+        n = pub_exp.size
+        sig, modulus, digest = _u8(sig), _u8(modulus), _u8(digest)
+        k = sig.size // n if n else 256
+        ok = out if out is not None else np.zeros(n, np.uint8)
+        self.rsa_verify_batch_ptr(k, hash, n, digest.ctypes.data, sig.ctypes.data, modulus.ctypes.data, pub_exp.ctypes.data, ok.ctypes.data)
+        return ok
+
+    def rsa_verify_batch_ptr(self, mod_bytes, hash, n, digest, sig, modulus, pub_exp, ok):
+        """Raw host pointers (ints) — used with pinned buffers."""
+        vp = C.c_void_p
+        self._check(self._lib.sbv_rsa_verify_batch(self._h, C.c_uint32(mod_bytes), C.c_uint8(hash), C.c_size_t(n), vp(digest), vp(sig), vp(modulus),
+                                                   vp(pub_exp), vp(ok)), "sbv_rsa_verify_batch")
+
+    def rsa_hash_verify_batch(self, hash, msgs, off, sig, modulus, pub_exp, want_digest=False):
+        """rsa_verify_batch with H = hash(M) computed on the device; msgs concatenated with off[n+1] byte offsets.  Returns
+        the verdicts, and the n x hLen digests too with want_digest."""
+        msgs = _u8(msgs if len(msgs) else np.zeros(1, np.uint8))
+        off = np.ascontiguousarray(off, dtype=np.uint64)
+        pub_exp = np.ascontiguousarray(pub_exp, dtype=np.uint32)
+        sig, modulus = _u8(sig), _u8(modulus)
+        n = off.size - 1
+        k = sig.size // n if n else 256
+        ok = np.zeros(n, np.uint8)
+        dig = np.zeros((n, HASH_BYTES[hash]), np.uint8) if want_digest else None
+        self.rsa_hash_verify_batch_ptr(k, hash, n, msgs.ctypes.data, off.ctypes.data, sig.ctypes.data, modulus.ctypes.data, pub_exp.ctypes.data,
+                                       dig.ctypes.data if want_digest else 0, ok.ctypes.data)
+        return (ok, dig) if want_digest else ok
+
+    def rsa_hash_verify_batch_ptr(self, mod_bytes, hash, n, msgs, off, sig, modulus, pub_exp, digest_out, ok):
+        """Raw host pointers (ints; digest_out may be 0) — used with pinned buffers."""
+        vp = C.c_void_p
+        self._check(self._lib.sbv_rsa_hash_verify_batch(self._h, C.c_uint32(mod_bytes), C.c_uint8(hash), C.c_size_t(n), vp(msgs), vp(off), vp(sig),
+                                                        vp(modulus), vp(pub_exp), vp(digest_out or None), vp(ok)), "sbv_rsa_hash_verify_batch")
 
     def hash384_verify_batch_ptr(self, curve, n, msgs, off, r, s, qx, qy, digest_out, ok):
         """Raw host pointers (ints; digest_out may be 0) — used with pinned buffers."""

@@ -177,6 +177,17 @@ int sbv_lane_ensure_mix(sbv_engine *e, Dev::Lane &ln, size_t bytes) {
     ln.mix_cap = cap;
     return 0;
 }
+int sbv_lane_ensure_rsa(sbv_engine *e, Dev::Lane &ln, size_t bytes) {
+    if (bytes <= ln.rsa_cap) return 0;
+    CU(e, cudaStreamSynchronize(ln.stream));
+    if (ln.d_rsa) cudaFree(ln.d_rsa);
+    ln.d_rsa = nullptr;
+    ln.rsa_cap = 0;
+    const size_t cap = bytes + bytes / 8 + 4096;
+    CU(e, cudaMalloc(&ln.d_rsa, cap));
+    ln.rsa_cap = cap;
+    return 0;
+}
 int sbv_launch_length_sort(sbv_engine *e, size_t n, const uint64_t *d_off, uint32_t *d_perm, cudaStream_t st, const uint32_t **perm) {
     *perm = nullptr;
     if (d_perm && n >= 2048) {  // sort by block count so that a warp's 32 messages have equal length
@@ -351,10 +362,12 @@ int gather_unpack(sbv_engine *e, int lane, const Shards &s, const std::vector<ui
 }
 
 // The hash that turns the messages of an ECDSA call into its digests (e = their leftmost field bytes).
-enum class MsgHash : uint8_t { sha256, sha384 };
-uint32_t hash_bytes(MsgHash h) { return h == MsgHash::sha384 ? 48u : 32u; }
+// (SHA-512 serves the RSA calls only.)  The values are the SBV_HASH_* tags.
+enum class MsgHash : uint8_t { sha256, sha384, sha512 };
+uint32_t hash_bytes(MsgHash h) { return h == MsgHash::sha512 ? 64u : h == MsgHash::sha384 ? 48u : 32u; }
 int launch_hash(sbv_engine *e, MsgHash h, size_t n, const uint8_t *d_msgs, const uint64_t *d_off, uint64_t base, uint8_t *d_digest, uint32_t *d_perm,
                 cudaStream_t st) {
+    if (h == MsgHash::sha512) return sbv_launch_sha512(e, n, d_msgs, d_off, base, d_digest, d_perm, st);
     return h == MsgHash::sha384 ? sbv_launch_sha384(e, n, d_msgs, d_off, base, d_digest, d_perm, st)
                                 : sbv_launch_sha256(e, n, d_msgs, d_off, base, d_digest, d_perm, st);
 }
@@ -511,7 +524,7 @@ void sbv_destroy(sbv_engine *e) {
         sbv_ed_keys_free(d);
         sbv_key_cache_free(d);
         for (auto &ln : d.lanes) {
-            void *lp[] = {ln.d_r, ln.d_s, ln.d_qx, ln.d_qy, ln.d_dig, ln.d_ok, ln.d_slot, ln.d_msgs, ln.d_off, ln.d_perm, ln.d_aux, ln.d_mix};
+            void *lp[] = {ln.d_r, ln.d_s, ln.d_qx, ln.d_qy, ln.d_dig, ln.d_ok, ln.d_slot, ln.d_msgs, ln.d_off, ln.d_perm, ln.d_aux, ln.d_mix, ln.d_rsa};
             for (void *p : lp) if (p) cudaFree(p);
             if (ln.h_pin) cudaFreeHost(ln.h_pin);
             if (ln.h_aux) cudaFreeHost(ln.h_aux);
@@ -735,6 +748,7 @@ double sbv_probe_mad_rate(sbv_engine *e) {
 }  // extern "C"
 
 #include "engine_more.inc"
+#include "engine_rsa.inc"
 
 // ---- profiling hooks (bench.py's roofline leg): CUDA-event timing inside every verify launch ----
 extern "C" {

@@ -79,6 +79,9 @@ struct Dev {
         // device scratch of a mixed ECDSA / Ed25519 shard (inst_mixed.cu: sbv_mix_carve)
         uint8_t *d_mix = nullptr;
         size_t mix_cap = 0;
+        // device scratch of an RSA shard (engine_rsa.inc: rsa_carve)
+        uint8_t *d_rsa = nullptr;
+        size_t rsa_cap = 0;
     } lanes[SBV_LANES];
     // generic scratch of the entry points that serialise on the engine lock
     uint8_t *d_scratch = nullptr;
@@ -285,6 +288,7 @@ int sbv_lane_ensure(sbv_engine *e, Dev &d, Dev::Lane &ln, size_t n, size_t pinne
 int sbv_lane_ensure_msgs(sbv_engine *e, Dev::Lane &ln, size_t bytes, size_t n_off);
 int sbv_lane_ensure_aux(sbv_engine *e, Dev::Lane &ln, size_t bytes);
 int sbv_lane_ensure_mix(sbv_engine *e, Dev::Lane &ln, size_t bytes);
+int sbv_lane_ensure_rsa(sbv_engine *e, Dev::Lane &ln, size_t bytes);
 int sbv_lane_stream2(sbv_engine *e, Dev::Lane &ln);  // creates the lane's second stream and its two events on first use
 // d_perm: n + 3072 words of scratch (may be null: no length sort)
 int sbv_launch_sha256(sbv_engine *e, size_t n, const uint8_t *d_msgs, const uint64_t *d_off, uint64_t base, uint8_t *d_digest, uint32_t *d_perm,
@@ -292,6 +296,15 @@ int sbv_launch_sha256(sbv_engine *e, size_t n, const uint8_t *d_msgs, const uint
 // the same with SHA-384: 48 bytes per message into d_digest
 int sbv_launch_sha384(sbv_engine *e, size_t n, const uint8_t *d_msgs, const uint64_t *d_off, uint64_t base, uint8_t *d_digest, uint32_t *d_perm,
                       cudaStream_t st);
+// ---- inst_rsa.cu: RSA (enqueue only, no sync) ----
+// the same with SHA-512 (sha512_batch.cuh: k_sha512): 64 bytes per message into d_digest
+int sbv_launch_sha512(sbv_engine *e, size_t n, const uint8_t *d_msgs, const uint64_t *d_off, uint64_t base, uint8_t *d_digest, uint32_t *d_perm,
+                      cudaStream_t st);
+// k_rsa_verify over n items of mod_bytes (256, 384 or 512) bytes each: d_sig and d_mod n * mod_bytes bytes (big-endian),
+// d_exp n words, d_digest n * hLen bytes (hash 0 / 1 / 2: SHA-256 / SHA-384 / SHA-512), verdicts into d_ok.  Every pointer
+// 4-byte aligned.
+int sbv_launch_rsa(sbv_engine *e, uint32_t mod_bytes, uint8_t hash, size_t n, const uint8_t *d_sig, const uint8_t *d_mod, const uint32_t *d_exp,
+                   const uint8_t *d_digest, uint8_t *d_ok, cudaStream_t st);
 // mixed_hash.cuh: k_mix_alg over the n uploaded tags of a mixed shard (tags 3 and 4 to their family, flags into d_alg)
 int sbv_launch_mix_alg(sbv_engine *e, size_t n, uint8_t *d_tag, uint8_t *d_alg, cudaStream_t st);
 // mixed_hash.cuh: k_sha2_sel over the n items of one family (d_idx: their shard indices, d_alg: the shard's flags), dlen

@@ -122,6 +122,35 @@ int sbv_hash384_verify_batch(sbv_engine *e, uint8_t curve, size_t n, const uint8
 int sbv_hash384_verify_registered(sbv_engine *e, uint8_t curve, size_t n, const uint8_t *msgs, const uint64_t *msg_off,
                                   const uint32_t *key_slot, const uint8_t *r, const uint8_t *s, uint8_t *ok);
 
+/* ---- RSA PKCS #1 v1.5 (RSASSA-PKCS1-v1_5, RFC 8017 §8.2.2), for a Verifier whose identities hold crypto/rsa keys
+ * (crypto/x509 SHA256WithRSA, SHA384WithRSA, SHA512WithRSA).  Hash tags: */
+enum { SBV_HASH_SHA256 = 0, SBV_HASH_SHA384 = 1, SBV_HASH_SHA512 = 2 };
+/* Accept set = Go crypto/rsa.VerifyPKCS1v15(pub, hash, H, S).  k = mod_bytes (256, 384 or 512), modulus N (k bytes,
+ * big-endian), public exponent e (uint32), digest H (hLen = 32, 48 or 64 bytes by the hash tag, taken as given: no
+ * truncation), signature S (k bytes, big-endian):
+ *  1. Key: reject unless N is odd, N's leading byte is nonzero (so Go's pub.Size() equals k and its k != len(sig)
+ *     check passes) and 2 <= e <= 2^31 - 1 (the bounds of Go's checkPub).  The rule on N's parity is the engine's:
+ *     Go's behaviour on an even modulus is not pinned by any test here, and no real key has one.
+ *  2. Range: reject if S >= N (Go's bigmod SetBytes fails there), so S + N, the twin of a valid S, rejects.
+ *  3. Recover: EM = S^e mod N as k bytes, big-endian.
+ *  4. Compare: accept iff EM = 00 || 01 || FF..FF || 00 || DigestInfo(hash) || H byte for byte, the FF run k - tLen - 3
+ *     bytes long, tLen = |DigestInfo| + hLen, with the DigestInfo prefixes of RFC 8017 §9.2 note 1 WITH the NULL
+ *     parameters (the form without them rejects, as in Go).
+ * RSA-PSS is not offered.  The checks: SBV_ERR_ARG for a mod_bytes other than 256 / 384 / 512, a hash tag above
+ * SBV_HASH_SHA512, a null buffer (msgs may be NULL when every message is empty), n >= 2^31 and decreasing offsets, all
+ * before anything is written or launched.  Multi-device engines shard by item as sbv_hash_verify_batch does.  Each
+ * device's shard is uploaded whole (no chunked upload).  Out of scope: registered RSA keys, RSA items in the mixed and
+ * commit-vote calls, and _device / _ranked forms. */
+/* SHA-512 over a ragged batch (msgs / msg_off as in sbv_sha256_batch); digest_out = 64n bytes. */
+int sbv_sha512_batch(sbv_engine *e, size_t n, const uint8_t *msgs, const uint64_t *msg_off, uint8_t *digest_out);
+/* digests supplied: digest = n x hLen bytes; sig, modulus = n x mod_bytes bytes; pub_exp = n x uint32 */
+int sbv_rsa_verify_batch(sbv_engine *e, uint32_t mod_bytes, uint8_t hash, size_t n, const uint8_t *digest,
+                         const uint8_t *sig, const uint8_t *modulus, const uint32_t *pub_exp, uint8_t *ok);
+/* fused SHA-2 -> RSA: H = hash(M) never leaves the device; digest_out (n x hLen) may be NULL */
+int sbv_rsa_hash_verify_batch(sbv_engine *e, uint32_t mod_bytes, uint8_t hash, size_t n, const uint8_t *msgs,
+                              const uint64_t *msg_off, const uint8_t *sig, const uint8_t *modulus,
+                              const uint32_t *pub_exp, uint8_t *digest_out, uint8_t *ok);
+
 /* Mixed-curve batch: curve_tag[i] in {SBV_P256, SBV_P384}; every field is stored in a 48-byte
  * slot (P-256 values right-aligned, i.e. 16 leading zero bytes); digest is 32 bytes per item. */
 int sbv_verify_mixed(sbv_engine *e, size_t n, const uint8_t *curve_tag, const uint8_t *r48, const uint8_t *s48,

@@ -29,6 +29,8 @@ namespace sbv { uint32_t tab[1 << 18]; }
 #include "../../consensus_b200/csrc/shards.h"
 #include "../../consensus_b200/csrc/mixed.cuh"
 #include "../../consensus_b200/csrc/mixed_hash.cuh"
+#include "../../consensus_b200/csrc/rsa.cuh"
+#include "../../consensus_b200/csrc/sha512_batch.cuh"
 
 using namespace sbv;
 
@@ -896,4 +898,62 @@ extern "C" uint32_t hs_kca_set(int fam, const uint8_t *a, const uint8_t *b, uint
         *fp = kca_fp(w, seed);
     });
     return set;
+}
+
+// ---- RSA (rsa.cuh) and SHA-512 (sha512_batch.cuh) ----
+extern "C" int hs_sha512(size_t n, const uint8_t *msgs, const uint64_t *off, uint64_t base, const uint32_t *perm, uint8_t *digest_out) {
+    run_grid((unsigned)((n + 127) / 128), 128, [&] { k_sha512((uint32_t)n, msgs, off, base, digest_out, perm); });
+    return 0;
+}
+
+// k_rsa_verify over n items of k = 64 * nl bytes, two groups of 16 lanes per simulated warp, in lockstep
+extern "C" int hs_rsa_verify(int nl, size_t n, uint32_t hash, const uint8_t *sig, const uint8_t *mod, const uint32_t *pub_exp, const uint8_t *digest,
+                             uint8_t *ok) {
+    const unsigned blocks = (unsigned)((n * RSA_GROUP + 31) / 32);
+    if (nl == 4) run_grid_lockstep(blocks, 32, [&] { k_rsa_verify<4>((uint32_t)n, hash, sig, mod, pub_exp, digest, ok); });
+    else if (nl == 6) run_grid_lockstep(blocks, 32, [&] { k_rsa_verify<6>((uint32_t)n, hash, sig, mod, pub_exp, digest, ok); });
+    else if (nl == 8) run_grid_lockstep(blocks, 32, [&] { k_rsa_verify<8>((uint32_t)n, hash, sig, mod, pub_exp, digest, ok); });
+    else return -1;
+    return 0;
+}
+
+// The arithmetic of rsa.cuh item by item (k = 64 * NL bytes, big-endian): op 0: out = a * b * R^-1 mod N (a, b < N);
+// op 1: out = R^2 mod N, and ninv[i] = -N^-1 mod 2^32; op 2: out = a - N, ninv[i] = the borrow out (1: a < N); op 3: the
+// end of a product (rsa_resolve) on the limbs a and the lazy words b (16 little-endian words per item, one per lane).
+template <int NL>
+static void rsa_op_t(int op, size_t n, const uint8_t *a, const uint8_t *b, const uint8_t *mod, uint8_t *out, uint32_t *ninv) {
+    constexpr uint32_t k = 64 * NL;
+    run_grid_lockstep((unsigned)((n * RSA_GROUP + 31) / 32), 32, [&] {
+        const size_t i = (blockIdx.x * blockDim.x + threadIdx.x) / RSA_GROUP;
+        if (i >= n) return;
+        const RsaLanes g = rsa_lanes();
+        uint32_t x[NL], y[NL], nn[NL], r[NL];
+        rsa_load(g, nn, mod + i * k, k);
+        if (op == 3) {
+            rsa_load(g, r, a + i * k, k);
+            rsa_resolve(g, r, reinterpret_cast<const uint32_t *>(b)[i * RSA_GROUP + g.l], nn);
+        } else if (op == 2) {
+            rsa_load(g, x, a + i * k, k);
+            const uint32_t bo = rsa_sub(g, r, x, nn);
+            if (g.l == 0) ninv[i] = bo;
+        } else {
+            const uint32_t ni = rsa_ninv(g, nn);
+            if (g.l == 0) ninv[i] = ni;
+            if (op == 0) {
+                rsa_load(g, x, a + i * k, k);
+                rsa_load(g, y, b + i * k, k);
+                rsa_mont(g, r, x, y, nn, ni);
+            } else {
+                rsa_r2(g, r, nn, ni);
+            }
+        }
+        rsa_store(g, out + i * k, r, k);
+    });
+}
+extern "C" int hs_rsa_op(int nl, int op, size_t n, const uint8_t *a, const uint8_t *b, const uint8_t *mod, uint8_t *out, uint32_t *ninv) {
+    if (nl == 4) rsa_op_t<4>(op, n, a, b, mod, out, ninv);
+    else if (nl == 6) rsa_op_t<6>(op, n, a, b, mod, out, ninv);
+    else if (nl == 8) rsa_op_t<8>(op, n, a, b, mod, out, ninv);
+    else return -1;
+    return 0;
 }

@@ -52,6 +52,7 @@ KEY_CACHE_EVICT = ["tests/test_hostsim_key_cache_evict.py"]
 SEEDED = ["tests/test_hostsim_seeded_passes.py"]
 COMB_WARP = ["tests/test_hostsim_comb_warp.py"]  # the comb build a warp per key against the one-thread-per-chain reference  # the first entry of a pass loaded, not added (pt_seed)
 TABLE_SHAPES = ["tests/test_hostsim_table_shapes.py"]
+RSA = ["tests/test_hostsim_rsa.py"]  # rsa.cuh and k_sha512 (sha512_batch.cuh)
 MIXED384 = ["tests/test_hostsim_mixed384.py"]  # k_mix_alg and k_sha2_sel (mixed_hash.cuh)  # every entry of the per-key tables at the key counts where the builds turn over
 
 
@@ -348,6 +349,34 @@ CATALOGUE = [
     M("quorum_scan_other_instance", "quorum.cuh", "if (instance[j] - inst_base != inst) break;", "(void)0;", ECDSA),
     M("quorum_reached_gt", "quorum.cuh", "reached[i] = valid_count[i] >= threshold ? 1 : 0;", "reached[i] = valid_count[i] > threshold ? 1 : 0;", ECDSA),
     M("pack_bits_tail", "quorum.cuh", "const uint32_t bit = (i < n && ok[i]) ? 1u : 0u;", "const uint32_t bit = ok[i] ? 1u : 0u;", ECDSA),
+    # ---------------------------------------------------------------- rsa.cuh: carries, final subtraction, range, encoding, exponent
+    M("rsa_lazy_word_dropped", "rsa.cuh", "    if (g.l == 0) c = 0;", "    c = 0;", RSA),
+    M("rsa_carry_propagate_ignored", "rsa.cuh", "const uint32_t cin = ((gen << 1) + prop) ^ prop;", "const uint32_t cin = gen << 1;", RSA),
+    M("rsa_carry_out_of_top_dropped", "rsa.cuh", "const uint32_t top = ((cin >> 16) & 1) + rsa_from(g, czl, RSA_GROUP - 1);",
+      "const uint32_t top = rsa_from(g, czl, RSA_GROUP - 1);", RSA),
+    M("rsa_final_sub_ignores_top", "rsa.cuh", "if (top || !borrow) {", "if (!borrow) {", RSA),
+    M("rsa_final_sub_ignores_borrow", "rsa.cuh", "if (top || !borrow) {", "if (top) {", RSA),
+    M("rsa_borrow_propagate_ignored", "rsa.cuh", "const uint32_t bin = ((gen << 1) + prop) ^ prop;", "const uint32_t bin = gen << 1;", RSA),
+    M("rsa_key_leading_byte_dropped", "rsa.cuh", "if (!(n0 & 1) || (ntop >> 24) == 0 || e < 2 || e > 0x7fffffffu) return false;",
+      "if (!(n0 & 1) || e < 2 || e > 0x7fffffffu) return false;", RSA),
+    M("rsa_key_e_lower_bound", "rsa.cuh", "if (!(n0 & 1) || (ntop >> 24) == 0 || e < 2 || e > 0x7fffffffu) return false;",
+      "if (!(n0 & 1) || (ntop >> 24) == 0 || e < 1 || e > 0x7fffffffu) return false;", RSA),
+    M("rsa_key_e_upper_bound", "rsa.cuh", "if (!(n0 & 1) || (ntop >> 24) == 0 || e < 2 || e > 0x7fffffffu) return false;",
+      "if (!(n0 & 1) || (ntop >> 24) == 0 || e < 2) return false;", RSA),
+    M("rsa_range_check_dropped", "rsa.cuh", "if (!rsa_sub(g, x, s, n)) return false;", "rsa_sub(g, x, s, n);", RSA),
+    M("rsa_ff_run_short", "rsa.cuh", "else if (r < k - 2) v = 0xff;", "else if (r < k - 3) v = 0xff;", RSA),
+    M("rsa_separator_byte", "rsa.cuh", "else if (r == tl) v = 0x00;", "else if (r == tl) v = 0xff;", RSA),
+    M("rsa_digest_info_of_sha256", "rsa.cuh", "v = RSA_DIGEST_INFO[hash][tl - 1 - r];", "v = RSA_DIGEST_INFO[0][tl - 1 - r];", RSA),
+    M("rsa_block_type_byte", "rsa.cuh", "else if (r == k - 2) v = 0x01;", "else if (r == k - 2) v = 0x02;", RSA),
+    M("rsa_compare_lane_local", "rsa.cuh", "return rsa_bits(g, bad != 0) == 0;", "return bad == 0;", RSA),
+    M("rsa_exp_multiply_bit", "rsa.cuh", "else if ((e >> i) & 1) mul = true;", "else if ((e >> i) & 2) mul = true;", RSA),
+    M("rsa_exp_top_bit", "rsa.cuh", "int i = 30 - __clz((int)e);", "int i = 31 - __clz((int)e);", RSA),
+    M("rsa_exp_square_skipped", "rsa.cuh", "if (mul) { mul = false; i--; }", "if (mul) { mul = false; i -= 2; }", RSA),
+    M("rsa_r2_doublings", "rsa.cuh", "for (int i = 0; i < 33 * K - b + 1; i++) {", "for (int i = 0; i < 33 * K - b; i++) {", RSA),
+    M("rsa_quotient_digit", "rsa.cuh", "const uint32_t q = rsa_from(g, t[0], 0) * ninv;", "const uint32_t q = t[0] * ninv;", RSA),
+    # ---------------------------------------------------------------- sha512_batch.cuh
+    M("sha512_batch_length_bytes", "sha512_batch.cuh", "w[15] = len << 3;", "w[15] = len;", RSA),
+    M("sha512_batch_iv", "sha512_batch.cuh", "0x5be0cd19137e2179ull", "0x47b5481dbefa4fa4ull", RSA),
     # ---------------------------------------------------------------- mixed_hash.cuh
     M("mix_alg_tag_map", "mixed_hash.cuh", "tag[i] = (uint8_t)(wide ? t - MIX_TAG_SHA384 : t);", "tag[i] = (uint8_t)t;", MIXED384),
     M("mix_alg_flag", "mixed_hash.cuh", "sha384[i] = wide ? 1 : 0;", "sha384[i] = 0;", MIXED384),
