@@ -4,6 +4,7 @@
 #include "engine.h"
 #include "debug_ops.cuh"
 #include "ed25519_debug.cuh"
+#include "rsa_debug.cuh"
 using namespace sbv;
 // debug.cu — arithmetic-layer test hooks (used only by tests/; not part of include/sbv.h).
 // Operands are little-endian 32-bit limb arrays, 2N limbs per slot (unused limbs zero).
@@ -125,6 +126,41 @@ extern "C" int sbv_debug_ed25519_sha512(sbv_engine *e, size_t n, const uint8_t *
             for (int b = 0; b < 4; b++) dig_out[i * 64 + 4 * w + b] = (uint8_t)(dig[i * 16 + w] >> (8 * b));
         for (int w = 0; w < 8; w++) k_out[i * 8 + w] = kw[(size_t)w * n + i];
     }
+    return SBV_OK;
+}
+
+// The RSA arithmetic of rsa.cuh on device 0: op and the item layout of rsa_debug.cuh (a, b, mod, out: mod_bytes bytes per
+// item; exp, aux: one word), k_rsa_debug in blocks of 128 threads as k_rsa_verify runs.  SBV_ERR_ARG, with nothing
+// written, for a modulus size outside 256 / 384 / 512, an op outside 0-4, a null buffer or n >= 2^31.
+extern "C" int sbv_debug_rsa(sbv_engine *e, uint32_t mod_bytes, int op, size_t n, const uint8_t *a, const uint8_t *b, const uint8_t *mod,
+                             const uint32_t *exp, uint8_t *out, uint32_t *aux) {
+    if (!e || !rsa_debug_args_ok(mod_bytes, op, n, a, b, mod, exp, out, aux)) return SBV_ERR_ARG;
+    if (n == 0) return SBV_OK;
+    std::lock_guard<std::mutex> lk(e->mu);
+    Dev &d = e->devs[0];
+    CU(e, cudaSetDevice(d.ordinal));
+    const size_t bytes = n * mod_bytes, words = (n * 4 + 255) & ~(size_t)255;
+    int rc = sbv_ensure_scratch(e, d, 4 * bytes + 2 * words + 1024);
+    if (rc) return rc;
+    uint8_t *p = d.d_scratch;
+    uint8_t *da = p; p += bytes;
+    uint8_t *db = p; p += bytes;
+    uint8_t *dmod = p; p += bytes;
+    uint8_t *dout = p; p += bytes;
+    uint32_t *dexp = (uint32_t *)p; p += words;
+    uint32_t *daux = (uint32_t *)p;
+    CU(e, cudaMemcpyAsync(da, a, bytes, cudaMemcpyHostToDevice, d.stream));
+    CU(e, cudaMemcpyAsync(db, b, bytes, cudaMemcpyHostToDevice, d.stream));
+    CU(e, cudaMemcpyAsync(dmod, mod, bytes, cudaMemcpyHostToDevice, d.stream));
+    CU(e, cudaMemcpyAsync(dexp, exp, n * 4, cudaMemcpyHostToDevice, d.stream));
+    const uint32_t blocks = (uint32_t)((n * RSA_GROUP + 127) / 128);
+    if (mod_bytes == 256) k_rsa_debug<4><<<blocks, 128, 0, d.stream>>>(op, (uint32_t)n, da, db, dmod, dexp, dout, daux);
+    else if (mod_bytes == 384) k_rsa_debug<6><<<blocks, 128, 0, d.stream>>>(op, (uint32_t)n, da, db, dmod, dexp, dout, daux);
+    else k_rsa_debug<8><<<blocks, 128, 0, d.stream>>>(op, (uint32_t)n, da, db, dmod, dexp, dout, daux);
+    CU(e, cudaGetLastError());
+    CU(e, cudaMemcpyAsync(out, dout, bytes, cudaMemcpyDeviceToHost, d.stream));
+    CU(e, cudaMemcpyAsync(aux, daux, n * 4, cudaMemcpyDeviceToHost, d.stream));
+    CU(e, cudaStreamSynchronize(d.stream));
     return SBV_OK;
 }
 

@@ -96,7 +96,17 @@ class Key:
             p, q = _prime((bits + 1) // 2, rng), _prime(bits // 2, rng)
             if p != q and (p * q).bit_length() == bits:
                 break
-        self.p, self.q, self.n, self.bits = p, q, p * q, bits
+        self._set(p, q)
+
+    @classmethod
+    def from_primes(cls, p: int, q: int) -> "Key":
+        """The key of two given primes (a committed fixture, or primes of a special form)."""
+        key = cls.__new__(cls)
+        key._set(p, q)
+        return key
+
+    def _set(self, p: int, q: int) -> None:
+        self.p, self.q, self.n, self.bits = p, q, p * q, (p * q).bit_length()
         self.lam = math.lcm(p - 1, q - 1)
 
     def mod_bytes(self, k: int) -> bytes:

@@ -1,23 +1,25 @@
 """The RSA device code (rsa.cuh) and k_sha512 (sha512_batch.cuh) in the CPU simulation (tools/hostsim), a group of 16
 lanes per item run in lockstep, one OS thread per lane:
 
-- Montgomery products against Python integers for 0, 1, N - 1, operands near R and random operands, on moduli at both
-  ends (an all-ones top limb, and 2^(8k-8) + 1) and on real keys, for every size;
-- S - N and its borrow, n0' = -N^-1 mod 2^32 and R^2 mod N for every size;
-- the carry resolution that ends a product, on redundant forms that reach every branch of its ballot;
+- the arithmetic sets of tests/rsa_arith.py through hs_rsa_debug (k_rsa_debug of rsa_debug.cuh, as sbv_debug_rsa runs it on
+  the device): Montgomery products through every outcome of the final subtraction, R^2 mod N and n0', S - N with its
+  borrow generated in every lane, the carry resolution that ends a product in every lane, and S^e mod N; the products,
+  R^2 and S^e on a subset of the modulus shapes (test_gpu_rsa_arith.py runs every shape);
 - a handful of whole verifications per class of tests/rsa_cases.py, against oracle_rsa.ref;
+- one item of every class of tests/rsa_edges.py per size (test_gpu_rsa_edges.py runs every item);
 - k_sha512 against hashlib at the padding boundaries and unaligned starts.
-The GPU twin of this file is test_gpu_rsa.py."""
+The GPU twins of this file are test_gpu_rsa.py, test_gpu_rsa_arith.py and test_gpu_rsa_edges.py."""
 import ctypes as C
 import hashlib
 import os
-import random
 import subprocess
 
 import numpy as np
 import pytest
 
+import rsa_arith as arith
 import rsa_cases as rc
+import rsa_edges as edges
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 HS_DIR = os.path.join(ROOT, "tools", "hostsim")
@@ -30,26 +32,16 @@ def hs():
 
 
 def _p(a):
-    return a.ctypes.data_as(C.c_void_p)
+    return None if a is None else a.ctypes.data_as(C.c_void_p)
 
 
-def _rows(vals, k):
-    return np.frombuffer(b"".join(v.to_bytes(k, "big") for v in vals), np.uint8).reshape(len(vals), k).copy()
+def _call(hs):
+    return lambda mb, op, n, *bufs: hs.hs_rsa_debug(C.c_uint32(mb), C.c_int(op), C.c_size_t(n), *map(_p, bufs))
 
 
-def _op(hs, k, op, a, b, n):
-    cnt = len(n)
-    A, B, N = _rows(a, k), _rows(b, k), _rows(n, k)
-    out, ninv = np.zeros((cnt, k), np.uint8), np.zeros(cnt, np.uint32)
-    assert hs.hs_rsa_op(C.c_int(k // 64), C.c_int(op), C.c_size_t(cnt), _p(A), _p(B), _p(N), _p(out), _p(ninv)) == 0
-    return [int.from_bytes(r.tobytes(), "big") for r in out], [int(x) for x in ninv]
-
-
-def _moduli(k):
-    """Odd moduli at both ends of the size: an all-ones top limb, 2^(8k-8) + 1 (the smallest with a nonzero leading byte),
-    a random one with the top bit set, and a real key."""
-    rng = random.Random(k)
-    return [2 ** (8 * k) - 1 - 2 * rng.getrandbits(8 * k - 40), 2 ** (8 * k - 8) + 1, rng.getrandbits(8 * k) | 1 | (1 << (8 * k - 1)), rc.key(8 * k).n]
+@pytest.fixture(scope="module")
+def run(hs):
+    return arith.runner(_call(hs))
 
 
 def _ragged(lens, lead, seed):
@@ -72,88 +64,32 @@ def test_sha512_lengths_and_offsets(hs, start):
 
 
 @pytest.mark.parametrize("k", rc.SIZES)
-def test_montgomery_products(hs, k):
-    R = 2 ** (8 * k)
-    rng = random.Random(100 + k)
-    a, b, n = [], [], []
-    for N in _moduli(k):
-        near_r = [N - 1, N - 2, (R - 1) % N, (R - 2**32) % N]
-        ops = [0, 1, N - 1, rng.randrange(N), rng.randrange(N)] + near_r
-        pairs = [(0, rng.randrange(N)), (1, 1), (N - 1, N - 1), (N - 1, 1), (ops[3], ops[4]), (near_r[2], near_r[2]), (near_r[3], near_r[0]),
-                 (rng.randrange(N), rng.randrange(N))]
-        for x, y in pairs:
-            a.append(x); b.append(y); n.append(N)
-    got, ninv = _op(hs, k, 0, a, b, n)
-    rinv = {N: pow(R, -1, N) for N in set(n)}
-    for i, (x, y, N) in enumerate(zip(a, b, n)):
-        assert got[i] == x * y * rinv[N] % N, (i, hex(N)[:12])
-        assert ninv[i] == (-pow(N, -1, 2**32)) % 2**32
+def test_montgomery_products(run, k):
+    arith.check_products(run, k, full=False)
 
 
 @pytest.mark.parametrize("k", rc.SIZES)
-def test_r2_and_ninv(hs, k):
-    ns = _moduli(k)
-    got, ninv = _op(hs, k, 1, [0] * len(ns), [0] * len(ns), ns)
-    for N, r2, ni in zip(ns, got, ninv):
-        assert r2 == 2 ** (16 * k) % N
-        assert ni == (-pow(N, -1, 2**32)) % 2**32
+def test_r2_and_ninv(run, k):
+    arith.check_r2_ninv(run, k, full=False)
 
 
 @pytest.mark.parametrize("k", rc.SIZES)
-def test_subtraction_borrow(hs, k):
-    """S - N with its borrows resolved across the group: the range check S < N."""
-    N = rc.key(8 * k).n
-    R = 2 ** (8 * k)
-    a = [0, 1, N - 1, N, N + 1, R - 1, N + (1 << 200), N - (1 << 300), (N >> 64) << 64]
-    got, bo = _op(hs, k, 2, a, [0] * len(a), [N] * len(a))
-    for x, d, b in zip(a, got, bo):
-        assert d == (x - N) % R and b == (1 if x < N else 0), hex(x)[:20]
+def test_subtraction_borrow(run, k):
+    arith.check_sub(run, k)
 
 
 @pytest.mark.parametrize("k", rc.SIZES)
-def test_carry_resolution(hs, k):
-    """The end of a product (rsa_resolve) on redundant forms built to reach every branch of the ballot: lanes that are all
-    ones after the lazy word below lands (propagate), lanes whose add carries out (generate), chains of both up to and
-    out of the top lane, and values on both sides of N.  A form is limbs t plus a lazy word cz_l <= 3 per lane at the
-    weight of lane l + 1's first limb; the value is below 2N, and the result must be that value mod N."""
-    K = k // 4
-    NL = K // 16
-    W = 32 * NL  # bits per lane
-    R = 2 ** (8 * k)
-    rng = random.Random(200 + k)
-    N = 2 ** (8 * k) - 1 - 2 * rng.getrandbits(8 * k - 40)  # top 40 bits all ones, so R - small < 2N
-    lane_ones = (1 << W) - 1
-    forms = []
+def test_carry_resolution(run, k):
+    assert arith.check_resolve(run, k) > 150
 
-    def add(t, cz):
-        v = t + sum(c << (W * (l + 1)) for l, c in enumerate(cz))
-        if 0 <= t < R and v < 2 * N:
-            forms.append((t, cz, v))
 
-    add(R - 4, [0] * 16)                           # no lazy words: lanes 1..15 all ones, nothing moves
-    add(R - 3, [2] + [0] * 15)                     # lane 1 overflows; lanes 2..15 propagate; the carry leaves the top
-    add(R - 1 - (3 << W), [3] + [0] * 15)          # lane 1 becomes all ones: it propagates, nothing to propagate
-    add(R - (3 << W), [3] + [0] * 15)              # value R: lane 1 overflows and the carry leaves the top
-    add(R - (1 << (W * 15)), [0] * 14 + [1, 0])    # lane 15 overflows on its lazy word alone
-    add(N - 1, [0] * 16)
-    add(N, [0] * 16)
-    add(N - (2 << (W * 3)), [0, 0, 2] + [0] * 13)
-    for _ in range(40):
-        cz = [rng.randrange(4) if rng.random() < 0.7 else 0 for _ in range(15)] + [0]
-        # limbs mostly all ones, so that carries meet propagating lanes
-        t = 0
-        for l in range(16):
-            t |= (lane_ones - (rng.randrange(4) if rng.random() < 0.3 else 0)) << (W * l)
-        add(t - rng.randrange(2 ** 20), cz)
-        add(rng.randrange(2 * N) - sum(c << (W * (l + 1)) for l, c in enumerate(cz)), cz)
-    assert len(forms) > 40
-    A = _rows([f[0] for f in forms], k)
-    B = np.array([f[1] for f in forms], np.uint32)
-    Nr = _rows([N] * len(forms), k)
-    out, dummy = np.zeros((len(forms), k), np.uint8), np.zeros(len(forms), np.uint32)
-    assert hs.hs_rsa_op(C.c_int(NL), C.c_int(3), C.c_size_t(len(forms)), _p(A), _p(B), _p(Nr), _p(out), _p(dummy)) == 0
-    for (t, cz, v), o in zip(forms, out):
-        assert int.from_bytes(o.tobytes(), "big") == v % N, (hex(t)[:20], cz)
+@pytest.mark.parametrize("k", rc.SIZES)
+def test_pow_chains(run, k):
+    arith.check_pow(run, k, full=False)
+
+
+def test_hook_refuses_bad_calls(hs):
+    arith.check_refused(_call(hs))
 
 
 def _verify(hs, c, idx):
@@ -181,3 +117,26 @@ def test_whole_verifications_per_class(hs, k, hash):
     bad = [c["cls"][i] for i, g, w in zip(idx, ok, want) if g != w]
     assert not bad, bad
     assert 0 < want.sum() < len(idx)
+
+
+# one hash per size, so that the three pairs cover every hash and the 4096-bit size meets SHA-384
+EDGE_HASH = {256: edges.ref.SHA256, 384: edges.ref.SHA512, 512: edges.ref.SHA384}
+
+
+@pytest.mark.parametrize("k", rc.SIZES)
+def test_edge_classes(hs, k):
+    """One item of every class of tests/rsa_edges.py: the shortest key's valid and corrupted signatures, the longest odd
+    exponent with alternating bits, an even exponent accepted (S and N - S) and refused (-EM), a changed DigestInfo
+    byte, the separator, a digest byte and one changed byte in a middle lane."""
+    h = EDGE_HASH[k]
+    K, NL = k // 4, k // 64
+    sets = [(edges.bitlen(k, h), [f"bitlen{8 * k - 7}_valid", f"bitlen{8 * k - 7}_valid_bit", f"bitlen{8 * k - 4}_n-1"]),
+            (edges.oddexp(k, h), ["oddexp_0x55555555"]),
+            (edges.evenexp(k, h), ["evenexp_0x2_n-s", "evenexp_0x7ffffffe_s", "evenexp_0x4_minus_em"]),
+            (edges.encoding(k, h, limbs=[7 * NL + 2]), ["encoding_good", "encoding_digest_info9", "encoding_separator", "encoding_digest17",
+                                                         f"encoding_limb{7 * NL + 2}"])]
+    for c, names in sets:
+        idx = np.array([c["cls"].index(nm) for nm in names])
+        ok = _verify(hs, c, idx)
+        assert list(ok) == list(c["want"][idx]), list(zip(names, ok))
+    assert K > 7 * NL + 2

@@ -30,6 +30,7 @@ namespace sbv { uint32_t tab[1 << 18]; }
 #include "../../consensus_b200/csrc/mixed.cuh"
 #include "../../consensus_b200/csrc/mixed_hash.cuh"
 #include "../../consensus_b200/csrc/rsa.cuh"
+#include "../../consensus_b200/csrc/rsa_debug.cuh"
 #include "../../consensus_b200/csrc/sha512_batch.cuh"
 
 using namespace sbv;
@@ -917,43 +918,32 @@ extern "C" int hs_rsa_verify(int nl, size_t n, uint32_t hash, const uint8_t *sig
     return 0;
 }
 
-// The arithmetic of rsa.cuh item by item (k = 64 * NL bytes, big-endian): op 0: out = a * b * R^-1 mod N (a, b < N);
-// op 1: out = R^2 mod N, and ninv[i] = -N^-1 mod 2^32; op 2: out = a - N, ninv[i] = the borrow out (1: a < N); op 3: the
-// end of a product (rsa_resolve) on the limbs a and the lazy words b (16 little-endian words per item, one per lane).
-template <int NL>
-static void rsa_op_t(int op, size_t n, const uint8_t *a, const uint8_t *b, const uint8_t *mod, uint8_t *out, uint32_t *ninv) {
-    constexpr uint32_t k = 64 * NL;
-    run_grid_lockstep((unsigned)((n * RSA_GROUP + 31) / 32), 32, [&] {
-        const size_t i = (blockIdx.x * blockDim.x + threadIdx.x) / RSA_GROUP;
-        if (i >= n) return;
-        const RsaLanes g = rsa_lanes();
-        uint32_t x[NL], y[NL], nn[NL], r[NL];
-        rsa_load(g, nn, mod + i * k, k);
-        if (op == 3) {
-            rsa_load(g, r, a + i * k, k);
-            rsa_resolve(g, r, reinterpret_cast<const uint32_t *>(b)[i * RSA_GROUP + g.l], nn);
-        } else if (op == 2) {
-            rsa_load(g, x, a + i * k, k);
-            const uint32_t bo = rsa_sub(g, r, x, nn);
-            if (g.l == 0) ninv[i] = bo;
-        } else {
-            const uint32_t ni = rsa_ninv(g, nn);
-            if (g.l == 0) ninv[i] = ni;
-            if (op == 0) {
-                rsa_load(g, x, a + i * k, k);
-                rsa_load(g, y, b + i * k, k);
-                rsa_mont(g, r, x, y, nn, ni);
-            } else {
-                rsa_r2(g, r, nn, ni);
-            }
-        }
-        rsa_store(g, out + i * k, r, k);
-    });
-}
-extern "C" int hs_rsa_op(int nl, int op, size_t n, const uint8_t *a, const uint8_t *b, const uint8_t *mod, uint8_t *out, uint32_t *ninv) {
-    if (nl == 4) rsa_op_t<4>(op, n, a, b, mod, out, ninv);
-    else if (nl == 6) rsa_op_t<6>(op, n, a, b, mod, out, ninv);
-    else if (nl == 8) rsa_op_t<8>(op, n, a, b, mod, out, ninv);
-    else return -1;
+// The arithmetic of rsa.cuh item by item: k_rsa_debug (rsa_debug.cuh) as libsbv.so's sbv_debug_rsa runs it, in blocks of
+// 128 threads, with the same arguments.  -1 (and nothing written) for the calls rsa_debug_args_ok refuses.
+extern "C" int hs_rsa_debug(uint32_t mod_bytes, int op, size_t n, const uint8_t *a, const uint8_t *b, const uint8_t *mod, const uint32_t *exp,
+                            uint8_t *out, uint32_t *aux) {
+    if (!rsa_debug_args_ok(mod_bytes, op, n, a, b, mod, exp, out, aux)) return -1;
+    const unsigned blocks = (unsigned)((n * RSA_GROUP + 127) / 128);
+    if (mod_bytes == 256) run_grid_lockstep(blocks, 128, [&] { k_rsa_debug<4>(op, (uint32_t)n, a, b, mod, exp, out, aux); });
+    else if (mod_bytes == 384) run_grid_lockstep(blocks, 128, [&] { k_rsa_debug<6>(op, (uint32_t)n, a, b, mod, exp, out, aux); });
+    else run_grid_lockstep(blocks, 128, [&] { k_rsa_debug<8>(op, (uint32_t)n, a, b, mod, exp, out, aux); });
     return 0;
+}
+
+// Ops 0-3 of hs_rsa_debug in the older layout: k = 64 * nl bytes, ninv[i] = aux, and for op 3 the 16 lazy words of item i
+// packed at b + 64 i (not spread over a k-byte row).
+extern "C" int hs_rsa_op(int nl, int op, size_t n, const uint8_t *a, const uint8_t *b, const uint8_t *mod, uint8_t *out, uint32_t *ninv) {
+    if (op < RSA_DBG_MONT || op > RSA_DBG_RESOLVE || nl <= 0) return -1;
+    const size_t k = 64 * (size_t)nl;
+    std::vector<uint8_t> rows;
+    if (op == RSA_DBG_RESOLVE && b) {
+        rows.assign(n * k, 0);
+        for (size_t i = 0; i < n; i++) memcpy(&rows[i * k], b + i * 64, 64);
+        b = rows.data();
+    }
+    std::vector<uint32_t> exp(n, 0), aux(n);
+    const int rc = hs_rsa_debug((uint32_t)k, op, n, a, b, mod, exp.data(), out, aux.data());
+    if (rc == 0 && op != RSA_DBG_RESOLVE)
+        for (size_t i = 0; i < n; i++) ninv[i] = aux[i];
+    return rc;
 }

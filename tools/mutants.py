@@ -374,6 +374,15 @@ CATALOGUE = [
     M("rsa_exp_square_skipped", "rsa.cuh", "if (mul) { mul = false; i--; }", "if (mul) { mul = false; i -= 2; }", RSA),
     M("rsa_r2_doublings", "rsa.cuh", "for (int i = 0; i < 33 * K - b + 1; i++) {", "for (int i = 0; i < 33 * K - b; i++) {", RSA),
     M("rsa_quotient_digit", "rsa.cuh", "const uint32_t q = rsa_from(g, t[0], 0) * ninv;", "const uint32_t q = t[0] * ninv;", RSA),
+    # the bit length of N in rsa_r2 taken as 32K: wrong for every modulus whose top bit is clear
+    M("rsa_r2_bit_length_32k", "rsa.cuh", "const int b = 32 * K - __clz((int)ntop);", "const int b = 32 * K;", RSA),
+    M("rsa_resolve_lazy_word_lane", "rsa.cuh", "uint32_t c = rsa_from(g, czl, g.l ? g.l - 1 : 0)", "uint32_t c = rsa_from(g, czl, g.l > 1 ? g.l - 2 : 0)", RSA),
+    # a byte-index slip confined to SHA-384 at 4096 bits: the whole verifications of test_hostsim_rsa.py skip that pair, the
+    # edge classes run it
+    M("rsa_encoding_byte_index_sha384_4096", "rsa.cuh", "const uint32_t r = 4 * (g.l * NL + j) + q;",
+      "const uint32_t r = 4 * (g.l * NL + j) + (hash == 1 && NL == 8 ? q ^ 1 : q);", RSA),
+    # an exponent whose bit 0 is clear ends on a squaring: only the even exponents of the edge classes reach it
+    M("rsa_exp_last_square_dropped", "rsa.cuh", "while (i >= 0) {", "while (i > 0 || (i == 0 && (mul || (e & 1)))) {", RSA),
     # ---------------------------------------------------------------- sha512_batch.cuh
     M("sha512_batch_length_bytes", "sha512_batch.cuh", "w[15] = len << 3;", "w[15] = len;", RSA),
     M("sha512_batch_iv", "sha512_batch.cuh", "0x5be0cd19137e2179ull", "0x47b5481dbefa4fa4ull", RSA),
