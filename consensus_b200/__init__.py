@@ -19,6 +19,7 @@ P256_SHA384, P384_SHA384 = 3, 4  # ECDSA over SHA-384: scheme tags of the mixed3
 FIELD_BYTES = {P256: 32, P384: 48}
 SHA256, SHA384, SHA512 = 0, 1, 2  # hash tags of the RSA calls (SBV_HASH_*)
 HASH_BYTES = {SHA256: 32, SHA384: 48, SHA512: 64}
+PSS_SALT_EQUALS_HASH, PSS_SALT_AUTO = -1, 0  # salt_len of the RSA-PSS calls (Go's PSSOptions.SaltLength)
 
 SYMBOLS = [
     "sbv_create", "sbv_destroy", "sbv_last_error", "sbv_device_count", "sbv_verify_batch",
@@ -33,6 +34,7 @@ SYMBOLS = [
     "sbv_key_cache_reserve", "sbv_key_cache_stats", "sbv_key_cache_reserve_evicting", "sbv_key_cache_stats_ex",
     "sbv_mixed384_verify_registered", "sbv_mixed384_verify_batch", "sbv_mixed384_verify_quorum",
     "sbv_sha512_batch", "sbv_rsa_verify_batch", "sbv_rsa_hash_verify_batch",
+    "sbv_rsa_pss_verify_batch", "sbv_rsa_pss_hash_verify_batch",
 ]
 
 
@@ -311,6 +313,46 @@ class Engine:
         vp = C.c_void_p
         self._check(self._lib.sbv_rsa_hash_verify_batch(self._h, C.c_uint32(mod_bytes), C.c_uint8(hash), C.c_size_t(n), vp(msgs), vp(off), vp(sig),
                                                         vp(modulus), vp(pub_exp), vp(digest_out or None), vp(ok)), "sbv_rsa_hash_verify_batch")
+
+    def rsa_pss_verify_batch(self, hash, salt_len, digest, sig, modulus, pub_exp, out=None) -> np.ndarray:
+        """RSA-PSS (Go crypto/rsa.VerifyPSS, MGF1 over the same hash) over supplied digests: salt_len = PSS_SALT_EQUALS_HASH,
+        PSS_SALT_AUTO or the exact salt length; the other arguments as in rsa_verify_batch."""
+        pub_exp = np.ascontiguousarray(pub_exp, dtype=np.uint32)
+        n = pub_exp.size
+        sig, modulus, digest = _u8(sig), _u8(modulus), _u8(digest)
+        k = sig.size // n if n else 256
+        ok = out if out is not None else np.zeros(n, np.uint8)
+        self.rsa_pss_verify_batch_ptr(k, hash, salt_len, n, digest.ctypes.data, sig.ctypes.data, modulus.ctypes.data, pub_exp.ctypes.data,
+                                      ok.ctypes.data)
+        return ok
+
+    def rsa_pss_verify_batch_ptr(self, mod_bytes, hash, salt_len, n, digest, sig, modulus, pub_exp, ok):
+        """Raw host pointers (ints) — used with pinned buffers."""
+        vp = C.c_void_p
+        self._check(self._lib.sbv_rsa_pss_verify_batch(self._h, C.c_uint32(mod_bytes), C.c_uint8(hash), C.c_int32(salt_len), C.c_size_t(n), vp(digest),
+                                                       vp(sig), vp(modulus), vp(pub_exp), vp(ok)), "sbv_rsa_pss_verify_batch")
+
+    def rsa_pss_hash_verify_batch(self, hash, salt_len, msgs, off, sig, modulus, pub_exp, want_digest=False):
+        """rsa_pss_verify_batch with H = hash(M) computed on the device; msgs concatenated with off[n+1] byte offsets.
+        Returns the verdicts, and the n x hLen digests too with want_digest."""
+        msgs = _u8(msgs if len(msgs) else np.zeros(1, np.uint8))
+        off = np.ascontiguousarray(off, dtype=np.uint64)
+        pub_exp = np.ascontiguousarray(pub_exp, dtype=np.uint32)
+        sig, modulus = _u8(sig), _u8(modulus)
+        n = off.size - 1
+        k = sig.size // n if n else 256
+        ok = np.zeros(n, np.uint8)
+        dig = np.zeros((n, HASH_BYTES[hash]), np.uint8) if want_digest else None
+        self.rsa_pss_hash_verify_batch_ptr(k, hash, salt_len, n, msgs.ctypes.data, off.ctypes.data, sig.ctypes.data, modulus.ctypes.data,
+                                           pub_exp.ctypes.data, dig.ctypes.data if want_digest else 0, ok.ctypes.data)
+        return (ok, dig) if want_digest else ok
+
+    def rsa_pss_hash_verify_batch_ptr(self, mod_bytes, hash, salt_len, n, msgs, off, sig, modulus, pub_exp, digest_out, ok):
+        """Raw host pointers (ints; digest_out may be 0) — used with pinned buffers."""
+        vp = C.c_void_p
+        self._check(self._lib.sbv_rsa_pss_hash_verify_batch(self._h, C.c_uint32(mod_bytes), C.c_uint8(hash), C.c_int32(salt_len), C.c_size_t(n),
+                                                            vp(msgs), vp(off), vp(sig), vp(modulus), vp(pub_exp), vp(digest_out or None), vp(ok)),
+                    "sbv_rsa_pss_hash_verify_batch")
 
     def hash384_verify_batch_ptr(self, curve, n, msgs, off, r, s, qx, qy, digest_out, ok):
         """Raw host pointers (ints; digest_out may be 0) — used with pinned buffers."""

@@ -305,6 +305,10 @@ int sbv_launch_sha512(sbv_engine *e, size_t n, const uint8_t *d_msgs, const uint
 // 4-byte aligned.
 int sbv_launch_rsa(sbv_engine *e, uint32_t mod_bytes, uint8_t hash, size_t n, const uint8_t *d_sig, const uint8_t *d_mod, const uint32_t *d_exp,
                    const uint8_t *d_digest, uint8_t *d_ok, cudaStream_t st);
+// RSA-PSS (rsa_pss.cuh): k_rsa_em over the same buffers, EM written over d_sig, then k_rsa_pss for the hash tag with
+// salt_len as in sbv_rsa_pss_verify_batch (>= -1); verdicts into d_ok.  Two launches.
+int sbv_launch_rsa_pss(sbv_engine *e, uint32_t mod_bytes, uint8_t hash, int32_t salt_len, size_t n, uint8_t *d_sig, const uint8_t *d_mod,
+                       const uint32_t *d_exp, const uint8_t *d_digest, uint8_t *d_ok, cudaStream_t st);
 // mixed_hash.cuh: k_mix_alg over the n uploaded tags of a mixed shard (tags 3 and 4 to their family, flags into d_alg)
 int sbv_launch_mix_alg(sbv_engine *e, size_t n, uint8_t *d_tag, uint8_t *d_alg, cudaStream_t st);
 // mixed_hash.cuh: k_sha2_sel over the n items of one family (d_idx: their shard indices, d_alg: the shard's flags), dlen

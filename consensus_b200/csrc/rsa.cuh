@@ -1,5 +1,6 @@
 // rsa.cuh — RSA PKCS #1 v1.5 signature verification (RFC 8017 §8.2.2, Go's crypto/rsa.VerifyPKCS1v15) for moduli of
-// 2048, 3072 and 4096 bits (k = 256, 384 or 512 bytes), a group of 16 lanes per signature, two signatures per warp.
+// 2048, 3072 and 4096 bits (k = 256, 384 or 512 bytes), a group of 16 lanes per signature, two signatures per warp.  The
+// key rule, the range check and the exponentiation (rsa_recover) serve RSA-PSS too (rsa_pss.cuh).
 //
 // Layout.  A k-byte number is K = k/4 little-endian 32-bit limbs; lane l of the group holds limbs [l*NL, l*NL + NL),
 // NL = K/16 = 4, 6 or 8, of every operand.  Values cross the group only by shuffle and ballot under the group's mask.
@@ -209,10 +210,11 @@ SBV_DEV void rsa_r2(const RsaLanes &g, uint32_t (&x)[NL], const uint32_t (&n)[NL
     for (int i = 0; i < 5; i++) rsa_mont(g, x, x, x, n, ninv);
 }
 
-// The verdict of one item (the same in every lane of the group).  sig, mod: k bytes big-endian; e: the public exponent;
-// h: the hLen-byte digest, hash 0 / 1 / 2 = SHA-256 / SHA-384 / SHA-512.
-template <int NL>
-SBV_DEV bool rsa_verify_item(const RsaLanes &g, const uint8_t *sig, const uint8_t *mod, uint32_t e, const uint8_t *h, uint32_t hash) {
+// Steps 1-3 of both paddings (the same in every lane of the group): false if the key rule or S < N refuses the item, else
+// tail(em), em = S^e mod N, this lane's limbs.  sig, mod: k bytes big-endian; e: the public exponent.  The padding's part
+// is a callable rather than a caller testing a flag, so that every refusal returns straight out of the kernel's item.
+template <int NL, class Tail>
+SBV_DEV bool rsa_recover(const RsaLanes &g, const uint8_t *sig, const uint8_t *mod, uint32_t e, Tail &&tail) {
     constexpr int K = RSA_GROUP * NL;
     constexpr uint32_t k = 4 * K;
     uint32_t n[NL], s[NL], x[NL];
@@ -245,27 +247,37 @@ SBV_DEV bool rsa_verify_item(const RsaLanes &g, const uint8_t *sig, const uint8_
 #pragma unroll
     for (int j = 0; j < NL; j++) x[j] = (g.l == 0 && j == 0) ? 1u : 0u;
     rsa_mont(g, acc, acc, x, n, ninv);  // EM = S^e mod N
-    // EM = 00 || 01 || FF..FF || 00 || DigestInfo || H, by bytes counted from the end (r = 0 is the last byte)
-    const uint32_t hl = 32 + 16 * hash, tl = hl + 19;
-    uint32_t bad = 0;
+    return tail(acc);
+}
+
+// The PKCS #1 v1.5 verdict of one item (the same in every lane of the group).  sig, mod: k bytes big-endian; e: the public
+// exponent; h: the hLen-byte digest, hash 0 / 1 / 2 = SHA-256 / SHA-384 / SHA-512.
+template <int NL>
+SBV_DEV bool rsa_verify_item(const RsaLanes &g, const uint8_t *sig, const uint8_t *mod, uint32_t e, const uint8_t *h, uint32_t hash) {
+    return rsa_recover<NL>(g, sig, mod, e, [&](const uint32_t (&acc)[NL]) {
+        constexpr uint32_t k = 64 * NL;
+        // EM = 00 || 01 || FF..FF || 00 || DigestInfo || H, by bytes counted from the end (r = 0 is the last byte)
+        const uint32_t hl = 32 + 16 * hash, tl = hl + 19;
+        uint32_t bad = 0;
 #pragma unroll
-    for (int j = 0; j < NL; j++) {
-        uint32_t w = 0;
+        for (int j = 0; j < NL; j++) {
+            uint32_t w = 0;
 #pragma unroll
-        for (int q = 0; q < 4; q++) {
-            const uint32_t r = 4 * (g.l * NL + j) + q;
-            uint32_t v;
-            if (r < hl) v = h[hl - 1 - r];
-            else if (r < tl) v = RSA_DIGEST_INFO[hash][tl - 1 - r];
-            else if (r == tl) v = 0x00;
-            else if (r < k - 2) v = 0xff;
-            else if (r == k - 2) v = 0x01;
-            else v = 0x00;
-            w |= v << (8 * q);
+            for (int q = 0; q < 4; q++) {
+                const uint32_t r = 4 * (g.l * NL + j) + q;
+                uint32_t v;
+                if (r < hl) v = h[hl - 1 - r];
+                else if (r < tl) v = RSA_DIGEST_INFO[hash][tl - 1 - r];
+                else if (r == tl) v = 0x00;
+                else if (r < k - 2) v = 0xff;
+                else if (r == k - 2) v = 0x01;
+                else v = 0x00;
+                w |= v << (8 * q);
+            }
+            bad |= w ^ acc[j];
         }
-        bad |= w ^ acc[j];
-    }
-    return rsa_bits(g, bad != 0) == 0;
+        return rsa_bits(g, bad != 0) == 0;
+    });
 }
 
 // One item per group of 16 lanes: ok[i] = 1 iff sig i (k bytes) is a valid PKCS #1 v1.5 signature of digest i (hLen

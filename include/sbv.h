@@ -136,8 +136,8 @@ enum { SBV_HASH_SHA256 = 0, SBV_HASH_SHA384 = 1, SBV_HASH_SHA512 = 2 };
  *  4. Compare: accept iff EM = 00 || 01 || FF..FF || 00 || DigestInfo(hash) || H byte for byte, the FF run k - tLen - 3
  *     bytes long, tLen = |DigestInfo| + hLen, with the DigestInfo prefixes of RFC 8017 §9.2 note 1 WITH the NULL
  *     parameters (the form without them rejects, as in Go).
- * RSA-PSS is not offered.  The checks: SBV_ERR_ARG for a mod_bytes other than 256 / 384 / 512, a hash tag above
- * SBV_HASH_SHA512, a null buffer (msgs may be NULL when every message is empty), n >= 2^31 and decreasing offsets, all
+ * RSA-PSS has calls of its own, below.  The checks: SBV_ERR_ARG for a mod_bytes other than 256 / 384 / 512, a hash
+ * tag above SBV_HASH_SHA512, a null buffer (msgs may be NULL when every message is empty), n >= 2^31 and decreasing offsets, all
  * before anything is written or launched.  Multi-device engines shard by item as sbv_hash_verify_batch does.  Each
  * device's shard is uploaded whole (no chunked upload).  Out of scope: registered RSA keys, RSA items in the mixed and
  * commit-vote calls, and _device / _ranked forms. */
@@ -150,6 +150,35 @@ int sbv_rsa_verify_batch(sbv_engine *e, uint32_t mod_bytes, uint8_t hash, size_t
 int sbv_rsa_hash_verify_batch(sbv_engine *e, uint32_t mod_bytes, uint8_t hash, size_t n, const uint8_t *msgs,
                               const uint64_t *msg_off, const uint8_t *sig, const uint8_t *modulus,
                               const uint32_t *pub_exp, uint8_t *digest_out, uint8_t *ok);
+
+/* ---- RSA-PSS (RSASSA-PSS, RFC 8017 §8.1.2 and EMSA-PSS §9.1.2), for crypto/x509 SHA256WithRSAPSS, SHA384WithRSAPSS,
+ * SHA512WithRSAPSS and the rsa_pss_rsae_* signatures of TLS 1.3.  salt_len as Go's PSSOptions.SaltLength: */
+enum { SBV_PSS_SALT_EQUALS_HASH = -1, SBV_PSS_SALT_AUTO = 0 };
+/* Accept set = Go crypto/rsa.VerifyPSS(pub, hash, H, S, &PSSOptions{SaltLength: salt_len}), MGF1 over the message hash.
+ * k, N, e, H (hLen bytes, taken as given) and S as for PKCS #1 v1.5 above; salt_len is -1 (the salt is hLen bytes), 0
+ * (auto-detect) or > 0 (exactly that many bytes):
+ *  1. Key, range and recovery: steps 1-3 of PKCS #1 v1.5 above (one key rule and one code path for both paddings).
+ *  2. emBits = bitlen(N) - 1, emLen = ceil(emBits / 8).  When bitlen(N) = 8k - 7 (N's leading byte is 01), emLen = k - 1:
+ *     reject unless EM's leading byte is 0, then drop it (Go's "strip leading zeroes").
+ *  3. sLen = hLen if salt_len = -1, else salt_len (0 for auto); reject if emLen < hLen + sLen + 2, compared in 64 bits
+ *     (salt_len = 2^31 - 1 rejects every item).
+ *  4. Reject unless EM's last byte is 0xBC.
+ *  5. maskedDB = the first dbLen = emLen - hLen - 1 bytes of EM, H_em the next hLen; reject if any of the top
+ *     8 emLen - emBits bits of maskedDB[0] is set.
+ *  6. DB = maskedDB XOR MGF1(H_em, dbLen), block c = Hash(H_em || BE32(c)); clear the top 8 emLen - emBits bits of DB[0].
+ *  7. Explicit sLen: reject unless the first dbLen - sLen - 1 bytes of DB are zero and the next is 01.  Auto: the first
+ *     nonzero byte of DB must be 01 (reject if there is none); the salt is everything after it.
+ *  8. Accept iff Hash(00 x 8 || H || salt) = H_em.
+ * The checks of the PKCS #1 v1.5 calls, plus SBV_ERR_ARG for salt_len < -1 (Go returns an error of its own there, not
+ * ErrVerification), all before anything is written or launched; any salt_len >= -1 is a valid argument.  Buffers,
+ * sharding and the out-of-scope forms as for PKCS #1 v1.5. */
+int sbv_rsa_pss_verify_batch(sbv_engine *e, uint32_t mod_bytes, uint8_t hash, int32_t salt_len, size_t n,
+                             const uint8_t *digest, const uint8_t *sig, const uint8_t *modulus,
+                             const uint32_t *pub_exp, uint8_t *ok);
+/* fused SHA-2 -> RSA-PSS: H = hash(M) never leaves the device; digest_out (n x hLen) may be NULL */
+int sbv_rsa_pss_hash_verify_batch(sbv_engine *e, uint32_t mod_bytes, uint8_t hash, int32_t salt_len, size_t n,
+                                  const uint8_t *msgs, const uint64_t *msg_off, const uint8_t *sig,
+                                  const uint8_t *modulus, const uint32_t *pub_exp, uint8_t *digest_out, uint8_t *ok);
 
 /* Mixed-curve batch: curve_tag[i] in {SBV_P256, SBV_P384}; every field is stored in a 48-byte
  * slot (P-256 values right-aligned, i.e. 16 leading zero bytes); digest is 32 bytes per item. */

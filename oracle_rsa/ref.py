@@ -1,11 +1,14 @@
-"""Go's crypto/rsa.VerifyPKCS1v15 restated in Python integers (the accept set of include/sbv.h), a seeded RSA key
-generator and a CRT signer.  TEST INFRASTRUCTURE ONLY.
+"""Go's crypto/rsa.VerifyPKCS1v15 and crypto/rsa.VerifyPSS restated in Python integers (the accept sets of include/sbv.h),
+a seeded RSA key generator and a CRT signer.  TEST INFRASTRUCTURE ONLY.
 
 verify(k, hash, H, S, N, e):
   1. key: N odd, N's leading byte (of k) nonzero, 2 <= e <= 2^31 - 1;
   2. range: S < N;
   3. EM = S^e mod N as k bytes, big-endian;
   4. accept iff EM == 00 || 01 || FF * (k - tLen - 3) || 00 || DigestInfo(hash) || H.
+
+pss_verify(k, hash, H, S, N, e, salt_len): steps 1-3 as above, then the EMSA-PSS decoding of RFC 8017 §9.1.2 as Go's
+emsaPSSVerify writes it, MGF1 over the message hash; salt_len as Go's PSSOptions.SaltLength (-1: hLen, 0: auto).
 """
 from __future__ import annotations
 
@@ -50,6 +53,77 @@ def verify_batch(k, hash, digest, sig, mod, exp) -> np.ndarray:
     digest = np.asarray(digest, np.uint8).reshape(n, HLEN[hash])
     sig, mod = np.asarray(sig, np.uint8).reshape(n, k), np.asarray(mod, np.uint8).reshape(n, k)
     return np.array([verify(k, hash, digest[i].tobytes(), sig[i].tobytes(), mod[i].tobytes(), int(exp[i])) for i in range(n)], np.uint8)
+
+
+# ---- RSA-PSS ----------------------------------------------------------------------------------------------------------
+SALT_EQUALS_HASH, SALT_AUTO = -1, 0
+
+
+def mgf1(seed: bytes, length: int, hash: int) -> bytes:
+    """MGF1 (RFC 8017 §B.2.1): Hash(seed || BE32(c)) for c = 0, 1, ... cut to length bytes."""
+    out = b"".join(HASHLIB[hash](seed + c.to_bytes(4, "big")).digest() for c in range(-(-length // HLEN[hash])))
+    return out[:length]
+
+
+def pss_encode(em_bits: int, hash: int, digest: bytes, salt: bytes) -> bytes:
+    """EMSA-PSS-ENCODE (RFC 8017 §9.1.1) of a digest with the given salt: emLen = ceil(emBits / 8) bytes."""
+    hl, em_len = HLEN[hash], (em_bits + 7) // 8
+    assert em_len >= hl + len(salt) + 2
+    h = HASHLIB[hash](bytes(8) + bytes(digest) + bytes(salt)).digest()
+    db = bytes(em_len - len(salt) - hl - 2) + b"\x01" + bytes(salt)
+    masked = bytearray(x ^ y for x, y in zip(db, mgf1(h, len(db), hash)))
+    masked[0] &= 0xFF >> (8 * em_len - em_bits)
+    return bytes(masked) + h + b"\xbc"
+
+
+def pss_verify(k: int, hash: int, digest: bytes, sig: bytes, mod: bytes, e: int, salt_len: int) -> bool:
+    assert salt_len >= SALT_EQUALS_HASH, "salt_len < -1 is an argument error, not a verdict"
+    mod, sig = bytes(mod), bytes(sig)
+    assert len(mod) == k and len(sig) == k and len(digest) == HLEN[hash]
+    n = int.from_bytes(mod, "big")
+    if n % 2 == 0 or mod[0] == 0 or not 2 <= e <= E_MAX:
+        return False
+    s = int.from_bytes(sig, "big")
+    if s >= n:
+        return False
+    em = pow(s, e, n).to_bytes(k, "big")
+    em_bits = n.bit_length() - 1
+    em_len = (em_bits + 7) // 8
+    while len(em) > em_len:  # Go's "strip leading zeroes"
+        if em[0] != 0:
+            return False
+        em = em[1:]
+    hl = HLEN[hash]
+    s_len = hl if salt_len == SALT_EQUALS_HASH else salt_len
+    if em_len < hl + s_len + 2:
+        return False
+    if em[-1] != 0xBC:
+        return False
+    db_len = em_len - hl - 1
+    masked, h = em[:db_len], em[db_len:db_len + hl]
+    keep = 0xFF >> (8 * em_len - em_bits)
+    if masked[0] & ~keep & 0xFF:
+        return False
+    db = bytearray(x ^ y for x, y in zip(masked, mgf1(h, db_len, hash)))
+    db[0] &= keep
+    if salt_len == SALT_AUTO:  # Go: the first 01 byte is the separator
+        ps_len = db.find(b"\x01")
+        if ps_len < 0:
+            return False
+        s_len = db_len - ps_len - 1
+    ps_len = em_len - hl - s_len - 2
+    if any(db[:ps_len]) or db[ps_len] != 0x01:
+        return False
+    salt = bytes(db[db_len - s_len:])
+    return HASHLIB[hash](bytes(8) + bytes(digest) + salt).digest() == h
+
+
+def pss_verify_batch(k, hash, digest, sig, mod, exp, salt_len) -> np.ndarray:
+    n = len(exp)
+    digest = np.asarray(digest, np.uint8).reshape(n, HLEN[hash])
+    sig, mod = np.asarray(sig, np.uint8).reshape(n, k), np.asarray(mod, np.uint8).reshape(n, k)
+    return np.array([pss_verify(k, hash, digest[i].tobytes(), sig[i].tobytes(), mod[i].tobytes(), int(exp[i]), salt_len) for i in range(n)],
+                    np.uint8)
 
 
 # ---- keys and signatures ----------------------------------------------------------------------------------------------
@@ -125,3 +199,7 @@ class Key:
 
     def sign(self, k: int, hash: int, digest: bytes, e: int = 65537) -> bytes:
         return self.sign_em(encode(k, hash, digest), e, k)
+
+    def sign_pss(self, k: int, hash: int, digest: bytes, salt: bytes, e: int = 65537) -> bytes:
+        """An RSA-PSS signature (k bytes) of the digest with the given salt: emBits = bitlen(N) - 1."""
+        return self.sign_em(pss_encode(self.bits - 1, hash, digest, salt).rjust(k, b"\0"), e, k)

@@ -31,6 +31,7 @@ namespace sbv { uint32_t tab[1 << 18]; }
 #include "../../consensus_b200/csrc/mixed_hash.cuh"
 #include "../../consensus_b200/csrc/rsa.cuh"
 #include "../../consensus_b200/csrc/rsa_debug.cuh"
+#include "../../consensus_b200/csrc/rsa_pss.cuh"
 #include "../../consensus_b200/csrc/sha512_batch.cuh"
 
 using namespace sbv;
@@ -946,4 +947,31 @@ extern "C" int hs_rsa_op(int nl, int op, size_t n, const uint8_t *a, const uint8
     if (rc == 0 && op != RSA_DBG_RESOLVE)
         for (size_t i = 0; i < n; i++) ninv[i] = aux[i];
     return rc;
+}
+
+// sbv_launch_rsa_pss with the same arguments: k_rsa_em in lockstep, in blocks of 128 threads (EM written over sig), then
+// k_rsa_pss one thread at a time.  -1 (and nothing written) for a size or hash tag outside the set or salt_len < -1.
+extern "C" int hs_rsa_pss_verify(uint32_t mod_bytes, uint8_t hash, int32_t salt_len, size_t n, uint8_t *sig, const uint8_t *mod, const uint32_t *pub_exp,
+                                 const uint8_t *digest, uint8_t *ok) {
+    if ((mod_bytes != 256 && mod_bytes != 384 && mod_bytes != 512) || hash > 2 || salt_len < PSS_SALT_EQUALS_HASH) return -1;
+    const unsigned blocks = (unsigned)((n * RSA_GROUP + 127) / 128), tblocks = (unsigned)((n + 127) / 128);
+    if (mod_bytes == 256) run_grid_lockstep(blocks, 128, [&] { k_rsa_em<4>((uint32_t)n, sig, mod, pub_exp, ok); });
+    else if (mod_bytes == 384) run_grid_lockstep(blocks, 128, [&] { k_rsa_em<6>((uint32_t)n, sig, mod, pub_exp, ok); });
+    else run_grid_lockstep(blocks, 128, [&] { k_rsa_em<8>((uint32_t)n, sig, mod, pub_exp, ok); });
+    if (hash == 0) run_grid(tblocks, 128, [&] { k_rsa_pss<0>((uint32_t)n, mod_bytes, salt_len, sig, mod, digest, ok); });
+    else if (hash == 1) run_grid(tblocks, 128, [&] { k_rsa_pss<1>((uint32_t)n, mod_bytes, salt_len, sig, mod, digest, ok); });
+    else run_grid(tblocks, 128, [&] { k_rsa_pss<2>((uint32_t)n, mod_bytes, salt_len, sig, mod, digest, ok); });
+    return 0;
+}
+
+// k_rsa_pss alone, one thread at a time, over EMs given in sig (ok: the key and range verdicts k_rsa_em would write, ANDed
+// with the PSS verdicts): the decoding checked item by item without the exponentiation.
+extern "C" int hs_rsa_pss_decode(uint32_t mod_bytes, uint8_t hash, int32_t salt_len, size_t n, uint8_t *em, const uint8_t *mod, const uint8_t *digest,
+                                 uint8_t *ok) {
+    if ((mod_bytes != 256 && mod_bytes != 384 && mod_bytes != 512) || hash > 2 || salt_len < PSS_SALT_EQUALS_HASH) return -1;
+    const unsigned tblocks = (unsigned)((n + 127) / 128);
+    if (hash == 0) run_grid(tblocks, 128, [&] { k_rsa_pss<0>((uint32_t)n, mod_bytes, salt_len, em, mod, digest, ok); });
+    else if (hash == 1) run_grid(tblocks, 128, [&] { k_rsa_pss<1>((uint32_t)n, mod_bytes, salt_len, em, mod, digest, ok); });
+    else run_grid(tblocks, 128, [&] { k_rsa_pss<2>((uint32_t)n, mod_bytes, salt_len, em, mod, digest, ok); });
+    return 0;
 }

@@ -53,6 +53,7 @@ SEEDED = ["tests/test_hostsim_seeded_passes.py"]
 COMB_WARP = ["tests/test_hostsim_comb_warp.py"]  # the comb build a warp per key against the one-thread-per-chain reference  # the first entry of a pass loaded, not added (pt_seed)
 TABLE_SHAPES = ["tests/test_hostsim_table_shapes.py"]
 RSA = ["tests/test_hostsim_rsa.py"]  # rsa.cuh and k_sha512 (sha512_batch.cuh)
+RSA_PSS = ["tests/test_hostsim_rsa_pss.py"]  # k_rsa_em and k_rsa_pss (rsa_pss.cuh)
 MIXED384 = ["tests/test_hostsim_mixed384.py"]  # k_mix_alg and k_sha2_sel (mixed_hash.cuh)  # every entry of the per-key tables at the key counts where the builds turn over
 
 
@@ -383,6 +384,26 @@ CATALOGUE = [
       "const uint32_t r = 4 * (g.l * NL + j) + (hash == 1 && NL == 8 ? q ^ 1 : q);", RSA),
     # an exponent whose bit 0 is clear ends on a squaring: only the even exponents of the edge classes reach it
     M("rsa_exp_last_square_dropped", "rsa.cuh", "while (i >= 0) {", "while (i > 0 || (i == 0 && (mul || (e & 1)))) {", RSA),
+    # ---------------------------------------------------------------- rsa_pss.cuh: one entry per decision of k_rsa_pss
+    M("pss_trailer", "rsa_pss.cuh", "if (em[emLen - 1] != 0xbc) return false;", "(void)0;", RSA_PSS),
+    M("pss_top_bits_unchecked", "rsa_pss.cuh", "if (em[0] & ~keep) return false;", "(void)0;", RSA_PSS),
+    M("pss_lead_byte_unchecked", "rsa_pss.cuh", "if (lead && em[0] != 0) return false;", "(void)0;", RSA_PSS),
+    M("pss_lead_byte_kept", "rsa_pss.cuh", "em += lead;", "(void)0;", RSA_PSS),
+    M("pss_mgf1_counter_plus1", "rsa_pss.cuh", "j == HW ? c : j == HW + 1", "j == HW ? c + 1 : j == HW + 1", RSA_PSS),
+    M("pss_mgf1_counter_le", "rsa_pss.cuh", "j == HW ? c : j == HW + 1", "j == HW ? __byte_perm(c, 0, 0x0123) : j == HW + 1", RSA_PSS),
+    M("pss_ps_nonzero_skipped", "rsa_pss.cuh", "while (ps < dbLen && db[ps] == 0) ps++;", "while (ps < dbLen && db[ps] != 1) ps++;", RSA_PSS),
+    M("pss_separator_any_nonzero", "rsa_pss.cuh", "if (ps == dbLen || db[ps] != 0x01) return false;", "if (ps == dbLen) return false;", RSA_PSS),
+    M("pss_salt_equals_hash_as_auto", "rsa_pss.cuh", "if (salt_len != PSS_SALT_AUTO && (int64_t)slen != sl) return false;",
+      "if (salt_len > PSS_SALT_AUTO && (int64_t)slen != sl) return false;", RSA_PSS),
+    M("pss_salt_auto_as_empty", "rsa_pss.cuh", "if (salt_len != PSS_SALT_AUTO && (int64_t)slen != sl) return false;",
+      "if ((int64_t)slen != sl) return false;", RSA_PSS),
+    M("pss_salt_explicit_at_most", "rsa_pss.cuh", "if (salt_len != PSS_SALT_AUTO && (int64_t)slen != sl) return false;",
+      "if (salt_len != PSS_SALT_AUTO && (int64_t)slen > sl) return false;", RSA_PSS),
+    M("pss_mprime_zeros7", "rsa_pss.cuh", "B = 4 * BW, Z = 8;", "B = 4 * BW, Z = 7;", RSA_PSS),
+    M("pss_compare_first_word", "rsa_pss.cuh", "for (uint32_t j = 0; j < HW; j++) diff |= s.word(j)", "for (uint32_t j = 0; j < 1; j++) diff |= s.word(j)",
+      RSA_PSS),
+    M("pss_compare_dropped", "rsa_pss.cuh", "return diff == 0;", "return true;", RSA_PSS),
+    M("pss_em_key_verdict", "rsa_pss.cuh", "if (i >= n || !ok[i]) return;", "if (i >= n) return;", RSA_PSS),
     # ---------------------------------------------------------------- sha512_batch.cuh
     M("sha512_batch_length_bytes", "sha512_batch.cuh", "w[15] = len << 3;", "w[15] = len;", RSA),
     M("sha512_batch_iv", "sha512_batch.cuh", "0x5be0cd19137e2179ull", "0x47b5481dbefa4fa4ull", RSA),

@@ -1,8 +1,10 @@
-"""RSA PKCS #1 v1.5 verification through the C ABI (sbv_rsa_hash_verify_batch), per modulus size, against OpenSSL on every
-core.
+"""RSA verification through the C ABI (sbv_rsa_hash_verify_batch, or sbv_rsa_pss_hash_verify_batch with --padding pss),
+per modulus size, against OpenSSL on every core.
 
     python tools/rsa_bench.py [--steps 20] [--warmup 3] [--sizes 256 384 512]
-    python tools/rsa_bench.py --profile      # k_rsa_verify / k_sha256 kernel times (torch.profiler), nothing timed
+    python tools/rsa_bench.py --padding pss [--salt-len -1]   # RSA-PSS, MGF1-SHA-256; salt_len as sbv.h (-1: 32 bytes)
+    python tools/rsa_bench.py --padding both  # PKCS #1 v1.5 and PSS over the same keys and messages, calls alternated
+    python tools/rsa_bench.py --profile      # k_rsa_verify / k_rsa_em / k_rsa_pss / k_sha256 kernel times (torch.profiler)
 
 Workload per size: 65,536 items over 1,024 key rows, 256-byte messages, SHA-256, e = 65537.  The keys come from OpenSSL
 (--distinct-keys of them per size, default 16, each filling 1,024 / 16 of the key rows), the signatures from OpenSSL too:
@@ -12,7 +14,9 @@ live in pinned host memory (sbv_host_alloc); every timed call's verdicts are che
 best call time and verifies/s, the wide MADs per verify from the algorithm and their share of sbv_probe_mad_rate, and
 OpenSSL verifies/s on all usable cores (each worker parses a key once and reuses it, as a Verifier keeps its clients'
 parsed certificates; with 16 distinct keys that reuse is kinder to the CPU's caches than 1,024 would be).  The card's
-name and power limit are read in the same run.  Prints one JSON line.
+name and power limit are read in the same run.  Prints one JSON line.  With --padding pss the keys are signed with
+RSA-PSS (salt of --salt-len bytes, hLen for -1 and auto) and the keys are reported with a _pss suffix; with both, each size
+reports both, the two calls alternating step by step, and the ratio pss / pkcs1 of their median times.
 """
 from __future__ import annotations
 
@@ -51,19 +55,26 @@ def _keys(bits, count):
     return [rsa.generate_private_key(public_exponent=65537, key_size=bits) for _ in range(count)]
 
 
+def _padding(pad, salt_len):
+    from cryptography.hazmat.primitives import hashes
+    from cryptography.hazmat.primitives.asymmetric import padding
+    if pad == "pkcs1":
+        return padding.PKCS1v15()
+    return padding.PSS(mgf=padding.MGF1(hashes.SHA256()), salt_length=salt_len if salt_len > 0 else padding.PSS.DIGEST_LENGTH)
+
+
 def _sign(args):
     from cryptography.hazmat.primitives import hashes, serialization
-    from cryptography.hazmat.primitives.asymmetric import padding
-    pem, msgs = args
+    pem, msgs, pad, salt_len = args
     key = serialization.load_pem_private_key(pem, password=None)
-    return [key.sign(m, padding.PKCS1v15(), hashes.SHA256()) for m in msgs]
+    return [key.sign(m, _padding(pad, salt_len), hashes.SHA256()) for m in msgs]
 
 
 def _cpu_verify(args):
     from cryptography.exceptions import InvalidSignature
     from cryptography.hazmat.primitives import hashes
-    from cryptography.hazmat.primitives.asymmetric import padding, rsa
-    items = args
+    from cryptography.hazmat.primitives.asymmetric import rsa
+    items, pad, salt_len = args
     cache, good = {}, 0
     t0 = time.perf_counter()
     for n, m, s in items:
@@ -71,14 +82,15 @@ def _cpu_verify(args):
         if pub is None:
             pub = cache[n] = rsa.RSAPublicNumbers(65537, n).public_key()
         try:
-            pub.verify(s, m, padding.PKCS1v15(), hashes.SHA256())
+            pub.verify(s, m, _padding(pad, salt_len), hashes.SHA256())
             good += 1
         except InvalidSignature:
             pass
     return good, time.perf_counter() - t0
 
 
-def corpus(k, items, key_rows, distinct, msg_len, seed, pool):
+def corpus(k, items, key_rows, distinct, msg_len, seed, pool, pads=("pkcs1",), salt_len=-1):
+    """The items of one size, signed under each padding of pads (sig_<pad>, cpu_<pad>) over the same keys and messages."""
     from cryptography.hazmat.primitives import serialization
     rng = np.random.default_rng(seed)
     keys = _keys(8 * k, distinct)
@@ -88,11 +100,13 @@ def corpus(k, items, key_rows, distinct, msg_len, seed, pool):
     row = np.arange(uniq) % key_rows  # key row of each distinct message
     owner = row % distinct
     pems = [kk.private_bytes(serialization.Encoding.PEM, serialization.PrivateFormat.PKCS8, serialization.NoEncryption()) for kk in keys]
-    sigs = [None] * uniq
-    jobs = [(pems[d], [msgs[i] for i in range(uniq) if owner[i] == d]) for d in range(distinct)]
-    for d, out in enumerate(pool.map(_sign, jobs)):
-        for i, s in zip([i for i in range(uniq) if owner[i] == d], out):
-            sigs[i] = s
+    sigs = {}
+    for pad in pads:
+        sigs[pad] = [None] * uniq
+        jobs = [(pems[d], [msgs[i] for i in range(uniq) if owner[i] == d], pad, salt_len) for d in range(distinct)]
+        for d, out in enumerate(pool.map(_sign, jobs)):
+            for i, s in zip([i for i in range(uniq) if owner[i] == d], out):
+                sigs[pad][i] = s
     idx = np.arange(items) % uniq
     m = [bytearray(msgs[i]) for i in idx]
     want = np.ones(items, np.uint8)
@@ -100,9 +114,12 @@ def corpus(k, items, key_rows, distinct, msg_len, seed, pool):
         m[j][j % msg_len] ^= 1
         want[j] = 0
     off = np.arange(items + 1, dtype=np.uint64) * msg_len
-    return dict(msgs=np.frombuffer(b"".join(m), np.uint8), off=off, sig=np.frombuffer(b"".join(sigs[i] for i in idx), np.uint8),
-                mod=np.frombuffer(b"".join(nints[owner[i]].to_bytes(k, "big") for i in idx), np.uint8),
-                exp=np.full(items, 65537, np.uint32), want=want, cpu=[(nints[owner[i]], bytes(m[j]), sigs[i]) for j, i in enumerate(idx)])
+    out = dict(msgs=np.frombuffer(b"".join(m), np.uint8), off=off, mod=np.frombuffer(b"".join(nints[owner[i]].to_bytes(k, "big") for i in idx), np.uint8),
+               exp=np.full(items, 65537, np.uint32), want=want)
+    for pad in pads:
+        out[f"sig_{pad}"] = np.frombuffer(b"".join(sigs[pad][i] for i in idx), np.uint8)
+        out[f"cpu_{pad}"] = [(nints[owner[i]], bytes(m[j]), sigs[pad][i]) for j, i in enumerate(idx)]
+    return out
 
 
 def main():
@@ -116,7 +133,10 @@ def main():
     ap.add_argument("--sizes", type=int, nargs="+", default=[256, 384, 512])
     ap.add_argument("--cpu-items", type=int, default=16384, help="items of the OpenSSL arm (0: skip it)")
     ap.add_argument("--profile", action="store_true", help="kernel times from torch.profiler instead of timing the calls")
+    ap.add_argument("--padding", choices=("pkcs1", "pss", "both"), default="pkcs1")
+    ap.add_argument("--salt-len", type=int, default=-1, help="salt_len of the PSS calls (-1: equals hash, 0: auto, > 0: exact)")
     args = ap.parse_args()
+    pads = ("pkcs1", "pss") if args.padding == "both" else (args.padding,)
 
     import torch
 
@@ -128,16 +148,18 @@ def main():
     vp = C.c_void_p
     ncpu = len(os.sched_getaffinity(0))
     res = {"metric": "rsa_verifies_per_s", "unit": "verifies/s", "items": args.items, "key_rows": args.keys, "distinct_keys": args.distinct_keys,
-           "msg_bytes": args.msg_len, "hash": "SHA-256", "e": 65537, "cpu_cores": ncpu}
+           "msg_bytes": args.msg_len, "hash": "SHA-256", "e": 65537, "cpu_cores": ncpu, "padding": args.padding}
+    if args.padding != "pkcs1":
+        res["salt_len"] = args.salt_len
     all_good = True
     eng = sbv.Engine(n_devices=1)
     res["mad_rate_per_s"] = eng.probe_mad_rate()
     try:
         with ProcessPoolExecutor(ncpu) as pool:
             for k in args.sizes:
-                c = corpus(k, args.items, args.keys, args.distinct_keys, args.msg_len, seed=k, pool=pool)
+                c = corpus(k, args.items, args.keys, args.distinct_keys, args.msg_len, seed=k, pool=pool, pads=pads, salt_len=args.salt_len)
                 n = args.items
-                arrays = [c["msgs"], c["off"], c["sig"], c["mod"], c["exp"], np.zeros(n, np.uint8)]
+                arrays = [c["msgs"], c["off"], c["mod"], c["exp"], np.zeros(n, np.uint8)] + [c[f"sig_{p}"] for p in pads]
                 bufs = []
                 try:
                     views = []
@@ -148,10 +170,14 @@ def main():
                         v = np.ctypeslib.as_array((C.c_uint8 * a.nbytes).from_address(p))
                         v[:] = a.view(np.uint8).reshape(-1)
                         views.append(v)
-                    ok = views[5]
+                    ok = views[4]
+                    sigbuf = dict(zip(pads, bufs[5:]))
 
-                    def call():
-                        eng.rsa_hash_verify_batch_ptr(k, sbv.SHA256, n, *bufs[:5], 0, bufs[5])
+                    def call(pad):
+                        if pad == "pss":
+                            eng.rsa_pss_hash_verify_batch_ptr(k, sbv.SHA256, args.salt_len, n, bufs[0], bufs[1], sigbuf[pad], bufs[2], bufs[3], 0, bufs[4])
+                        else:
+                            eng.rsa_hash_verify_batch_ptr(k, sbv.SHA256, n, bufs[0], bufs[1], sigbuf[pad], bufs[2], bufs[3], 0, bufs[4])
 
                     def check():
                         good = bool(np.array_equal(ok, c["want"]))
@@ -163,16 +189,18 @@ def main():
                     res[f"{tag}_wide_mads_per_verify"] = mads_per_verify(k)
                     if args.profile:
                         from torch.profiler import ProfilerActivity, profile
-                        call()
-                        all_good &= check()
+                        for pad in pads:
+                            call(pad)
+                            all_good &= check()
                         torch.cuda.synchronize()
                         with profile(activities=[ProfilerActivity.CUDA]) as prof:
                             for _ in range(5):
-                                call()
-                                all_good &= check()
+                                for pad in pads:
+                                    call(pad)
+                                    all_good &= check()
                             torch.cuda.synchronize()
                         for ev in prof.key_averages():
-                            for name in ("k_rsa_verify", "k_sha256"):
+                            for name in ("k_rsa_verify", "k_rsa_em", "k_rsa_pss", "k_sha256"):
                                 if re.search(r"\b" + name + r"\b", ev.key):
                                     t = getattr(ev, "device_time", None) or getattr(ev, "cuda_time", 0.0)  # average µs per launch
                                     res[f"{tag}_{name}_us"] = round(float(t), 1)
@@ -183,35 +211,42 @@ def main():
                             res[f"{tag}_kernel_mad_share"] = round(n * mads_per_verify(k) / kt / res["mad_rate_per_s"], 3)
                     else:
                         for _ in range(args.warmup):
-                            call()
-                            all_good &= check()
-                        times = []
+                            for pad in pads:
+                                call(pad)
+                                all_good &= check()
+                        times = {pad: [] for pad in pads}
                         for _ in range(args.steps):
-                            t0 = time.perf_counter()
-                            call()
-                            times.append(time.perf_counter() - t0)
-                            all_good &= check()
-                        med = float(np.median(times))
-                        res[f"{tag}_median_ms"] = round(med * 1e3, 3)
-                        res[f"{tag}_best_ms"] = round(min(times) * 1e3, 3)
-                        res[f"{tag}_verifies_per_s"] = round(n / med)
-                        res[f"{tag}_call_mad_share"] = round(n * mads_per_verify(k) / med / res["mad_rate_per_s"], 3)
-                        if args.cpu_items:
-                            items = c["cpu"][:args.cpu_items]
-                            parts = [items[i::ncpu] for i in range(ncpu)]
-                            t0 = time.perf_counter()
-                            out = list(pool.map(_cpu_verify, parts))
-                            wall = time.perf_counter() - t0
-                            good = sum(o[0] for o in out)
-                            all_good &= good == int(c["want"][:len(items)].sum())
-                            res[f"{tag}_openssl_verifies_per_s"] = round(len(items) / wall)
+                            for pad in pads:  # alternated: both paddings see the same state of the card
+                                t0 = time.perf_counter()
+                                call(pad)
+                                times[pad].append(time.perf_counter() - t0)
+                                all_good &= check()
+                        for pad in pads:
+                            sfx = "" if pad == "pkcs1" else "_pss"
+                            med = float(np.median(times[pad]))
+                            res[f"{tag}{sfx}_median_ms"] = round(med * 1e3, 3)
+                            res[f"{tag}{sfx}_best_ms"] = round(min(times[pad]) * 1e3, 3)
+                            res[f"{tag}{sfx}_verifies_per_s"] = round(n / med)
+                            res[f"{tag}{sfx}_call_mad_share"] = round(n * mads_per_verify(k) / med / res["mad_rate_per_s"], 3)
+                            if args.cpu_items:
+                                items = c[f"cpu_{pad}"][:args.cpu_items]
+                                parts = [(items[i::ncpu], pad, args.salt_len) for i in range(ncpu)]
+                                t0 = time.perf_counter()
+                                out = list(pool.map(_cpu_verify, parts))
+                                wall = time.perf_counter() - t0
+                                good = sum(o[0] for o in out)
+                                all_good &= good == int(c["want"][:len(items)].sum())
+                                res[f"{tag}{sfx}_openssl_verifies_per_s"] = round(len(items) / wall)
+                        if len(pads) == 2:
+                            res[f"{tag}_pss_over_pkcs1_time"] = round(res[f"{tag}_pss_median_ms"] / res[f"{tag}_median_ms"], 4)
                 finally:
                     for p in bufs:
                         lib.sbv_host_free(C.c_void_p(p))
     finally:
         eng.close()
-    if not args.profile and f"k{args.sizes[0]}_verifies_per_s" in res:
-        res["value"] = res[f"k{args.sizes[0]}_verifies_per_s"]
+    first = f"k{args.sizes[0]}" + ("_pss" if args.padding == "pss" else "") + "_verifies_per_s"
+    if not args.profile and first in res:
+        res["value"] = res[first]
     res["outputs_match_expected"] = bool(all_good)
     res["device"] = torch.cuda.get_device_properties(0).name
     res["power_limit_w"] = power_limit_w()
