@@ -17,6 +17,7 @@
 #include <cstring>
 #include <mutex>
 #include <string>
+#include <type_traits>
 #include <vector>
 
 #include "engine.h"
@@ -36,6 +37,9 @@ int env_int(const char *name, int dflt) {
 }
 
 size_t fbytes(uint8_t curve) { return curve == SBV_P256 ? 32 : 48; }
+
+// a digest length the verify calls accept: whole 32-bit words, 4 to 64 bytes
+bool digest_len_ok(uint8_t dl) { return dl != 0 && (dl & 3) == 0 && dl <= 64; }
 
 bool is_pinned(const void *p) {
     cudaPointerAttributes a;
@@ -59,17 +63,55 @@ __global__ void k_mad_probe(uint32_t *out, uint32_t iters) {
     if (s == 0x1234567) out[0] = (uint32_t)s;
 }
 
+void buf_free(DevBuf &b) { if (b.p) cudaFree(b.p); b = DevBuf{}; }
+void buf_free(PinBuf &b) { if (b.p) cudaFreeHost(b.p); b = PinBuf{}; }
+// Replaces b's memory with `bytes` fresh bytes (its contents are not kept); on a fault b is left empty.
+template <class Buf>
+cudaError_t buf_regrow(Buf &b, size_t bytes) {
+    buf_free(b);
+    const cudaError_t err = std::is_base_of<PinBuf, Buf>::value ? cudaHostAlloc(&b.p, bytes, cudaHostAllocPortable) : cudaMalloc(&b.p, bytes);
+    if (err == cudaSuccess) b.bytes = bytes; else b.p = nullptr;
+    return err;
+}
+
+// Every buffer of lane ln, once: visit(buffer, need, alloc) with the bytes the call uses (need) and the bytes to allocate
+// when the buffer must grow (alloc: the buffer's headroom rule).
+template <class V>
+void each_lane_buffer(Dev::Lane &ln, const LaneNeeds &s, V &&visit) {
+    const size_t n = s.items, ni = n + n / 8 + 1024, o = s.offsets, oi = o + o / 8 + 1024;
+    visit(ln.d_r, n * 48, ni * 48);
+    visit(ln.d_s, n * 48, ni * 48);
+    visit(ln.d_qx, n * 48, ni * 48);
+    visit(ln.d_qy, n * 48, ni * 48);
+    visit(ln.d_dig, n * 64, ni * 64);
+    visit(ln.d_ok, n, ni);
+    visit(ln.d_slot, n * 4, ni * 4);
+    visit(ln.d_msgs, s.msg_bytes, s.msg_bytes + s.msg_bytes / 8 + 4096);
+    visit(ln.d_off, o * 8, oi * 8);
+    visit(ln.d_perm, o ? (o + 3 * 1024) * 4 : 0, (oi + 3 * 1024) * 4);
+    visit(ln.h_pin, s.pinned, s.pinned + s.pinned / 4 + 4096);
+    visit(ln.d_aux, s.aux, s.aux + s.aux / 4 + 4096);
+    visit(ln.h_aux, s.aux, s.aux + s.aux / 4 + 4096);
+    visit(ln.d_carve, s.carve, s.carve + s.carve / 8 + 4096);
+}
+
+// Frees every buffer, both streams and every event of lane ln; caller has set the device and drained it.
+void lane_free(Dev::Lane &ln) {
+    each_lane_buffer(ln, LaneNeeds{}, [](auto &b, size_t, size_t) { buf_free(b); });
+    if (ln.stream) cudaStreamDestroy(ln.stream);
+    if (ln.stream2) cudaStreamDestroy(ln.stream2);
+    if (ln.ev_a) cudaEventDestroy(ln.ev_a);
+    if (ln.ev_b) cudaEventDestroy(ln.ev_b);
+    for (cudaEvent_t ev : ln.ev_chunk) if (ev) cudaEventDestroy(ev);
+    ln = Dev::Lane{};
+}
+
 }  // namespace
 
 int sbv_ensure_scratch(sbv_engine *e, Dev &d, size_t bytes) {
-    if (bytes <= d.scratch_cap) return 0;
+    if (bytes <= d.d_scratch.bytes) return 0;
     CU(e, cudaSetDevice(d.ordinal));
-    if (d.d_scratch) cudaFree(d.d_scratch);
-    d.d_scratch = nullptr;
-    d.scratch_cap = 0;
-    size_t cap = bytes + bytes / 4 + 4096;
-    CU(e, cudaMalloc(&d.d_scratch, cap));
-    d.scratch_cap = cap;
+    CU(e, buf_regrow(d.d_scratch, bytes + bytes / 4 + 4096));
     return 0;
 }
 
@@ -88,74 +130,19 @@ void sbv_lane_release(sbv_engine *e, int lane) {
     { std::lock_guard<std::mutex> lk(e->mu); e->lane_busy[lane] = false; }
     e->lane_cv.notify_one();
 }
-// caller has set the device.  Only the owner of the lane touches it, so no lock is needed here.
-int sbv_lane_ensure(sbv_engine *e, Dev &d, Dev::Lane &ln, size_t n, size_t pinned_bytes) {
+// Only the owner of the lane touches it, so no lock is needed here.
+int sbv_lane_reserve(sbv_engine *e, Dev::Lane &ln, const LaneNeeds &needs) {
     if (!ln.stream) CU(e, cudaStreamCreateWithFlags(&ln.stream, cudaStreamNonBlocking));
-    if (n > ln.cap) {
-        CU(e, cudaStreamSynchronize(ln.stream));
-        uint8_t **ptrs[] = {&ln.d_r, &ln.d_s, &ln.d_qx, &ln.d_qy, &ln.d_dig, &ln.d_ok};
-        for (auto p : ptrs) { if (*p) cudaFree(*p); *p = nullptr; }
-        if (ln.d_slot) cudaFree(ln.d_slot);
-        ln.d_slot = nullptr;
-        ln.cap = 0;
-        const size_t cap = n + n / 8 + 1024;
-        CU(e, cudaMalloc(&ln.d_r, cap * 48));
-        CU(e, cudaMalloc(&ln.d_s, cap * 48));
-        CU(e, cudaMalloc(&ln.d_qx, cap * 48));
-        CU(e, cudaMalloc(&ln.d_qy, cap * 48));
-        CU(e, cudaMalloc(&ln.d_dig, cap * 64));
-        CU(e, cudaMalloc(&ln.d_ok, cap));
-        CU(e, cudaMalloc(&ln.d_slot, cap * 4));
-        ln.cap = cap;
-    }
-    if (pinned_bytes > ln.h_pin_cap) {
-        CU(e, cudaStreamSynchronize(ln.stream));
-        if (ln.h_pin) cudaFreeHost(ln.h_pin);
-        ln.h_pin = nullptr;
-        ln.h_pin_cap = 0;
-        const size_t cap = pinned_bytes + pinned_bytes / 4 + 4096;
-        CU(e, cudaHostAlloc(&ln.h_pin, cap, cudaHostAllocPortable));
-        ln.h_pin_cap = cap;
-    }
-    (void)d;
-    return 0;
-}
-int sbv_lane_ensure_msgs(sbv_engine *e, Dev::Lane &ln, size_t bytes, size_t n_off) {
-    if (!ln.stream) CU(e, cudaStreamCreateWithFlags(&ln.stream, cudaStreamNonBlocking));
-    if (bytes > ln.msg_cap) {
-        CU(e, cudaStreamSynchronize(ln.stream));
-        if (ln.d_msgs) cudaFree(ln.d_msgs);
-        ln.d_msgs = nullptr;
-        ln.msg_cap = 0;
-        const size_t cap = bytes + bytes / 8 + 4096;
-        CU(e, cudaMalloc(&ln.d_msgs, cap));
-        ln.msg_cap = cap;
-    }
-    if (n_off > ln.off_cap) {
-        CU(e, cudaStreamSynchronize(ln.stream));
-        if (ln.d_off) cudaFree(ln.d_off);
-        if (ln.d_perm) cudaFree(ln.d_perm);
-        ln.d_off = nullptr;
-        ln.d_perm = nullptr;
-        ln.off_cap = 0;
-        const size_t cap = n_off + n_off / 8 + 1024;
-        CU(e, cudaMalloc(&ln.d_off, cap * sizeof(uint64_t)));
-        CU(e, cudaMalloc(&ln.d_perm, (cap + 3 * 1024) * sizeof(uint32_t)));
-        ln.off_cap = cap;
-    }
-    return 0;
-}
-int sbv_lane_ensure_aux(sbv_engine *e, Dev::Lane &ln, size_t bytes) {
-    if (!ln.stream) CU(e, cudaStreamCreateWithFlags(&ln.stream, cudaStreamNonBlocking));
-    if (bytes <= ln.aux_cap) return 0;
+    bool grows = false;
+    each_lane_buffer(ln, needs, [&](DevBuf &b, size_t need, size_t) { grows = grows || need > b.bytes; });
+    if (!grows) return 0;
     CU(e, cudaStreamSynchronize(ln.stream));
-    if (ln.d_aux) cudaFree(ln.d_aux);
-    if (ln.h_aux) cudaFreeHost(ln.h_aux);
-    ln.d_aux = nullptr; ln.h_aux = nullptr; ln.aux_cap = 0;
-    const size_t cap = bytes + bytes / 4 + 4096;
-    CU(e, cudaMalloc(&ln.d_aux, cap));
-    CU(e, cudaHostAlloc(&ln.h_aux, cap, cudaHostAllocPortable));
-    ln.aux_cap = cap;
+    if (ln.stream2) CU(e, cudaStreamSynchronize(ln.stream2));
+    cudaError_t err = cudaSuccess;
+    each_lane_buffer(ln, needs, [&](auto &b, size_t need, size_t alloc) {
+        if (err == cudaSuccess && need > b.bytes) err = buf_regrow(b, alloc);
+    });
+    CU(e, err);
     return 0;
 }
 int sbv_lane_stream2(sbv_engine *e, Dev::Lane &ln) {
@@ -163,29 +150,6 @@ int sbv_lane_stream2(sbv_engine *e, Dev::Lane &ln) {
     CU(e, cudaStreamCreateWithFlags(&ln.stream2, cudaStreamNonBlocking));
     CU(e, cudaEventCreateWithFlags(&ln.ev_a, cudaEventDisableTiming));
     CU(e, cudaEventCreateWithFlags(&ln.ev_b, cudaEventDisableTiming));
-    return 0;
-}
-int sbv_lane_ensure_mix(sbv_engine *e, Dev::Lane &ln, size_t bytes) {
-    if (bytes <= ln.mix_cap) return 0;
-    CU(e, cudaStreamSynchronize(ln.stream));
-    if (ln.stream2) CU(e, cudaStreamSynchronize(ln.stream2));
-    if (ln.d_mix) cudaFree(ln.d_mix);
-    ln.d_mix = nullptr;
-    ln.mix_cap = 0;
-    const size_t cap = bytes + bytes / 8 + 4096;
-    CU(e, cudaMalloc(&ln.d_mix, cap));
-    ln.mix_cap = cap;
-    return 0;
-}
-int sbv_lane_ensure_rsa(sbv_engine *e, Dev::Lane &ln, size_t bytes) {
-    if (bytes <= ln.rsa_cap) return 0;
-    CU(e, cudaStreamSynchronize(ln.stream));
-    if (ln.d_rsa) cudaFree(ln.d_rsa);
-    ln.d_rsa = nullptr;
-    ln.rsa_cap = 0;
-    const size_t cap = bytes + bytes / 8 + 4096;
-    CU(e, cudaMalloc(&ln.d_rsa, cap));
-    ln.rsa_cap = cap;
     return 0;
 }
 int sbv_launch_length_sort(sbv_engine *e, size_t n, const uint64_t *d_off, uint32_t *d_perm, cudaStream_t st, const uint32_t **perm) {
@@ -245,7 +209,7 @@ int sbv_lane_h2d(sbv_engine *e, Dev::Lane &ln, void *dst, const void *src, size_
     if (is_pinned(src)) {
         CU(e, cudaMemcpyAsync(dst, src, bytes, cudaMemcpyHostToDevice, st));
     } else {
-        if (stage_off + bytes > ln.h_pin_cap) return fail(e, SBV_ERR_NOMEM, "pinned staging area too small (%zu + %zu > %zu)", stage_off, bytes, ln.h_pin_cap);
+        if (stage_off + bytes > ln.h_pin.bytes) return fail(e, SBV_ERR_NOMEM, "pinned staging area too small (%zu + %zu > %zu)", stage_off, bytes, ln.h_pin.bytes);
         memcpy(ln.h_pin + stage_off, src, bytes);
         CU(e, cudaMemcpyAsync(dst, ln.h_pin + stage_off, bytes, cudaMemcpyHostToDevice, st));
         stage_off += (bytes + 255) & ~(size_t)255;
@@ -387,13 +351,13 @@ struct BatchSrc {
 // the rest of the batch is still being copied.  A LARGE shard (>= chunk_items) then arrives in chunks on the lane's
 // second stream while the lane's first stream hashes and verifies the chunks that are already there: the call costs
 // max(upload, arithmetic) instead of their sum (C3: 1,048,576 requests of 256 B are 411 MB of upload).
-// extra_pinned / so_out: the caller stages more arrays behind ours (the quorum columns) in the lane's pinned area.
-int stage_and_verify(sbv_engine *e, Dev &d, int lane, uint8_t curve, size_t lo, size_t cnt, const BatchSrc &b, size_t extra_pinned = 0,
+// more / so_out: the caller's own needs of the lane (the pinned bytes and aux area of the quorum columns, or a gather
+// buffer), reserved with ours; the caller stages its arrays behind ours in the lane's pinned area.
+int stage_and_verify(sbv_engine *e, Dev &d, Dev::Lane &ln, uint8_t curve, size_t lo, size_t cnt, const BatchSrc &b, const LaneNeeds &more = {},
                      size_t *so_out = nullptr) {
     const size_t L = fbytes(curve);
     const bool hashing = b.digest == nullptr;
     const uint32_t dlen = hashing ? hash_bytes(b.hash) : b.digest_len;
-    Dev::Lane &ln = d.lanes[lane];
     CU(e, cudaSetDevice(d.ordinal));
     const uint64_t base = hashing ? b.msg_off[lo] : 0, bytes = hashing ? b.msg_off[lo + cnt] - base : 0;
     int chunks = 1;
@@ -401,9 +365,12 @@ int stage_and_verify(sbv_engine *e, Dev &d, int lane, uint8_t curve, size_t lo, 
         chunks = (int)std::min<size_t>(std::max<size_t>(cnt / (size_t)e->chunk_items, 2), SBV_MAX_CHUNKS);
     }
     const size_t per = (((cnt + chunks - 1) / chunks) + 255) & ~(size_t)255;   // items per chunk
-    int rc = sbv_lane_ensure(e, d, ln, cnt ? cnt : 1, cnt * (4 * L + dlen + 1) + bytes + (cnt + 1) * 8 + (size_t)(4 * chunks + 8) * 256 + extra_pinned);
+    LaneNeeds need = more;
+    need.items = cnt;
+    need.pinned += cnt * (4 * L + dlen + 1) + bytes + (cnt + 1) * 8 + (size_t)(4 * chunks + 8) * 256;
+    if (hashing) need.msgs(bytes, cnt);
+    int rc = sbv_lane_reserve(e, ln, need);
     if (rc) return rc;
-    if (hashing && (rc = sbv_lane_ensure_msgs(e, ln, bytes + 16, cnt + 1))) return rc;
     cudaStream_t up = ln.stream;   // the stream the rest of the batch is uploaded on
     if (chunks > 1) {
         if (int rc2 = sbv_lane_stream2(e, ln)) return rc2;
@@ -517,22 +484,14 @@ void sbv_destroy(sbv_engine *e) {
     }
     for (Dev &d : e->devs) {
         cudaSetDevice(d.ordinal);
-        void *ptrs[] = {d.gtab[0], d.gtab[1], d.ed_btab, d.d_scratch};
+        void *ptrs[] = {d.gtab[0], d.gtab[1], d.ed_btab};
         for (void *p : ptrs) if (p) cudaFree(p);
+        buf_free(d.d_scratch);
         sbv_scratch_free(d);
         sbv_keys_free(d);
         sbv_ed_keys_free(d);
         sbv_key_cache_free(d);
-        for (auto &ln : d.lanes) {
-            void *lp[] = {ln.d_r, ln.d_s, ln.d_qx, ln.d_qy, ln.d_dig, ln.d_ok, ln.d_slot, ln.d_msgs, ln.d_off, ln.d_perm, ln.d_aux, ln.d_mix, ln.d_rsa};
-            for (void *p : lp) if (p) cudaFree(p);
-            if (ln.h_pin) cudaFreeHost(ln.h_pin);
-            if (ln.h_aux) cudaFreeHost(ln.h_aux);
-            if (ln.stream) cudaStreamDestroy(ln.stream);
-            if (ln.stream2) cudaStreamDestroy(ln.stream2);
-            if (ln.ev_a) cudaEventDestroy(ln.ev_a);
-            if (ln.ev_b) cudaEventDestroy(ln.ev_b);
-        }
+        for (auto &ln : d.lanes) lane_free(ln);
         for (cudaEvent_t ev : d.prof_events) cudaEventDestroy(ev);
         if (d.stream) cudaStreamDestroy(d.stream);
     }
@@ -575,8 +534,7 @@ int sbv_verify_batch_device(sbv_engine *e, int device_index, uint8_t curve, size
 
 int sbv_verify_batch(sbv_engine *e, uint8_t curve, size_t n, const uint8_t *r, const uint8_t *s, const uint8_t *qx,
                      const uint8_t *qy, const uint8_t *digest, uint8_t digest_len, uint8_t *ok) {
-    if (!e || curve > SBV_P384 || digest_len == 0 || (digest_len & 3) || digest_len > 64)
-        return fail(e, SBV_ERR_ARG, "sbv_verify_batch: bad argument");
+    if (!e || curve > SBV_P384 || !digest_len_ok(digest_len)) return fail(e, SBV_ERR_ARG, "sbv_verify_batch: bad argument");
     if (n == 0) return SBV_OK;
     if (!r || !s || !qx || !qy || !digest || !ok) return fail(e, SBV_ERR_ARG, "null buffer");
     if (n > 0x7fffffffu) return fail(e, SBV_ERR_ARG, "n too large");
@@ -591,13 +549,13 @@ int sbv_verify_batch(sbv_engine *e, uint8_t curve, size_t n, const uint8_t *r, c
         Dev &d = e->devs[g];
         Dev::Lane &ln = d.lanes[lane];
         const Range v = sh.vr[g];
-        int rc = 0;
-        if (v.n && (rc = stage_and_verify(e, d, lane, curve, v.lo, v.n, BatchSrc{r, s, qx, qy, digest, digest_len, nullptr, nullptr}))) return rc;
-        if (G > 1) {  // the aux area holds the gather buffer
-            CU(e, cudaSetDevice(d.ordinal));
-            if ((rc = sbv_lane_ensure_aux(e, ln, sh.wp() * G * 4))) return rc;
-            gbuf[g] = (uint32_t *)ln.d_aux;
-        }
+        LaneNeeds gather;  // the aux area holds the gather buffer
+        gather.aux = G > 1 ? sh.wp() * G * 4 : 0;
+        CU(e, cudaSetDevice(d.ordinal));
+        int rc = v.n ? stage_and_verify(e, d, ln, curve, v.lo, v.n, BatchSrc{r, s, qx, qy, digest, digest_len, nullptr, nullptr}, gather)
+                     : sbv_lane_reserve(e, ln, gather);
+        if (rc) return rc;
+        gbuf[g] = (uint32_t *)ln.d_aux;
         if ((rc = shard_out(e, ln, sh, g, gbuf[g], ln.d_ok, nullptr, ok, nullptr))) return rc;
     }
     return gather_unpack(e, lane, sh, gbuf, ok, nullptr);
@@ -689,7 +647,7 @@ int sbv_gather_words_device(sbv_engine *e, int channel, uint32_t *d_all, size_t 
 // one channel are issued in the same order on every rank.
 int sbv_verify_batch_ranked(sbv_engine *e, int channel, uint8_t curve, size_t n, const uint8_t *r, const uint8_t *s, const uint8_t *qx,
                             const uint8_t *qy, const uint8_t *digest, uint8_t digest_len, uint8_t *ok, uint32_t *mask_all) {
-    if (!e || curve > SBV_P384 || digest_len == 0 || (digest_len & 3) || digest_len > 64 || e->devs.size() != 1)
+    if (!e || curve > SBV_P384 || !digest_len_ok(digest_len) || e->devs.size() != 1)
         return fail(e, SBV_ERR_ARG, "sbv_verify_batch_ranked: bad argument");
     if (n == 0 || n > 0x7fffffffu) return fail(e, SBV_ERR_ARG, "n must be in [1, 2^31)");
     if (!r || !s || !qx || !qy || !digest || !ok || !mask_all) return fail(e, SBV_ERR_ARG, "null buffer");
@@ -697,10 +655,11 @@ int sbv_verify_batch_ranked(sbv_engine *e, int channel, uint8_t curve, size_t n,
     const int lane = guard.lane;
     Dev &d = e->devs[0];
     Dev::Lane &ln = d.lanes[lane];
-    int rc = stage_and_verify(e, d, lane, curve, 0, n, BatchSrc{r, s, qx, qy, digest, digest_len, nullptr, nullptr});
-    if (rc) return rc;
     const size_t wp = (n + 31) / 32;
-    if ((rc = sbv_lane_ensure_aux(e, ln, wp * (size_t)e->nranks * 4))) return rc;
+    LaneNeeds masks;  // the aux area holds the masks of all ranks
+    masks.aux = wp * (size_t)e->nranks * 4;
+    int rc = stage_and_verify(e, d, ln, curve, 0, n, BatchSrc{r, s, qx, qy, digest, digest_len, nullptr, nullptr}, masks);
+    if (rc) return rc;
     CU(e, cudaMemcpyAsync(ok, ln.d_ok, n, cudaMemcpyDeviceToHost, ln.stream));
     if ((rc = sbv_gather_verdicts_device(e, channel, ln.d_ok, n, (uint32_t *)ln.d_aux, ln.stream))) return rc;
     CU(e, cudaMemcpyAsync(mask_all, ln.d_aux, wp * (size_t)e->nranks * 4, cudaMemcpyDeviceToHost, ln.stream));

@@ -19,15 +19,23 @@ constexpr int SBV_LANES = 6;    // concurrent host-buffer calls per engine
 constexpr int SBV_SCRATCH = 8;  // scratch sets per device (> SBV_LANES + 1: a launch may be held open per lane)
 constexpr int SBV_MAX_CHUNKS = 32;  // a large host-buffer batch is uploaded and verified in at most this many chunks
 
-// A device buffer with the bytes allocated for it; reads as a T *.
+// A device buffer with the bytes allocated for it; DevArray<T> reads as a T * (and casts to other pointer types as a
+// raw pointer would).  PinBuf / PinArray: the same in pinned host memory (cudaHostAllocPortable).
 struct DevBuf {
     void *p = nullptr;
     size_t bytes = 0;
 };
-template <class T>
-struct DevArray : DevBuf {
-    operator T *() const { return static_cast<T *>(p); }
+struct PinBuf : DevBuf {};
+template <class T, class Buf>
+struct TypedBuf : Buf {
+    operator T *() const { return static_cast<T *>(this->p); }
+    template <class U>
+    explicit operator U *() const { return static_cast<U *>(this->p); }
 };
+template <class T>
+using DevArray = TypedBuf<T, DevBuf>;
+template <class T>
+using PinArray = TypedBuf<T, PinBuf>;
 
 struct Dev {
     int ordinal = 0;
@@ -58,34 +66,28 @@ struct Dev {
     unsigned ws_next = 0;
     // Per-call lanes of the host-buffer entry points: own stream, input/verdict buffers and pinned staging, so that
     // SBV_LANES host threads can have a call in flight each (H2D / kernels / D2H of one overlap the others').
+    // The buffers are sized, grown and freed from one list (engine.cu: each_lane_buffer).
     struct Lane {
         cudaStream_t stream = nullptr;
-        size_t cap = 0;
-        uint8_t *d_r = nullptr, *d_s = nullptr, *d_qx = nullptr, *d_qy = nullptr, *d_dig = nullptr, *d_ok = nullptr;
-        uint32_t *d_slot = nullptr;
-        uint8_t *d_msgs = nullptr;
-        uint64_t *d_off = nullptr;
-        uint32_t *d_perm = nullptr;  // off_cap entries + 3 * 1024 words of sort state
-        size_t msg_cap = 0, off_cap = 0;
-        uint8_t *h_pin = nullptr;
-        size_t h_pin_cap = 0;
+        DevArray<uint8_t> d_r, d_s, d_qx, d_qy, d_dig, d_ok;  // per item: 48, 48, 48, 48, 64 and 1 bytes
+        DevArray<uint32_t> d_slot;
+        DevArray<uint8_t> d_msgs;
+        DevArray<uint64_t> d_off;
+        DevArray<uint32_t> d_perm;  // an entry per offset + 3 * 1024 words of sort state
+        PinArray<uint8_t> h_pin;    // staging of pageable caller buffers
         // small device scratch (quorum inputs / counts, packed verdict masks) and its pinned mirror
-        uint8_t *d_aux = nullptr, *h_aux = nullptr;
-        size_t aux_cap = 0;
+        DevArray<uint8_t> d_aux;
+        PinArray<uint8_t> h_aux;
+        // device scratch of a mixed ECDSA / Ed25519 shard (inst_mixed.cu: sbv_mix_carve) or of an RSA shard
+        // (engine_rsa.inc: rsa_carve); a lane serves one call at a time
+        DevArray<uint8_t> d_carve;
         // second stream of the call (mixed-curve batches run their two pipelines side by side)
         cudaStream_t stream2 = nullptr;
         cudaEvent_t ev_a = nullptr, ev_b = nullptr;
         cudaEvent_t ev_chunk[SBV_MAX_CHUNKS] = {};  // "chunk c has arrived" (recorded on stream2, the upload stream of a chunked call)
-        // device scratch of a mixed ECDSA / Ed25519 shard (inst_mixed.cu: sbv_mix_carve)
-        uint8_t *d_mix = nullptr;
-        size_t mix_cap = 0;
-        // device scratch of an RSA shard (engine_rsa.inc: rsa_carve)
-        uint8_t *d_rsa = nullptr;
-        size_t rsa_cap = 0;
     } lanes[SBV_LANES];
     // generic scratch of the entry points that serialise on the engine lock
-    uint8_t *d_scratch = nullptr;
-    size_t scratch_cap = 0;
+    DevArray<uint8_t> d_scratch;
     // registered keys (sbv_set_keys): per-curve tables (8-bit signed windows), validity flags, slot -> table index
     uint32_t *ktab[2] = {nullptr, nullptr};
     uint8_t *keyflags[2] = {nullptr, nullptr};
@@ -137,7 +139,6 @@ struct sbv_engine {
     uint32_t hash_seed = 0x9e3779b9u;
     bool profiling = false;
     // NCCL (loaded lazily with dlopen so single-device, single-rank users never touch it)
-    void *nccl_lib = nullptr;
     std::vector<void *> nccl_comms;  // one per device of a multi-device engine
     // one-process-per-GPU deployments: this engine is rank `rank` of `nranks`.  One communicator per CHANNEL: the
     // collectives of a channel must be issued in the same order on every rank, so concurrent host threads take one each.
@@ -284,11 +285,21 @@ constexpr size_t SBV_ED_BTAB_ENTRIES = 32 * 128, SBV_ED_BTAB_ENTRY_WORDS = 24;
 // ---- engine.cu helpers shared with the other translation units ----
 int sbv_lane_acquire(sbv_engine *e);            // blocks until a lane index is free; returns it
 void sbv_lane_release(sbv_engine *e, int lane);
-int sbv_lane_ensure(sbv_engine *e, Dev &d, Dev::Lane &ln, size_t n, size_t pinned_bytes);
-int sbv_lane_ensure_msgs(sbv_engine *e, Dev::Lane &ln, size_t bytes, size_t n_off);
-int sbv_lane_ensure_aux(sbv_engine *e, Dev::Lane &ln, size_t bytes);
-int sbv_lane_ensure_mix(sbv_engine *e, Dev::Lane &ln, size_t bytes);
-int sbv_lane_ensure_rsa(sbv_engine *e, Dev::Lane &ln, size_t bytes);
+// What one call uses of a lane's buffers on one device, in bytes unless noted (most calls: LaneNeeds{items, pinned}).
+struct LaneNeeds {
+    size_t items = 0;      // d_r, d_s, d_qx, d_qy, d_dig, d_ok and d_slot for this many items
+    size_t pinned = 0;     // h_pin
+    size_t msg_bytes = 0;  // d_msgs
+    size_t offsets = 0;    // d_off and d_perm: this many offsets
+    size_t aux = 0;        // d_aux and h_aux
+    size_t carve = 0;      // d_carve
+    // the messages of cnt items, `bytes` in all (engine_more.inc: stage_msgs)
+    void msgs(uint64_t bytes, size_t cnt) { msg_bytes = bytes + 16, offsets = cnt + 1; }
+};
+// Caller has set the device and owns the lane.  Creates the lane's stream on first use; if any buffer must grow, drains
+// both of the lane's streams once and regrows only those buffers (with headroom, so that a steady stream of calls of one
+// shape allocates nothing after its first).  Call it before enqueuing anything that uses the lane's buffers.
+int sbv_lane_reserve(sbv_engine *e, Dev::Lane &ln, const LaneNeeds &needs);
 int sbv_lane_stream2(sbv_engine *e, Dev::Lane &ln);  // creates the lane's second stream and its two events on first use
 // d_perm: n + 3072 words of scratch (may be null: no length sort)
 int sbv_launch_sha256(sbv_engine *e, size_t n, const uint8_t *d_msgs, const uint64_t *d_off, uint64_t base, uint8_t *d_digest, uint32_t *d_perm,
