@@ -35,6 +35,8 @@ SYMBOLS = [
     "sbv_mixed384_verify_registered", "sbv_mixed384_verify_batch", "sbv_mixed384_verify_quorum",
     "sbv_sha512_batch", "sbv_rsa_verify_batch", "sbv_rsa_hash_verify_batch",
     "sbv_rsa_pss_verify_batch", "sbv_rsa_pss_hash_verify_batch",
+    "sbv_rsa_set_keys", "sbv_rsa_verify_registered", "sbv_rsa_hash_verify_registered", "sbv_rsa_pss_verify_registered",
+    "sbv_rsa_pss_hash_verify_registered",
 ]
 
 
@@ -353,6 +355,96 @@ class Engine:
         self._check(self._lib.sbv_rsa_pss_hash_verify_batch(self._h, C.c_uint32(mod_bytes), C.c_uint8(hash), C.c_int32(salt_len), C.c_size_t(n),
                                                             vp(msgs), vp(off), vp(sig), vp(modulus), vp(pub_exp), vp(digest_out or None), vp(ok)),
                     "sbv_rsa_pss_hash_verify_batch")
+
+    def rsa_set_keys(self, mod_bytes, modulus, pub_exp):
+        """Replaces the RSA key registry: slot i = (modulus i, pub_exp[i]), modulus i being mod_bytes[i] bytes (256, 384 or
+        512) big-endian, the moduli concatenated in slot order; no keys empties it.  n0' and R^2 mod N are built once per
+        key on every device; a slot whose key fails the key rule is kept, and its items reject."""
+        mod_bytes = np.ascontiguousarray(mod_bytes, dtype=np.uint32).reshape(-1)
+        pub_exp = np.ascontiguousarray(pub_exp, dtype=np.uint32).reshape(-1)
+        modulus = _u8(modulus).reshape(-1)
+        n = mod_bytes.size
+        if pub_exp.size != n or modulus.size != int(mod_bytes.sum(dtype=np.uint64)):
+            raise ValueError("pub_exp must hold one exponent and modulus mod_bytes[i] bytes per key")
+        vp = C.c_void_p
+        self._check(self._lib.sbv_rsa_set_keys(self._h, C.c_size_t(n), vp(mod_bytes.ctypes.data if n else None), vp(modulus.ctypes.data if n else None),
+                                               vp(pub_exp.ctypes.data if n else None)), "sbv_rsa_set_keys")
+
+    def rsa_verify_registered(self, hash, key_slot, digest, sig, out=None) -> np.ndarray:
+        """rsa_verify_batch with the key of item i taken from registry slot key_slot[i] (rsa_set_keys); sig = n x k bytes,
+        k the call's modulus size (a slot of another size rejects)."""
+        key_slot = np.ascontiguousarray(key_slot, dtype=np.uint32)
+        n = key_slot.size
+        sig, digest = _u8(sig), _u8(digest)
+        k = sig.size // n if n else 256
+        ok = out if out is not None else np.zeros(n, np.uint8)
+        self.rsa_verify_registered_ptr(k, hash, n, key_slot.ctypes.data, digest.ctypes.data, sig.ctypes.data, ok.ctypes.data)
+        return ok
+
+    def rsa_verify_registered_ptr(self, mod_bytes, hash, n, key_slot, digest, sig, ok):
+        """Raw host pointers (ints) — used with pinned buffers."""
+        vp = C.c_void_p
+        self._check(self._lib.sbv_rsa_verify_registered(self._h, C.c_uint32(mod_bytes), C.c_uint8(hash), C.c_size_t(n), vp(key_slot), vp(digest),
+                                                        vp(sig), vp(ok)), "sbv_rsa_verify_registered")
+
+    def rsa_hash_verify_registered(self, hash, msgs, off, key_slot, sig, want_digest=False):
+        """rsa_verify_registered with H = hash(M) computed on the device; msgs concatenated with off[n+1] byte offsets.
+        Returns the verdicts, and the n x hLen digests too with want_digest."""
+        msgs = _u8(msgs if len(msgs) else np.zeros(1, np.uint8))
+        off = np.ascontiguousarray(off, dtype=np.uint64)
+        key_slot = np.ascontiguousarray(key_slot, dtype=np.uint32)
+        sig = _u8(sig)
+        n = off.size - 1
+        k = sig.size // n if n else 256
+        ok = np.zeros(n, np.uint8)
+        dig = np.zeros((n, HASH_BYTES[hash]), np.uint8) if want_digest else None
+        self.rsa_hash_verify_registered_ptr(k, hash, n, msgs.ctypes.data, off.ctypes.data, key_slot.ctypes.data, sig.ctypes.data,
+                                            dig.ctypes.data if want_digest else 0, ok.ctypes.data)
+        return (ok, dig) if want_digest else ok
+
+    def rsa_hash_verify_registered_ptr(self, mod_bytes, hash, n, msgs, off, key_slot, sig, digest_out, ok):
+        """Raw host pointers (ints; digest_out may be 0) — used with pinned buffers."""
+        vp = C.c_void_p
+        self._check(self._lib.sbv_rsa_hash_verify_registered(self._h, C.c_uint32(mod_bytes), C.c_uint8(hash), C.c_size_t(n), vp(msgs), vp(off),
+                                                             vp(key_slot), vp(sig), vp(digest_out or None), vp(ok)), "sbv_rsa_hash_verify_registered")
+
+    def rsa_pss_verify_registered(self, hash, salt_len, key_slot, digest, sig, out=None) -> np.ndarray:
+        """rsa_pss_verify_batch with the key of item i taken from registry slot key_slot[i] (rsa_set_keys)."""
+        key_slot = np.ascontiguousarray(key_slot, dtype=np.uint32)
+        n = key_slot.size
+        sig, digest = _u8(sig), _u8(digest)
+        k = sig.size // n if n else 256
+        ok = out if out is not None else np.zeros(n, np.uint8)
+        self.rsa_pss_verify_registered_ptr(k, hash, salt_len, n, key_slot.ctypes.data, digest.ctypes.data, sig.ctypes.data, ok.ctypes.data)
+        return ok
+
+    def rsa_pss_verify_registered_ptr(self, mod_bytes, hash, salt_len, n, key_slot, digest, sig, ok):
+        """Raw host pointers (ints) — used with pinned buffers."""
+        vp = C.c_void_p
+        self._check(self._lib.sbv_rsa_pss_verify_registered(self._h, C.c_uint32(mod_bytes), C.c_uint8(hash), C.c_int32(salt_len), C.c_size_t(n),
+                                                            vp(key_slot), vp(digest), vp(sig), vp(ok)), "sbv_rsa_pss_verify_registered")
+
+    def rsa_pss_hash_verify_registered(self, hash, salt_len, msgs, off, key_slot, sig, want_digest=False):
+        """rsa_pss_verify_registered with H = hash(M) computed on the device; msgs concatenated with off[n+1] byte offsets.
+        Returns the verdicts, and the n x hLen digests too with want_digest."""
+        msgs = _u8(msgs if len(msgs) else np.zeros(1, np.uint8))
+        off = np.ascontiguousarray(off, dtype=np.uint64)
+        key_slot = np.ascontiguousarray(key_slot, dtype=np.uint32)
+        sig = _u8(sig)
+        n = off.size - 1
+        k = sig.size // n if n else 256
+        ok = np.zeros(n, np.uint8)
+        dig = np.zeros((n, HASH_BYTES[hash]), np.uint8) if want_digest else None
+        self.rsa_pss_hash_verify_registered_ptr(k, hash, salt_len, n, msgs.ctypes.data, off.ctypes.data, key_slot.ctypes.data, sig.ctypes.data,
+                                                dig.ctypes.data if want_digest else 0, ok.ctypes.data)
+        return (ok, dig) if want_digest else ok
+
+    def rsa_pss_hash_verify_registered_ptr(self, mod_bytes, hash, salt_len, n, msgs, off, key_slot, sig, digest_out, ok):
+        """Raw host pointers (ints; digest_out may be 0) — used with pinned buffers."""
+        vp = C.c_void_p
+        self._check(self._lib.sbv_rsa_pss_hash_verify_registered(self._h, C.c_uint32(mod_bytes), C.c_uint8(hash), C.c_int32(salt_len), C.c_size_t(n),
+                                                                 vp(msgs), vp(off), vp(key_slot), vp(sig), vp(digest_out or None), vp(ok)),
+                    "sbv_rsa_pss_hash_verify_registered")
 
     def hash384_verify_batch_ptr(self, curve, n, msgs, off, r, s, qx, qy, digest_out, ok):
         """Raw host pointers (ints; digest_out may be 0) — used with pinned buffers."""

@@ -462,3 +462,19 @@ extern "C" int sbv_debug_key_cache_sets(sbv_engine *e, int device_index, uint8_t
     out[1] = k.amap.sets;
     return 1;
 }
+
+// Copies the record of RSA registry slot `slot` on device 0 (sbv_rsa_set_keys; rsa_keyed.cuh): out[0..8) = {k, valid, ntop,
+// n0', e, limb offset (2 words), 0}, then the K = k / 4 little-endian limbs of N and the K of R^2 mod N, 8 + 2K words (at
+// most 264).  SBV_ERR_ARG for a slot outside the registry.
+extern "C" int sbv_debug_rsa_key(sbv_engine *e, uint32_t slot, uint32_t *out) {
+    if (!e || !out || e->devs.empty()) return SBV_ERR_ARG;
+    std::shared_lock<std::shared_mutex> reg(e->ed_reg_mu);
+    std::lock_guard<std::mutex> lk(e->mu);
+    Dev &d = e->devs[0];
+    if (slot >= d.rsa_n_slots) return SBV_ERR_ARG;
+    CU(e, cudaSetDevice(d.ordinal));
+    CU(e, cudaMemcpy(out, d.rsa_rec + 2 * (size_t)slot, 32, cudaMemcpyDeviceToHost));
+    const uint64_t off = ((uint64_t)out[6] << 32) | out[5];
+    CU(e, cudaMemcpy(out + 8, d.rsa_pool + off, (size_t)out[0] * 2, cudaMemcpyDeviceToHost));  // 2K words
+    return SBV_OK;
+}

@@ -490,6 +490,7 @@ void sbv_destroy(sbv_engine *e) {
         sbv_scratch_free(d);
         sbv_keys_free(d);
         sbv_ed_keys_free(d);
+        sbv_rsa_keys_free(d);
         sbv_key_cache_free(d);
         for (auto &ln : d.lanes) lane_free(ln);
         for (cudaEvent_t ev : d.prof_events) cudaEventDestroy(ev);

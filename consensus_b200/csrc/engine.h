@@ -37,6 +37,18 @@ using DevArray = TypedBuf<T, DevBuf>;
 template <class T>
 using PinArray = TypedBuf<T, PinBuf>;
 
+struct DevTemp {  // device temporaries of one registry build, freed on every exit path
+    std::vector<void *> p;
+    ~DevTemp() { for (void *x : p) cudaFree(x); }
+    template <class T>
+    cudaError_t alloc(T **out, size_t bytes) {
+        void *q = nullptr;
+        const cudaError_t st = cudaMalloc(&q, bytes);
+        if (st == cudaSuccess) { p.push_back(q); *out = static_cast<T *>(q); }
+        return st;
+    }
+};
+
 struct Dev {
     int ordinal = 0;
     cudaStream_t stream = nullptr;
@@ -99,6 +111,11 @@ struct Dev {
     int32_t *ed_slot2local = nullptr;
     uint32_t *ed_ktab = nullptr;
     uint32_t ed_n_slots = 0, ed_n_local = 0;
+    // registered RSA keys (sbv_rsa_set_keys): two uint4 of record per slot and the limbs of N and R^2 mod N of every slot
+    // (rsa_keyed.cuh)
+    uint4 *rsa_rec = nullptr;
+    uint32_t *rsa_pool = nullptr;
+    uint32_t rsa_n_slots = 0;
     // the opt-in cache of grouped-key tables across launches (sbv_key_cache_reserve), per scheme tag: one allocation holding
     // the pool, the counters, the map (key_cache.cuh) and one launch area per scratch set (2 + SBV_GROUP_MAX_KEYS words:
     // the lookup's miss and hit counts and the renumbered keylist of the launch holding that set).  An evicting cache
@@ -124,8 +141,9 @@ struct sbv_engine {
     std::vector<Dev> devs;
     std::mutex mu;       // kernel enqueue + workspace growth
     std::mutex err_mu;   // last-error string
-    // the Ed25519 registry: sbv_ed25519_set_keys holds it exclusively, sbv_ed25519_verify_registered shared for the
-    // enqueue of all its shards, so every shard of one call reads the same registry (taken before mu, never inside it)
+    // the Ed25519 and RSA registries: sbv_ed25519_set_keys and sbv_rsa_set_keys hold it exclusively, the registered calls
+    // of both families shared for the enqueue of all their shards, so every shard of one call reads the same registry
+    // (taken before mu, never inside it)
     std::shared_mutex ed_reg_mu;
     std::condition_variable lane_cv;
     bool lane_busy[SBV_LANES] = {};
@@ -320,6 +338,17 @@ int sbv_launch_rsa(sbv_engine *e, uint32_t mod_bytes, uint8_t hash, size_t n, co
 // salt_len as in sbv_rsa_pss_verify_batch (>= -1); verdicts into d_ok.  Two launches.
 int sbv_launch_rsa_pss(sbv_engine *e, uint32_t mod_bytes, uint8_t hash, int32_t salt_len, size_t n, uint8_t *d_sig, const uint8_t *d_mod,
                        const uint32_t *d_exp, const uint8_t *d_digest, uint8_t *d_ok, cudaStream_t st);
+// registered RSA keys (rsa_keyed.cuh).  sbv_rsa_keys_build: caller holds e->mu; waits for the device to drain, frees the old
+// registry of device d and builds one from the n keys (mod_bytes[i] in {256, 384, 512}, checked by the caller; the moduli
+// concatenated, big-endian); a fault leaves d's registry empty.
+int sbv_rsa_keys_build(sbv_engine *e, Dev &d, size_t n, const uint32_t *mod_bytes, const uint8_t *modulus, const uint32_t *pub_exp);
+void sbv_rsa_keys_free(Dev &d);
+// sbv_launch_rsa and sbv_launch_rsa_pss with the key of each item read from device d's RSA registry by slot (d_slot, n
+// words) in place of d_mod and d_exp; the same launches.  The caller holds the registry (ed_reg_mu shared) while enqueuing.
+int sbv_launch_rsa_reg(sbv_engine *e, Dev &d, uint32_t mod_bytes, uint8_t hash, size_t n, const uint8_t *d_sig, const uint32_t *d_slot,
+                       const uint8_t *d_digest, uint8_t *d_ok, cudaStream_t st);
+int sbv_launch_rsa_pss_reg(sbv_engine *e, Dev &d, uint32_t mod_bytes, uint8_t hash, int32_t salt_len, size_t n, uint8_t *d_sig, const uint32_t *d_slot,
+                           const uint8_t *d_digest, uint8_t *d_ok, cudaStream_t st);
 // mixed_hash.cuh: k_mix_alg over the n uploaded tags of a mixed shard (tags 3 and 4 to their family, flags into d_alg)
 int sbv_launch_mix_alg(sbv_engine *e, size_t n, uint8_t *d_tag, uint8_t *d_alg, cudaStream_t st);
 // mixed_hash.cuh: k_sha2_sel over the n items of one family (d_idx: their shard indices, d_alg: the shard's flags), dlen

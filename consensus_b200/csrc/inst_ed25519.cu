@@ -213,18 +213,6 @@ void sbv_ed_keys_free(Dev &d) {
 }
 
 namespace {
-struct DevTemp {  // device temporaries of one registry build, freed on every exit path
-    std::vector<void *> p;
-    ~DevTemp() { for (void *x : p) cudaFree(x); }
-    template <class T>
-    cudaError_t alloc(T **out, size_t bytes) {
-        void *q = nullptr;
-        const cudaError_t st = cudaMalloc(&q, bytes);
-        if (st == cudaSuccess) { p.push_back(q); *out = static_cast<T *>(q); }
-        return st;
-    }
-};
-
 // The registry of device d from the n keys of pub: the registered bytes, k_ed_kdecode for the flags, the map of the
 // decodable slots to tables, and k_ed_ktab_build for their tables, at most ED_KBUILD_MAX keys per launch.
 int ed_keys_fill(sbv_engine *e, Dev &d, size_t n, const uint8_t *pub) {

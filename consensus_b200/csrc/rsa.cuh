@@ -1,6 +1,7 @@
 // rsa.cuh — RSA PKCS #1 v1.5 signature verification (RFC 8017 §8.2.2, Go's crypto/rsa.VerifyPKCS1v15) for moduli of
 // 2048, 3072 and 4096 bits (k = 256, 384 or 512 bytes), a group of 16 lanes per signature, two signatures per warp.  The
-// key rule, the range check and the exponentiation (rsa_recover) serve RSA-PSS too (rsa_pss.cuh).
+// key rule, the range check and the exponentiation (rsa_recover) serve RSA-PSS too (rsa_pss.cuh); the exponentiation from
+// S * R onward (rsa_pow_tail) and the encoding compare (rsa_pkcs1_match) serve the registered keys (rsa_keyed.cuh).
 //
 // Layout.  A k-byte number is K = k/4 little-endian 32-bit limbs; lane l of the group holds limbs [l*NL, l*NL + NL),
 // NL = K/16 = 4, 6 or 8, of every operand.  Values cross the group only by shuffle and ballot under the group's mask.
@@ -210,24 +211,13 @@ SBV_DEV void rsa_r2(const RsaLanes &g, uint32_t (&x)[NL], const uint32_t (&n)[NL
     for (int i = 0; i < 5; i++) rsa_mont(g, x, x, x, n, ninv);
 }
 
-// Steps 1-3 of both paddings (the same in every lane of the group): false if the key rule or S < N refuses the item, else
-// tail(em), em = S^e mod N, this lane's limbs.  sig, mod: k bytes big-endian; e: the public exponent.  The padding's part
-// is a callable rather than a caller testing a flag, so that every refusal returns straight out of the kernel's item.
+// Step 3 from S * R onward, shared by the keys carried per item (rsa_recover) and the registered keys (rsa_keyed.cuh):
+// s = S < N, x = R^2 mod N on entry (scratch after), ninv = -N^-1 mod 2^32, e the public exponent; returns tail(em), em =
+// S^e mod N, this lane's limbs.  sm (S * R) and acc are the caller's arrays: declared there, ahead of rsa_r2, the keys-per-
+// item kernels compile to the same instructions as before this function was split out.
 template <int NL, class Tail>
-SBV_DEV bool rsa_recover(const RsaLanes &g, const uint8_t *sig, const uint8_t *mod, uint32_t e, Tail &&tail) {
-    constexpr int K = RSA_GROUP * NL;
-    constexpr uint32_t k = 4 * K;
-    uint32_t n[NL], s[NL], x[NL];
-    rsa_load(g, n, mod, k);
-    rsa_load(g, s, sig, k);
-    // the key: N odd, N's leading byte nonzero, 2 <= e <= 2^31 - 1
-    const uint32_t n0 = rsa_from(g, n[0], 0), ntop = rsa_from(g, n[NL - 1], RSA_GROUP - 1);
-    if (!(n0 & 1) || (ntop >> 24) == 0 || e < 2 || e > 0x7fffffffu) return false;
-    // the range: S < N
-    if (!rsa_sub(g, x, s, n)) return false;
-    const uint32_t ninv = rsa_ninv(g, n);
-    uint32_t sm[NL], acc[NL];
-    rsa_r2(g, x, n, ninv);
+SBV_DEV bool rsa_pow_tail(const RsaLanes &g, const uint32_t (&s)[NL], uint32_t (&x)[NL], const uint32_t (&n)[NL], uint32_t ninv, uint32_t e,
+                          uint32_t (&sm)[NL], uint32_t (&acc)[NL], Tail &&tail) {
     rsa_mont(g, sm, s, x, n, ninv);  // S * R mod N
     // left to right over the bits of e below its top bit: square, and multiply by S*R where the bit is set
 #pragma unroll
@@ -250,34 +240,60 @@ SBV_DEV bool rsa_recover(const RsaLanes &g, const uint8_t *sig, const uint8_t *m
     return tail(acc);
 }
 
+// Steps 1-3 of both paddings (the same in every lane of the group): false if the key rule or S < N refuses the item, else
+// tail(em), em = S^e mod N, this lane's limbs.  sig, mod: k bytes big-endian; e: the public exponent.  The padding's part
+// is a callable rather than a caller testing a flag, so that every refusal returns straight out of the kernel's item.
+template <int NL, class Tail>
+SBV_DEV bool rsa_recover(const RsaLanes &g, const uint8_t *sig, const uint8_t *mod, uint32_t e, Tail &&tail) {
+    constexpr int K = RSA_GROUP * NL;
+    constexpr uint32_t k = 4 * K;
+    uint32_t n[NL], s[NL], x[NL];
+    rsa_load(g, n, mod, k);
+    rsa_load(g, s, sig, k);
+    // the key: N odd, N's leading byte nonzero, 2 <= e <= 2^31 - 1
+    const uint32_t n0 = rsa_from(g, n[0], 0), ntop = rsa_from(g, n[NL - 1], RSA_GROUP - 1);
+    if (!(n0 & 1) || (ntop >> 24) == 0 || e < 2 || e > 0x7fffffffu) return false;
+    // the range: S < N
+    if (!rsa_sub(g, x, s, n)) return false;
+    const uint32_t ninv = rsa_ninv(g, n);
+    uint32_t sm[NL], acc[NL];
+    rsa_r2(g, x, n, ninv);
+    return rsa_pow_tail<NL>(g, s, x, n, ninv, e, sm, acc, tail);
+}
+
+// Step 4 of PKCS #1 v1.5 (the same in every lane of the group): em = this lane's limbs of S^e mod N; h: the hLen-byte
+// digest, hash 0 / 1 / 2 = SHA-256 / SHA-384 / SHA-512.
+template <int NL>
+SBV_DEV bool rsa_pkcs1_match(const RsaLanes &g, const uint32_t (&acc)[NL], const uint8_t *h, uint32_t hash) {
+    constexpr uint32_t k = 64 * NL;
+    // EM = 00 || 01 || FF..FF || 00 || DigestInfo || H, by bytes counted from the end (r = 0 is the last byte)
+    const uint32_t hl = 32 + 16 * hash, tl = hl + 19;
+    uint32_t bad = 0;
+#pragma unroll
+    for (int j = 0; j < NL; j++) {
+        uint32_t w = 0;
+#pragma unroll
+        for (int q = 0; q < 4; q++) {
+            const uint32_t r = 4 * (g.l * NL + j) + q;
+            uint32_t v;
+            if (r < hl) v = h[hl - 1 - r];
+            else if (r < tl) v = RSA_DIGEST_INFO[hash][tl - 1 - r];
+            else if (r == tl) v = 0x00;
+            else if (r < k - 2) v = 0xff;
+            else if (r == k - 2) v = 0x01;
+            else v = 0x00;
+            w |= v << (8 * q);
+        }
+        bad |= w ^ acc[j];
+    }
+    return rsa_bits(g, bad != 0) == 0;
+}
+
 // The PKCS #1 v1.5 verdict of one item (the same in every lane of the group).  sig, mod: k bytes big-endian; e: the public
 // exponent; h: the hLen-byte digest, hash 0 / 1 / 2 = SHA-256 / SHA-384 / SHA-512.
 template <int NL>
 SBV_DEV bool rsa_verify_item(const RsaLanes &g, const uint8_t *sig, const uint8_t *mod, uint32_t e, const uint8_t *h, uint32_t hash) {
-    return rsa_recover<NL>(g, sig, mod, e, [&](const uint32_t (&acc)[NL]) {
-        constexpr uint32_t k = 64 * NL;
-        // EM = 00 || 01 || FF..FF || 00 || DigestInfo || H, by bytes counted from the end (r = 0 is the last byte)
-        const uint32_t hl = 32 + 16 * hash, tl = hl + 19;
-        uint32_t bad = 0;
-#pragma unroll
-        for (int j = 0; j < NL; j++) {
-            uint32_t w = 0;
-#pragma unroll
-            for (int q = 0; q < 4; q++) {
-                const uint32_t r = 4 * (g.l * NL + j) + q;
-                uint32_t v;
-                if (r < hl) v = h[hl - 1 - r];
-                else if (r < tl) v = RSA_DIGEST_INFO[hash][tl - 1 - r];
-                else if (r == tl) v = 0x00;
-                else if (r < k - 2) v = 0xff;
-                else if (r == k - 2) v = 0x01;
-                else v = 0x00;
-                w |= v << (8 * q);
-            }
-            bad |= w ^ acc[j];
-        }
-        return rsa_bits(g, bad != 0) == 0;
-    });
+    return rsa_recover<NL>(g, sig, mod, e, [&](const uint32_t (&acc)[NL]) { return rsa_pkcs1_match<NL>(g, acc, h, hash); });
 }
 
 // One item per group of 16 lanes: ok[i] = 1 iff sig i (k bytes) is a valid PKCS #1 v1.5 signature of digest i (hLen

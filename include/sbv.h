@@ -139,8 +139,8 @@ enum { SBV_HASH_SHA256 = 0, SBV_HASH_SHA384 = 1, SBV_HASH_SHA512 = 2 };
  * RSA-PSS has calls of its own, below.  The checks: SBV_ERR_ARG for a mod_bytes other than 256 / 384 / 512, a hash
  * tag above SBV_HASH_SHA512, a null buffer (msgs may be NULL when every message is empty), n >= 2^31 and decreasing offsets, all
  * before anything is written or launched.  Multi-device engines shard by item as sbv_hash_verify_batch does.  Each
- * device's shard is uploaded whole (no chunked upload).  Out of scope: registered RSA keys, RSA items in the mixed and
- * commit-vote calls, and _device / _ranked forms. */
+ * device's shard is uploaded whole (no chunked upload).  Registered keys have calls of their own (sbv_rsa_set_keys, below).
+ * Out of scope: RSA items in the mixed and commit-vote calls, and _device / _ranked forms. */
 /* SHA-512 over a ragged batch (msgs / msg_off as in sbv_sha256_batch); digest_out = 64n bytes. */
 int sbv_sha512_batch(sbv_engine *e, size_t n, const uint8_t *msgs, const uint64_t *msg_off, uint8_t *digest_out);
 /* digests supplied: digest = n x hLen bytes; sig, modulus = n x mod_bytes bytes; pub_exp = n x uint32 */
@@ -179,6 +179,41 @@ int sbv_rsa_pss_verify_batch(sbv_engine *e, uint32_t mod_bytes, uint8_t hash, in
 int sbv_rsa_pss_hash_verify_batch(sbv_engine *e, uint32_t mod_bytes, uint8_t hash, int32_t salt_len, size_t n,
                                   const uint8_t *msgs, const uint64_t *msg_off, const uint8_t *sig,
                                   const uint8_t *modulus, const uint32_t *pub_exp, uint8_t *digest_out, uint8_t *ok);
+
+/* ---- Registered RSA keys: client keys are configuration, as consenter keys are (they change only with a reconfiguration),
+ * so the key-only work of the calls above (the key rule, n0' = -N^-1 mod 2^32 and R^2 mod N) runs once per key set in
+ * sbv_rsa_set_keys, and the verify calls upload only signatures, slots and digests or messages.
+ *  - Accept set: ok[i] equals, byte for byte, what the keys-per-item call of the same padding returns for item i given the
+ *    slot's registered modulus bytes and exponent.  The key rule (odd N, nonzero leading byte, 2 <= e <= 2^31 - 1) runs
+ *    once, in sbv_rsa_set_keys; a slot whose key fails it is kept as invalid, and its items reject.
+ *  - Slots that reject, without a fault: key_slot[i] >= n of the registry (every slot while the registry is empty), and a
+ *    slot whose key size differs from the call's mod_bytes (one call takes one modulus size, as the other RSA calls do).
+ *  - Registry: a call replaces the whole registry; every device holds all of it; the call waits for the launches that may
+ *    still read the old registry; every shard of one verify call, on every device, reads the same registry; a device
+ *    fault leaves the registry empty on every device.  It is independent of the ECDSA and Ed25519 registries.
+ *  - Checks, all SBV_ERR_ARG before anything is written, launched or replaced (a refused sbv_rsa_set_keys leaves the old
+ *    registry in place): sbv_rsa_set_keys refuses a mod_bytes[i] other than 256 / 384 / 512 (its index in sbv_last_error),
+ *    null buffers when n > 0 and n >= 2^31; the verify calls make the checks of their keys-per-item counterparts, plus a
+ *    null key_slot.
+ *  - Multi-device engines shard by item; digest_out may be NULL.
+ * 32 + 2 * mod_bytes bytes of device memory per slot on every device. */
+/* Slot i = (modulus i, pub_exp[i]), modulus i being mod_bytes[i] bytes (256, 384 or 512) big-endian, the moduli
+ * concatenated in slot order; n = 0 empties the registry. */
+int sbv_rsa_set_keys(sbv_engine *e, size_t n, const uint32_t *mod_bytes, const uint8_t *modulus, const uint32_t *pub_exp);
+/* sbv_rsa_verify_batch with the key of item i taken from registry slot key_slot[i] */
+int sbv_rsa_verify_registered(sbv_engine *e, uint32_t mod_bytes, uint8_t hash, size_t n, const uint32_t *key_slot,
+                              const uint8_t *digest, const uint8_t *sig, uint8_t *ok);
+/* sbv_rsa_hash_verify_batch with registered keys; digest_out (n x hLen) may be NULL */
+int sbv_rsa_hash_verify_registered(sbv_engine *e, uint32_t mod_bytes, uint8_t hash, size_t n, const uint8_t *msgs,
+                                   const uint64_t *msg_off, const uint32_t *key_slot, const uint8_t *sig,
+                                   uint8_t *digest_out, uint8_t *ok);
+/* sbv_rsa_pss_verify_batch with registered keys */
+int sbv_rsa_pss_verify_registered(sbv_engine *e, uint32_t mod_bytes, uint8_t hash, int32_t salt_len, size_t n,
+                                  const uint32_t *key_slot, const uint8_t *digest, const uint8_t *sig, uint8_t *ok);
+/* sbv_rsa_pss_hash_verify_batch with registered keys; digest_out (n x hLen) may be NULL */
+int sbv_rsa_pss_hash_verify_registered(sbv_engine *e, uint32_t mod_bytes, uint8_t hash, int32_t salt_len, size_t n,
+                                       const uint8_t *msgs, const uint64_t *msg_off, const uint32_t *key_slot,
+                                       const uint8_t *sig, uint8_t *digest_out, uint8_t *ok);
 
 /* Mixed-curve batch: curve_tag[i] in {SBV_P256, SBV_P384}; every field is stored in a 48-byte
  * slot (P-256 values right-aligned, i.e. 16 leading zero bytes); digest is 32 bytes per item. */

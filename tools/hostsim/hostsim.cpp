@@ -32,6 +32,7 @@ namespace sbv { uint32_t tab[1 << 18]; }
 #include "../../consensus_b200/csrc/rsa.cuh"
 #include "../../consensus_b200/csrc/rsa_debug.cuh"
 #include "../../consensus_b200/csrc/rsa_pss.cuh"
+#include "../../consensus_b200/csrc/rsa_keyed.cuh"
 #include "../../consensus_b200/csrc/sha512_batch.cuh"
 
 using namespace sbv;
@@ -973,5 +974,58 @@ extern "C" int hs_rsa_pss_decode(uint32_t mod_bytes, uint8_t hash, int32_t salt_
     if (hash == 0) run_grid(tblocks, 128, [&] { k_rsa_pss<0>((uint32_t)n, mod_bytes, salt_len, em, mod, digest, ok); });
     else if (hash == 1) run_grid(tblocks, 128, [&] { k_rsa_pss<1>((uint32_t)n, mod_bytes, salt_len, em, mod, digest, ok); });
     else run_grid(tblocks, 128, [&] { k_rsa_pss<2>((uint32_t)n, mod_bytes, salt_len, em, mod, digest, ok); });
+    return 0;
+}
+
+// ---- registered RSA keys (rsa_keyed.cuh) ----
+// The registry of sbv_rsa_set_keys from the n keys (mod_bytes[i] in {256, 384, 512}, the moduli concatenated): k_rsa_kprep
+// in lockstep, in blocks of 128 threads, one launch per size over the slots of that size, as the engine launches it.  rec:
+// 8 words per slot; pool: (sum of mod_bytes) / 2 words.  -1 (and nothing written) for a size outside the set.
+extern "C" int hs_rsa_kprep(size_t n, const uint32_t *mod_bytes, const uint8_t *modulus, const uint32_t *pub_exp, uint32_t *rec, uint32_t *pool) {
+    for (size_t i = 0; i < n; i++)
+        if (mod_bytes[i] != 256 && mod_bytes[i] != 384 && mod_bytes[i] != 512) return -1;
+    std::vector<uint64_t> off(n);
+    std::vector<uint32_t> slots(n);
+    size_t first[4];
+    rsa_reg_layout(n, mod_bytes, off.data(), slots.data(), first);
+    uint4 *r = reinterpret_cast<uint4 *>(rec);
+    for (int c = 0; c < 3; c++) {
+        const uint32_t cnt = (uint32_t)(first[c + 1] - first[c]);
+        if (cnt == 0) continue;
+        const unsigned blocks = (unsigned)(((size_t)cnt * RSA_GROUP + 127) / 128);
+        const uint32_t *sl = slots.data() + first[c];
+        if (c == 0) run_grid_lockstep(blocks, 128, [&] { k_rsa_kprep<4>(cnt, sl, modulus, off.data(), pub_exp, r, pool); });
+        else if (c == 1) run_grid_lockstep(blocks, 128, [&] { k_rsa_kprep<6>(cnt, sl, modulus, off.data(), pub_exp, r, pool); });
+        else run_grid_lockstep(blocks, 128, [&] { k_rsa_kprep<8>(cnt, sl, modulus, off.data(), pub_exp, r, pool); });
+    }
+    return 0;
+}
+
+// sbv_launch_rsa_reg with the same arguments over a registry of nslots slots (rec, pool as hs_rsa_kprep wrote them):
+// k_rsa_verify_reg in lockstep, in blocks of 128 threads.  -1 (and nothing written) for a size or hash tag outside the set.
+extern "C" int hs_rsa_verify_registered(uint32_t mod_bytes, uint8_t hash, size_t n, const uint8_t *sig, const uint32_t *key_slot, uint32_t nslots,
+                                        const uint32_t *rec, const uint32_t *pool, const uint8_t *digest, uint8_t *ok) {
+    if ((mod_bytes != 256 && mod_bytes != 384 && mod_bytes != 512) || hash > 2) return -1;
+    const unsigned blocks = (unsigned)((n * RSA_GROUP + 127) / 128);
+    const uint4 *r = reinterpret_cast<const uint4 *>(rec);
+    if (mod_bytes == 256) run_grid_lockstep(blocks, 128, [&] { k_rsa_verify_reg<4>((uint32_t)n, hash, sig, key_slot, nslots, r, pool, digest, ok); });
+    else if (mod_bytes == 384) run_grid_lockstep(blocks, 128, [&] { k_rsa_verify_reg<6>((uint32_t)n, hash, sig, key_slot, nslots, r, pool, digest, ok); });
+    else run_grid_lockstep(blocks, 128, [&] { k_rsa_verify_reg<8>((uint32_t)n, hash, sig, key_slot, nslots, r, pool, digest, ok); });
+    return 0;
+}
+
+// sbv_launch_rsa_pss_reg with the same arguments: k_rsa_em_reg in lockstep (EM written over sig), then k_rsa_pss_reg one
+// thread at a time.  -1 (and nothing written) for a size or hash tag outside the set or salt_len < -1.
+extern "C" int hs_rsa_pss_verify_registered(uint32_t mod_bytes, uint8_t hash, int32_t salt_len, size_t n, uint8_t *sig, const uint32_t *key_slot,
+                                            uint32_t nslots, const uint32_t *rec, const uint32_t *pool, const uint8_t *digest, uint8_t *ok) {
+    if ((mod_bytes != 256 && mod_bytes != 384 && mod_bytes != 512) || hash > 2 || salt_len < PSS_SALT_EQUALS_HASH) return -1;
+    const unsigned blocks = (unsigned)((n * RSA_GROUP + 127) / 128), tblocks = (unsigned)((n + 127) / 128);
+    const uint4 *r = reinterpret_cast<const uint4 *>(rec);
+    if (mod_bytes == 256) run_grid_lockstep(blocks, 128, [&] { k_rsa_em_reg<4>((uint32_t)n, sig, key_slot, nslots, r, pool, ok); });
+    else if (mod_bytes == 384) run_grid_lockstep(blocks, 128, [&] { k_rsa_em_reg<6>((uint32_t)n, sig, key_slot, nslots, r, pool, ok); });
+    else run_grid_lockstep(blocks, 128, [&] { k_rsa_em_reg<8>((uint32_t)n, sig, key_slot, nslots, r, pool, ok); });
+    if (hash == 0) run_grid(tblocks, 128, [&] { k_rsa_pss_reg<0>((uint32_t)n, mod_bytes, salt_len, sig, key_slot, r, digest, ok); });
+    else if (hash == 1) run_grid(tblocks, 128, [&] { k_rsa_pss_reg<1>((uint32_t)n, mod_bytes, salt_len, sig, key_slot, r, digest, ok); });
+    else run_grid(tblocks, 128, [&] { k_rsa_pss_reg<2>((uint32_t)n, mod_bytes, salt_len, sig, key_slot, r, digest, ok); });
     return 0;
 }

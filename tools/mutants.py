@@ -54,6 +54,7 @@ COMB_WARP = ["tests/test_hostsim_comb_warp.py"]  # the comb build a warp per key
 TABLE_SHAPES = ["tests/test_hostsim_table_shapes.py"]
 RSA = ["tests/test_hostsim_rsa.py"]  # rsa.cuh and k_sha512 (sha512_batch.cuh)
 RSA_PSS = ["tests/test_hostsim_rsa_pss.py"]  # k_rsa_em and k_rsa_pss (rsa_pss.cuh)
+RSA_REG = ["tests/test_hostsim_rsa_registered.py"]  # registered RSA keys (rsa_keyed.cuh)
 MIXED384 = ["tests/test_hostsim_mixed384.py"]  # k_mix_alg and k_sha2_sel (mixed_hash.cuh)  # every entry of the per-key tables at the key counts where the builds turn over
 
 
@@ -404,6 +405,14 @@ CATALOGUE = [
       RSA_PSS),
     M("pss_compare_dropped", "rsa_pss.cuh", "return diff == 0;", "return true;", RSA_PSS),
     M("pss_em_key_verdict", "rsa_pss.cuh", "if (i >= n || !ok[i]) return;", "if (i >= n) return;", RSA_PSS),
+    # ---------------------------------------------------------------- rsa_keyed.cuh: the registry's record and the checks of its readers
+    M("rsa_reg_slot_bound", "rsa_keyed.cuh", "    if (slot >= nslots) return false;\n", "", RSA_REG),
+    M("rsa_reg_size_mismatch", "rsa_keyed.cuh", "    if (r0.x != k) return false;\n", "", RSA_REG),
+    M("rsa_reg_valid_flag", "rsa_keyed.cuh", "    if (r0.y == 0) return false;\n", "", RSA_REG),
+    M("rsa_reg_r2_of_slot0", "rsa_keyed.cuh", "rsa_limbs_load(x, p + K);  // R^2 mod N", "rsa_limbs_load(x, pool + K + g.l * NL);  // R^2 mod N", RSA_REG),
+    M("rsa_reg_ninv_of_slot0", "rsa_keyed.cuh", "rsa_pow_tail<NL>(g, s, x, n, r0.w, r1.x,", "rsa_pow_tail<NL>(g, s, x, n, rec[0].w, r1.x,", RSA_REG),
+    M("rsa_reg_ntop_stored", "rsa_keyed.cuh", "valid ? 1u : 0u, hi >> 24, ninv}", "valid ? 1u : 0u, 1u, ninv}", RSA_REG),
+    M("rsa_kprep_rule_lead_byte", "rsa_keyed.cuh", "hi >= (1u << 24)", "hi != 0", RSA_REG),
     # ---------------------------------------------------------------- sha512_batch.cuh
     M("sha512_batch_length_bytes", "sha512_batch.cuh", "w[15] = len << 3;", "w[15] = len;", RSA),
     M("sha512_batch_iv", "sha512_batch.cuh", "0x5be0cd19137e2179ull", "0x47b5481dbefa4fa4ull", RSA),
