@@ -278,16 +278,44 @@ class Engine:
         vp = C.c_void_p
         self._check(self._lib.sbv_sha512_batch(self._h, C.c_size_t(n), vp(msgs), vp(off), vp(digest_out)), "sbv_sha512_batch")
 
+    @staticmethod
+    def _rsa_keys(modulus, pub_exp, key_slot):
+        """The key arrays of an RSA call by their _ptr parameter names, and the item count they give: key_slot (registered), or
+        modulus and pub_exp."""
+        if key_slot is not None:
+            key_slot = np.ascontiguousarray(key_slot, dtype=np.uint32)
+            return {"key_slot": key_slot}, key_slot.size
+        pub_exp = np.ascontiguousarray(pub_exp, dtype=np.uint32)
+        return {"modulus": _u8(modulus), "pub_exp": pub_exp}, pub_exp.size
+
+    def _rsa_digests(self, ptr, digest, sig, out, modulus=None, pub_exp=None, key_slot=None, **scalars):
+        """The numpy form of the RSA calls over supplied digests: n = the keys' item count, k = the bytes per signature, and
+        ptr (the call's _ptr form) given every array by keyword with the call's scalars.  Returns the verdicts (into out)."""
+        keys, n = self._rsa_keys(modulus, pub_exp, key_slot)
+        sig, digest = _u8(sig), _u8(digest)
+        ok = out if out is not None else np.zeros(n, np.uint8)
+        ptr(mod_bytes=sig.size // n if n else 256, n=n, digest=digest.ctypes.data, sig=sig.ctypes.data, ok=ok.ctypes.data,
+            **{name: a.ctypes.data for name, a in keys.items()}, **scalars)
+        return ok
+
+    def _rsa_messages(self, ptr, hash, msgs, off, sig, want_digest, modulus=None, pub_exp=None, key_slot=None, **scalars):
+        """The numpy form of the RSA calls that hash on the device: msgs concatenated with off[n+1] byte offsets, the rest as
+        in _rsa_digests.  Returns the verdicts, and the n x hLen digests too with want_digest."""
+        msgs = _u8(msgs if len(msgs) else np.zeros(1, np.uint8))
+        off = np.ascontiguousarray(off, dtype=np.uint64)
+        keys, _ = self._rsa_keys(modulus, pub_exp, key_slot)
+        sig = _u8(sig)
+        n = off.size - 1
+        ok = np.zeros(n, np.uint8)
+        dig = np.zeros((n, HASH_BYTES[hash]), np.uint8) if want_digest else None
+        ptr(mod_bytes=sig.size // n if n else 256, hash=hash, n=n, msgs=msgs.ctypes.data, off=off.ctypes.data, sig=sig.ctypes.data,
+            digest_out=dig.ctypes.data if want_digest else 0, ok=ok.ctypes.data, **{name: a.ctypes.data for name, a in keys.items()}, **scalars)
+        return (ok, dig) if want_digest else ok
+
     def rsa_verify_batch(self, hash, digest, sig, modulus, pub_exp, out=None) -> np.ndarray:
         """RSA PKCS #1 v1.5 (Go crypto/rsa.VerifyPKCS1v15) over supplied digests: hash in {SHA256, SHA384, SHA512};
         digest = n x hLen bytes, sig and modulus = n x k bytes big-endian (k = 256, 384 or 512), pub_exp = n uint32."""
-        pub_exp = np.ascontiguousarray(pub_exp, dtype=np.uint32)
-        n = pub_exp.size
-        sig, modulus, digest = _u8(sig), _u8(modulus), _u8(digest)
-        k = sig.size // n if n else 256
-        ok = out if out is not None else np.zeros(n, np.uint8)
-        self.rsa_verify_batch_ptr(k, hash, n, digest.ctypes.data, sig.ctypes.data, modulus.ctypes.data, pub_exp.ctypes.data, ok.ctypes.data)
-        return ok
+        return self._rsa_digests(self.rsa_verify_batch_ptr, digest, sig, out, hash=hash, modulus=modulus, pub_exp=pub_exp)
 
     def rsa_verify_batch_ptr(self, mod_bytes, hash, n, digest, sig, modulus, pub_exp, ok):
         """Raw host pointers (ints) — used with pinned buffers."""
@@ -298,17 +326,7 @@ class Engine:
     def rsa_hash_verify_batch(self, hash, msgs, off, sig, modulus, pub_exp, want_digest=False):
         """rsa_verify_batch with H = hash(M) computed on the device; msgs concatenated with off[n+1] byte offsets.  Returns
         the verdicts, and the n x hLen digests too with want_digest."""
-        msgs = _u8(msgs if len(msgs) else np.zeros(1, np.uint8))
-        off = np.ascontiguousarray(off, dtype=np.uint64)
-        pub_exp = np.ascontiguousarray(pub_exp, dtype=np.uint32)
-        sig, modulus = _u8(sig), _u8(modulus)
-        n = off.size - 1
-        k = sig.size // n if n else 256
-        ok = np.zeros(n, np.uint8)
-        dig = np.zeros((n, HASH_BYTES[hash]), np.uint8) if want_digest else None
-        self.rsa_hash_verify_batch_ptr(k, hash, n, msgs.ctypes.data, off.ctypes.data, sig.ctypes.data, modulus.ctypes.data, pub_exp.ctypes.data,
-                                       dig.ctypes.data if want_digest else 0, ok.ctypes.data)
-        return (ok, dig) if want_digest else ok
+        return self._rsa_messages(self.rsa_hash_verify_batch_ptr, hash, msgs, off, sig, want_digest, modulus=modulus, pub_exp=pub_exp)
 
     def rsa_hash_verify_batch_ptr(self, mod_bytes, hash, n, msgs, off, sig, modulus, pub_exp, digest_out, ok):
         """Raw host pointers (ints; digest_out may be 0) — used with pinned buffers."""
@@ -319,14 +337,7 @@ class Engine:
     def rsa_pss_verify_batch(self, hash, salt_len, digest, sig, modulus, pub_exp, out=None) -> np.ndarray:
         """RSA-PSS (Go crypto/rsa.VerifyPSS, MGF1 over the same hash) over supplied digests: salt_len = PSS_SALT_EQUALS_HASH,
         PSS_SALT_AUTO or the exact salt length; the other arguments as in rsa_verify_batch."""
-        pub_exp = np.ascontiguousarray(pub_exp, dtype=np.uint32)
-        n = pub_exp.size
-        sig, modulus, digest = _u8(sig), _u8(modulus), _u8(digest)
-        k = sig.size // n if n else 256
-        ok = out if out is not None else np.zeros(n, np.uint8)
-        self.rsa_pss_verify_batch_ptr(k, hash, salt_len, n, digest.ctypes.data, sig.ctypes.data, modulus.ctypes.data, pub_exp.ctypes.data,
-                                      ok.ctypes.data)
-        return ok
+        return self._rsa_digests(self.rsa_pss_verify_batch_ptr, digest, sig, out, hash=hash, salt_len=salt_len, modulus=modulus, pub_exp=pub_exp)
 
     def rsa_pss_verify_batch_ptr(self, mod_bytes, hash, salt_len, n, digest, sig, modulus, pub_exp, ok):
         """Raw host pointers (ints) — used with pinned buffers."""
@@ -337,17 +348,8 @@ class Engine:
     def rsa_pss_hash_verify_batch(self, hash, salt_len, msgs, off, sig, modulus, pub_exp, want_digest=False):
         """rsa_pss_verify_batch with H = hash(M) computed on the device; msgs concatenated with off[n+1] byte offsets.
         Returns the verdicts, and the n x hLen digests too with want_digest."""
-        msgs = _u8(msgs if len(msgs) else np.zeros(1, np.uint8))
-        off = np.ascontiguousarray(off, dtype=np.uint64)
-        pub_exp = np.ascontiguousarray(pub_exp, dtype=np.uint32)
-        sig, modulus = _u8(sig), _u8(modulus)
-        n = off.size - 1
-        k = sig.size // n if n else 256
-        ok = np.zeros(n, np.uint8)
-        dig = np.zeros((n, HASH_BYTES[hash]), np.uint8) if want_digest else None
-        self.rsa_pss_hash_verify_batch_ptr(k, hash, salt_len, n, msgs.ctypes.data, off.ctypes.data, sig.ctypes.data, modulus.ctypes.data,
-                                           pub_exp.ctypes.data, dig.ctypes.data if want_digest else 0, ok.ctypes.data)
-        return (ok, dig) if want_digest else ok
+        return self._rsa_messages(self.rsa_pss_hash_verify_batch_ptr, hash, msgs, off, sig, want_digest, salt_len=salt_len, modulus=modulus,
+                                  pub_exp=pub_exp)
 
     def rsa_pss_hash_verify_batch_ptr(self, mod_bytes, hash, salt_len, n, msgs, off, sig, modulus, pub_exp, digest_out, ok):
         """Raw host pointers (ints; digest_out may be 0) — used with pinned buffers."""
@@ -373,13 +375,7 @@ class Engine:
     def rsa_verify_registered(self, hash, key_slot, digest, sig, out=None) -> np.ndarray:
         """rsa_verify_batch with the key of item i taken from registry slot key_slot[i] (rsa_set_keys); sig = n x k bytes,
         k the call's modulus size (a slot of another size rejects)."""
-        key_slot = np.ascontiguousarray(key_slot, dtype=np.uint32)
-        n = key_slot.size
-        sig, digest = _u8(sig), _u8(digest)
-        k = sig.size // n if n else 256
-        ok = out if out is not None else np.zeros(n, np.uint8)
-        self.rsa_verify_registered_ptr(k, hash, n, key_slot.ctypes.data, digest.ctypes.data, sig.ctypes.data, ok.ctypes.data)
-        return ok
+        return self._rsa_digests(self.rsa_verify_registered_ptr, digest, sig, out, hash=hash, key_slot=key_slot)
 
     def rsa_verify_registered_ptr(self, mod_bytes, hash, n, key_slot, digest, sig, ok):
         """Raw host pointers (ints) — used with pinned buffers."""
@@ -390,17 +386,7 @@ class Engine:
     def rsa_hash_verify_registered(self, hash, msgs, off, key_slot, sig, want_digest=False):
         """rsa_verify_registered with H = hash(M) computed on the device; msgs concatenated with off[n+1] byte offsets.
         Returns the verdicts, and the n x hLen digests too with want_digest."""
-        msgs = _u8(msgs if len(msgs) else np.zeros(1, np.uint8))
-        off = np.ascontiguousarray(off, dtype=np.uint64)
-        key_slot = np.ascontiguousarray(key_slot, dtype=np.uint32)
-        sig = _u8(sig)
-        n = off.size - 1
-        k = sig.size // n if n else 256
-        ok = np.zeros(n, np.uint8)
-        dig = np.zeros((n, HASH_BYTES[hash]), np.uint8) if want_digest else None
-        self.rsa_hash_verify_registered_ptr(k, hash, n, msgs.ctypes.data, off.ctypes.data, key_slot.ctypes.data, sig.ctypes.data,
-                                            dig.ctypes.data if want_digest else 0, ok.ctypes.data)
-        return (ok, dig) if want_digest else ok
+        return self._rsa_messages(self.rsa_hash_verify_registered_ptr, hash, msgs, off, sig, want_digest, key_slot=key_slot)
 
     def rsa_hash_verify_registered_ptr(self, mod_bytes, hash, n, msgs, off, key_slot, sig, digest_out, ok):
         """Raw host pointers (ints; digest_out may be 0) — used with pinned buffers."""
@@ -410,13 +396,7 @@ class Engine:
 
     def rsa_pss_verify_registered(self, hash, salt_len, key_slot, digest, sig, out=None) -> np.ndarray:
         """rsa_pss_verify_batch with the key of item i taken from registry slot key_slot[i] (rsa_set_keys)."""
-        key_slot = np.ascontiguousarray(key_slot, dtype=np.uint32)
-        n = key_slot.size
-        sig, digest = _u8(sig), _u8(digest)
-        k = sig.size // n if n else 256
-        ok = out if out is not None else np.zeros(n, np.uint8)
-        self.rsa_pss_verify_registered_ptr(k, hash, salt_len, n, key_slot.ctypes.data, digest.ctypes.data, sig.ctypes.data, ok.ctypes.data)
-        return ok
+        return self._rsa_digests(self.rsa_pss_verify_registered_ptr, digest, sig, out, hash=hash, salt_len=salt_len, key_slot=key_slot)
 
     def rsa_pss_verify_registered_ptr(self, mod_bytes, hash, salt_len, n, key_slot, digest, sig, ok):
         """Raw host pointers (ints) — used with pinned buffers."""
@@ -427,17 +407,7 @@ class Engine:
     def rsa_pss_hash_verify_registered(self, hash, salt_len, msgs, off, key_slot, sig, want_digest=False):
         """rsa_pss_verify_registered with H = hash(M) computed on the device; msgs concatenated with off[n+1] byte offsets.
         Returns the verdicts, and the n x hLen digests too with want_digest."""
-        msgs = _u8(msgs if len(msgs) else np.zeros(1, np.uint8))
-        off = np.ascontiguousarray(off, dtype=np.uint64)
-        key_slot = np.ascontiguousarray(key_slot, dtype=np.uint32)
-        sig = _u8(sig)
-        n = off.size - 1
-        k = sig.size // n if n else 256
-        ok = np.zeros(n, np.uint8)
-        dig = np.zeros((n, HASH_BYTES[hash]), np.uint8) if want_digest else None
-        self.rsa_pss_hash_verify_registered_ptr(k, hash, salt_len, n, msgs.ctypes.data, off.ctypes.data, key_slot.ctypes.data, sig.ctypes.data,
-                                                dig.ctypes.data if want_digest else 0, ok.ctypes.data)
-        return (ok, dig) if want_digest else ok
+        return self._rsa_messages(self.rsa_pss_hash_verify_registered_ptr, hash, msgs, off, sig, want_digest, salt_len=salt_len, key_slot=key_slot)
 
     def rsa_pss_hash_verify_registered_ptr(self, mod_bytes, hash, salt_len, n, msgs, off, key_slot, sig, digest_out, ok):
         """Raw host pointers (ints; digest_out may be 0) — used with pinned buffers."""

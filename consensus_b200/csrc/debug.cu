@@ -153,10 +153,9 @@ extern "C" int sbv_debug_rsa(sbv_engine *e, uint32_t mod_bytes, int op, size_t n
     CU(e, cudaMemcpyAsync(db, b, bytes, cudaMemcpyHostToDevice, d.stream));
     CU(e, cudaMemcpyAsync(dmod, mod, bytes, cudaMemcpyHostToDevice, d.stream));
     CU(e, cudaMemcpyAsync(dexp, exp, n * 4, cudaMemcpyHostToDevice, d.stream));
-    const uint32_t blocks = (uint32_t)((n * RSA_GROUP + 127) / 128);
-    if (mod_bytes == 256) k_rsa_debug<4><<<blocks, 128, 0, d.stream>>>(op, (uint32_t)n, da, db, dmod, dexp, dout, daux);
-    else if (mod_bytes == 384) k_rsa_debug<6><<<blocks, 128, 0, d.stream>>>(op, (uint32_t)n, da, db, dmod, dexp, dout, daux);
-    else k_rsa_debug<8><<<blocks, 128, 0, d.stream>>>(op, (uint32_t)n, da, db, dmod, dexp, dout, daux);
+    rsa_nl(mod_bytes, [&](auto nl) {
+        k_rsa_debug<decltype(nl)::value><<<rsa_grid(n, RSA_GROUP), RSA_BLOCK, 0, d.stream>>>(op, (uint32_t)n, da, db, dmod, dexp, dout, daux);
+    });
     CU(e, cudaGetLastError());
     CU(e, cudaMemcpyAsync(out, dout, bytes, cudaMemcpyDeviceToHost, d.stream));
     CU(e, cudaMemcpyAsync(aux, daux, n * 4, cudaMemcpyDeviceToHost, d.stream));
@@ -468,7 +467,7 @@ extern "C" int sbv_debug_key_cache_sets(sbv_engine *e, int device_index, uint8_t
 // most 264).  SBV_ERR_ARG for a slot outside the registry.
 extern "C" int sbv_debug_rsa_key(sbv_engine *e, uint32_t slot, uint32_t *out) {
     if (!e || !out || e->devs.empty()) return SBV_ERR_ARG;
-    std::shared_lock<std::shared_mutex> reg(e->ed_reg_mu);
+    std::shared_lock<std::shared_mutex> reg(e->registry_mu);
     std::lock_guard<std::mutex> lk(e->mu);
     Dev &d = e->devs[0];
     if (slot >= d.rsa_n_slots) return SBV_ERR_ARG;

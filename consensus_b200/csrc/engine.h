@@ -14,6 +14,7 @@
 
 #include "../../include/sbv.h"
 #include "ops.h"
+#include "rsa_shard.h"
 
 constexpr int SBV_LANES = 6;    // concurrent host-buffer calls per engine
 constexpr int SBV_SCRATCH = 8;  // scratch sets per device (> SBV_LANES + 1: a launch may be held open per lane)
@@ -141,10 +142,10 @@ struct sbv_engine {
     std::vector<Dev> devs;
     std::mutex mu;       // kernel enqueue + workspace growth
     std::mutex err_mu;   // last-error string
-    // the Ed25519 and RSA registries: sbv_ed25519_set_keys and sbv_rsa_set_keys hold it exclusively, the registered calls
-    // of both families shared for the enqueue of all their shards, so every shard of one call reads the same registry
-    // (taken before mu, never inside it)
-    std::shared_mutex ed_reg_mu;
+    // the Ed25519 and RSA registries: sbv_ed25519_set_keys and sbv_rsa_set_keys hold it exclusively (replace_registry), the
+    // registered calls of both families shared for the enqueue of all their shards, so every shard of one call reads the
+    // same registry (taken before mu, never inside it)
+    std::shared_mutex registry_mu;
     std::condition_variable lane_cv;
     bool lane_busy[SBV_LANES] = {};
     std::string err;
@@ -329,26 +330,14 @@ int sbv_launch_sha384(sbv_engine *e, size_t n, const uint8_t *d_msgs, const uint
 // the same with SHA-512 (sha512_batch.cuh: k_sha512): 64 bytes per message into d_digest
 int sbv_launch_sha512(sbv_engine *e, size_t n, const uint8_t *d_msgs, const uint64_t *d_off, uint64_t base, uint8_t *d_digest, uint32_t *d_perm,
                       cudaStream_t st);
-// k_rsa_verify over n items of mod_bytes (256, 384 or 512) bytes each: d_sig and d_mod n * mod_bytes bytes (big-endian),
-// d_exp n words, d_digest n * hLen bytes (hash 0 / 1 / 2: SHA-256 / SHA-384 / SHA-512), verdicts into d_ok.  Every pointer
-// 4-byte aligned.
-int sbv_launch_rsa(sbv_engine *e, uint32_t mod_bytes, uint8_t hash, size_t n, const uint8_t *d_sig, const uint8_t *d_mod, const uint32_t *d_exp,
-                   const uint8_t *d_digest, uint8_t *d_ok, cudaStream_t st);
-// RSA-PSS (rsa_pss.cuh): k_rsa_em over the same buffers, EM written over d_sig, then k_rsa_pss for the hash tag with
-// salt_len as in sbv_rsa_pss_verify_batch (>= -1); verdicts into d_ok.  Two launches.
-int sbv_launch_rsa_pss(sbv_engine *e, uint32_t mod_bytes, uint8_t hash, int32_t salt_len, size_t n, uint8_t *d_sig, const uint8_t *d_mod,
-                       const uint32_t *d_exp, const uint8_t *d_digest, uint8_t *d_ok, cudaStream_t st);
+// The kernels of one RSA shard (rsa_keyed.cuh: rsa_launch_shard) on st, both paddings and both key sources; every pointer
+// 4-byte aligned.  With a slot per item the caller holds the registry (registry_mu shared) while enqueuing.
+int sbv_launch_rsa(sbv_engine *e, const sbv::RsaShard &shard, cudaStream_t st);
 // registered RSA keys (rsa_keyed.cuh).  sbv_rsa_keys_build: caller holds e->mu; waits for the device to drain, frees the old
 // registry of device d and builds one from the n keys (mod_bytes[i] in {256, 384, 512}, checked by the caller; the moduli
 // concatenated, big-endian); a fault leaves d's registry empty.
 int sbv_rsa_keys_build(sbv_engine *e, Dev &d, size_t n, const uint32_t *mod_bytes, const uint8_t *modulus, const uint32_t *pub_exp);
 void sbv_rsa_keys_free(Dev &d);
-// sbv_launch_rsa and sbv_launch_rsa_pss with the key of each item read from device d's RSA registry by slot (d_slot, n
-// words) in place of d_mod and d_exp; the same launches.  The caller holds the registry (ed_reg_mu shared) while enqueuing.
-int sbv_launch_rsa_reg(sbv_engine *e, Dev &d, uint32_t mod_bytes, uint8_t hash, size_t n, const uint8_t *d_sig, const uint32_t *d_slot,
-                       const uint8_t *d_digest, uint8_t *d_ok, cudaStream_t st);
-int sbv_launch_rsa_pss_reg(sbv_engine *e, Dev &d, uint32_t mod_bytes, uint8_t hash, int32_t salt_len, size_t n, uint8_t *d_sig, const uint32_t *d_slot,
-                           const uint8_t *d_digest, uint8_t *d_ok, cudaStream_t st);
 // mixed_hash.cuh: k_mix_alg over the n uploaded tags of a mixed shard (tags 3 and 4 to their family, flags into d_alg)
 int sbv_launch_mix_alg(sbv_engine *e, size_t n, uint8_t *d_tag, uint8_t *d_alg, cudaStream_t st);
 // mixed_hash.cuh: k_sha2_sel over the n items of one family (d_idx: their shard indices, d_alg: the shard's flags), dlen

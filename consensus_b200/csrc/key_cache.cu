@@ -82,7 +82,7 @@ int kca_alloc(sbv_engine *e, Dev &d, int s, size_t cap) {
 // does: the registry lock, the engine lock, then a drain of every device, so no launch still reads or fills the old maps.
 // A fault frees them all.
 int reserve(sbv_engine *e, const size_t cap[3], bool evicting) {
-    std::unique_lock<std::shared_mutex> reg(e->ed_reg_mu);
+    std::unique_lock<std::shared_mutex> reg(e->registry_mu);
     std::lock_guard<std::mutex> lk(e->mu);
     for (Dev &d : e->devs) {
         CU(e, cudaSetDevice(d.ordinal));

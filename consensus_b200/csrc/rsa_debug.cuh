@@ -13,6 +13,7 @@
 #include <stddef.h>
 
 #include "rsa.cuh"
+#include "rsa_shard.h"
 
 namespace sbv {
 
@@ -21,7 +22,7 @@ enum RsaDebugOp { RSA_DBG_MONT = 0, RSA_DBG_R2 = 1, RSA_DBG_SUB = 2, RSA_DBG_RES
 // The calls the hook runs: a modulus size of rsa.cuh, a known op, every buffer present and n < 2^31.
 inline bool rsa_debug_args_ok(uint32_t mod_bytes, int op, size_t n, const void *a, const void *b, const void *mod, const void *exp, const void *out,
                               const void *aux) {
-    return (mod_bytes == 256 || mod_bytes == 384 || mod_bytes == 512) && op >= RSA_DBG_MONT && op <= RSA_DBG_POW && a && b && mod && exp && out && aux &&
+    return rsa_size_ok(mod_bytes) && op >= RSA_DBG_MONT && op <= RSA_DBG_POW && a && b && mod && exp && out && aux &&
            n < ((size_t)1 << 31);
 }
 

@@ -25,6 +25,7 @@
 
 #include "rsa.cuh"
 #include "rsa_pss.cuh"
+#include "rsa_shard.h"
 
 namespace sbv {
 
@@ -179,6 +180,67 @@ inline uint64_t rsa_reg_layout(size_t n, const uint32_t *mod_bytes, uint64_t *mo
     }
     first[3] = m;
     return t;
+}
+
+// ---- the launch plan of the RSA kernels, for the engine and the CPU simulation alike ----
+// launch(kernel, lanes, items, args...) runs kernel(args...) over rsa_grid(items, lanes) blocks of RSA_BLOCK threads and
+// returns 0 or an error code; lanes = RSA_GROUP for the kernels of a group per item, 1 for one thread per item.
+
+// The shards the plan launches: a size and a hash tag of the set, and for PSS a salt length >= -1.
+inline bool rsa_shard_ok(const RsaShard &s) {
+    return rsa_size_ok(s.k) && rsa_hash_ok(s.hash) && (s.pad == RsaPad::pkcs1 || s.salt_len >= PSS_SALT_EQUALS_HASH);
+}
+
+// The PSS decoding of a shard alone: k_rsa_pss (with a slot per item k_rsa_pss_reg) over the EMs in s.sig, for the items
+// s.ok accepts.  -1 with nothing launched for a shard rsa_shard_ok refuses.
+template <class Launch>
+int rsa_launch_pss_decode(const RsaShard &s, Launch &&launch) {
+    if (!rsa_shard_ok(s)) return -1;
+    if (s.n == 0) return 0;
+    const uint32_t n = (uint32_t)s.n;
+    int rc = 0;
+    rsa_h(s.hash, [&](auto h) {
+        constexpr int H = decltype(h)::value;
+        if (s.slot) rc = launch(k_rsa_pss_reg<H>, 1, s.n, n, s.k, s.salt_len, s.sig, s.slot, s.rec, s.digest, s.ok);
+        else rc = launch(k_rsa_pss<H>, 1, s.n, n, s.k, s.salt_len, s.sig, s.mod, s.digest, s.ok);
+    });
+    return rc;
+}
+
+// The kernels of one shard: PKCS #1 v1.5 k_rsa_verify; PSS k_rsa_em, which writes EM over s.sig, then the decoding.  With a
+// slot per item, their _reg forms.  -1 with nothing launched for a shard rsa_shard_ok refuses; n = 0 launches nothing.
+template <class Launch>
+int rsa_launch_shard(const RsaShard &s, Launch &&launch) {
+    if (!rsa_shard_ok(s)) return -1;
+    if (s.n == 0) return 0;
+    const bool pss = s.pad == RsaPad::pss, reg = s.slot != nullptr;
+    const uint32_t n = (uint32_t)s.n;
+    int rc = 0;
+    rsa_nl(s.k, [&](auto nl) {
+        constexpr int NL = decltype(nl)::value;
+        if (!pss && reg) rc = launch(k_rsa_verify_reg<NL>, RSA_GROUP, s.n, n, s.hash, s.sig, s.slot, s.nslots, s.rec, s.pool, s.digest, s.ok);
+        else if (!pss) rc = launch(k_rsa_verify<NL>, RSA_GROUP, s.n, n, s.hash, s.sig, s.mod, s.exp, s.digest, s.ok);
+        else if (reg) rc = launch(k_rsa_em_reg<NL>, RSA_GROUP, s.n, n, s.sig, s.slot, s.nslots, s.rec, s.pool, s.ok);
+        else rc = launch(k_rsa_em<NL>, RSA_GROUP, s.n, n, s.sig, s.mod, s.exp, s.ok);
+    });
+    if (rc || !pss) return rc;
+    return rsa_launch_pss_decode(s, launch);
+}
+
+// The registry build: one k_rsa_kprep launch per modulus size present, over the slots of that size (slots, first and
+// mod_off as rsa_reg_layout wrote them; mods and exps the registered moduli and exponents).
+template <class Launch>
+int rsa_launch_kprep(const uint32_t *slots, const size_t (&first)[4], const uint8_t *mods, const uint64_t *mod_off, const uint32_t *exps, uint4 *rec,
+                     uint32_t *pool, Launch &&launch) {
+    int rc = 0;
+    for (int c = 0; c < 3 && !rc; c++) {
+        const uint32_t cnt = (uint32_t)(first[c + 1] - first[c]);
+        if (cnt == 0) continue;
+        rsa_nl(256 + 128 * c, [&](auto nl) {
+            rc = launch(k_rsa_kprep<decltype(nl)::value>, RSA_GROUP, cnt, cnt, slots + first[c], mods, mod_off, exps, rec, pool);
+        });
+    }
+    return rc;
 }
 
 }  // namespace sbv

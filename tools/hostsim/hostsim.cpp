@@ -909,15 +909,21 @@ extern "C" int hs_sha512(size_t n, const uint8_t *msgs, const uint64_t *off, uin
     return 0;
 }
 
-// k_rsa_verify over n items of k = 64 * nl bytes, two groups of 16 lanes per simulated warp, in lockstep
+// The launch of rsa_keyed.cuh's plan in the simulation: blocks of RSA_BLOCK threads, in lockstep where a group of lanes
+// shares an item.
+static const auto hs_rsa_launch = [](auto kernel, uint32_t lanes, size_t items, auto... args) {
+    if (lanes > 1) run_grid_lockstep(rsa_grid(items, lanes), RSA_BLOCK, [&] { kernel(args...); });
+    else run_grid(rsa_grid(items, lanes), RSA_BLOCK, [&] { kernel(args...); });
+    return 0;
+};
+
+// sbv_launch_rsa over n PKCS #1 v1.5 items of k = 64 * nl bytes with keys per item.  -1 (and nothing written) for a size
+// or hash tag outside the set.
 extern "C" int hs_rsa_verify(int nl, size_t n, uint32_t hash, const uint8_t *sig, const uint8_t *mod, const uint32_t *pub_exp, const uint8_t *digest,
                              uint8_t *ok) {
-    const unsigned blocks = (unsigned)((n * RSA_GROUP + 31) / 32);
-    if (nl == 4) run_grid_lockstep(blocks, 32, [&] { k_rsa_verify<4>((uint32_t)n, hash, sig, mod, pub_exp, digest, ok); });
-    else if (nl == 6) run_grid_lockstep(blocks, 32, [&] { k_rsa_verify<6>((uint32_t)n, hash, sig, mod, pub_exp, digest, ok); });
-    else if (nl == 8) run_grid_lockstep(blocks, 32, [&] { k_rsa_verify<8>((uint32_t)n, hash, sig, mod, pub_exp, digest, ok); });
-    else return -1;
-    return 0;
+    if (nl <= 0 || nl > 8) return -1;
+    // sig is only read with PKCS #1 v1.5
+    return rsa_launch_shard(RsaShard{64u * nl, hash, RsaPad::pkcs1, 0, n, const_cast<uint8_t *>(sig), digest, ok, mod, pub_exp}, hs_rsa_launch);
 }
 
 // The arithmetic of rsa.cuh item by item: k_rsa_debug (rsa_debug.cuh) as libsbv.so's sbv_debug_rsa runs it, in blocks of
@@ -925,10 +931,7 @@ extern "C" int hs_rsa_verify(int nl, size_t n, uint32_t hash, const uint8_t *sig
 extern "C" int hs_rsa_debug(uint32_t mod_bytes, int op, size_t n, const uint8_t *a, const uint8_t *b, const uint8_t *mod, const uint32_t *exp,
                             uint8_t *out, uint32_t *aux) {
     if (!rsa_debug_args_ok(mod_bytes, op, n, a, b, mod, exp, out, aux)) return -1;
-    const unsigned blocks = (unsigned)((n * RSA_GROUP + 127) / 128);
-    if (mod_bytes == 256) run_grid_lockstep(blocks, 128, [&] { k_rsa_debug<4>(op, (uint32_t)n, a, b, mod, exp, out, aux); });
-    else if (mod_bytes == 384) run_grid_lockstep(blocks, 128, [&] { k_rsa_debug<6>(op, (uint32_t)n, a, b, mod, exp, out, aux); });
-    else run_grid_lockstep(blocks, 128, [&] { k_rsa_debug<8>(op, (uint32_t)n, a, b, mod, exp, out, aux); });
+    rsa_nl(mod_bytes, [&](auto nl) { hs_rsa_launch(k_rsa_debug<decltype(nl)::value>, RSA_GROUP, n, op, (uint32_t)n, a, b, mod, exp, out, aux); });
     return 0;
 }
 
@@ -950,82 +953,49 @@ extern "C" int hs_rsa_op(int nl, int op, size_t n, const uint8_t *a, const uint8
     return rc;
 }
 
-// sbv_launch_rsa_pss with the same arguments: k_rsa_em in lockstep, in blocks of 128 threads (EM written over sig), then
-// k_rsa_pss one thread at a time.  -1 (and nothing written) for a size or hash tag outside the set or salt_len < -1.
+// sbv_launch_rsa over n PSS items with keys per item: k_rsa_em in lockstep (EM written over sig), then k_rsa_pss one thread
+// at a time.  -1 (and nothing written) for a size or hash tag outside the set or salt_len < -1.
 extern "C" int hs_rsa_pss_verify(uint32_t mod_bytes, uint8_t hash, int32_t salt_len, size_t n, uint8_t *sig, const uint8_t *mod, const uint32_t *pub_exp,
                                  const uint8_t *digest, uint8_t *ok) {
-    if ((mod_bytes != 256 && mod_bytes != 384 && mod_bytes != 512) || hash > 2 || salt_len < PSS_SALT_EQUALS_HASH) return -1;
-    const unsigned blocks = (unsigned)((n * RSA_GROUP + 127) / 128), tblocks = (unsigned)((n + 127) / 128);
-    if (mod_bytes == 256) run_grid_lockstep(blocks, 128, [&] { k_rsa_em<4>((uint32_t)n, sig, mod, pub_exp, ok); });
-    else if (mod_bytes == 384) run_grid_lockstep(blocks, 128, [&] { k_rsa_em<6>((uint32_t)n, sig, mod, pub_exp, ok); });
-    else run_grid_lockstep(blocks, 128, [&] { k_rsa_em<8>((uint32_t)n, sig, mod, pub_exp, ok); });
-    if (hash == 0) run_grid(tblocks, 128, [&] { k_rsa_pss<0>((uint32_t)n, mod_bytes, salt_len, sig, mod, digest, ok); });
-    else if (hash == 1) run_grid(tblocks, 128, [&] { k_rsa_pss<1>((uint32_t)n, mod_bytes, salt_len, sig, mod, digest, ok); });
-    else run_grid(tblocks, 128, [&] { k_rsa_pss<2>((uint32_t)n, mod_bytes, salt_len, sig, mod, digest, ok); });
-    return 0;
+    return rsa_launch_shard(RsaShard{mod_bytes, hash, RsaPad::pss, salt_len, n, sig, digest, ok, mod, pub_exp}, hs_rsa_launch);
 }
 
-// k_rsa_pss alone, one thread at a time, over EMs given in sig (ok: the key and range verdicts k_rsa_em would write, ANDed
-// with the PSS verdicts): the decoding checked item by item without the exponentiation.
+// k_rsa_pss alone (rsa_launch_pss_decode), one thread at a time, over EMs given in em (ok: the key and range verdicts
+// k_rsa_em would write, ANDed with the PSS verdicts): the decoding checked item by item without the exponentiation.
 extern "C" int hs_rsa_pss_decode(uint32_t mod_bytes, uint8_t hash, int32_t salt_len, size_t n, uint8_t *em, const uint8_t *mod, const uint8_t *digest,
                                  uint8_t *ok) {
-    if ((mod_bytes != 256 && mod_bytes != 384 && mod_bytes != 512) || hash > 2 || salt_len < PSS_SALT_EQUALS_HASH) return -1;
-    const unsigned tblocks = (unsigned)((n + 127) / 128);
-    if (hash == 0) run_grid(tblocks, 128, [&] { k_rsa_pss<0>((uint32_t)n, mod_bytes, salt_len, em, mod, digest, ok); });
-    else if (hash == 1) run_grid(tblocks, 128, [&] { k_rsa_pss<1>((uint32_t)n, mod_bytes, salt_len, em, mod, digest, ok); });
-    else run_grid(tblocks, 128, [&] { k_rsa_pss<2>((uint32_t)n, mod_bytes, salt_len, em, mod, digest, ok); });
-    return 0;
+    return rsa_launch_pss_decode(RsaShard{mod_bytes, hash, RsaPad::pss, salt_len, n, em, digest, ok, mod}, hs_rsa_launch);
 }
 
 // ---- registered RSA keys (rsa_keyed.cuh) ----
 // The registry of sbv_rsa_set_keys from the n keys (mod_bytes[i] in {256, 384, 512}, the moduli concatenated): k_rsa_kprep
-// in lockstep, in blocks of 128 threads, one launch per size over the slots of that size, as the engine launches it.  rec:
-// 8 words per slot; pool: (sum of mod_bytes) / 2 words.  -1 (and nothing written) for a size outside the set.
+// in lockstep, one launch per size over the slots of that size (rsa_launch_kprep).  rec: 8 words per slot; pool: (sum of
+// mod_bytes) / 2 words.  -1 (and nothing written) for a size outside the set.
 extern "C" int hs_rsa_kprep(size_t n, const uint32_t *mod_bytes, const uint8_t *modulus, const uint32_t *pub_exp, uint32_t *rec, uint32_t *pool) {
     for (size_t i = 0; i < n; i++)
-        if (mod_bytes[i] != 256 && mod_bytes[i] != 384 && mod_bytes[i] != 512) return -1;
+        if (!rsa_size_ok(mod_bytes[i])) return -1;
     std::vector<uint64_t> off(n);
     std::vector<uint32_t> slots(n);
     size_t first[4];
     rsa_reg_layout(n, mod_bytes, off.data(), slots.data(), first);
-    uint4 *r = reinterpret_cast<uint4 *>(rec);
-    for (int c = 0; c < 3; c++) {
-        const uint32_t cnt = (uint32_t)(first[c + 1] - first[c]);
-        if (cnt == 0) continue;
-        const unsigned blocks = (unsigned)(((size_t)cnt * RSA_GROUP + 127) / 128);
-        const uint32_t *sl = slots.data() + first[c];
-        if (c == 0) run_grid_lockstep(blocks, 128, [&] { k_rsa_kprep<4>(cnt, sl, modulus, off.data(), pub_exp, r, pool); });
-        else if (c == 1) run_grid_lockstep(blocks, 128, [&] { k_rsa_kprep<6>(cnt, sl, modulus, off.data(), pub_exp, r, pool); });
-        else run_grid_lockstep(blocks, 128, [&] { k_rsa_kprep<8>(cnt, sl, modulus, off.data(), pub_exp, r, pool); });
-    }
-    return 0;
+    return rsa_launch_kprep(slots.data(), first, modulus, off.data(), pub_exp, reinterpret_cast<uint4 *>(rec), pool, hs_rsa_launch);
 }
 
-// sbv_launch_rsa_reg with the same arguments over a registry of nslots slots (rec, pool as hs_rsa_kprep wrote them):
-// k_rsa_verify_reg in lockstep, in blocks of 128 threads.  -1 (and nothing written) for a size or hash tag outside the set.
+// sbv_launch_rsa over n PKCS #1 v1.5 items with a slot per item, over a registry of nslots slots (rec, pool as hs_rsa_kprep
+// wrote them).  -1 (and nothing written) for a size or hash tag outside the set.
 extern "C" int hs_rsa_verify_registered(uint32_t mod_bytes, uint8_t hash, size_t n, const uint8_t *sig, const uint32_t *key_slot, uint32_t nslots,
                                         const uint32_t *rec, const uint32_t *pool, const uint8_t *digest, uint8_t *ok) {
-    if ((mod_bytes != 256 && mod_bytes != 384 && mod_bytes != 512) || hash > 2) return -1;
-    const unsigned blocks = (unsigned)((n * RSA_GROUP + 127) / 128);
-    const uint4 *r = reinterpret_cast<const uint4 *>(rec);
-    if (mod_bytes == 256) run_grid_lockstep(blocks, 128, [&] { k_rsa_verify_reg<4>((uint32_t)n, hash, sig, key_slot, nslots, r, pool, digest, ok); });
-    else if (mod_bytes == 384) run_grid_lockstep(blocks, 128, [&] { k_rsa_verify_reg<6>((uint32_t)n, hash, sig, key_slot, nslots, r, pool, digest, ok); });
-    else run_grid_lockstep(blocks, 128, [&] { k_rsa_verify_reg<8>((uint32_t)n, hash, sig, key_slot, nslots, r, pool, digest, ok); });
-    return 0;
+    // sig is only read with PKCS #1 v1.5
+    return rsa_launch_shard(RsaShard{mod_bytes, hash, RsaPad::pkcs1, 0, n, const_cast<uint8_t *>(sig), digest, ok, nullptr, nullptr, key_slot, nslots,
+                                     reinterpret_cast<const uint4 *>(rec), pool},
+                            hs_rsa_launch);
 }
 
-// sbv_launch_rsa_pss_reg with the same arguments: k_rsa_em_reg in lockstep (EM written over sig), then k_rsa_pss_reg one
-// thread at a time.  -1 (and nothing written) for a size or hash tag outside the set or salt_len < -1.
+// sbv_launch_rsa over n PSS items with a slot per item: k_rsa_em_reg in lockstep (EM written over sig), then k_rsa_pss_reg
+// one thread at a time.  -1 (and nothing written) for a size or hash tag outside the set or salt_len < -1.
 extern "C" int hs_rsa_pss_verify_registered(uint32_t mod_bytes, uint8_t hash, int32_t salt_len, size_t n, uint8_t *sig, const uint32_t *key_slot,
                                             uint32_t nslots, const uint32_t *rec, const uint32_t *pool, const uint8_t *digest, uint8_t *ok) {
-    if ((mod_bytes != 256 && mod_bytes != 384 && mod_bytes != 512) || hash > 2 || salt_len < PSS_SALT_EQUALS_HASH) return -1;
-    const unsigned blocks = (unsigned)((n * RSA_GROUP + 127) / 128), tblocks = (unsigned)((n + 127) / 128);
-    const uint4 *r = reinterpret_cast<const uint4 *>(rec);
-    if (mod_bytes == 256) run_grid_lockstep(blocks, 128, [&] { k_rsa_em_reg<4>((uint32_t)n, sig, key_slot, nslots, r, pool, ok); });
-    else if (mod_bytes == 384) run_grid_lockstep(blocks, 128, [&] { k_rsa_em_reg<6>((uint32_t)n, sig, key_slot, nslots, r, pool, ok); });
-    else run_grid_lockstep(blocks, 128, [&] { k_rsa_em_reg<8>((uint32_t)n, sig, key_slot, nslots, r, pool, ok); });
-    if (hash == 0) run_grid(tblocks, 128, [&] { k_rsa_pss_reg<0>((uint32_t)n, mod_bytes, salt_len, sig, key_slot, r, digest, ok); });
-    else if (hash == 1) run_grid(tblocks, 128, [&] { k_rsa_pss_reg<1>((uint32_t)n, mod_bytes, salt_len, sig, key_slot, r, digest, ok); });
-    else run_grid(tblocks, 128, [&] { k_rsa_pss_reg<2>((uint32_t)n, mod_bytes, salt_len, sig, key_slot, r, digest, ok); });
-    return 0;
+    return rsa_launch_shard(RsaShard{mod_bytes, hash, RsaPad::pss, salt_len, n, sig, digest, ok, nullptr, nullptr, key_slot, nslots,
+                                     reinterpret_cast<const uint4 *>(rec), pool},
+                            hs_rsa_launch);
 }

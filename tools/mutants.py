@@ -413,6 +413,15 @@ CATALOGUE = [
     M("rsa_reg_ninv_of_slot0", "rsa_keyed.cuh", "rsa_pow_tail<NL>(g, s, x, n, r0.w, r1.x,", "rsa_pow_tail<NL>(g, s, x, n, rec[0].w, r1.x,", RSA_REG),
     M("rsa_reg_ntop_stored", "rsa_keyed.cuh", "valid ? 1u : 0u, hi >> 24, ninv}", "valid ? 1u : 0u, 1u, ninv}", RSA_REG),
     M("rsa_kprep_rule_lead_byte", "rsa_keyed.cuh", "hi >= (1u << 24)", "hi != 0", RSA_REG),
+    # ---------------------------------------------------------------- rsa_shard.h and rsa_keyed.cuh: the launch plan, which the engine and the simulation share
+    M("rsa_plan_hash_rotated", "rsa_shard.h",
+      "        case 0: f(std::integral_constant<int, 0>{}); return true;\n        case 1: f(std::integral_constant<int, 1>{}); return true;\n"
+      "        case 2: f(std::integral_constant<int, 2>{}); return true;",
+      "        case 0: f(std::integral_constant<int, 1>{}); return true;\n        case 1: f(std::integral_constant<int, 2>{}); return true;\n"
+      "        case 2: f(std::integral_constant<int, 0>{}); return true;", RSA_PSS + RSA_REG),
+    M("rsa_plan_group_grid_items", "rsa_shard.h", "(items * lanes + RSA_BLOCK - 1)", "(items + RSA_BLOCK - 1)", RSA + RSA_PSS + RSA_REG),
+    M("rsa_plan_pss_salt_auto", "rsa_keyed.cuh", "launch(k_rsa_pss<H>, 1, s.n, n, s.k, s.salt_len,", "launch(k_rsa_pss<H>, 1, s.n, n, s.k, PSS_SALT_AUTO,",
+      RSA_PSS),
     # ---------------------------------------------------------------- sha512_batch.cuh
     M("sha512_batch_length_bytes", "sha512_batch.cuh", "w[15] = len << 3;", "w[15] = len;", RSA),
     M("sha512_batch_iv", "sha512_batch.cuh", "0x5be0cd19137e2179ull", "0x47b5481dbefa4fa4ull", RSA),
