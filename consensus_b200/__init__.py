@@ -36,7 +36,7 @@ SYMBOLS = [
     "sbv_sha512_batch", "sbv_rsa_verify_batch", "sbv_rsa_hash_verify_batch",
     "sbv_rsa_pss_verify_batch", "sbv_rsa_pss_hash_verify_batch",
     "sbv_rsa_set_keys", "sbv_rsa_verify_registered", "sbv_rsa_hash_verify_registered", "sbv_rsa_pss_verify_registered",
-    "sbv_rsa_pss_hash_verify_registered",
+    "sbv_rsa_pss_hash_verify_registered", "sbv_rsa_verify_quorum", "sbv_rsa_pss_verify_quorum",
 ]
 
 
@@ -415,6 +415,62 @@ class Engine:
         self._check(self._lib.sbv_rsa_pss_hash_verify_registered(self._h, C.c_uint32(mod_bytes), C.c_uint8(hash), C.c_int32(salt_len), C.c_size_t(n),
                                                                  vp(msgs), vp(off), vp(key_slot), vp(sig), vp(digest_out or None), vp(ok)),
                     "sbv_rsa_pss_hash_verify_registered")
+
+    def rsa_verify_quorum(self, hash, msgs, off, key_slot, sig, sig_off, instance, sender, signer, digest_match, n_instances, threshold,
+                          self_id=None, _salt_len=None):
+        """RSA commit votes against registered keys of any mix of sizes (rsa_set_keys): vote i's message msgs[off[i]:off[i+1]]
+        is hashed on the device with `hash`, its signature sig[sig_off[i]:sig_off[i+1]] verified (PKCS #1 v1.5) under slot
+        key_slot[i] at the size its length gives (a length other than 256, 384 or 512 bytes rejects), and the verdicts counted
+        on the device; votes grouped by non-decreasing instance.  Returns (ok, valid_count, reached)."""
+        msgs = _u8(msgs if len(msgs) else np.zeros(1, np.uint8))
+        sig = _u8(sig if len(sig) else np.zeros(1, np.uint8))
+        off = np.ascontiguousarray(off, dtype=np.uint64)
+        sig_off = np.ascontiguousarray(sig_off, dtype=np.uint64)
+        key_slot = np.ascontiguousarray(key_slot, dtype=np.uint32)
+        instance = np.ascontiguousarray(instance, dtype=np.uint32)
+        sender = np.ascontiguousarray(sender, dtype=np.uint16)
+        signer = np.ascontiguousarray(signer, dtype=np.uint16)
+        digest_match = _u8(digest_match)
+        n = instance.size
+        if off.size != n + 1 or sig_off.size != n + 1 or key_slot.size != n or sender.size != n or signer.size != n or digest_match.size != n:
+            raise ValueError("off and sig_off must hold n + 1 offsets and every other column one entry per vote")
+        ok = np.zeros(n, np.uint8)
+        cnt = np.zeros(n_instances, np.uint32)
+        reached = np.zeros(n_instances, np.uint8)
+        if self_id is not None:
+            self_id = np.ascontiguousarray(self_id, dtype=np.uint16)
+        args = dict(n=n, msgs=msgs.ctypes.data, off=off.ctypes.data, key_slot=key_slot.ctypes.data, sig=sig.ctypes.data, sig_off=sig_off.ctypes.data,
+                    instance=instance.ctypes.data, sender=sender.ctypes.data, signer=signer.ctypes.data, digest_match=digest_match.ctypes.data,
+                    n_instances=n_instances, self_id=None if self_id is None else self_id.ctypes.data, threshold=threshold, ok=ok.ctypes.data,
+                    valid_count=cnt.ctypes.data, reached=reached.ctypes.data)
+        if _salt_len is None:
+            self.rsa_verify_quorum_ptr(hash, **args)
+        else:
+            self.rsa_pss_verify_quorum_ptr(hash, _salt_len, **args)
+        return ok, cnt, reached
+
+    def rsa_verify_quorum_ptr(self, hash, n, msgs, off, key_slot, sig, sig_off, instance, sender, signer, digest_match, n_instances, self_id,
+                              threshold, ok, valid_count, reached):
+        """Raw host pointers (ints; self_id may be None) — used with pinned buffers."""
+        vp = C.c_void_p
+        self._check(self._lib.sbv_rsa_verify_quorum(self._h, C.c_uint8(hash), C.c_size_t(n), vp(msgs), vp(off), vp(key_slot), vp(sig), vp(sig_off),
+                                                    vp(instance), vp(sender), vp(signer), vp(digest_match), C.c_size_t(n_instances), vp(self_id),
+                                                    C.c_uint32(threshold), vp(ok), vp(valid_count), vp(reached)), "sbv_rsa_verify_quorum")
+
+    def rsa_pss_verify_quorum(self, hash, salt_len, msgs, off, key_slot, sig, sig_off, instance, sender, signer, digest_match, n_instances,
+                              threshold, self_id=None):
+        """rsa_verify_quorum with RSA-PSS verdicts (salt_len as in rsa_pss_verify_batch)."""
+        return self.rsa_verify_quorum(hash, msgs, off, key_slot, sig, sig_off, instance, sender, signer, digest_match, n_instances, threshold,
+                                      self_id, _salt_len=salt_len)
+
+    def rsa_pss_verify_quorum_ptr(self, hash, salt_len, n, msgs, off, key_slot, sig, sig_off, instance, sender, signer, digest_match, n_instances,
+                                  self_id, threshold, ok, valid_count, reached):
+        """Raw host pointers (ints; self_id may be None) — used with pinned buffers."""
+        vp = C.c_void_p
+        self._check(self._lib.sbv_rsa_pss_verify_quorum(self._h, C.c_uint8(hash), C.c_int32(salt_len), C.c_size_t(n), vp(msgs), vp(off), vp(key_slot),
+                                                        vp(sig), vp(sig_off), vp(instance), vp(sender), vp(signer), vp(digest_match),
+                                                        C.c_size_t(n_instances), vp(self_id), C.c_uint32(threshold), vp(ok), vp(valid_count), vp(reached)),
+                    "sbv_rsa_pss_verify_quorum")
 
     def hash384_verify_batch_ptr(self, curve, n, msgs, off, r, s, qx, qy, digest_out, ok):
         """Raw host pointers (ints; digest_out may be 0) — used with pinned buffers."""

@@ -295,6 +295,23 @@ size_t sbv_mix_carve(uint8_t *base, size_t n, const uint32_t m[3], uint64_t byte
 // the families
 int sbv_launch_mix_split(sbv_engine *e, const MixBufs &b, size_t n, const uint32_t m[3], const uint8_t *d_msgs, const uint64_t *d_off, uint64_t base,
                          cudaStream_t st);
+// The device scratch of a shard of n RSA votes (engine_rsa.inc: stage_rsa_votes), m[f] of family f and sig_bytes of
+// signatures, carved from one buffer, each area 256-byte aligned: the split's plan in mb (the uploaded tags and slots, the
+// tile prefixes, the compacted signatures in blob, and per family the indices, slots, hlen-byte digest rows in r, offsets
+// and verdicts), the staged signatures (16 bytes of read slack for k_mix_compact) and their offsets, and the vote-order
+// digests.  base == nullptr only sizes; returns the bytes the carve takes.
+struct RsaVoteBufs {
+    MixBufs mb;
+    uint8_t *sig, *dig;
+    uint64_t *sig_off;
+};
+size_t sbv_rsa_vote_carve(uint8_t *base, size_t n, const uint32_t m[3], uint64_t sig_bytes, uint32_t hlen, RsaVoteBufs *out);
+// The split of a staged shard of n RSA votes (rsa_quorum.cuh), m[f] of family f: b.tag and b.slot_in uploaded, d_dig the
+// vote-order digests (hlen bytes each), the signatures at d_sig with offsets d_sig_off from base (readable 16 bytes past
+// the last one).  b carries no sig96, key96, s or qx / qy: its r[f] are the families' digest rows, its blob the compacted
+// signatures (rsa_family_start).
+int sbv_launch_rsa_split(sbv_engine *e, const MixBufs &b, size_t n, const uint32_t m[3], const uint8_t *d_dig, uint32_t hlen, const uint8_t *d_sig,
+                         const uint64_t *d_sig_off, uint64_t base, cudaStream_t st);
 // the family verdicts b.ok[f] back into item order in d_ok
 int sbv_launch_mix_ok(sbv_engine *e, const MixBufs &b, size_t n, const uint32_t m[3], uint8_t *d_ok, cudaStream_t st);
 

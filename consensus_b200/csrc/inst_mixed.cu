@@ -1,7 +1,8 @@
-// inst_mixed.cu — launchers of the split / scatter kernels of mixed ECDSA / Ed25519 shards (mixed.cuh) behind engine.h,
-// and the layout of their device scratch.
+// inst_mixed.cu — launchers of the split / scatter kernels of mixed ECDSA / Ed25519 shards (mixed.cuh) and of RSA vote
+// shards (rsa_quorum.cuh) behind engine.h, and the layout of both kinds of shard's device scratch.
 #include "engine.h"
 #include "mixed.cuh"
+#include "rsa_quorum.cuh"
 
 using namespace sbv;
 
@@ -68,6 +69,51 @@ int sbv_launch_mix_split(sbv_engine *e, const MixBufs &b, size_t n, const uint32
         k_mix_split<<<(ntiles + 255) / 256, 256, 0, st>>>(nn, b.tag, b.slot_in, b.sig96, d_off, ntiles, b.tile_cnt, b.tile_bytes, p);
     k_mix_compact<<<(uint32_t)(((uint64_t)n * MIX_LANES + 255) / 256), 256, 0, st>>>(nn, m[0], m[1], d_msgs, d_off, base, p);
     e->launches += 4;
+    CU(e, cudaGetLastError());
+    return 0;
+}
+
+size_t sbv_rsa_vote_carve(uint8_t *base, size_t n, const uint32_t m[3], uint64_t sig_bytes, uint32_t hlen, RsaVoteBufs *out) {
+    RsaVoteBufs b{};
+    size_t at = 0;
+    auto take = [&](size_t sz) {
+        uint8_t *p = base ? base + at : nullptr;
+        at += al256(sz);
+        return p;
+    };
+    const size_t ntiles = (n + MIX_TILE - 1) / MIX_TILE;
+    const uint32_t mf[RSA_FAMILIES] = {m[0], m[1], m[2]};
+    b.mb.tag = take(n);
+    b.mb.slot_in = (uint32_t *)take(n * 4);
+    b.mb.tile_cnt = (uint32_t *)take(ntiles * RSA_FAMILIES * 4);
+    b.mb.tile_bytes = (uint64_t *)take(ntiles * RSA_FAMILIES * 8);
+    b.mb.blob = take(rsa_family_start(mf, RSA_FAMILIES));
+    for (int f = 0; f < RSA_FAMILIES; f++) {
+        b.mb.idx[f] = (uint32_t *)take(m[f] * 4);
+        b.mb.slot[f] = (uint32_t *)take(m[f] * 4);
+        b.mb.r[f] = take(m[f] * hlen);
+        b.mb.off[f] = (uint64_t *)take((m[f] + 1) * 8);
+        b.mb.ok[f] = take(m[f]);
+    }
+    b.sig = take(sig_bytes + 16);
+    b.sig_off = (uint64_t *)take((n + 1) * 8);
+    b.dig = take(n * hlen);
+    if (out) *out = b;
+    return at;
+}
+
+int sbv_launch_rsa_split(sbv_engine *e, const MixBufs &b, size_t n, const uint32_t m[3], const uint8_t *d_dig, uint32_t hlen, const uint8_t *d_sig,
+                         const uint64_t *d_sig_off, uint64_t base, cudaStream_t st) {
+    const uint32_t nn = (uint32_t)n, ntiles = (uint32_t)((n + MIX_TILE - 1) / MIX_TILE), fam = m[0] + m[1] + m[2];
+    const MixPlan p = plan_of(b);
+    k_mix_count<<<(ntiles + 255) / 256, 256, 0, st>>>(nn, b.tag, d_sig_off, ntiles, b.tile_cnt, b.tile_bytes);
+    k_mix_scan<<<1, MIX_SCAN_THREADS, 0, st>>>(ntiles, b.tile_cnt, b.tile_bytes, p);
+    k_rsa_split<<<(ntiles + 255) / 256, 256, 0, st>>>(nn, b.tag, b.slot_in, d_dig, hlen, d_sig_off, ntiles, b.tile_cnt, b.tile_bytes, p);
+    e->launches += 3;
+    if (fam) {
+        k_mix_compact<<<(uint32_t)(((uint64_t)fam * MIX_LANES + 255) / 256), 256, 0, st>>>(fam, m[0], m[1], d_sig, d_sig_off, base, p);
+        e->launches += 1;
+    }
     CU(e, cudaGetLastError());
     return 0;
 }

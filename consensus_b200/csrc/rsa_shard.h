@@ -59,6 +59,21 @@ bool rsa_h(uint32_t h, F &&f) {
 inline bool rsa_size_ok(uint32_t k) { return rsa_nl(k, [](auto) {}); }
 inline bool rsa_hash_ok(uint32_t h) { return rsa_h(h, [](auto) {}); }
 
+// The RSA commit votes (sbv_rsa_verify_quorum) carry signatures of the signer's key size, and the length alone decides a
+// vote's family, as Go's VerifyPKCS1v15 / VerifyPSS reject len(sig) != pub.Size(): 0 / 1 / 2 for 256 / 384 / 512 bytes,
+// RSA_NO_FAMILY for any other length (the vote rejects without reaching a kernel).
+constexpr int RSA_FAMILIES = 3;
+constexpr uint8_t RSA_NO_FAMILY = 3;
+inline uint8_t rsa_family(uint64_t len) { return len == 256 ? 0 : len == 384 ? 1 : len == 512 ? 2 : RSA_NO_FAMILY; }
+inline uint32_t rsa_family_k(int f) { return 256u + 128u * (uint32_t)f; }
+// Where family f's k-byte rows start in the compacted signature buffer of a split shard with m[c] votes of family c: the
+// region starts k_mix_scan lays out (each 16-byte aligned, after the previous region and 16 bytes of slack).
+inline uint64_t rsa_family_start(const uint32_t (&m)[RSA_FAMILIES], int f) {
+    uint64_t at = 0;
+    for (int c = 0; c < f; c++) at += ((uint64_t)m[c] * rsa_family_k(c) + 16 + 15) & ~(uint64_t)15;
+    return at;
+}
+
 // Every RSA kernel runs in blocks of 128 threads, `lanes` threads per item (a group of 16, or 1): the grid of `items`.
 constexpr uint32_t RSA_BLOCK = 128;
 inline uint32_t rsa_grid(size_t items, uint32_t lanes) { return (uint32_t)((items * lanes + RSA_BLOCK - 1) / RSA_BLOCK); }

@@ -140,7 +140,8 @@ enum { SBV_HASH_SHA256 = 0, SBV_HASH_SHA384 = 1, SBV_HASH_SHA512 = 2 };
  * tag above SBV_HASH_SHA512, a null buffer (msgs may be NULL when every message is empty), n >= 2^31 and decreasing offsets, all
  * before anything is written or launched.  Multi-device engines shard by item as sbv_hash_verify_batch does.  Each
  * device's shard is uploaded whole (no chunked upload).  Registered keys have calls of their own (sbv_rsa_set_keys, below).
- * Out of scope: RSA items in the mixed and commit-vote calls, and _device / _ranked forms. */
+ * Commit votes with registered keys have calls of their own (sbv_rsa_verify_quorum, below).  Out of scope: RSA items in
+ * the mixed calls, and _device / _ranked forms. */
 /* SHA-512 over a ragged batch (msgs / msg_off as in sbv_sha256_batch); digest_out = 64n bytes. */
 int sbv_sha512_batch(sbv_engine *e, size_t n, const uint8_t *msgs, const uint64_t *msg_off, uint8_t *digest_out);
 /* digests supplied: digest = n x hLen bytes; sig, modulus = n x mod_bytes bytes; pub_exp = n x uint32 */
@@ -289,6 +290,37 @@ int sbv_ed25519_verify_quorum(sbv_engine *e, size_t n_votes, const uint8_t *msgs
                               const uint16_t *sender, const uint16_t *signer, const uint8_t *digest_match,
                               size_t n_instances, const uint16_t *self_id, uint32_t threshold, uint8_t *ok,
                               uint32_t *valid_count, uint8_t *reached);
+
+/* sbv_verify_quorum for consenters with registered crypto/rsa keys (sbv_rsa_set_keys) of any mix of sizes: each consenter
+ * picks its own key size, so one call takes the votes as the wire carries them.  Vote i has its message
+ * msgs[msg_off[i]..msg_off[i+1]), hashed on the device with the call's hash tag (msgs may be NULL when every message is
+ * empty); its signature sig[sig_off[i]..sig_off[i+1]) of any length (sig may be NULL when every signature is empty); and
+ * the key of registry slot key_slot[i].
+ *  - ok[i]: for L = the signature's length in {256, 384, 512}, byte for byte what sbv_rsa_hash_verify_registered(L, hash,
+ *    ...) returns for vote i alone (sbv_rsa_pss_hash_verify_registered(L, hash, salt_len, ...) for the PSS form); 0 for
+ *    any other length, 0 included.  That is Go's VerifyPKCS1v15 / VerifyPSS, which reject len(sig) != pub.Size(), under
+ *    the registry's key rule: a slot >= n, a slot whose key failed the key rule, an empty registry and a slot whose key
+ *    size is not L reject.
+ *  - valid_count / reached = sbv_quorum over those verdicts, with the vote rules, self_id (NULL = no self filter),
+ *    threshold (the caller passes Quorum-1), ordering (votes grouped by non-decreasing instance, arrival order inside an
+ *    instance) and outputs of sbv_ed25519_verify_quorum; n_instances == 0 does nothing.  The verdicts stay on the device.
+ *  - Checks, all SBV_ERR_ARG before anything is written or launched: those of sbv_ed25519_verify_quorum, a hash tag above
+ *    SBV_HASH_SHA512, salt_len < -1 (PSS), and sig_off as msg_off (present, non-decreasing, sig NULL only when every
+ *    signature is empty).
+ *  - A multi-device engine shards BY INSTANCE, and every shard of one call reads the same registry.  Shards are uploaded
+ *    whole, not in chunks.  Each device's shard is split by key size on the device and every size present runs the
+ *    registered kernels of sbv_rsa_hash_verify_registered.
+ * Outputs: ok[n_votes], valid_count[n_instances], reached[n_instances]. */
+int sbv_rsa_verify_quorum(sbv_engine *e, uint8_t hash, size_t n_votes, const uint8_t *msgs, const uint64_t *msg_off,
+                          const uint32_t *key_slot, const uint8_t *sig, const uint64_t *sig_off, const uint32_t *instance,
+                          const uint16_t *sender, const uint16_t *signer, const uint8_t *digest_match, size_t n_instances,
+                          const uint16_t *self_id, uint32_t threshold, uint8_t *ok, uint32_t *valid_count, uint8_t *reached);
+/* sbv_rsa_verify_quorum with RSA-PSS verdicts; salt_len as in sbv_rsa_pss_verify_batch */
+int sbv_rsa_pss_verify_quorum(sbv_engine *e, uint8_t hash, int32_t salt_len, size_t n_votes, const uint8_t *msgs,
+                              const uint64_t *msg_off, const uint32_t *key_slot, const uint8_t *sig, const uint64_t *sig_off,
+                              const uint32_t *instance, const uint16_t *sender, const uint16_t *signer,
+                              const uint8_t *digest_match, size_t n_instances, const uint16_t *self_id, uint32_t threshold,
+                              uint8_t *ok, uint32_t *valid_count, uint8_t *reached);
 
 /* Registered-key batch whose items may be of any scheme (a consenter or client set that mixes ECDSA and Ed25519 keys,
  * e.g. while it moves from one to the other).  scheme[i] in {SBV_P256, SBV_P384, SBV_ED25519}; msgs concatenated with

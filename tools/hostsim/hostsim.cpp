@@ -34,6 +34,7 @@ namespace sbv { uint32_t tab[1 << 18]; }
 #include "../../consensus_b200/csrc/rsa_pss.cuh"
 #include "../../consensus_b200/csrc/rsa_keyed.cuh"
 #include "../../consensus_b200/csrc/sha512_batch.cuh"
+#include "../../consensus_b200/csrc/rsa_quorum.cuh"
 
 using namespace sbv;
 
@@ -998,4 +999,52 @@ extern "C" int hs_rsa_pss_verify_registered(uint32_t mod_bytes, uint8_t hash, in
     return rsa_launch_shard(RsaShard{mod_bytes, hash, RsaPad::pss, salt_len, n, sig, digest, ok, nullptr, nullptr, key_slot, nslots,
                                      reinterpret_cast<const uint4 *>(rec), pool},
                             hs_rsa_launch);
+}
+
+// ---- RSA commit votes (rsa_quorum.cuh, sbv_rsa_verify_quorum) ----
+// The device part of one shard of n RSA votes as stage_rsa_votes enqueues it, from the digests on: each vote's family from
+// its signature's length (rsa_family), then k_mix_count, k_mix_scan (as one thread), k_rsa_split and k_mix_compact over the
+// signatures (sig with offsets sig_off[0..n], read from a copy with 16 bytes of slack), rsa_launch_shard for every family
+// with votes against the registry of hs_rsa_kprep (nslots slots; rec, pool), and k_mix_ok over zeroed verdicts.  digest:
+// n rows of hLen bytes in vote order; pss: 0 PKCS #1 v1.5, 1 PSS with salt_len.  -1 (and nothing written) for a hash tag
+// outside the set or salt_len < -1.
+extern "C" int hs_rsa_quorum_shard(uint8_t hash, int pss, int32_t salt_len, size_t n, const uint8_t *digest, const uint32_t *slot_in, const uint8_t *sig,
+                                   const uint64_t *sig_off, uint32_t nslots, const uint32_t *rec, const uint32_t *pool, uint8_t *ok) {
+    if (!rsa_hash_ok(hash) || salt_len < PSS_SALT_EQUALS_HASH) return -1;
+    if (n == 0) return 0;
+    const uint32_t hl = 32 + 16 * hash, nn = (uint32_t)n, ntiles = (uint32_t)((n + MIX_TILE - 1) / MIX_TILE);
+    std::vector<uint8_t> tag(n);
+    uint32_t m[RSA_FAMILIES] = {0, 0, 0};
+    for (size_t i = 0; i < n; i++) {
+        tag[i] = rsa_family(sig_off[i + 1] - sig_off[i]);
+        if (tag[i] != RSA_NO_FAMILY) m[tag[i]]++;
+    }
+    const uint64_t base = sig_off[0], bytes = sig_off[n] - base;
+    std::vector<uint8_t> src(bytes + 16, 0), blob(rsa_family_start(m, RSA_FAMILIES), 0), okv(n, 0);
+    if (bytes) memcpy(src.data(), sig + base, bytes);
+    std::vector<uint32_t> tc((size_t)MIX_FAMILIES * ntiles), idx[RSA_FAMILIES], slot[RSA_FAMILIES];
+    std::vector<uint64_t> tb((size_t)MIX_FAMILIES * ntiles), off[RSA_FAMILIES];
+    std::vector<uint8_t> dig[RSA_FAMILIES], okf[RSA_FAMILIES];
+    MixPlan p;
+    for (int f = 0; f < RSA_FAMILIES; f++) {
+        idx[f].resize(m[f] + 1), slot[f].resize(m[f] + 1), off[f].resize(m[f] + 1), dig[f].resize((size_t)m[f] * hl + 1), okf[f].resize(m[f] + 1);
+        p.f[f] = MixFamily{idx[f].data(), slot[f].data(), dig[f].data(), nullptr, off[f].data(), okf[f].data()};
+    }
+    p.blob = blob.data();
+    run_grid((ntiles + 255) / 256, 256, [&] { k_mix_count(nn, tag.data(), sig_off, ntiles, tc.data(), tb.data()); });
+    run_grid(1, 1, [&] { k_mix_scan(ntiles, tc.data(), tb.data(), p); });
+    run_grid((ntiles + 255) / 256, 256, [&] { k_rsa_split(nn, tag.data(), slot_in, digest, hl, sig_off, ntiles, tc.data(), tb.data(), p); });
+    const uint32_t fam = m[0] + m[1] + m[2];
+    if (fam) run_grid((unsigned)(((uint64_t)fam * MIX_LANES + 255) / 256), 256, [&] { k_mix_compact(fam, m[0], m[1], src.data(), sig_off, base, p); });
+    for (int f = 0; f < RSA_FAMILIES; f++) {
+        if (!m[f]) continue;
+        RsaShard shard{rsa_family_k(f), hash, pss ? RsaPad::pss : RsaPad::pkcs1, salt_len, m[f], blob.data() + rsa_family_start(m, f), dig[f].data(),
+                       okf[f].data()};
+        shard.slot = slot[f].data();
+        shard.nslots = nslots, shard.rec = reinterpret_cast<const uint4 *>(rec), shard.pool = pool;
+        if (int rc = rsa_launch_shard(shard, hs_rsa_launch)) return rc;
+    }
+    if (fam) run_grid((unsigned)((fam + 255) / 256), 256, [&] { k_mix_ok(fam, m[0], m[1], p, okv.data()); });
+    memcpy(ok, okv.data(), n);
+    return 0;
 }

@@ -55,6 +55,7 @@ TABLE_SHAPES = ["tests/test_hostsim_table_shapes.py"]
 RSA = ["tests/test_hostsim_rsa.py"]  # rsa.cuh and k_sha512 (sha512_batch.cuh)
 RSA_PSS = ["tests/test_hostsim_rsa_pss.py"]  # k_rsa_em and k_rsa_pss (rsa_pss.cuh)
 RSA_REG = ["tests/test_hostsim_rsa_registered.py"]  # registered RSA keys (rsa_keyed.cuh)
+RSA_QUORUM = ["tests/test_hostsim_rsa_quorum.py"]  # RSA commit votes: rsa_family and k_rsa_split (rsa_quorum.cuh)
 MIXED384 = ["tests/test_hostsim_mixed384.py"]  # k_mix_alg and k_sha2_sel (mixed_hash.cuh)  # every entry of the per-key tables at the key counts where the builds turn over
 
 
@@ -422,6 +423,12 @@ CATALOGUE = [
     M("rsa_plan_group_grid_items", "rsa_shard.h", "(items * lanes + RSA_BLOCK - 1)", "(items + RSA_BLOCK - 1)", RSA + RSA_PSS + RSA_REG),
     M("rsa_plan_pss_salt_auto", "rsa_keyed.cuh", "launch(k_rsa_pss<H>, 1, s.n, n, s.k, s.salt_len,", "launch(k_rsa_pss<H>, 1, s.n, n, s.k, PSS_SALT_AUTO,",
       RSA_PSS),
+    # ---------------------------------------------------------------- rsa_shard.h and rsa_quorum.cuh: the split of RSA commit votes by key size
+    M("rsa_family_384_as_2048", "rsa_shard.h", "len == 384 ? 1 :", "len == 384 ? 0 :", RSA_QUORUM),
+    M("rsa_family_start_no_slack", "rsa_shard.h", "rsa_family_k(c) + 16 + 15)", "rsa_family_k(c) + 15)", RSA_QUORUM),
+    M("rsa_split_digest_at_rank", "rsa_quorum.cuh", "dig + (size_t)i * hlen,", "dig + (size_t)j * hlen,", RSA_QUORUM),
+    M("rsa_split_slot_of_tile_head", "rsa_quorum.cuh", "F.slot[j] = slot[i];", "F.slot[j] = slot[lo];", RSA_QUORUM),
+    M("rsa_split_index_at_rank", "rsa_quorum.cuh", "F.idx[j] = i;", "F.idx[j] = lo + j % MIX_TILE;", RSA_QUORUM),
     # ---------------------------------------------------------------- sha512_batch.cuh
     M("sha512_batch_length_bytes", "sha512_batch.cuh", "w[15] = len << 3;", "w[15] = len;", RSA),
     M("sha512_batch_iv", "sha512_batch.cuh", "0x5be0cd19137e2179ull", "0x47b5481dbefa4fa4ull", RSA),
